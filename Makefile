@@ -1,6 +1,6 @@
-# Builds libb200exec.so (the product: CUDA kernels + C-ABI host engine) for sm_100a, in-tree.
+# Builds libb200exec.so (the product: CUDA kernels + C-ABI host engine) for sm_90a, in-tree.
 NVCC      ?= nvcc
-ARCH      := -gencode arch=compute_100a,code=sm_100a
+ARCH      := -gencode arch=compute_90a,code=sm_90a
 PKG       := datafusion-ballista_b200
 SRC       := $(PKG)/csrc
 OUT       := $(PKG)/lib

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- TPC-H through the B200 execution engine; headline: q1 SF10 (BASELINE.json configs[1]).
+"""bench.py -- TPC-H through the CUDA execution engine; headline: q1 SF10 (BASELINE.json configs[1]).
 
 One "step" = one full pass of the hot path over the resident synthetic lineitem table:
   stage 1  scan -> FilterExec -> ProjectionExec -> AggregateExec(Partial) -> hash ShuffleWriter
@@ -7,13 +7,16 @@ One "step" = one full pass of the hot path over the resident synthetic lineitem 
   stage 3  ShuffleReader -> SortPreservingMergeExec -> ShuffleWriter(None)
 exactly the stage shapes Ballista's planner emits for q1 (ballista/scheduler/src/planner.rs:655-670).
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--dump-outputs DIR]
 N>1 is launched by the driver under torchrun (one rank per GPU, NCCL); every rank owns SF10 worth
 of lineitem rows (weak scaling: the global table is SF(10*N)), the partial aggregate states are
 exchanged with an NCCL all-to-all, and `value` is global rows / max-over-ranks device time.
 
 `--impl reference` times the CPU restatement of the reference path (oracle/, all host threads) on
 a bounded sample of the same workload: the reference itself (Rust) cannot be built offline.
+
+`--dump-outputs DIR` writes, after the timed steps, the result tables of the last timed step as DIR/<query>.<column>.npy
+(float64; see dump_outputs) so that two builds can be compared output for output on identical generated inputs.
 """
 from __future__ import annotations
 
@@ -156,13 +159,13 @@ def measured_hbm_peak():
         with open(p) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md)"
+        return 3350.0, "data sheet (H100 SXM HBM3, 3.35 TB/s; not a measured peak)"
 
 
 # ---- CPU arm (oracle) -------------------------------------------------------------------------------
 def usable_cpus() -> int:
-    """CPUs this process may actually use: the cgroup quota when there is one (the B200 boxes expose 128
-    hardware threads under a 16-CPU quota; oversubscribing it only adds throttling), else os.cpu_count()."""
+    """CPUs this process may actually use: the cgroup quota when there is one (a container may expose many more
+    hardware threads than its quota; oversubscribing it only adds throttling), else os.cpu_count()."""
     n = os.cpu_count() or 1
     try:
         quota, period = open("/sys/fs/cgroup/cpu.max").read().split()[:2]
@@ -405,6 +408,8 @@ def run_b200(args):
     ms = e0.elapsed_time(e1)
     launches = eng.kernel_launches() - launches0
     exch_timed = dict(exch)   # the e2e passes below go through the same step()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, {"q1": pa.Table.from_batches([res])})
     clocks = sampler.stop() if rank == 0 else None
     if world > 1:
         t = torch.tensor([ms], dtype=torch.float64, device=device)
@@ -447,14 +452,7 @@ def run_b200(args):
         kern_s = (agg_ns[0] / max(agg_ns[1], 1)) / 1e9
         alg_bytes = ROWS_SF10 * BYTES_PER_ROW + 4 * (2 * 5 + 13 * 16)
         achieved = alg_bytes / kern_s / 1e9 if kern_s > 0 else 0.0
-        traffic, traffic_src = None, None
-        tp = os.path.join(ROOT, "profiles", "q1_stage1_traffic.json")
-        if os.path.exists(tp):
-            try:
-                tj = json.load(open(tp))
-                traffic, traffic_src = tj.get("dram_bytes_per_launch"), tj.get("source")
-            except Exception:
-                traffic = None
+        traffic, traffic_src = None, "not measured"
         line = {
             "metric": METRIC, "value": value, "unit": "rows/s", "n_gpus": world, "steps": args.steps,
             "warmup": max(args.warmup, 3), "ms_per_step": ms / args.steps, "higher_is_better": True,
@@ -462,7 +460,7 @@ def run_b200(args):
             "q1_steps_per_hour": 3600.0 / (ms / 1e3 / args.steps),
             "config": {"workload": "TPC-H q1 SF10 (BASELINE.json configs[1]): lineitem 59,986,052 rows x 7 columns, "
                                    "Arrow layout resident in HBM, 1 GPU executor per GPU", "rows_per_gpu": ROWS_SF10,
-                       "target_partitions": P, "l2_policy": "inputs (4.68 GB per GPU) far larger than the 126 MB L2",
+                       "target_partitions": P, "l2_policy": "inputs (4.68 GB per GPU) far larger than the 50 MB L2",
                        "stages": "scan+filter+project+partial-agg+hash-shuffle | final-agg+sort | merge",
                        "exchange": "in-library NCCL send/recv (b200_exchange_stage): hash repartition + gather to the merge task" if world > 1 else "none (1 executor)"},
             "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
@@ -612,6 +610,8 @@ def run_workload(args):
     clocks = sampler.stop() if rank == 0 else None
     launches = eng.kernel_launches() - launches0
     kstats = eng.kernel_stats(reset=True)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, res)
     # self-consistency at full scale (the oracle cannot hold SF100): a different shuffle fan-out must give the same table
     consistent = None
     if not args.no_parity:
@@ -643,7 +643,7 @@ def run_workload(args):
             "vs_baseline": None, "dtype": "decimal128/i128 (+f64 where the SQL forces it)", "data": "synthetic",
             "config": {"workload": f"TPC-H {args.workload} SF{sf:g}, {world} GPU executors, hash joins (prefer_hash_join=true), "
                                    f"target_partitions={P}, tables resident in HBM (row-range partitioned, nation/region replicated)",
-                       "queries": names, "l2_policy": "inputs far larger than the 126 MB L2", "timing": "per query: max over ranks of the wall clock between barriers (device synchronised)"},
+                       "queries": names, "l2_policy": "inputs far larger than the 50 MB L2", "timing": "per query: max over ranks of the wall clock between barriers (device synchronised)"},
             "per_query_ms": {nme: 1e3 * sec[nme] for nme in names},
             "queries_per_hour": len(names) * 3600.0 / total_s,
             "base_rows_scanned": rows,
@@ -723,6 +723,68 @@ def measure_e2e(eng, bb, pa, torch, dist, step, rank, world, device, steps):
                     "Decimal128 sign-extension bytes, H2D of h2d_bytes_per_step, device widens) -> 3 stages (+ exchanges) -> b200_partition_export (D2H)"}
 
 
+DUMP_LIMIT_BYTES = 63 << 20  # + the .npy headers: under 64 MB in all
+
+
+def _string_chunks(col, width):
+    """A Utf8 column as a (rows, 1 + width) array: the UTF-8 byte length, then the bytes in 6-byte big-endian chunks
+    (each exact in float64), zero-padded; a NULL row is all NaN.  Distinct strings give distinct rows."""
+    import numpy as np
+    out = np.zeros((len(col), 1 + width), dtype=np.float64)
+    for r, v in enumerate(col.to_pylist()):
+        if v is None:
+            out[r] = np.nan
+            continue
+        b = v.encode()
+        out[r, 0] = len(b)
+        for k in range(0, len(b), 6):
+            out[r, 1 + k // 6] = int.from_bytes(b[k:k + 6].ljust(6, b"\0"), "big")
+    return out
+
+
+def dump_outputs(out_dir, tables):
+    """Writes every column of every result table as out_dir/<query>.<column>.npy, float64, one row per result row: integers,
+    decimals (value / 10^scale) and dates (days since the epoch) as one number, NULL as NaN; strings as (rows, 1 + chunks)
+    arrays (see _string_chunks), so the whole string is compared.  When the tables would take more than 64 MB in all, every
+    table is cut to the same fraction of its rows by a fixed, seeded sample (the same rows for the same row count)."""
+    import numpy as np
+    import pyarrow as pa
+    import pyarrow.compute as pc
+    os.makedirs(out_dir, exist_ok=True)
+    tables = {q: t for q, t in tables.items() if t is not None}
+    widths, total = {}, 0
+    for q, t in tables.items():
+        for name in t.column_names:
+            ty = t.column(name).type
+            if pa.types.is_string(ty) or pa.types.is_large_string(ty):
+                longest = pc.max(pc.binary_length(t.column(name))).as_py() or 0
+                widths[q, name] = -(-longest // 6)
+                total += 8 * (1 + widths[q, name]) * t.num_rows
+            else:
+                total += 8 * t.num_rows
+    keep_frac = min(1.0, DUMP_LIMIT_BYTES / total) if total else 1.0
+    for q, t in tables.items():
+        rows = t.num_rows
+        if keep_frac < 1.0:
+            keep = np.sort(np.random.default_rng(0).choice(rows, int(rows * keep_frac), replace=False))
+            t = t.take(pa.array(keep))
+        for name in t.column_names:
+            col = t.column(name).combine_chunks()
+            ty = col.type
+            if (q, name) in widths:
+                v = _string_chunks(col, widths[q, name])
+            elif pa.types.is_decimal(ty):
+                v = np.array([np.nan if d is None else float(d) for d in col.to_pylist()])
+            else:
+                if pa.types.is_date32(ty):
+                    col = col.cast(pa.int32())
+                elif pa.types.is_boolean(ty):
+                    col = col.cast(pa.int8())
+                v = pc.cast(col, pa.float64()).to_numpy(zero_copy_only=False)
+            np.save(os.path.join(out_dir, f"{q}.{name}.npy"), np.asarray(v, dtype=np.float64))
+    log(f"wrote the outputs of {len(tables)} quer{'y' if len(tables) == 1 else 'ies'} to {out_dir}")
+
+
 _REAL_STDOUT = None
 
 
@@ -754,6 +816,7 @@ def main():
     ap.add_argument("--no-fused-shuffle", action="store_true", help="N>1: always shuffle in two steps (writer, then NCCL exchange)")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-parity", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="after the timed steps, write the last timed step's result tables as DIR/<query>.<column>.npy")
     args = ap.parse_args()
     if args.impl == "reference":
         run_reference(args)

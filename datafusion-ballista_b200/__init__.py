@@ -1,4 +1,4 @@
-"""B200-native execution engine for Apache DataFusion Ballista's executor hot path.
+"""CUDA-native (H100, sm_90a) execution engine for Apache DataFusion Ballista's executor hot path.
 
 Host-side mirror (Python harness) of the reference plug-in interface
 ``ExecutionEngine`` / ``QueryStageExecutor`` (ballista/executor/src/execution_engine.rs:45-81) on

@@ -1,4 +1,4 @@
-// FilterExec (+ column projection) without the tile VM (sm_100a): predicates that are boolean combinations of comparisons
+// FilterExec (+ column projection) without the tile VM (sm_90a): predicates that are boolean combinations of comparisons
 // between plain columns and literals -- every TPC-H scan filter except LIKE -- evaluated per row in registers, the
 // surviving rows of the forwarded columns compacted in input order.
 //

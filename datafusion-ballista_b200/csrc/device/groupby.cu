@@ -1,4 +1,4 @@
-// High-cardinality GROUP BY kernel (sm_100a): AggregateExec(Partial | Final*) whose keys are one or two integer-like
+// High-cardinality GROUP BY kernel (sm_90a): AggregateExec(Partial | Final*) whose keys are one or two integer-like
 // columns and whose aggregates are COUNT / SUM (AVG = SUM + COUNT) over plain columns or decimal products.
 //
 // Reference operator: AggregateExec + GroupsAccumulator [EXT, DataFusion 53.1] (wire surface
@@ -11,7 +11,7 @@
 // (the slot word holds mix64(key image), a bijection, so ONE 8-byte compare identifies the group exactly) and updates
 // the accumulators with L2 atomics: COUNT is a fire-and-forget reduction, a 128-bit SUM is one 64-bit atomic add plus a
 // second one only when a carry or a non-zero high word exists.  Table traffic is random access: while the table fits the
-// 126 MB L2 the kernel runs at the column-scan rate, beyond that it is bound by 32-byte-sector DRAM accesses.
+// 50 MB L2 the kernel runs at the column-scan rate, beyond that it is bound by 32-byte-sector DRAM accesses.
 // Anything outside the pattern (wide decimal operands, keys that do not fit the image) raises `bail` and the host
 // re-runs the aggregate on the general tile-VM sink: same results by construction.
 #include <cuda_runtime.h>

@@ -1,4 +1,4 @@
-// Hash join kernels (sm_100a): HashJoinExec build + single-pass probe.
+// Hash join kernels (sm_90a): HashJoinExec build + single-pass probe.
 //
 // Reference operator: HashJoinExec [EXT, DataFusion 53.1] (wire surface ballista/core/proto/datafusion.proto:1134-1144):
 // the build side is collected into one batch + a chained hash map, probe batches are hashed, candidate pairs are
@@ -25,7 +25,7 @@ namespace b200 {
 static inline int join_grid(int64_t n, int block, int per_thread) {
   int64_t g = (n + (int64_t)block * per_thread - 1) / ((int64_t)block * per_thread);
   if (g < 1) g = 1;
-  if (g > 148 * 16) g = 148 * 16;
+  if (g > 132 * 16) g = 132 * 16;
   return (int)g;
 }
 

@@ -1,4 +1,4 @@
-// Auxiliary CUDA kernels (sm_100a): aggregate-table init/extraction, prefix sums, hash-partition
+// Auxiliary CUDA kernels (sm_90a): aggregate-table init/extraction, prefix sums, hash-partition
 // rank + scatter (ShuffleWriter), gathers, string view <-> Arrow Utf8 conversion, hash-join
 // build/probe, LSD radix sort, and the synthetic TPC-H generator.
 //
@@ -21,7 +21,7 @@ typedef unsigned __int128 u128;
 static inline int grid_for(int64_t n, int block, int per_thread = 1) {
   int64_t g = (n + (int64_t)block * per_thread - 1) / ((int64_t)block * per_thread);
   if (g < 1) g = 1;
-  if (g > 148 * 16) g = 148 * 16;  // grid-stride loops; a multiple of the SM count
+  if (g > 132 * 16) g = 132 * 16;  // grid-stride loops; a multiple of the SM count (H100 SXM: 132)
   return (int)g;
 }
 

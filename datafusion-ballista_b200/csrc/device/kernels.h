@@ -1,4 +1,4 @@
-// Host-callable launchers of every CUDA kernel in libb200exec (sm_100a).
+// Host-callable launchers of every CUDA kernel in libb200exec (sm_90a).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>

@@ -1,4 +1,4 @@
-// Parquet page decode on the GPU (sm_100a): definition levels, dictionaries, PLAIN and RLE_DICTIONARY values ->
+// Parquet page decode on the GPU (sm_90a): definition levels, dictionaries, PLAIN and RLE_DICTIONARY values ->
 // the engine's HBM column layout (Arrow fixed-width values, 16-byte string views into the raw page bytes, validity bytes).
 //
 // Reference path: DataSourceExec + ParquetSource (ballista/core/proto/datafusion.proto:1058-1077) -> parquet 58.1 [EXT]

@@ -1,4 +1,4 @@
-// Fused pipeline kernel for sm_100a:  scan -> [FilterExec | ProjectionExec]* -> sink
+// Fused pipeline kernel for sm_90a:  scan -> [FilterExec | ProjectionExec]* -> sink
 // (sink = materialise/compact | partial-or-final hash aggregate).
 //
 // Reference operators replaced (SURVEY.md 8(a) R9a-R9c): DataFusion FilterExec, ProjectionExec and

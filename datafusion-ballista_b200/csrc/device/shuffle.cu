@@ -1,4 +1,4 @@
-// Shuffle-side CUDA kernels (sm_100a): one-pass stable radix partition (ShuffleWriterExec /
+// Shuffle-side CUDA kernels (sm_90a): one-pass stable radix partition (ShuffleWriterExec /
 // SortShuffleWriterExec), the exchange message packer, and the small-result export packer.
 //
 // Reference behaviour being reproduced:

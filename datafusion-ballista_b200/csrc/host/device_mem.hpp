@@ -1,4 +1,4 @@
-// Device-resident columnar batch model (HBM layout) of the B200 engine.
+// Device-resident columnar batch model (HBM layout) of the engine.
 //
 // Layout = Arrow's, as delivered at the ExecutionPlan boundary (SURVEY.md 8 "Conventions"):
 //   fixed width  : values buffer, `width` bytes per row (Decimal128: 16-byte LE two's complement)

@@ -69,7 +69,7 @@ struct OpMetrics {
 struct b200_engine {
   int device = 0;
   int rank = 0, world = 1;
-  int sm_count = 148;
+  int sm_count = 132;
   cudaStream_t own_stream = nullptr;
   cudaStream_t stream = nullptr;
   std::mutex mu;
@@ -521,8 +521,7 @@ void ingest_decimal_narrowed(b200_engine* e, const uint8_t* src, uint8_t* dst, i
   std::lock_guard<std::mutex> ingest_guard(e->ingest_mu);
   if (!e->pool) {
     // default pool size: 1.5 x the CPUs this process may use (cgroup quota if there is one; the loops
-    // are memory-latency bound, a few more threads than cores help, many more get throttled) --
-    // measured on the B200 box (16-CPU quota): 12/16/24/32 threads -> 59.8/58.1/48.7/57.9 ms for SF10 lineitem
+    // are memory-latency bound, a few more threads than cores help, many more get throttled)
     int cpus = (int)std::thread::hardware_concurrency();
     if (cpus <= 0) cpus = 8;
     if (FILE* f = fopen("/sys/fs/cgroup/cpu.max", "r")) {
@@ -890,7 +889,9 @@ bool match_fast_filter(const Program& P, FastFilterSpec& S);
 // device (launch_groupby_plan): no host synchronisation between the partition and the aggregation.
 bool partition_for_groupby(const Exec& x, GroupBySpec& S, std::vector<DevPtr>& keep) {
   // b200.agg.partition_first.bucket_slots (default 2^19 slots ~ 32 MB of touched cells; 0 = never partition),
-  // b200.agg.partition_first.min_rows (default 2^22)
+  // b200.agg.partition_first.min_rows (default 2^22).  On an H100 SXM (700 W limit), GROUP BY l_partkey (2 M groups) /
+  // l_orderkey (15 M groups) over SF10 lineitem, SUM + COUNT, median of 3: 2^19 slots 4.99 / 7.88 ms, 2^18 5.05 / 7.74 ms,
+  // 2^17 5.46 / 7.95 ms, never partitioned 11.16 / 8.75 ms.  The min_rows threshold has not been measured on an H100.
   const uint64_t GB_PF_BUCKET_SLOTS = x.e->pf_bucket_slots;
   if (!GB_PF_BUCKET_SLOTS || S.n_keys < 1 || S.table.cap < GB_PF_BUCKET_SLOTS * 8 || S.n_rows < x.e->pf_min_rows || S.n_rows >= ((int64_t)1 << 32)) return false;
   for (int k = 0; k < S.n_keys; k++) {
@@ -1373,9 +1374,10 @@ bool match_fused(const Program& P, FusedPlan& FP) {
   for (int a = 0; a < P.n_acc; a++)
     if (!(P.acc[a].kind == ACC_SUM_I128 || P.acc[a].kind == ACC_COUNT || P.acc[a].kind == ACC_COUNT_STAR)) return false;
   // stage layout: every column of the program, one warp tile of 32*R rows each
-  // measured on B200 (profiles/r01_summary.md): 4 rows per thread amortise the per-tile work (claim, TMA
-  // issue, barrier wait) best; grouped shapes then fit 8 warps of up to 255 registers next to their
-  // shared-memory partials, scalar shapes 12 warps
+  // 4 rows per thread amortise the per-tile work (claim, TMA issue, barrier wait); grouped shapes then fit
+  // 8 warps of up to 255 registers next to their shared-memory partials, scalar shapes 12 warps.  On an
+  // H100 SXM (700 W limit) stage 1 of q1 at SF10 took 1.62-1.73 ms at R=4 / 256 threads against
+  // 1.69-1.83 ms for R=4 / 384 and R=2 / 256, 384, 512
   const int R = env_int("B200_FUSED_R", 4);
   if (!(R == 2 || R == 4)) return false;
   int block = env_int("B200_FUSED_B", (R == 4 && P.n_keys) ? 256 : 384);
@@ -4094,7 +4096,7 @@ static void setup_window(b200_engine* e) {
 
 extern "C" {
 
-const char* b200_version(void) { return "b200exec 0.1 sm_100a"; }
+const char* b200_version(void) { return "b200exec 0.1 sm_90a"; }
 const char* b200_last_error(void) { return g_err.c_str(); }
 
 // Ingest is a host<->GPU pipeline (pinned staging, a pool of narrowing threads, DMA): it only reaches the PCIe rate when
@@ -4147,7 +4149,7 @@ int b200_engine_create(int device, uint64_t pool_bytes, int rank, int world, b20
     int ndev = 0;
     cudaError_t ce = cudaGetDeviceCount(&ndev);
     if (ce != cudaSuccess || ndev == 0)
-      throw EngineError(B200_ERR_CUDA, std::string("no CUDA device available: the B200 engine has no CPU path (") + cudaGetErrorString(ce) + ")");
+      throw EngineError(B200_ERR_CUDA, std::string("no CUDA device available: the engine has no CPU path (") + cudaGetErrorString(ce) + ")");
     if (device < 0 || device >= ndev) throw EngineError(B200_ERR_INVALID, "bad device ordinal");
     CUDA_CHECK(cudaSetDevice(device));
     bind_to_gpu_numa_node(device);

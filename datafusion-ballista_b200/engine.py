@@ -92,7 +92,7 @@ def load_library():
         return _lib
     if not os.path.exists(LIB_PATH):
         raise RuntimeError(f"{LIB_PATH} is missing: run `make` (or __graft_entry__.build()); "
-                           "the B200 engine has no CPU fallback")
+                           "the engine has no CPU fallback")
     L = C.CDLL(LIB_PATH)
     vp, cp, i64, u64, ci = C.c_void_p, C.c_char_p, C.c_int64, C.c_uint64, C.c_int
     L.b200_engine_create.argtypes = [ci, u64, ci, ci, C.POINTER(vp)]

@@ -1,6 +1,6 @@
 /* Arrow C Data Interface structs (https://arrow.apache.org/docs/format/CDataInterface.html).
  * This is the ABI-stable layout both arrow-rs (`arrow::ffi::FFI_ArrowArray/FFI_ArrowSchema`)
- * and pyarrow (`_export_to_c`) produce; the B200 engine's C-ABI exchanges all column data
+ * and pyarrow (`_export_to_c`) produce; the engine's C-ABI exchanges all column data
  * with the host through these structs (SURVEY.md §8(b), last row).                      */
 #ifndef B200_ARROW_ABI_H
 #define B200_ARROW_ABI_H

@@ -1,4 +1,4 @@
-/* libb200exec -- C ABI of the B200-native Ballista execution engine.
+/* libb200exec -- C ABI of the CUDA-native (H100, sm_90a) Ballista execution engine.
  *
  * The reference defines NO C ABI: its plug-in point is the Rust trait pair
  *   ExecutionEngine::create_query_stage_exec   ballista/executor/src/execution_engine.rs:45-59
@@ -275,7 +275,7 @@ int b200_shuffle_read_file(b200_engine* e, const char* job_id, int64_t stage_id,
 void* b200_host_alloc_pinned(uint64_t bytes);
 void b200_host_free_pinned(void* p);
 
-/* Version / build info: "b200exec <ver> sm_100a" */
+/* Version / build info: "b200exec <ver> sm_90a" */
 const char* b200_version(void);
 
 #ifdef __cplusplus

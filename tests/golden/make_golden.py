@@ -1,7 +1,7 @@
 """Generates the committed golden fixtures from the reference's own test data.
 
-Run in the build container only (needs /root/reference):  python tests/golden/make_golden.py
-Outputs (committed; the GPU box never reads /root/reference):
+BALLISTA_SRC=<datafusion-ballista checkout> python tests/golden/make_golden.py
+Outputs (committed; the tests read only these):
   tests/golden/alltypes_plain.json      <- ballista/client/testdata/alltypes_plain.parquet
   tests/golden/aggregate_test_100.json  <- examples/testdata/aggregate_test_100.csv
   tests/golden/python_test.json         <- python/testdata/test.csv
@@ -14,7 +14,7 @@ import pyarrow as pa
 import pyarrow.csv as pacsv
 import pyarrow.parquet as pq
 
-REF = "/root/reference"
+REF = os.environ.get("BALLISTA_SRC", "")
 OUT = os.path.dirname(os.path.abspath(__file__))
 
 

@@ -1,6 +1,6 @@
 """Generate tests/golden/proto_plans.json: stage plans as the protobuf bytes a Ballista scheduler ships to an executor.
 
-    python tests/golden/make_proto_plans.py            (needs /root/reference: run in the build container, commit the output)
+    BALLISTA_SRC=<datafusion-ballista checkout> python tests/golden/make_proto_plans.py      (commit the output)
 
 For every stage of the 22 TPC-H queries (ballista_b200/tpch.py) and a few extra shapes, the stage-plan IR is typed by the
 engine's own plan front end (b200_plan_typed_json: resolved column indices, node schemas) and then ENCODED as
@@ -452,6 +452,52 @@ def main():
         json.dump({"generated_by": "tests/golden/make_proto_plans.py", "proto_files": "ballista/core/proto/{datafusion_common,datafusion,ballista}.proto",
                    "cases": cases, "tasks": tasks, "statuses": statuses}, fh, indent=0)
     print(len(cases), "plans,", sum(len(c["proto_b64"]) for c in cases) * 3 // 4, "proto bytes")
+    write_reference_checks(cases)
+    write_random_plans()
+
+
+def write_reference_checks(cases):
+    """What google.protobuf, given the reference's message definitions, reports for every fixture (tests/golden/proto_plans_checked.json):
+    the fixture parses completely and re-serialises byte-identically, which oneof its root and its Ballista node hold, and the field
+    numbers involved, so that tests/test_plan_proto.py can check the fixtures without the .proto files."""
+    import hashlib
+    P, E, B = C("datafusion.PhysicalPlanNode"), C("datafusion.PhysicalExtensionNode"), C("ballista.protobuf.BallistaPhysicalPlanNode")
+    checked = []
+    for c in cases:
+        raw = base64.b64decode(c["proto_b64"])
+        m = P()
+        m.ParseFromString(raw)
+        b = B()
+        b.ParseFromString(m.extension.node)
+        checked.append({"name": c["name"], "sha256": hashlib.sha256(raw).hexdigest(), "reserialises_identically": m.SerializeToString() == raw,
+                        "root_oneof": m.WhichOneof("PhysicalPlanType"), "ballista_oneof": b.WhichOneof("PhysicalPlanType"),
+                        "extension_inputs": len(m.extension.inputs)})
+    fields = {"PhysicalPlanNode.extension": P.DESCRIPTOR.fields_by_name["extension"].number,
+              "PhysicalExtensionNode.node": E.DESCRIPTOR.fields_by_name["node"].number,
+              "PhysicalExtensionNode.inputs": E.DESCRIPTOR.fields_by_name["inputs"].number,
+              "BallistaPhysicalPlanNode.shuffle_writer": B.DESCRIPTOR.fields_by_name["shuffle_writer"].number,
+              "BallistaPhysicalPlanNode.sort_shuffle_writer": B.DESCRIPTOR.fields_by_name["sort_shuffle_writer"].number}
+    with open(os.path.join(HERE, "proto_plans_checked.json"), "w") as fh:
+        json.dump({"generated_by": "tests/golden/make_proto_plans.py", "field_numbers": fields, "cases": checked}, fh, indent=0)
+
+
+def write_random_plans():
+    """The seeded random plans of tests/test_plan_proto_random.py, encoded (tests/golden/random_proto_plans.json.gz: seed -> bytes)."""
+    import gzip
+    sys.path.insert(0, os.path.dirname(HERE))
+    import test_plan_proto_random as T
+    from ballista_b200 import engine
+    protos = {}
+    for seed in range(T.N_SEEDS):
+        ir = json.dumps(T._plan(seed), separators=(",", ":"))
+        try:
+            engine.plan_typed_json(ir)
+        except engine.B200Error:
+            continue
+        protos[str(seed)] = base64.b64encode(encode(ir)).decode()
+    with gzip.GzipFile(os.path.join(HERE, "random_proto_plans.json.gz"), "wb", mtime=0) as fh:
+        fh.write(json.dumps({"generated_by": "tests/golden/make_proto_plans.py", "protos": protos}, separators=(",", ":")).encode())
+    print(len(protos), "random plans")
 
 
 if __name__ == "__main__":

@@ -8,6 +8,7 @@ the bytes under tests/golden/proto_plans.json are what a conforming protobuf enc
 restatement of them.  Supports what the three files use: messages (nested), enums, oneof, repeated / optional, map<,>,
 imports, packages, reserved, options (ignored), services (ignored).
 """
+import os
 import re
 
 from google.protobuf import descriptor_pb2, descriptor_pool, message_factory
@@ -252,7 +253,12 @@ def load(paths):
     return classes, pool
 
 
-def load_ballista(proto_dir="/root/reference/ballista/core/proto"):
+def load_ballista(proto_dir=None):
+    """The message classes of a datafusion-ballista checkout's ballista/core/proto (default: $BALLISTA_SRC/ballista/core/proto)."""
+    if proto_dir is None:
+        if not os.environ.get("BALLISTA_SRC"):
+            raise RuntimeError("set BALLISTA_SRC to a datafusion-ballista checkout")
+        proto_dir = os.path.join(os.environ["BALLISTA_SRC"], "ballista", "core", "proto")
     return load([("datafusion_common.proto", proto_dir + "/datafusion_common.proto"),
                  ("datafusion.proto", proto_dir + "/datafusion.proto"),
                  ("ballista.proto", proto_dir + "/ballista.proto")])

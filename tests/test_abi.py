@@ -26,7 +26,7 @@ def test_python_binding_lists_the_same_symbols():
 
 
 def test_version_string():
-    assert b"sm_100a" in bb.engine.load_library().b200_version()
+    assert b"sm_90a" in bb.engine.load_library().b200_version()
 
 
 def test_struct_layouts_match_header():
@@ -70,7 +70,7 @@ def test_header_is_plain_c_and_usable_without_python(tmp_path):
     out = subprocess.run([exe, str(plan)], capture_output=True, text=True, timeout=120)
     assert out.returncode == 0, out.stdout + out.stderr
     kv = dict(tok.split("=", 1) for line in out.stdout.splitlines() for tok in line.split() if "=" in tok)
-    assert "sm_100a" in out.stdout
+    assert "sm_90a" in out.stdout
     assert int(kv["sizeof_task_result"]) == C.sizeof(bb.engine.TaskResult)
     assert int(kv["sizeof_swp"]) == C.sizeof(bb.engine.ShuffleWritePartition) and int(kv["sizeof_metrics"]) == C.sizeof(bb.engine.OperatorMetrics)
     assert kv["has_job"] == "1" and int(kv["ir_bytes"]) > 100 and int(kv["typed_bytes"]) > 100

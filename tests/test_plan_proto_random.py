@@ -1,12 +1,13 @@
 """Randomised round trip of the protobuf plan decoder: seeded random well-typed stage plans (nested expressions of every kind
 over a seven-column schema, under Filter / Projection / Aggregate / HashJoin with residual filter / Sort / Limit) are encoded
-as datafusion.PhysicalPlanNode by the fixture generator (google.protobuf over the reference's .proto files) and decoded by
-csrc/common/plan_proto.hpp; typed(decoded) must equal typed(source).  Needs the reference's .proto files, so it runs in the
-build container (the GPU box runs only `-m gpu`)."""
+as datafusion.PhysicalPlanNode by the fixture generator (google.protobuf over the reference's .proto files; stored per seed in
+tests/golden/random_proto_plans.json.gz by tests/golden/make_proto_plans.py) and decoded by csrc/common/plan_proto.hpp;
+typed(decoded) must equal typed(source)."""
+import base64
+import gzip
 import json
 import os
 import random
-import sys
 
 import pytest
 
@@ -14,7 +15,7 @@ from ballista_b200 import engine
 from ballista_b200 import plan as P
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-pytestmark = pytest.mark.skipif(not os.path.exists("/root/reference/ballista/core/proto/datafusion.proto"), reason="needs the reference's .proto files")
+N_SEEDS = 600
 
 SCH = [P.field("k", "i64"), P.field("g", "utf8", True), P.field("x", P.dec(15, 2), True), P.field("y", "f64", True),
        P.field("d", "date32"), P.field("b", "bool", True), P.field("n", "i32", True)]
@@ -126,17 +127,18 @@ def _strip(t):
 
 
 def test_random_plans_round_trip():
-    sys.path.insert(0, os.path.join(HERE, "golden"))
-    import make_proto_plans as M
+    with gzip.open(os.path.join(HERE, "golden", "random_proto_plans.json.gz")) as fh:
+        protos = json.load(fh)["protos"]
     ok = rejected = 0
-    for seed in range(600):
+    for seed in range(N_SEEDS):
         ir = json.dumps(_plan(seed), separators=(",", ":"))
         try:
             want = json.loads(engine.plan_typed_json(ir))
         except engine.B200Error:
             rejected += 1          # an ill-typed combination (e.g. decimal precision overflow): not a plan
             continue
-        proto = M.encode(ir)
+        assert str(seed) in protos, f"seed {seed}: no stored encoding (regenerate with tests/golden/make_proto_plans.py)"
+        proto = base64.b64decode(protos[str(seed)])
         got = json.loads(engine.plan_typed_json(engine.plan_proto_to_json(proto)))
         assert _strip(got) == _strip(want), f"seed {seed}"
         ok += 1
