@@ -314,9 +314,12 @@ struct PqDecompJob {
   uint8_t* dst;         // where the page payload is rebuilt
   uint32_t src_len, dst_len;
   uint32_t raw_copy;    // 1: plain copy (sections that are never compressed)
-  uint32_t _pad;
+  uint32_t codec;       // the column chunk's parquet CompressionCodec: selects the kernel that runs the job
 };
+// One warp per job; a job that does not decode to exactly dst_len bytes sets a bit in *error: 1 Snappy, 2 GZIP, 4 LZ4_RAW.
 void launch_pq_snappy(const PqDecompJob* jobs, int n_jobs, unsigned int* error, cudaStream_t st);
+void launch_pq_inflate(const PqDecompJob* jobs, int n_jobs, unsigned int* error, cudaStream_t st);  // GZIP: gzip / zlib members
+void launch_pq_lz4(const PqDecompJob* jobs, int n_jobs, unsigned int* error, cudaStream_t st);      // LZ4_RAW: one LZ4 block
 void launch_pq_levels(const PqPage* pages, int n_pages, uint8_t* valid, uint32_t* nonnull, unsigned long long* total_nonnull, cudaStream_t st);
 void launch_pq_page_scan(const uint32_t* nonnull, int n_pages, unsigned long long* dense_base, cudaStream_t st);
 void launch_pq_dict(const PqColumn& C, const PqPage* dict_pages, int n_dicts, cudaStream_t st);

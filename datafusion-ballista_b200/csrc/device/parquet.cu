@@ -13,6 +13,7 @@
 //     engine's intermediate string layout is exactly that);
 //   * DELTA_* and BYTE_STREAM_SPLIT pages: validated first, then decoded by pq_values_delta_kernel (see that section);
 //   * nullable columns: values are stored densely, a second pass spreads them to their rows using the validity bytes.
+// Compressed pages (SNAPPY, GZIP, LZ4_RAW) are first rebuilt uncompressed in HBM by one warp per page (end of this file).
 // Integer/byte work, HBM bound: algorithmic bytes = encoded page bytes read + decoded column bytes written.
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -675,9 +676,516 @@ __global__ void __launch_bounds__(128) pq_snappy_kernel(const PqDecompJob* __res
   if (op != ulen && lane == 0) atomicExch(error, 1u);
 }
 
+// ---- shared by the GZIP and LZ4_RAW kernels ---------------------------------------------------------------------------------------
+// out[P, P+L) = the L bytes starting D bytes back (1 <= D <= P).  When D < L the source overlaps the destination and the
+// bytes repeat with period D, so byte k is out[P - D + k mod D]: every source byte lies before P, all lanes copy at once.
+__device__ __forceinline__ void pq_copy_match(uint8_t* out, uint64_t P, uint32_t L, uint32_t D, int lane) {
+  for (uint32_t k = lane; k < L; k += 32) out[P + k] = out[P - D + (k < D ? k : k % D)];
+}
+
+// ---- DEFLATE (RFC 1951) page decompression: one warp per job ---------------------------------------------------------------------
+// A GZIP page payload is what zlib's inflate accepts with header auto-detection (which pyarrow's reader uses): one or more
+// members back to back, each a gzip member (RFC 1952: header with optional FEXTRA / FNAME / FCOMMENT / FHCRC, deflate data,
+// CRC32 and ISIZE) or a zlib stream (RFC 1950: CMF/FLG header, deflate data, big-endian Adler-32); the outputs concatenate.
+// Raw deflate without a wrapper is refused, as zlib refuses it ("incorrect header check").
+//
+// Every lane runs the same bit reader and Huffman decode (broadcast loads from shared memory and the page), lane t keeping
+// token t of a batch of up to 32 (a literal byte, or a length / distance pair).  A batch is then executed by the warp: an
+// inclusive scan of the token lengths places every token, the literals are stored in parallel, and the matches run in order
+// (pq_copy_match).  A match reads only bytes before its own position, written by earlier tokens, so storing the batch's
+// literals first is safe.  Match distances reach back inside the member's own output, which is in HBM already: no window.
+//
+// Huffman tables (per warp, shared memory): a primary lookup on the next PQ_LIT_BITS / PQ_DIST_BITS bits giving
+// (symbol << 4 | code length); a code longer than that (or a bit pattern no code has) finds entry 0 and is decoded
+// canonically from the per-length counts and the symbols ordered by (length, symbol), as RFC 1951 §3.2.2 defines them.
+//
+// Validated, each failure refusing the page (error bit 2): CM = 8, reserved gzip flags, the zlib header check, window size
+// and FDICT, the FHCRC header CRC16; block type 3; stored LEN / NLEN; HLIT <= 286, HDIST <= 30, a repeat code with nothing
+// to repeat or running past the lengths, a literal/length code without end-of-block; over-subscribed code sets and
+// incomplete ones except a single code of length 1 (zlib's rules; a set without codes is legal until a symbol is read from
+// it); literal/length symbols 286-287 and distance symbols 30-31; a distance before the member's first output byte; the
+// CRC32 and ISIZE, or the Adler-32; output not exactly dst_len; input not consumed exactly.  Reads stay inside
+// [src, src+src_len) and writes inside [dst, dst+dst_len) whatever the bytes say.
+constexpr int PQ_LIT_BITS = 10, PQ_DIST_BITS = 8;
+struct PqHuff {
+  uint16_t lit[1 << PQ_LIT_BITS];   // literal/length primary lookup
+  uint16_t dist[1 << PQ_DIST_BITS];  // distance primary lookup (and the code-length code while the lengths are read)
+  uint16_t lit_sym[288], dist_sym[32];  // symbols ordered by (code length, symbol)
+  uint32_t lit_cnt[16], dist_cnt[16];   // codes per length
+  uint32_t first[16], offs[16], next[16];  // table build: first canonical code / first sorted index / running index per length
+  uint8_t lens[320];                // literal/length then distance code lengths
+  uint8_t clens[20];                // code-length code lengths
+};
+
+__constant__ uint16_t pq_len_base[29] = {3, 4, 5, 6, 7, 8, 9, 10, 11, 13, 15, 17, 19, 23, 27, 31, 35, 43, 51, 59, 67, 83, 99, 115, 131, 163, 195, 227, 258};
+__constant__ uint8_t pq_len_extra[29] = {0, 0, 0, 0, 0, 0, 0, 0, 1, 1, 1, 1, 2, 2, 2, 2, 3, 3, 3, 3, 4, 4, 4, 4, 5, 5, 5, 5, 0};
+__constant__ uint16_t pq_dist_base[30] = {1,   2,   3,   4,   5,   7,    9,    13,   17,   25,   33,   49,   65,    97,    129,
+                                          193, 257, 385, 513, 769, 1025, 1537, 2049, 3073, 4097, 6145, 8193, 12289, 16385, 24577};
+__constant__ uint8_t pq_dist_extra[30] = {0, 0, 0, 0, 1, 1, 2, 2, 3, 3, 4, 4, 5, 5, 6, 6, 7, 7, 8, 8, 9, 9, 10, 10, 11, 11, 12, 12, 13, 13};
+__constant__ uint8_t pq_clen_order[19] = {16, 17, 18, 0, 8, 7, 9, 6, 10, 5, 11, 4, 12, 3, 13, 2, 14, 1, 15};
+
+// LSB-first bit reader over [s, s+len).  Bytes past the end read as zero and still advance `pos`, so after byte alignment
+// `pos - cnt / 8` is the next unread byte and a value above `len` means the stream was truncated.
+struct PqBits {
+  const uint8_t* s;
+  uint32_t len, pos;
+  uint64_t buf;
+  int cnt;
+  __device__ __forceinline__ void fill() {
+    while (cnt <= 56) {
+      buf |= (uint64_t)(pos < len ? s[pos] : 0) << cnt;
+      pos++;
+      cnt += 8;
+    }
+  }
+  __device__ __forceinline__ uint32_t peek(int n) const { return (uint32_t)(buf & ((1ull << n) - 1ull)); }
+  __device__ __forceinline__ void drop(int n) {
+    buf >>= n;
+    cnt -= n;
+  }
+  __device__ __forceinline__ uint32_t get(int n) {
+    const uint32_t v = peek(n);
+    drop(n);
+    return v;
+  }
+  __device__ __forceinline__ uint32_t align() {  // skip to the next byte boundary; returns that byte's offset, buffer emptied
+    drop(cnt & 7);
+    const uint32_t p = pos - (uint32_t)(cnt >> 3);
+    buf = 0;
+    cnt = 0;
+    pos = p;
+    return p;
+  }
+};
+
+// Needs >= 15 buffered bits.  Returns the symbol, or -1 for a bit pattern no code has.
+__device__ __forceinline__ int pq_huff_decode(PqBits& b, const uint16_t* table, int P, const uint16_t* sym, const uint32_t* cnt) {
+  const uint16_t e = table[b.peek(P)];
+  if (e & 15) {
+    b.drop(e & 15);
+    return e >> 4;
+  }
+  int code = 0, first = 0, index = 0;  // canonical decode, one bit at a time (the code's first bit is its most significant)
+  for (int l = 1; l <= 15; l++) {
+    code |= (int)((b.buf >> (l - 1)) & 1);
+    const int count = (int)cnt[l];
+    if (code - first < count) {
+      b.drop(l);
+      return sym[index + code - first];
+    }
+    index += count;
+    first = (first + count) << 1;
+    code <<= 1;
+  }
+  return -1;
+}
+
+// Builds the lookup for `n` code lengths with the whole warp.  `codes`: the code-length code, which zlib never accepts
+// incomplete.  Returns false for a set zlib refuses.
+__device__ bool pq_huff_build(PqHuff& H, const uint8_t* lens, int n, int P, uint16_t* table, uint16_t* sym, uint32_t* cnt, bool codes, int lane) {
+  if (lane < 16) cnt[lane] = 0;
+  for (int k = lane; k < (1 << P); k += 32) table[k] = 0;
+  __syncwarp();
+  for (int s = lane; s < n; s += 32)
+    if (lens[s]) atomicAdd(&cnt[lens[s]], 1u);
+  __syncwarp();
+  int left = 1, maxl = 0;
+  bool over = false;
+  for (int l = 1; l <= 15; l++) {
+    left = (left << 1) - (int)cnt[l];
+    over |= left < 0;
+    if (cnt[l]) maxl = l;
+    if (over) break;
+  }
+  if (maxl == 0) return true;  // no codes: every lookup misses, a symbol read from it is an error
+  if (over || (left > 0 && (codes || maxl != 1))) return false;
+  if (lane == 0) {
+    uint32_t code = 0, o = 0;
+    for (int l = 1; l <= 15; l++) {
+      code = (code + cnt[l - 1]) << 1;  // cnt[0] == 0
+      H.first[l] = code;
+      H.offs[l] = H.next[l] = o;
+      o += cnt[l];
+    }
+  }
+  __syncwarp();
+  for (int s0 = 0; s0 < n; s0 += 32) {
+    const int s = s0 + lane;
+    const int L = s < n ? lens[s] : 0;
+    const unsigned peers = __match_any_sync(0xFFFFFFFFu, L);
+    const unsigned below = peers & ((1u << lane) - 1u);
+    const uint32_t idx = L ? H.next[L] + __popc(below) : 0;
+    __syncwarp();
+    if (L && below == 0) H.next[L] += __popc(peers);
+    __syncwarp();
+    if (L) {
+      sym[idx] = (uint16_t)s;
+      if (L <= P) {
+        const uint32_t rev = __brev(H.first[L] + (idx - H.offs[L])) >> (32 - L);
+        const uint16_t e = (uint16_t)((s << 4) | L);
+        for (uint32_t k = rev; k < (1u << P); k += (1u << L)) table[k] = e;
+      }
+    }
+  }
+  __syncwarp();
+  return true;
+}
+
+// Executes a batch of `nt` tokens (lane t holds token t: bit 31 match, bits 16-24 length, bits 0-15 distance or the literal)
+// at out + op.  False if the batch would write past dst_len or a match reaches before `mstart`.
+__device__ __forceinline__ bool pq_inflate_flush(uint8_t* out, uint32_t& op, uint32_t mstart, uint32_t dst_len, uint32_t tok, int nt, int lane) {
+  const bool on = lane < nt;
+  const uint32_t len = on ? (tok >> 16) & 0x1FF : 0;
+  uint32_t inc = len;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const uint32_t t = __shfl_up_sync(0xFFFFFFFFu, inc, o);
+    if (lane >= o) inc += t;
+  }
+  const uint32_t total = __shfl_sync(0xFFFFFFFFu, inc, 31);
+  if ((uint64_t)op + total > dst_len) return false;
+  const uint32_t pos = op + inc - len;
+  const bool match = on && (tok >> 31);
+  const uint32_t dist = tok & 0xFFFF;
+  if (__any_sync(0xFFFFFFFFu, match && dist > pos - mstart)) return false;
+  if (on && !match) out[pos] = (uint8_t)tok;
+  __syncwarp();
+  for (unsigned m = __ballot_sync(0xFFFFFFFFu, match); m; m &= m - 1) {
+    const int j = __ffs(m) - 1;
+    pq_copy_match(out, __shfl_sync(0xFFFFFFFFu, pos, j), __shfl_sync(0xFFFFFFFFu, len, j), __shfl_sync(0xFFFFFFFFu, dist, j), lane);
+    __syncwarp();
+  }
+  op += total;
+  return true;
+}
+
+// CRC-32 (gzip's, reflected polynomial 0xEDB88320) over the 2^k-th powers of x: crc32_combine's shift operator.
+__device__ uint32_t pq_multmodp(uint32_t a, uint32_t b) {  // a * b modulo the CRC polynomial (a != 0)
+  uint32_t m = 1u << 31, p = 0;
+  for (;;) {
+    if (a & m) {
+      p ^= b;
+      if ((a & (m - 1)) == 0) break;
+    }
+    m >>= 1;
+    b = (b & 1) ? (b >> 1) ^ 0xEDB88320u : b >> 1;
+  }
+  return p;
+}
+__device__ uint32_t pq_x8nmodp(uint64_t n, const uint32_t* x2n) {  // x^(8n) modulo the polynomial
+  uint32_t p = 1u << 31;
+  for (int k = 3; n; n >>= 1, k++)
+    if (n & 1) p = pq_multmodp(x2n[k & 31], p);
+  return p;
+}
+
+// CRC-32 of p[0, n) by the warp: each lane checksums a 1/32 slice, then the slices are combined in a tree.
+__device__ uint32_t pq_warp_crc32(const uint8_t* p, uint32_t n, const uint32_t* T, const uint32_t* x2n, int lane) {
+  const uint32_t a = (uint32_t)((uint64_t)n * lane / 32), e = (uint32_t)((uint64_t)n * (lane + 1) / 32);
+  uint32_t c = 0xFFFFFFFFu;
+  for (uint32_t k = a; k < e; k++) c = T[(c ^ p[k]) & 0xFF] ^ (c >> 8);
+  c = ~c;
+  uint32_t len = e - a;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const uint32_t c2 = __shfl_down_sync(0xFFFFFFFFu, c, o), l2 = __shfl_down_sync(0xFFFFFFFFu, len, o);
+    if ((lane & (2 * o - 1)) == 0) {
+      c = pq_multmodp(pq_x8nmodp(l2, x2n), c) ^ c2;
+      len += l2;
+    }
+  }
+  return __shfl_sync(0xFFFFFFFFu, c, 0);
+}
+
+// Adler-32 of p[0, n) by the warp: per-lane slice sums (a = sum of bytes, b = sum of running sums) combined in a tree.
+__device__ uint32_t pq_warp_adler32(const uint8_t* p, uint32_t n, int lane) {
+  const uint64_t M = 65521;
+  const uint32_t s = (uint32_t)((uint64_t)n * lane / 32), e = (uint32_t)((uint64_t)n * (lane + 1) / 32);
+  uint64_t a = 0, b = 0;
+  for (uint32_t k = s; k < e; k++) {
+    a += p[k];
+    b += a;
+    if (((k - s) & 4095) == 4095) {
+      a %= M;
+      b %= M;
+    }
+  }
+  a %= M;
+  b %= M;
+  uint64_t len = e - s;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const uint64_t a2 = __shfl_down_sync(0xFFFFFFFFu, a, o), b2 = __shfl_down_sync(0xFFFFFFFFu, b, o), l2 = __shfl_down_sync(0xFFFFFFFFu, len, o);
+    if ((lane & (2 * o - 1)) == 0) {
+      b = (b + b2 + (l2 % M) * a) % M;
+      a = (a + a2) % M;
+      len += l2;
+    }
+  }
+  a = __shfl_sync(0xFFFFFFFFu, a, 0);
+  b = __shfl_sync(0xFFFFFFFFu, b, 0);
+  return (uint32_t)((((b + (uint64_t)n) % M) << 16) | ((1 + a) % M));
+}
+
+// Parses a gzip or zlib member header at s[pos]; advances pos past it.
+__device__ bool pq_member_header(const uint8_t* s, uint32_t len, uint32_t& pos, bool& gz, const uint32_t* T, const uint32_t* x2n, int lane) {
+  if (len - pos < 2) return false;
+  const uint32_t b0 = s[pos], b1 = s[pos + 1];
+  gz = b0 == 0x1F && b1 == 0x8B;
+  if (!gz) {  // zlib: CM 8, window <= 32 KiB, (CMF*256 + FLG) % 31 == 0, no preset dictionary
+    if (((b0 << 8) | b1) % 31 != 0 || (b0 & 15) != 8 || (b0 >> 4) > 7 || (b1 & 0x20)) return false;
+    pos += 2;
+    return true;
+  }
+  const uint32_t h0 = pos;
+  if (len - pos < 10) return false;
+  const uint32_t flg = s[pos + 3];
+  if (s[pos + 2] != 8 || (flg & 0xE0)) return false;
+  pos += 10;
+  if (flg & 4) {  // FEXTRA
+    if (len - pos < 2) return false;
+    const uint32_t xlen = s[pos] | ((uint32_t)s[pos + 1] << 8);
+    pos += 2;
+    if (len - pos < xlen) return false;
+    pos += xlen;
+  }
+  for (uint32_t f = 8; f <= 16; f <<= 1) {  // FNAME, FCOMMENT: zero-terminated
+    if (!(flg & f)) continue;
+    while (pos < len && s[pos]) pos++;
+    if (pos >= len) return false;
+    pos++;
+  }
+  if (flg & 2) {  // FHCRC: the low 16 bits of the header's CRC-32
+    if (len - pos < 2) return false;
+    const uint32_t want = s[pos] | ((uint32_t)s[pos + 1] << 8);
+    if ((pq_warp_crc32(s + h0, pos - h0, T, x2n, lane) & 0xFFFF) != want) return false;
+    pos += 2;
+  }
+  return true;
+}
+
+// The deflate blocks of one member, starting at byte b.pos; on return b is aligned after the final block.
+__device__ bool pq_inflate_blocks(PqHuff& H, PqBits& b, uint8_t* out, uint32_t& op, uint32_t dst_len, int lane) {
+  const uint32_t mstart = op;
+  bool last = false;
+  while (!last) {
+    b.fill();
+    if (b.pos > b.len + 8) return false;  // reading past the end of the input
+    last = b.get(1);
+    const uint32_t type = b.get(2);
+    if (type == 0) {  // stored
+      uint32_t p = b.align();
+      if (p > b.len || b.len - p < 4) return false;
+      const uint32_t n = b.s[p] | ((uint32_t)b.s[p + 1] << 8), nn = b.s[p + 2] | ((uint32_t)b.s[p + 3] << 8);
+      p += 4;
+      if (n != (~nn & 0xFFFFu) || b.len - p < n || dst_len - op < n) return false;
+      for (uint32_t k = lane; k < n; k += 32) out[op + k] = b.s[p + k];
+      __syncwarp();
+      op += n;
+      b.pos = p + n;
+      continue;
+    }
+    if (type == 3) return false;
+    if (type == 1) {  // fixed Huffman codes
+      for (int s = lane; s < 320; s += 32) H.lens[s] = s < 144 ? 8 : s < 256 ? 9 : s < 280 ? 7 : s < 288 ? 8 : 5;
+      __syncwarp();
+      pq_huff_build(H, H.lens, 288, PQ_LIT_BITS, H.lit, H.lit_sym, H.lit_cnt, false, lane);
+      pq_huff_build(H, H.lens + 288, 32, PQ_DIST_BITS, H.dist, H.dist_sym, H.dist_cnt, false, lane);
+    } else {  // dynamic: the code lengths, themselves Huffman coded
+      const int hlit = (int)b.get(5) + 257, hdist = (int)b.get(5) + 1, hclen = (int)b.get(4) + 4;
+      if (hlit > 286 || hdist > 30) return false;
+      for (int k = 0; k < 19; k++) {
+        b.fill();
+        const uint8_t l = k < hclen ? (uint8_t)b.get(3) : 0;
+        if (lane == 0) H.clens[pq_clen_order[k]] = l;
+      }
+      __syncwarp();
+      if (!pq_huff_build(H, H.clens, 19, PQ_DIST_BITS, H.dist, H.dist_sym, H.dist_cnt, true, lane)) return false;
+      int i = 0;
+      uint8_t prev = 0;
+      while (i < hlit + hdist) {
+        b.fill();
+        const int sym = pq_huff_decode(b, H.dist, PQ_DIST_BITS, H.dist_sym, H.dist_cnt);
+        if (sym < 0) return false;
+        if (sym < 16) {
+          if (lane == 0) H.lens[i] = (uint8_t)sym;
+          prev = (uint8_t)sym;
+          i++;
+          continue;
+        }
+        int rep;
+        uint8_t v = 0;
+        if (sym == 16) {
+          if (i == 0) return false;
+          v = prev;
+          rep = 3 + (int)b.get(2);
+        } else {
+          rep = sym == 17 ? 3 + (int)b.get(3) : 11 + (int)b.get(7);
+        }
+        if (i + rep > hlit + hdist) return false;
+        if (lane == 0)
+          for (int k = 0; k < rep; k++) H.lens[i + k] = v;
+        prev = v;
+        i += rep;
+      }
+      __syncwarp();
+      if (H.lens[256] == 0) return false;  // no end-of-block code
+      if (!pq_huff_build(H, H.lens, hlit, PQ_LIT_BITS, H.lit, H.lit_sym, H.lit_cnt, false, lane)) return false;
+      if (!pq_huff_build(H, H.lens + hlit, hdist, PQ_DIST_BITS, H.dist, H.dist_sym, H.dist_cnt, false, lane)) return false;
+    }
+    int nt = 0;
+    uint32_t mytok = 0;
+    for (;;) {
+      b.fill();  // >= 57 bits: a token takes at most 15 + 5 + 15 + 13
+      if (b.pos > b.len + 8) return false;
+      const int sym = pq_huff_decode(b, H.lit, PQ_LIT_BITS, H.lit_sym, H.lit_cnt);
+      if (sym < 0 || sym > 285) return false;
+      if (sym == 256) break;
+      uint32_t tok;
+      if (sym < 256) {
+        tok = (1u << 16) | (uint32_t)sym;
+      } else {
+        const uint32_t len = pq_len_base[sym - 257] + b.get(pq_len_extra[sym - 257]);
+        const int ds = pq_huff_decode(b, H.dist, PQ_DIST_BITS, H.dist_sym, H.dist_cnt);
+        if (ds < 0 || ds > 29) return false;
+        tok = 0x80000000u | (len << 16) | (pq_dist_base[ds] + b.get(pq_dist_extra[ds]));
+      }
+      if (lane == nt) mytok = tok;
+      if (++nt == 32) {
+        if (!pq_inflate_flush(out, op, mstart, dst_len, mytok, nt, lane)) return false;
+        nt = 0;
+      }
+    }
+    if (nt && !pq_inflate_flush(out, op, mstart, dst_len, mytok, nt, lane)) return false;
+  }
+  b.align();
+  return b.pos <= b.len;
+}
+
+__global__ void __launch_bounds__(128) pq_inflate_kernel(const PqDecompJob* __restrict__ jobs, int n_jobs, unsigned int* __restrict__ error) {
+  __shared__ uint32_t crc_table[256], x2n[32];
+  __shared__ PqHuff huff[4];
+  for (int i = threadIdx.x; i < 256; i += blockDim.x) {
+    uint32_t c = (uint32_t)i;
+    for (int k = 0; k < 8; k++) c = (c & 1) ? (c >> 1) ^ 0xEDB88320u : c >> 1;
+    crc_table[i] = c;
+  }
+  if (threadIdx.x == 0) {
+    uint32_t p = 1u << 30;  // x^1
+    x2n[0] = p;
+    for (int k = 1; k < 32; k++) x2n[k] = p = pq_multmodp(p, p);
+  }
+  __syncthreads();
+  const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+  if (warp >= n_jobs) return;
+  const PqDecompJob J = jobs[warp];
+  if (J.raw_copy) {  // stored section: the host refuses one whose two sizes differ; never write past dst_len regardless
+    if (J.src_len != J.dst_len && lane == 0) atomicOr(error, 2u);
+    for (uint32_t k = lane; k < J.src_len && k < J.dst_len; k += 32) J.dst[k] = J.src[k];
+    return;
+  }
+  if (J.dst_len == 0) return;  // zlib's callers return an empty output without reading the input; so does pyarrow
+  PqHuff& H = huff[threadIdx.x >> 5];
+  uint32_t pos = 0, op = 0;
+  bool ok = J.src_len > 0;
+  while (ok && pos < J.src_len) {
+    bool gz;
+    ok = pq_member_header(J.src, J.src_len, pos, gz, crc_table, x2n, lane);
+    if (!ok) break;
+    const uint32_t mstart = op;
+    PqBits b{J.src, J.src_len, pos, 0ull, 0};
+    ok = pq_inflate_blocks(H, b, J.dst, op, J.dst_len, lane);
+    if (!ok) break;
+    pos = b.pos;
+    const uint8_t* t = J.src + pos;
+    if (gz) {
+      ok = J.src_len - pos >= 8;
+      if (!ok) break;
+      const uint32_t crc = t[0] | ((uint32_t)t[1] << 8) | ((uint32_t)t[2] << 16) | ((uint32_t)t[3] << 24);
+      const uint32_t isize = t[4] | ((uint32_t)t[5] << 8) | ((uint32_t)t[6] << 16) | ((uint32_t)t[7] << 24);
+      ok = isize == op - mstart && pq_warp_crc32(J.dst + mstart, op - mstart, crc_table, x2n, lane) == crc;
+      pos += 8;
+    } else {
+      ok = J.src_len - pos >= 4;
+      if (!ok) break;
+      const uint32_t adler = ((uint32_t)t[0] << 24) | ((uint32_t)t[1] << 16) | ((uint32_t)t[2] << 8) | t[3];
+      ok = pq_warp_adler32(J.dst + mstart, op - mstart, lane) == adler;
+      pos += 4;
+    }
+  }
+  if ((!ok || op != J.dst_len) && lane == 0) atomicOr(error, 2u);
+}
+
+// ---- LZ4 block format (LZ4_RAW) page decompression: one warp per job -----------------------------------------------------------
+// Format (lz4 Block_format.md): sequences of a token (high nibble literal length, low nibble match length - 4, 15 = more
+// bytes follow: each adds 0-255, 255 = continue), the literals, a 16-bit little-endian offset and the match length
+// continuation.  The final sequence ends after its literals.  Lane 0's parse is every lane's (broadcast loads); the warp moves
+// the bytes.  An empty input with an empty output is accepted (pyarrow reads such V2 values sections).  Refused (error bit 4): a field past the end of the input, offset 0 (which the format forbids; liblz4 accepts it
+// and writes unspecified bytes), an offset before the first output byte, output past dst_len or short of it.
+__global__ void __launch_bounds__(128) pq_lz4_kernel(const PqDecompJob* __restrict__ jobs, int n_jobs, unsigned int* __restrict__ error) {
+  const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+  if (warp >= n_jobs) return;
+  const PqDecompJob J = jobs[warp];
+  if (J.raw_copy) {  // stored section: the host refuses one whose two sizes differ; never write past dst_len regardless
+    if (J.src_len != J.dst_len && lane == 0) atomicOr(error, 4u);
+    for (uint32_t k = lane; k < J.src_len && k < J.dst_len; k += 32) J.dst[k] = J.src[k];
+    return;
+  }
+  const uint8_t* s = J.src;
+  const uint64_t n = J.src_len, cap = J.dst_len;
+  uint64_t ip = 0, op = 0;
+  bool ok = n == 0 && cap == 0;  // an empty section (the values of an all-NULL V2 page): nothing to decode
+  while (ip < n) {
+    const uint32_t token = s[ip++];
+    uint64_t lit = token >> 4;
+    if (lit == 15) {
+      uint32_t more;
+      do {
+        if (ip >= n) goto done;
+        more = s[ip++];
+        lit += more;
+      } while (more == 255);
+    }
+    if (lit > n - ip || lit > cap - op) break;
+    for (uint32_t k = lane; k < lit; k += 32) J.dst[op + k] = s[ip + k];
+    ip += lit;
+    op += lit;
+    if (ip == n) {  // the final sequence: literals only
+      ok = op == cap;
+      break;
+    }
+    if (n - ip < 2) break;
+    const uint32_t off = s[ip] | ((uint32_t)s[ip + 1] << 8);
+    ip += 2;
+    uint64_t ml = token & 15;
+    if (ml == 15) {
+      uint32_t more;
+      do {
+        if (ip >= n) goto done;
+        more = s[ip++];
+        ml += more;
+      } while (more == 255);
+    }
+    ml += 4;
+    if (off == 0 || off > op || ml > cap - op) break;
+    __syncwarp();
+    pq_copy_match(J.dst, op, (uint32_t)ml, off, lane);
+    __syncwarp();
+    op += ml;
+  }
+done:
+  if (!ok && lane == 0) atomicOr(error, 4u);
+}
+
 static inline unsigned pq_grid(int n_warps) { return (unsigned)((n_warps * 32 + 127) / 128); }
 void launch_pq_snappy(const PqDecompJob* jobs, int n_jobs, unsigned int* error, cudaStream_t st) {
   if (n_jobs > 0) pq_snappy_kernel<<<pq_grid(n_jobs), 128, 0, st>>>(jobs, n_jobs, error);
+}
+void launch_pq_inflate(const PqDecompJob* jobs, int n_jobs, unsigned int* error, cudaStream_t st) {
+  if (n_jobs > 0) pq_inflate_kernel<<<pq_grid(n_jobs), 128, 0, st>>>(jobs, n_jobs, error);
+}
+void launch_pq_lz4(const PqDecompJob* jobs, int n_jobs, unsigned int* error, cudaStream_t st) {
+  if (n_jobs > 0) pq_lz4_kernel<<<pq_grid(n_jobs), 128, 0, st>>>(jobs, n_jobs, error);
 }
 
 void launch_pq_levels(const PqPage* pages, int n_pages, uint8_t* valid, uint32_t* nonnull, unsigned long long* total_nonnull, cudaStream_t st) {

@@ -3665,8 +3665,9 @@ struct PqHostColumn {
   std::vector<PqPage> pages, dicts;
   int64_t rows = 0, dict_entries = 0;
   DevPtr raw;  // the column's chunks, back to back (as stored in the file: possibly compressed)
-  DevPtr dec;  // Snappy-compressed chunks: the pages' payloads rebuilt uncompressed
+  DevPtr dec;  // compressed chunks: the pages' payloads rebuilt uncompressed
   std::vector<PqDecompJob> jobs;
+  std::map<int32_t, uint64_t> codec_bytes;  // per compressed codec: its chunks' stored bytes + their rebuilt payload bytes
   std::vector<uint8_t> page_in_dec, dict_in_dec;  // per page: its payload pointer is an offset into `dec` until `dec` exists
   size_t dec_bytes = 0;
   int64_t delta_pages = 0, dba_pages = 0;  // data pages in PQ_ENC_DBP and above; of those, DELTA_BYTE_ARRAY
@@ -3754,9 +3755,11 @@ DevBatchPtr scan_parquet(const Exec& x, const std::string& path, const std::vect
     size_t dpos = 0;
     for (auto& rg : fm.row_groups) {
       const pq::ColumnChunkMeta& cm = rg.columns[(size_t)c.leaf];
-      if (cm.codec != 0 && cm.codec != 1)
-        throw EngineError(B200_ERR_UNSUPPORTED, "parquet: column " + c.se.name + " uses compression codec " + std::to_string(cm.codec) + " (the device scan reads UNCOMPRESSED and SNAPPY pages)");
-      const bool snappy = cm.codec == 1;
+      if (cm.codec != pq::C_UNCOMPRESSED && cm.codec != pq::C_SNAPPY && cm.codec != pq::C_GZIP && cm.codec != pq::C_LZ4_RAW)
+        throw EngineError(B200_ERR_UNSUPPORTED, "parquet: column " + c.se.name + " uses compression codec " + std::to_string(cm.codec) +
+                                                    " (the device scan reads UNCOMPRESSED, SNAPPY, GZIP and LZ4_RAW pages)");
+      const bool compressed = cm.codec != pq::C_UNCOMPRESSED;
+      const size_t dec_before = c.dec_bytes;
       int64_t start = cm.data_page_offset;
       if (cm.dictionary_page_offset > 0 && cm.dictionary_page_offset < start) start = cm.dictionary_page_offset;
       if (start < 0 || (size_t)start + (size_t)cm.total_compressed > fsize) throw EngineError(B200_ERR_INVALID, "parquet: column chunk outside the file");
@@ -3781,7 +3784,7 @@ DevBatchPtr scan_parquet(const Exec& x, const std::string& path, const std::vect
         uint32_t plen = (uint32_t)h.compressed_size;   // bytes of the payload the decode kernels will see
         const bool is_data = h.type == pq::P_DATA || h.type == pq::P_DATA_V2;
         const uint32_t v2_levels = h.type == pq::P_DATA_V2 ? (uint32_t)(h.rep_bytes + h.def_bytes) : 0;
-        const bool in_dec = snappy && (h.type == pq::P_DICTIONARY || is_data);
+        const bool in_dec = compressed && (h.type == pq::P_DICTIONARY || is_data);
         if (in_dec) {
           // the page payload is rebuilt, uncompressed, at c.dec + dec_bytes (the addresses are patched in once c.dec exists)
           plen = (uint32_t)h.uncompressed_size;
@@ -3794,6 +3797,7 @@ DevBatchPtr scan_parquet(const Exec& x, const std::string& path, const std::vect
             lv.dst = (uint8_t*)c.dec_bytes;
             lv.src_len = lv.dst_len = v2_levels;
             lv.raw_copy = 1;
+            lv.codec = (uint32_t)cm.codec;
             c.jobs.push_back(lv);
           }
           vj.src = dev_payload + v2_levels;
@@ -3801,6 +3805,10 @@ DevBatchPtr scan_parquet(const Exec& x, const std::string& path, const std::vect
           vj.src_len = (uint32_t)h.compressed_size - v2_levels;
           vj.dst_len = plen - v2_levels;
           vj.raw_copy = (h.type == pq::P_DATA_V2 && !h.v2_compressed) ? 1 : 0;
+          // a stored section is copied byte for byte: its two sizes must agree, or the copy would overrun the payload
+          if (vj.raw_copy && vj.src_len != vj.dst_len)
+            throw EngineError(B200_ERR_INVALID, "parquet: column " + c.se.name + ": uncompressed V2 page whose compressed and uncompressed sizes differ");
+          vj.codec = (uint32_t)cm.codec;
           c.jobs.push_back(vj);
           pg.data = (const uint8_t*)c.dec_bytes;   // offset for now
           c.dec_bytes += ((size_t)plen + 15) & ~(size_t)15;
@@ -3859,11 +3867,16 @@ DevBatchPtr scan_parquet(const Exec& x, const std::string& path, const std::vect
         }  // index pages etc.: skipped
         hp = payload + h.compressed_size;
       }
+      if (compressed) c.codec_bytes[cm.codec] += (uint64_t)cm.total_compressed + (uint64_t)(c.dec_bytes - dec_before);
       dpos += (size_t)cm.total_compressed;
     }
     if (c.rows != n_rows) throw EngineError(B200_ERR_INVALID, "parquet: column " + c.se.name + " has " + std::to_string(c.rows) + " values, the file " + std::to_string(n_rows) + " rows");
     if (c.dec_bytes) {
-      // Snappy: rebuild every page payload uncompressed in HBM (one warp per page), then decode as usual
+      // compressed chunks: rebuild every page payload uncompressed in HBM (one warp per job, each codec's jobs by its own
+      // kernel), then decode as usual
+      // The order matters for the error word: pq_snappy_kernel sets it with atomicExch(1), the other kernels OR in their
+      // bits, so Snappy (codec 1) must run before GZIP (2) and LZ4_RAW (7) on the stream or it would erase their bits.
+      std::stable_sort(c.jobs.begin(), c.jobs.end(), [](const PqDecompJob& a, const PqDecompJob& b) { return a.codec < b.codec; });
       c.dec = dev_alloc(c.dec_bytes + 64, st);
       uint8_t* base = (uint8_t*)c.dec->ptr;
       for (auto& j : c.jobs) j.dst = base + (size_t)j.dst;
@@ -3875,15 +3888,39 @@ DevBatchPtr scan_parquet(const Exec& x, const std::string& path, const std::vect
       CUDA_CHECK(cudaMemcpyAsync(dj->ptr, c.jobs.data(), c.jobs.size() * sizeof(PqDecompJob), cudaMemcpyHostToDevice, st));
       DevPtr err = dev_alloc(16, st);
       CUDA_CHECK(cudaMemsetAsync(err->ptr, 0, 16, st));
-      {
-        KernelTimer kt(x, "parquet_snappy", (uint64_t)c.raw->bytes + (uint64_t)c.dec_bytes);
-        launch_pq_snappy((const PqDecompJob*)dj->ptr, (int)c.jobs.size(), (unsigned int*)err->ptr, st);
-        x.count();
+      // a column of one codec keeps the Snappy kernel's historical byte count (the column's allocation + rebuilt bytes)
+      const bool one_codec = c.codec_bytes.size() == 1;
+      for (size_t j0 = 0; j0 < c.jobs.size();) {
+        size_t j1 = j0;
+        while (j1 < c.jobs.size() && c.jobs[j1].codec == c.jobs[j0].codec) j1++;
+        const int32_t codec = (int32_t)c.jobs[j0].codec;
+        const PqDecompJob* jobs = (const PqDecompJob*)dj->ptr + j0;
+        const uint64_t bytes = one_codec ? (uint64_t)c.raw->bytes + (uint64_t)c.dec_bytes : c.codec_bytes[codec];
+        unsigned int* e = (unsigned int*)err->ptr;
+        if (codec == pq::C_SNAPPY) {
+          KernelTimer kt(x, "parquet_snappy", bytes);
+          launch_pq_snappy(jobs, (int)(j1 - j0), e, st);
+          x.count();
+        } else if (codec == pq::C_GZIP) {
+          KernelTimer kt(x, "parquet_gzip", bytes);
+          launch_pq_inflate(jobs, (int)(j1 - j0), e, st);
+          x.count();
+        } else {
+          KernelTimer kt(x, "parquet_lz4", bytes);
+          launch_pq_lz4(jobs, (int)(j1 - j0), e, st);
+          x.count();
+        }
+        j0 = j1;
       }
       const unsigned int* herr = x.fetch<unsigned int>(err->ptr);
       const std::string cname = c.se.name;
       x.defer([herr, cname, dj, err]() {
-        if (*herr) throw EngineError(B200_ERR_INVALID, "parquet: corrupt Snappy data in column " + cname);
+        if (!*herr) return;
+        std::string what;
+        const char* names[3] = {"Snappy", "GZIP", "LZ4_RAW"};
+        for (int k = 0; k < 3; k++)
+          if (*herr & (1u << k)) what += (what.empty() ? "" : "/") + std::string(names[k]);
+        throw EngineError(B200_ERR_INVALID, "parquet: corrupt " + what + " data in column " + cname);
       });
     }
   }
@@ -4446,12 +4483,14 @@ int b200_parquet_describe(const char* path, char* out, uint64_t cap) {
     std::string j = "{\"num_rows\":" + std::to_string(fm.num_rows) + ",\"row_groups\":" + std::to_string(fm.row_groups.size()) + ",\"columns\":[";
     for (size_t i = 1; i < fm.schema.size(); i++) {
       const pq::SchemaElement& se = fm.schema[i];
-      int64_t data_pages = 0, dict_pages = 0, values = 0, dict_encoded = 0, codec = 0;
+      int64_t data_pages = 0, dict_pages = 0, values = 0, dict_encoded = 0, codec = 0;  // codec: the last row group's
       std::set<int32_t> encodings;  // value encodings named by the column's data and dictionary page headers
+      std::set<int32_t> codecs;     // compression codecs of all its chunks
       for (auto& rg : fm.row_groups) {
         if (i - 1 >= rg.columns.size()) continue;
         const pq::ColumnChunkMeta& cm = rg.columns[i - 1];
         codec = cm.codec;
+        codecs.insert(cm.codec);
         int64_t start = cm.data_page_offset;
         if (cm.dictionary_page_offset > 0 && cm.dictionary_page_offset < start) start = cm.dictionary_page_offset;
         const uint8_t* hp = buf.data() + start;
@@ -4481,6 +4520,12 @@ int b200_parquet_describe(const char* path, char* out, uint64_t cap) {
       bool first = true;
       for (int32_t e : encodings) {
         j += (first ? "" : ",") + std::to_string(e);
+        first = false;
+      }
+      j += "],\"codecs\":[";
+      first = true;
+      for (int32_t k : codecs) {
+        j += (first ? "" : ",") + std::to_string(k);
         first = false;
       }
       j += "]}";

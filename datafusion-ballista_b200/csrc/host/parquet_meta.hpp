@@ -9,7 +9,8 @@
 // Encodings.md: PLAIN, RLE/bit-packed hybrid, RLE_DICTIONARY, DELTA_*, BYTE_STREAM_SPLIT).  Supported: flat schemas, physical
 // types BOOLEAN / INT32 / INT64 / DOUBLE / BYTE_ARRAY / FIXED_LEN_BYTE_ARRAY, logical DECIMAL / DATE / STRING, encodings PLAIN,
 // [PLAIN|RLE]_DICTIONARY, DELTA_BINARY_PACKED, DELTA_LENGTH_BYTE_ARRAY, DELTA_BYTE_ARRAY and BYTE_STREAM_SPLIT, data pages V1
-// and V2, codecs UNCOMPRESSED and SNAPPY.  Everything else is reported as unsupported.
+// and V2, codecs UNCOMPRESSED, SNAPPY, GZIP and LZ4_RAW (a column may use a different codec in each row group).  Everything else,
+// including BROTLI, LZO, ZSTD and the deprecated Hadoop-framed LZ4, is reported as unsupported.
 #pragma once
 #include <cstdint>
 #include <cstring>
@@ -26,6 +27,7 @@ enum Encoding : int32_t {
   E_RLE_DICTIONARY = 8, E_BYTE_STREAM_SPLIT = 9
 };
 enum PageType : int32_t { P_DATA = 0, P_INDEX = 1, P_DICTIONARY = 2, P_DATA_V2 = 3 };
+enum Codec : int32_t { C_UNCOMPRESSED = 0, C_SNAPPY = 1, C_GZIP = 2, C_LZO = 3, C_BROTLI = 4, C_LZ4 = 5, C_ZSTD = 6, C_LZ4_RAW = 7 };
 
 struct ThriftReader {
   const uint8_t* p;

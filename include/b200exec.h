@@ -103,8 +103,9 @@ int b200_engine_register_batch(b200_engine* e, const char* table, int partition,
  * DELTA_BINARY_PACKED (INT32 / INT64), DELTA_LENGTH_BYTE_ARRAY (BYTE_ARRAY), DELTA_BYTE_ARRAY (BYTE_ARRAY,
  * FIXED_LEN_BYTE_ARRAY) and BYTE_STREAM_SPLIT (INT32 / INT64 / DOUBLE / FIXED_LEN_BYTE_ARRAY), mixed freely within a column
  * chunk; definition levels; INT32 / INT64 / DOUBLE / BOOLEAN / BYTE_ARRAY / FIXED_LEN_BYTE_ARRAY with DECIMAL / DATE / STRING
- * annotations; flat schemas; UNCOMPRESSED and SNAPPY codecs).  A malformed page returns B200_ERR_INVALID naming the column;
- * other encodings, codecs and types B200_ERR_UNSUPPORTED.  columns_csv = NULL: every column.  Replaces the table partition. */
+ * annotations; flat schemas; UNCOMPRESSED, SNAPPY, GZIP (gzip or zlib members) and LZ4_RAW codecs, which may differ from
+ * one row group to the next, all decompressed on the device).  A malformed page returns B200_ERR_INVALID naming the column;
+ * other encodings, codecs (BROTLI, LZO, ZSTD, Hadoop-framed LZ4) and types B200_ERR_UNSUPPORTED.  columns_csv = NULL: every column.  Replaces the table partition. */
 int b200_engine_register_parquet(b200_engine* e, const char* table, int partition, const char* path, const char* columns_csv);
 /* Host-only: JSON description (schema, rows, page inventory per column) of a Parquet file as the scan's metadata reader
  * sees it.  No CUDA call. */

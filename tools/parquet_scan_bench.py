@@ -1,10 +1,11 @@
 """Device Parquet scan of TPC-H lineitem's q1 columns in several page encodings (b200_engine_register_parquet).
 
-  python tools/parquet_scan_bench.py [--sf 10] [--steps 5] [--warmup 2] [--no-parity]
+  python tools/parquet_scan_bench.py [--sf 10] [--steps 5] [--warmup 2] [--codec snappy|gzip|lz4|none] [--no-parity]
 
-The columns come from the oracle's generator and are written by pyarrow, with Snappy, into a temporary directory in the
-encodings of FILES.  Per file: warmed-up median wall time of the registration, device time and achieved GB/s of the
-value decode (family parquet_decode_values; GB/s = (uncompressed page bytes read + decoded Arrow bytes written) / device
+The columns come from the oracle's generator and are written by pyarrow, with --codec (default Snappy), into a temporary
+directory in the encodings of FILES.  With gzip or lz4 each file also reports the GB/s of uncompressed page bytes its
+decompression kernel (family parquet_gzip / parquet_lz4) writes.  Per file: warmed-up median wall time of the
+registration, device time and achieved GB/s of the value decode (family parquet_decode_values; GB/s = (uncompressed page bytes read + decoded Arrow bytes written) / device
 time), the other scan kernels' device time and pages per column.  Then q1 on each scanned table is checked against the
 CPU oracle.  Prints one JSON line, with the card name and its power limit beside the numbers."""
 import argparse
@@ -21,6 +22,14 @@ sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 
 import bench  # noqa: E402  (cpu_q1, tables_equal, usable_cpus, measured_hbm_peak)
+
+# --codec -> (pyarrow write options, codec name in FILES' descriptions, decompression kernel family reported as GB/s).
+# gzip is written at zlib's default level 6, which Hadoop's and Spark's GzipCodec use; pyarrow's own default, level 9, is
+# about nine times slower to write (a minute per SF1 file).
+CODECS = {"snappy": (dict(compression="snappy"), "Snappy", None),
+          "gzip": (dict(compression="gzip", compression_level=6), "GZIP", "parquet_gzip"),
+          "lz4": (dict(compression="lz4"), "LZ4_RAW", "parquet_lz4"),
+          "none": (dict(compression="none"), "uncompressed", None)}
 
 FILES = {
     "default": "pyarrow's defaults: dictionary pages (PLAIN once a dictionary grows too large), decimals as FIXED_LEN_BYTE_ARRAY, Snappy",
@@ -63,6 +72,7 @@ def main():
     ap.add_argument("--sf", type=float, default=10.0)
     ap.add_argument("--steps", type=int, default=5)
     ap.add_argument("--warmup", type=int, default=2)
+    ap.add_argument("--codec", choices=sorted(CODECS), default="snappy")
     ap.add_argument("--no-parity", action="store_true")
     args = ap.parse_args()
 
@@ -90,7 +100,9 @@ def main():
     try:
         for kind in FILES:
             path = os.path.join(tmp, f"lineitem-{kind}.parquet")
-            pq.write_table(host, path, compression="snappy", **write_options(kind, host.schema))
+            print(f"{kind}: writing with {args.codec}", file=sys.stderr, flush=True)
+            pq.write_table(host, path, **CODECS[args.codec][0], **write_options(kind, host.schema))
+            print(f"{kind}: written ({os.path.getsize(path)} bytes), timing register_parquet", file=sys.stderr, flush=True)
             md = pq.ParquetFile(path).metadata
             page_bytes = sum(md.row_group(g).column(c).total_uncompressed_size for g in range(md.num_row_groups) for c in range(md.num_columns))
             desc = bb.engine.parquet_describe(path)
@@ -114,7 +126,7 @@ def main():
             results[kind] = driver.run_stages(eng, tpch.q1(1), f"pq-{kind}")
             eng.remove_job_data(f"pq-{kind}")
             out[kind] = {
-                "what": FILES[kind], "file_bytes": os.path.getsize(path), "uncompressed_page_bytes": page_bytes,
+                "what": FILES[kind].replace("Snappy", CODECS[args.codec][1]), "file_bytes": os.path.getsize(path), "uncompressed_page_bytes": page_bytes,
                 "register_parquet_ms": 1e3 * statistics.median(wall),
                 "decode_values_ms": dec_ms, "decode_values_gbs": dec_gbs, "decode_values_frac_of_hbm_peak": dec_gbs / peak,
                 "other_kernels_ms": {k: v["ms"] / args.steps for k, v in sorted(ks.items())
@@ -122,6 +134,11 @@ def main():
                 "pages_per_column": {c["name"]: c["data_pages"] for c in desc["columns"]},
                 "encodings": {c["name"]: c["encodings"] for c in desc["columns"]},
             }
+            family = CODECS[args.codec][2]
+            if family:
+                dms = ks.get(family, {"ms": 0.0})["ms"] / args.steps
+                out[kind]["decompress_ms"] = dms
+                out[kind]["decompress_gbs"] = page_bytes / (dms / 1e3) / 1e9 if dms > 0 else 0.0
             os.remove(path)
     finally:
         shutil.rmtree(tmp, ignore_errors=True)
@@ -140,7 +157,8 @@ def main():
                   "what": f"q1 on each scanned table == CPU oracle q1 on the same {rows} generated rows, bit-exact"}
     name, watts = card()
     line = {
-        "workload": f"device Parquet scan of TPC-H lineitem's q1 columns, SF{args.sf:g} ({rows} rows), written by pyarrow {pa.__version__}",
+        "workload": f"device Parquet scan of TPC-H lineitem's q1 columns, SF{args.sf:g} ({rows} rows), written by pyarrow {pa.__version__}"
+                    + ("" if args.codec == "snappy" else " with " + ", ".join(f"{k}={v}" for k, v in CODECS[args.codec][0].items())),
         "steps": args.steps, "warmup": max(args.warmup, 1), "gpu": name, "power_limit_w": watts,
         "timing": "register_parquet: median host wall time (file in the page cache); kernels: CUDA events per kernel family",
         "gbs": "(uncompressed page bytes + decoded Arrow bytes) / parquet_decode_values device time",
