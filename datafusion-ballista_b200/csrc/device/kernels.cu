@@ -40,6 +40,8 @@ __global__ void agg_table_init_kernel(AggTable T, AccKinds kinds) {
         case ACC_MAX_I128: lo = 0; hi = 0x8000000000000000ull; break;
         case ACC_MIN_F64: lo = 0x7FFFFFFFFFFFFFFFull; break;
         case ACC_MAX_F64: lo = 0x8000000000000000ull; break;
+        case ACC_MIN_STR:
+        case ACC_MAX_STR: hi = ACC_STR_NONE; break;
         default: break;
       }
       T.acc[((unsigned long long)a * T.cap + i) * 2 + 0] = lo;
@@ -114,6 +116,10 @@ __global__ void agg_extract_kernel(AggTable T, AggExtractArgs A) {
               ok = true;
               break;
             case AO_MINMAX_F64: ((double*)o.data)[pos] = f64_from_key((long long)lo); break;
+            case AO_MINMAX_STR:
+              ok = ok && hi != ACC_STR_NONE;
+              ((ulonglong2*)o.data)[pos] = ok ? make_ulonglong2(lo, hi) : make_ulonglong2(0ull, 0ull);
+              break;
             case AO_AVG_DEC: {
               i128 sum = mk128(lo, hi);
               i128 res = 0;

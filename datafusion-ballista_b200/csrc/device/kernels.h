@@ -31,7 +31,8 @@ enum AggOutKind : uint8_t {
   AO_MINMAX_F64,   // order-key -> double ; b count
   AO_AVG_DEC,      // a: sum acc, b: count acc, imm: 10^k multiplier exponent
   AO_AVG_F64,      // a: sum acc (f64), b: count acc
-  AO_KEY_PACKED    // a: key index holding a packed short string (OP_STR_PACK8); imm: bit position of the length; aux: 8 B/row chars
+  AO_KEY_PACKED,   // a: key index holding a packed short string (OP_STR_PACK8); imm: bit position of the length; aux: 8 B/row chars
+  AO_MINMAX_STR    // a: MIN_STR / MAX_STR acc -> string view (points at the input's characters); b count
 };
 struct AggOut {
   void* data;

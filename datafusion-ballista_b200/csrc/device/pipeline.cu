@@ -143,6 +143,19 @@ __device__ __noinline__ int str_cmp(StrRef a, StrRef b) {
   }
   return a.len < b.len ? -1 : (a.len > b.len ? 1 : 0);
 }
+// string MIN / MAX: does the view (xp, xl) order strictly before (MIN) / after (MAX) the view (cp, cl)?  A length of
+// ACC_STR_NONE is "no value": it never wins and loses to every value
+__device__ __noinline__ bool str_beats(bool is_min, uint64_t xp, uint64_t xl, uint64_t cp, uint64_t cl) {
+  if (xl == ACC_STR_NONE) return false;
+  if (cl == ACC_STR_NONE) return true;
+  StrRef x, c;
+  x.p = (const uint8_t*)xp;
+  x.len = (uint32_t)xl;
+  c.p = (const uint8_t*)cp;
+  c.len = (uint32_t)cl;
+  const int d = str_cmp(x, c);
+  return is_min ? d < 0 : d > 0;
+}
 __device__ __noinline__ bool str_eq(StrRef a, StrRef b) {
   if (a.len != b.len) return false;
   for (uint32_t i = 0; i < a.len; i++)
@@ -1618,6 +1631,49 @@ struct Acc128 {
   uint64_t lo, hi;
 };
 
+// single-copy-atomic 16-byte load and compare-and-swap of a table cell (sm_90: LDG.E.128 / ATOMG.E.CAS.128)
+__device__ __forceinline__ ulonglong2 ld_relaxed_b128(const unsigned long long* p) {
+  ulonglong2 r;
+  asm volatile(
+      "{\n\t.reg .b128 t;\n\t"
+      "ld.relaxed.gpu.global.b128 t, [%2];\n\t"
+      "mov.b128 {%0, %1}, t;\n\t}"
+      : "=l"(r.x), "=l"(r.y)
+      : "l"(p)
+      : "memory");
+  return r;
+}
+__device__ __forceinline__ ulonglong2 atom_cas_b128(unsigned long long* p, ulonglong2 cmp, ulonglong2 val) {
+  ulonglong2 r;
+  asm volatile(
+      "{\n\t.reg .b128 c, v, d;\n\t"
+      "mov.b128 c, {%3, %4};\n\t"
+      "mov.b128 v, {%5, %6};\n\t"
+      "atom.relaxed.gpu.global.cas.b128 d, [%2], c, v;\n\t"
+      "mov.b128 {%0, %1}, d;\n\t}"
+      : "=l"(r.x), "=l"(r.y)
+      : "l"(p), "l"(cmp.x), "l"(cmp.y), "l"(val.x), "l"(val.y)
+      : "memory");
+  return r;
+}
+
+// string MIN / MAX of a table cell: compare-and-swap of the whole 16-byte view, no lock.  The cell only ever moves
+// towards the final answer, so a row that does not beat the value it last read can stop -- most rows issue no atomic.
+// (The characters a view points at never change, so relaxed ordering suffices.)  Kept apart from table_merge, which the
+// fused kernel's and the add-only register sink's flushes call: they never see a string accumulator.
+__device__ __noinline__ void table_merge_str(int kind, unsigned long long slot, int a, Acc128 x) {
+  const AggTable& T = PROG.table;
+  unsigned long long* cell = T.acc + ((unsigned long long)a * T.cap + slot) * 2;
+  const bool is_min = kind == ACC_MIN_STR;
+  ulonglong2 cur = ld_relaxed_b128(cell);
+  const ulonglong2 val = make_ulonglong2(x.lo, x.hi);
+  while (str_beats(is_min, x.lo, x.hi, cur.x, cur.y)) {
+    const ulonglong2 seen = atom_cas_b128(cell, cur, val);
+    if (seen.x == cur.x && seen.y == cur.y) return;
+    cur = seen;
+  }
+}
+
 // merge one partial accumulator value into a table cell (atomics; 128-bit min/max under the lock)
 __device__ __noinline__ void table_merge(int kind, unsigned long long slot, int a, Acc128 x) {
   const AggTable& T = PROG.table;
@@ -1690,13 +1746,18 @@ __device__ __noinline__ uint32_t sink_agg_global(const Lane L, uint32_t active) 
       if (ad.kind == ACC_SUM_I128 || ad.kind == ACC_MIN_I128 || ad.kind == ACC_MAX_I128) {
         i128 v = ld1_i128(L, ad.src, r);
         x.lo = lo64(v);
-        x.hi = hi64(v);
+        x.hi = ad.zext ? 0ull : hi64(v);
+      } else if (ad.kind == ACC_MIN_STR || ad.kind == ACC_MAX_STR) {
+        const StrRef s = ld1_str(L, ad.src, r);
+        x.lo = (uint64_t)s.p;
+        x.hi = s.len;
       } else if (ad.kind == ACC_SUM_F64) {
         x.lo = (uint64_t)__double_as_longlong(ld1_f64(L, ad.src, r));
       } else if (ad.kind == ACC_MIN_F64 || ad.kind == ACC_MAX_F64) {
         x.lo = (uint64_t)f64_order_key(ld1_f64(L, ad.src, r));
       }
-      table_merge(ad.kind, slot, a, x);
+      if (ad.kind == ACC_MIN_STR || ad.kind == ACC_MAX_STR) table_merge_str(ad.kind, slot, a, x);
+      else table_merge(ad.kind, slot, a, x);
     }
   }
   return active;
@@ -1831,9 +1892,56 @@ __device__ __noinline__ void reg_merge_big(RegGroupTable* gt, int G, int g, int 
   table_merge(ACC_SUM_I128, slot, a, x);
 }
 
-template <int G, bool ADD_ONLY>
-__device__ __forceinline__ uint32_t sink_agg_reg(const Lane L, uint32_t active, RegAggState<G>& S, unsigned long long* hi, RegGroupTable* gt,
-                                                 unsigned long long (&dir)[G], uint32_t& dir_n, const AccOp* accops) {
+// ---- side accumulators of the general register sink: string MIN / MAX and UInt64 MIN / MAX ----------------------------
+// Their per-thread state lives in memory, not in the register matrix: the 64-bit value (string: the view's pointer) in
+// the acc_side scratch, a string's length in the acc_hi scratch (ACC_STR_NONE: no value yet).  They are folded in by one
+// rolled call per tile and merged by their own flush, all of it only in the pipeline_kernel variants instantiated with
+// SIDE = true (launched when the program has such an accumulator): every other variant, the fused kernel included,
+// compiles exactly as it does without them.
+__device__ __forceinline__ bool acc_is_side(const AccDesc& ad) { return ad.kind == ACC_MIN_STR || ad.kind == ACC_MAX_STR || ad.zext; }
+
+__device__ __noinline__ void reg_side_init(unsigned long long* hi, unsigned long long* side) {
+  for (int a = 0; a < PROG.n_acc && a < VM_REG_ACC; a++) {
+    const AccDesc ad = PROG.acc[a];
+    if (!acc_is_side(ad)) continue;
+    for (int g = 0; g < VM_REG_GROUPS; g++) {
+      const int w = g * VM_REG_ACC + a;
+      if (ad.zext) {
+        side[w] = ad.kind == ACC_MIN_I128 ? ~0ull : 0ull;  // UInt64 identities: no value orders below / above them
+      } else {
+        side[w] = 0;
+        hi[w] = ACC_STR_NONE;
+      }
+    }
+  }
+}
+
+// fold the tile's rows of this thread into its side accumulators; gp: group of row r in byte r
+__device__ __noinline__ void reg_side_rows(const Lane L, uint32_t active, uint32_t gp, unsigned long long* hi, unsigned long long* side) {
+  for (int a = 0; a < PROG.n_acc && a < VM_REG_ACC; a++) {
+    const AccDesc ad = PROG.acc[a];
+    if (!acc_is_side(ad)) continue;
+    const uint32_t v = ad.nullable ? (active & fetch_valid(L, ad.src)) : active;
+    for (int r = 0; r < VM_R; r++) {
+      if (!((v >> r) & 1)) continue;
+      const int w = (int)((gp >> (8 * r)) & 0xFFu) * VM_REG_ACC + a;
+      if (ad.zext) {
+        const uint64_t u = (uint64_t)ld1_i64(L, ad.src, r);
+        if (ad.kind == ACC_MIN_I128 ? u < side[w] : u > side[w]) side[w] = u;
+      } else {
+        const StrRef s = ld1_str(L, ad.src, r);
+        if (str_beats(ad.kind == ACC_MIN_STR, (uint64_t)s.p, s.len, side[w], hi[w])) {
+          side[w] = (uint64_t)s.p;
+          hi[w] = s.len;
+        }
+      }
+    }
+  }
+}
+
+template <int G, bool ADD_ONLY, bool SIDE>
+__device__ __forceinline__ uint32_t sink_agg_reg(const Lane L, uint32_t active, RegAggState<G>& S, unsigned long long* hi, unsigned long long* side,
+                                                 RegGroupTable* gt, unsigned long long (&dir)[G], uint32_t& dir_n, const AccOp* accops) {
   uint32_t gid[VM_R];
 #pragma unroll
   FOR_R gid[r] = 0;
@@ -1976,7 +2084,7 @@ __device__ __forceinline__ uint32_t sink_agg_reg(const Lane L, uint32_t active, 
             if (is_min ? k < cur : k > cur) S.lo[g][a] = (uint64_t)k;
           }
       }
-    } else {
+    } else if (!SIDE || !acc_is_side(ad)) {
       i128 vi[VM_R];
       fetch_i128(L, ad.src, vi);
       const bool is_min = ad.kind == ACC_MIN_I128;
@@ -1993,6 +2101,12 @@ __device__ __forceinline__ uint32_t sink_agg_reg(const Lane L, uint32_t active, 
           }
       }
     }
+  }
+  if (SIDE) {
+    uint32_t gp = 0;
+#pragma unroll
+    FOR_R gp |= gid[r] << (8 * r);
+    reg_side_rows(L, active, gp, hi, side);
   }
   return active;
 }
@@ -2015,14 +2129,32 @@ __device__ __noinline__ Acc128 acc_combine(int kind, Acc128 x, Acc128 y) {
   }
 }
 
-// rolled CTA reduction of scratch[a][thread] -> scratch[a][0], then merge into the global table
+// acc_combine plus the side accumulators (a zero-extended UInt64 compares correctly as a 128-bit integer)
+__device__ __noinline__ Acc128 acc_combine_side(int kind, Acc128 x, Acc128 y) {
+  if (kind == ACC_MIN_STR || kind == ACC_MAX_STR) return str_beats(kind == ACC_MIN_STR, y.lo, y.hi, x.lo, x.hi) ? y : x;
+  return acc_combine(kind, x, y);
+}
+
+// rolled CTA reduction of scratch[a][thread] -> scratch[a][0], then merge into the global table.  SIDE (general register
+// sink only): the side accumulators' values are taken from their scratch first, and strings merge by compare-and-swap.
+template <bool SIDE>
 __device__ __noinline__ void reg_flush_group(RegGroupTable* gt, Acc128* scratch, int g, int G, int tid, int B) {
   const int n_acc = PROG.n_acc, n_keys = PROG.n_keys;
+  if (SIDE) {
+    const size_t t = ((size_t)blockIdx.x * B + tid) * (VM_REG_GROUPS * VM_REG_ACC) + (size_t)g * VM_REG_ACC;
+    for (int a = 0; a < n_acc; a++)
+      if (acc_is_side(PROG.acc[a])) {
+        scratch[a * B + tid].lo = PROG.acc_side[t + a];
+        scratch[a * B + tid].hi = PROG.acc[a].zext ? 0ull : PROG.acc_hi[t + a];
+      }
+  }
   __syncthreads();
   for (int n = B; n > 1;) {  // B need not be a power of two
     const int half = (n + 1) >> 1;
     for (int a = 0; a < n_acc; a++)
-      if (tid < n - half) scratch[a * B + tid] = acc_combine(PROG.acc[a].kind, scratch[a * B + tid], scratch[a * B + tid + half]);
+      if (tid < n - half)
+        scratch[a * B + tid] = SIDE ? acc_combine_side(PROG.acc[a].kind, scratch[a * B + tid], scratch[a * B + tid + half])
+                                    : acc_combine(PROG.acc[a].kind, scratch[a * B + tid], scratch[a * B + tid + half]);
     __syncthreads();
     n = half;
   }
@@ -2042,7 +2174,11 @@ __device__ __noinline__ void reg_flush_group(RegGroupTable* gt, Acc128* scratch,
     if (slot == ~0ull) {
       atomicExch(&PROG.status->overflow, 1u);
     } else {
-      for (int a = 0; a < n_acc; a++) table_merge(PROG.acc[a].kind, slot, a, scratch[a * B]);
+      for (int a = 0; a < n_acc; a++) {
+        const int kind = PROG.acc[a].kind;
+        if (SIDE && (kind == ACC_MIN_STR || kind == ACC_MAX_STR)) table_merge_str(kind, slot, a, scratch[a * B]);
+        else table_merge(kind, slot, a, scratch[a * B]);
+      }
     }
   }
   __syncthreads();
@@ -2050,7 +2186,7 @@ __device__ __noinline__ void reg_flush_group(RegGroupTable* gt, Acc128* scratch,
 
 // End of kernel: reduce the per-thread matrices over the CTA (through shared memory, one group at a
 // time) and merge them into the global table with atomics.
-template <int G, bool ADD_ONLY>
+template <int G, bool ADD_ONLY, bool SIDE = false>
 __device__ __forceinline__ void reg_agg_flush(RegAggState<G>& S, const unsigned long long* hi, RegGroupTable* gt, Acc128* scratch /*[VM_REG_ACC][B]*/, int tid,
                                               int B) {
   const unsigned int ng = (G == 1) ? 1u : gt->n_groups;
@@ -2064,7 +2200,7 @@ __device__ __forceinline__ void reg_agg_flush(RegAggState<G>& S, const unsigned 
       x.hi = ADD_ONLY ? (uint64_t)((int64_t)S.lo[g][a] >> 63) : hi[g * VM_REG_ACC + a];
       scratch[a * B + tid] = x;
     }
-    reg_flush_group(gt, scratch, g, G, tid, B);
+    reg_flush_group<SIDE>(gt, scratch, g, G, tid, B);
   }
 }
 
@@ -2114,7 +2250,7 @@ __device__ __forceinline__ uint32_t addsub128(bool minus, uint64_t llo, uint64_t
 // ------------------------------------------------------------------------------------------------
 // The kernel
 // ------------------------------------------------------------------------------------------------
-template <int SINK, int G, bool ADD_ONLY>
+template <int SINK, int G, bool ADD_ONLY, bool SIDE>
 __global__ void __launch_bounds__(512, 1) pipeline_kernel() {
   extern __shared__ __align__(128) uint8_t smem[];
   __shared__ __align__(8) uint64_t full_bar[VM_MAX_STAGES];
@@ -2152,9 +2288,14 @@ __global__ void __launch_bounds__(512, 1) pipeline_kernel() {
   unsigned long long dir[G];
   uint32_t dir_n = 0;
   unsigned long long* acc_hi = nullptr;
+  unsigned long long* acc_side = nullptr;
   if (SINK == SINK_AGG_REG) {
     if (!ADD_ONLY) acc_hi = PROG.acc_hi + ((size_t)blockIdx.x * B + tid) * (VM_REG_GROUPS * VM_REG_ACC);
     reg_agg_init<G>(S_reg, acc_hi);
+    if (SIDE) {
+      acc_side = PROG.acc_side + ((size_t)blockIdx.x * B + tid) * (VM_REG_GROUPS * VM_REG_ACC);
+      reg_side_init(acc_hi, acc_side);
+    }
 #pragma unroll
     for (int q = 0; q < G; q++) dir[q] = 0xFFFFFFFFFFFFFFFFull;
   }
@@ -2212,7 +2353,7 @@ __global__ void __launch_bounds__(512, 1) pipeline_kernel() {
       active = sink_agg_global(L, active);
       live_rows += __popc(active);
     } else {
-      active = sink_agg_reg<G, ADD_ONLY>(L, active, S_reg, acc_hi, &gtable, dir, dir_n, accops);
+      active = sink_agg_reg<G, ADD_ONLY, SIDE>(L, active, S_reg, acc_hi, acc_side, &gtable, dir, dir_n, accops);
       live_rows += __popc(active);
     }
     // everyone is done with this stage buffer (and the VM registers); the sink-overflow flag is
@@ -2242,7 +2383,7 @@ __global__ void __launch_bounds__(512, 1) pipeline_kernel() {
     __syncthreads();
     // scalar aggregates emit their single group even when no CTA saw a row: CTA 0 always flushes
     const bool has_rows = tile_of(0) < n_tiles;
-    if (has_rows || (G == 1 && blockIdx.x == 0)) reg_agg_flush<G, ADD_ONLY>(S_reg, acc_hi, &gtable, (Acc128*)smem, tid, B);
+    if (has_rows || (G == 1 && blockIdx.x == 0)) reg_agg_flush<G, ADD_ONLY, SIDE>(S_reg, acc_hi, &gtable, (Acc128*)smem, tid, B);
   }
 }
 
@@ -2284,17 +2425,17 @@ struct GateLock {
   }
 };
 
-template <int SINK, int G, bool ADD_ONLY>
+template <int SINK, int G, bool ADD_ONLY, bool SIDE = false>
 static cudaError_t launch_one(int grid, int block, size_t smem, cudaStream_t st) {
   // the opt-in to large dynamic shared memory is per (function, device) and sticky: raise it only when needed
   static size_t granted[64] = {0};
   const int dev = GateLock::current_device() & 63;
   if (smem > granted[dev]) {
-    cudaError_t e = cudaFuncSetAttribute(pipeline_kernel<SINK, G, ADD_ONLY>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    cudaError_t e = cudaFuncSetAttribute(pipeline_kernel<SINK, G, ADD_ONLY, SIDE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
     granted[dev] = smem;
   }
-  pipeline_kernel<SINK, G, ADD_ONLY><<<grid, block, smem, st>>>();
+  pipeline_kernel<SINK, G, ADD_ONLY, SIDE><<<grid, block, smem, st>>>();
   return cudaGetLastError();
 }
 
@@ -2318,6 +2459,8 @@ cudaError_t launch_pipeline(const Program& P, int reg_groups, int grid, int bloc
     case SINK_MATERIALIZE: return launch_one<SINK_MATERIALIZE, 1, true>(grid, block, smem, st);
     case SINK_AGG_GLOBAL: return launch_one<SINK_AGG_GLOBAL, 1, true>(grid, block, smem, st);
     default:
+      // string / UInt64 MIN / MAX are never add-only
+      if (P.has_side_acc) return reg_groups <= 1 ? launch_one<SINK_AGG_REG, 1, false, true>(grid, block, smem, st) : launch_one<SINK_AGG_REG, VM_REG_GROUPS, false, true>(grid, block, smem, st);
       if (reg_groups <= 1) return add_only ? launch_one<SINK_AGG_REG, 1, true>(grid, block, smem, st) : launch_one<SINK_AGG_REG, 1, false>(grid, block, smem, st);
       return add_only ? launch_one<SINK_AGG_REG, VM_REG_GROUPS, true>(grid, block, smem, st) : launch_one<SINK_AGG_REG, VM_REG_GROUPS, false>(grid, block, smem, st);
   }

@@ -125,13 +125,23 @@ struct OutCol {
   uint8_t _pad[7];
 };
 
-enum AccKind : uint8_t { ACC_SUM_I128 = 0, ACC_SUM_F64, ACC_COUNT, ACC_MIN_I128, ACC_MAX_I128, ACC_MIN_F64, ACC_MAX_F64, ACC_COUNT_STAR };
+// Accumulators.  A cell is 16 bytes (lo, hi):
+//  SUM_I128 / MIN_I128 / MAX_I128: 128-bit two's complement; COUNT / COUNT_STAR: count in lo;
+//  SUM_F64: the double's bits in lo; MIN_F64 / MAX_F64: the total-order key of the double in lo;
+//  MIN_STR / MAX_STR: the string view {ptr, len} of the best value so far (unsigned bytewise order, a proper prefix
+//  first), len = ACC_STR_NONE while no value has been seen -- the identity of both (an empty string is a value).
+//  The characters stay where the rows had them; the host copies the extracted results into buffers of their own.
+//  String MIN / MAX and the zero-extended UInt64 MIN / MAX are the register sink's "side" accumulators (pipeline.cu).
+enum AccKind : uint8_t { ACC_SUM_I128 = 0, ACC_SUM_F64, ACC_COUNT, ACC_MIN_I128, ACC_MAX_I128, ACC_MIN_F64, ACC_MAX_F64, ACC_COUNT_STAR,
+                         ACC_MIN_STR, ACC_MAX_STR };
+static const unsigned long long ACC_STR_NONE = ~0ull;
 
 struct AccDesc {
   Operand src;      // value operand (ignored for ACC_COUNT_STAR)
   uint8_t kind;     // AccKind
   uint8_t nullable; // operand may be NULL
-  uint8_t _pad[2];
+  uint8_t zext;     // MIN_I128 / MAX_I128 over UInt64: the operand's 64 bits are zero-extended, not sign-extended
+  uint8_t _pad;
 };
 
 // Global aggregate hash table (SoA), shared by both aggregate sinks and by the extraction kernel.
@@ -180,13 +190,15 @@ struct Program {
   Operand keys[VM_MAX_KEYS];    // aggregate sinks: group keys
   Operand key_hash;             // aggregate sinks: I64 register holding the row hash (OPD_NONE if no keys)
   uint8_t keys_all_i64;         // every key is an integer-like 64-bit value (ints, dates, bools, packed strings)
-  uint8_t _pad1[3];
+  uint8_t has_side_acc;         // some accumulator is a string MIN / MAX or a UInt64 MIN / MAX (zext)
+  uint8_t _pad1[2];
   AccDesc acc[VM_MAX_ACC];
   AggTable table;
   unsigned long long* acc_hi;   // register sink: high 64-bit words [cta][thread][group][acc], pre-zeroed
   RunStatus* status;
   unsigned long long* tile_state;  // materialize sink: one look-back word per tile, zeroed before the launch
   int64_t n_rows;
+  unsigned long long* acc_side; // register sink with has_side_acc: the side accumulators' 64-bit values, laid out as acc_hi
 };
 
 // ---- fused fast path (scan -> filter -> decimal products -> <=4-group SUM/COUNT aggregate) -----------

@@ -1166,6 +1166,7 @@ int add_acc(PipelineBuilder& pb, AggLowered& L, uint8_t kind, const ColRef* src)
   a.kind = kind;
   a.src = so;
   a.nullable = nullable ? 1 : 0;
+  a.zext = (src && src->type.id == TypeId::UInt64 && (kind == ACC_MIN_I128 || kind == ACC_MAX_I128)) ? 1 : 0;
   L.accs.push_back(a);
   if (src) {
     pb.pin(*src);
@@ -1266,6 +1267,16 @@ void lower_aggregate(PipelineBuilder& pb, const PlanNode& node, AggLowered& L, i
     L.outs.push_back(r);
   };
   auto sum_out_kind = [](const DataType& t) -> uint8_t { return t.pk() == PK::F64 ? AO_ACC_F64 : (t.pk() == PK::I128 ? AO_ACC_I128 : AO_ACC_I64); };
+  // MIN / MAX of a value (raw rows or a partial state column): strings as views, floats by their total-order key,
+  // everything else (integers, UInt64 zero-extended, decimals, bools) as 128-bit integers
+  auto push_minmax = [&](bool mn, const ColRef& v, const DataType& t, const std::string& name) {
+    const bool s = v.type.pk() == PK::Str, f = v.type.pk() == PK::F64;
+    const uint8_t kind = s ? (mn ? ACC_MIN_STR : ACC_MAX_STR) : f ? (mn ? ACC_MIN_F64 : ACC_MAX_F64) : (mn ? ACC_MIN_I128 : ACC_MAX_I128);
+    int a = add_acc(pb, L, kind, &v);
+    int c = v.nullable ? add_acc(pb, L, ACC_COUNT, &v) : star;
+    push(s ? AO_MINMAX_STR : f ? AO_MINMAX_F64 : sum_out_kind(t), a, c, t, name, v.nullable || scalar);
+    if (s) L.outs.back().phys = PH_STRVIEW;  // copied into a buffer of its own after the extraction
+  };
   for (size_t ai = 0; ai < node.aggs.size(); ai++) {
     const AggExpr& ae = node.aggs[ai];
     const std::string& nm = ae.name;
@@ -1286,11 +1297,7 @@ void lower_aggregate(PipelineBuilder& pb, const PlanNode& node, AggLowered& L, i
         }
         case AggFn::Min:
         case AggFn::Max: {
-          if (s0.type.pk() == PK::Str) throw EngineError(B200_ERR_UNSUPPORTED, "MIN/MAX over Utf8");
-          bool f = s0.type.pk() == PK::F64, mn = ae.fn == AggFn::Min;
-          int a = add_acc(pb, L, f ? (mn ? ACC_MIN_F64 : ACC_MAX_F64) : (mn ? ACC_MIN_I128 : ACC_MAX_I128), &s0);
-          int c = s0.nullable ? add_acc(pb, L, ACC_COUNT, &s0) : star;
-          push(f ? AO_MINMAX_F64 : sum_out_kind(ae.result_type), a, c, ae.result_type, nm, s0.nullable || scalar);
+          push_minmax(ae.fn == AggFn::Min, s0, ae.result_type, nm);
           break;
         }
         case AggFn::Avg: {
@@ -1326,12 +1333,8 @@ void lower_aggregate(PipelineBuilder& pb, const PlanNode& node, AggLowered& L, i
       }
       case AggFn::Min:
       case AggFn::Max: {
-        if (arg.type.pk() == PK::Str) throw EngineError(B200_ERR_UNSUPPORTED, "MIN/MAX over Utf8");
-        if (arg.type.id == TypeId::UInt64) throw EngineError(B200_ERR_UNSUPPORTED, "MIN/MAX over UInt64");
-        bool f = arg.type.pk() == PK::F64, mn = ae.fn == AggFn::Min;
-        int a = add_acc(pb, L, f ? (mn ? ACC_MIN_F64 : ACC_MAX_F64) : (mn ? ACC_MIN_I128 : ACC_MAX_I128), &arg);
-        int c = arg.nullable ? add_acc(pb, L, ACC_COUNT, &arg) : star;
-        push(f ? AO_MINMAX_F64 : sum_out_kind(ae.sum_type), a, c, ae.sum_type, emit_states ? nm + (mn ? "[min]" : "[max]") : nm, arg.nullable || scalar);
+        const bool mn = ae.fn == AggFn::Min;
+        push_minmax(mn, arg, ae.sum_type, emit_states ? nm + (mn ? "[min]" : "[max]") : nm);
         break;
       }
       case AggFn::Avg: {
@@ -1961,6 +1964,14 @@ DevBatchPtr run_aggregate(const Exec& x, const BuilderFactory& make_pb, const Pl
       DevPtr hi = dev_alloc(hi_bytes, x.st());
       tm.keep.push_back(hi);
       P.acc_hi = (unsigned long long*)hi->ptr;
+      // string / UInt64 MIN / MAX keep their per-thread values in a scratch of their own (initialised by the kernel)
+      for (size_t a = 0; a < L.accs.size(); a++)
+        P.has_side_acc |= (L.accs[a].kind == ACC_MIN_STR || L.accs[a].kind == ACC_MAX_STR || L.accs[a].zext) ? 1 : 0;
+      if (P.has_side_acc) {
+        DevPtr side = dev_alloc(hi_bytes, x.st());
+        tm.keep.push_back(side);
+        P.acc_side = (unsigned long long*)side->ptr;
+      }
     }
     // First sight of a large integer-keyed aggregate: group the first 16 K rows on the hash kernel to learn whether the
     // 4-group register sink can apply at all and which table class to start with, instead of discovering it by running
@@ -2070,6 +2081,11 @@ DevBatchPtr run_aggregate(const Exec& x, const BuilderFactory& make_pb, const Pl
   }
   launch_agg_extract(tm.T, A, x.st());
   x.count();
+  // string MIN / MAX results are views of the input's characters (or of a literal of the pipeline): copy them into a
+  // buffer of their own, so that the result outlives the input and a few strings do not pin a multi-GB character buffer.
+  // The character total is not known on the host: each such column costs three launches and one read-back of it.
+  for (size_t j = 0; j < L.outs.size(); j++)
+    if (L.outs[j].kind == AO_MINMAX_STR) out->cols[j] = as_utf8(x, out->cols[j]);
   {
     // the extraction's overflow flag (decimal AVG / SUM precision) only has to be seen before the task returns
     const unsigned int* herr = x.fetch<unsigned int>(A.error);

@@ -10,6 +10,9 @@ engine's own CUDA-event timing (b200_engine_kernel_stats) can be read for the sa
   filter     q3's lineitem filter (l_shipdate > date) forwarding 3 columns                            -> fast_filter_kernel
   parquet    lineitem q1 columns written by pyarrow (uncompressed), scanned by the device decoder      -> pq_values_kernel
   q1         stage 1 of q1                                                                             -> fused_kernel
+  minmax_str lineitem MIN/MAX(l_comment) GROUP BY l_returnflag, l_linestatus (4 groups)              -> pipeline_agg_reg
+             and MAX(l_comment) GROUP BY l_orderkey (15 M groups at SF10)                             -> pipeline_agg_global
+             (each result checked against the CPU oracle unless ORACLE=0)
 """
 import json
 import os
@@ -86,6 +89,45 @@ elif op == "parquet":
 elif op == "q1":
     load("lineitem", tpch.Q1_COLUMNS)
     run([tpch.q1(1)[0]], [1])
+elif op == "minmax_str":
+    cols = ["l_orderkey", "l_returnflag", "l_linestatus", "l_comment"]
+    n = load("lineitem", cols)
+    host = eng.export_table("lineitem", 0)
+    comment = host.column(3)
+    arrow_bytes = {"offsets": 4 * (n + 1), "chars": comment.buffers()[2].size, "flags": 2 * (4 * (n + 1) + n), "orderkey": 8 * n}
+    del host, comment
+    scan = tpch.table_scan("lineitem", cols)
+    queries = {
+        "reg_4_groups": (P.aggregate("Single", [(c(1), "l_returnflag"), (c(2), "l_linestatus")],
+                                     [P.agg("min", c(3), "mn"), P.agg("max", c(3), "mx")], scan),
+                         arrow_bytes["offsets"] + arrow_bytes["chars"] + arrow_bytes["flags"]),
+        "global_orderkey": (P.aggregate("Single", [(c(0), "l_orderkey")], [P.agg("max", c(3), "mx")], scan),
+                            arrow_bytes["offsets"] + arrow_bytes["chars"] + arrow_bytes["orderkey"]),
+    }
+    report = {}
+    oracle = None
+    if os.environ.get("ORACLE", "1") != "0":
+        sys.path.insert(0, os.path.join(ROOT, "tests"))
+        import oracle_ffi
+        from util import assert_tables_equal
+        from ballista_b200 import driver
+        oracle = oracle_ffi.OracleEngine()
+        oracle.tpch_generate("lineitem", msf, 0, 0, n, cols)
+    for name, (plan, nbytes) in queries.items():
+        st = [P.Stage(1, P.shuffle_writer(plan, 1))]
+        eng.kernel_stats(reset=True)
+        run(st, [1])
+        ks = eng.kernel_stats(reset=True)
+        fam = {k: v for k, v in ks.items() if k.startswith("pipeline_") or k == "groupby_hash_agg"}
+        ms = {k: round(v["ms"] / reps, 3) for k, v in fam.items()}
+        report[name] = {"kernel_ms_per_run": ms, "arrow_bytes_read": nbytes,
+                        "GB_per_s": {k: round(nbytes / (v * 1e-3) / 1e9, 1) for k, v in ms.items() if v > 0}}
+        if oracle is not None:
+            got = driver.run_stages(eng, st, f"chk-{name}")
+            want = driver.run_stages(oracle, st, f"chk-{name}")
+            assert_tables_equal(got, want)
+            report[name]["matches_oracle"] = True
+    print(json.dumps({op: report, "rows": n}, indent=1))
 else:
     raise SystemExit(__doc__)
 print(json.dumps({op: eng.kernel_stats()}, indent=1))
