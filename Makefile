@@ -5,7 +5,7 @@ PKG       := datafusion-ballista_b200
 SRC       := $(PKG)/csrc
 OUT       := $(PKG)/lib
 NVFLAGS   := $(ARCH) -lineinfo -O3 -std=c++17 -Xcompiler -fPIC -Xcompiler -Wno-unused-function
-OBJS      := $(OUT)/pipeline.o $(OUT)/kernels.o $(OUT)/shuffle.o $(OUT)/join.o $(OUT)/groupby.o $(OUT)/parquet.o $(OUT)/filter.o $(OUT)/engine.o $(OUT)/host_narrow.o
+OBJS      := $(OUT)/pipeline.o $(OUT)/kernels.o $(OUT)/shuffle.o $(OUT)/join.o $(OUT)/nlj.o $(OUT)/groupby.o $(OUT)/parquet.o $(OUT)/filter.o $(OUT)/engine.o $(OUT)/host_narrow.o
 CXX       ?= g++
 COMMON    := $(wildcard $(SRC)/common/*.hpp) $(wildcard $(SRC)/device/*.h) $(wildcard $(SRC)/device/*.cuh) $(wildcard $(SRC)/host/*.hpp) include/b200exec.h include/b200_arrow_abi.h
 
@@ -27,6 +27,9 @@ $(OUT)/groupby.o: $(SRC)/device/groupby.cu $(COMMON)
 	@mkdir -p $(OUT)
 	$(NVCC) $(NVFLAGS) -c $< -o $@
 $(OUT)/join.o: $(SRC)/device/join.cu $(COMMON)
+	@mkdir -p $(OUT)
+	$(NVCC) $(NVFLAGS) -c $< -o $@
+$(OUT)/nlj.o: $(SRC)/device/nlj.cu $(COMMON)
 	@mkdir -p $(OUT)
 	$(NVCC) $(NVFLAGS) -c $< -o $@
 $(OUT)/shuffle.o: $(SRC)/device/shuffle.cu $(COMMON)

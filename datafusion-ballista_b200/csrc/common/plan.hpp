@@ -586,6 +586,7 @@ struct PlanNode {
   std::vector<std::pair<ExprPtr, ExprPtr>> on;
   bool null_equals_null = false;
   ExprPtr join_filter;  // over concat(left schema, right schema)
+  bool nested_loop = false;  // NestedLoopJoinExec: no keys, every (build, probe) pair is tested against the filter
   // Sort / SPM / Limit
   std::vector<SortKey> sort_keys;
   int64_t fetch = -1;
@@ -779,18 +780,24 @@ inline PlanPtr parse_plan(const Json& j) {
         n->schema.push_back(Field{ae.name, ae.result_type, ae.fn != AggFn::Count});
       }
     }
-  } else if (op == "HashJoinExec" || op == "SortMergeJoinExec") {
+  } else if (op == "HashJoinExec" || op == "SortMergeJoinExec" || op == "NestedLoopJoinExec") {
     // SortMergeJoinExec (datafusion.proto:1433, Ballista's default join, extension.rs:683): same matching
     // semantics as the hash join over co-partitioned inputs; its contract adds an output ordered by the
     // join keys (sort_options), which both engines establish by sorting the join result.
+    // NestedLoopJoinExec (datafusion.proto:1301-1307): a join without equality keys.  DataFusion requires a single
+    // partition on its left input, so the left side is the build side and every task reads it whole (CollectLeft).
     const bool smj = op == "SortMergeJoinExec";
+    const bool nlj = op == "NestedLoopJoinExec";
     n->op = PlanNode::HashJoin;
+    n->nested_loop = nlj;
     PlanNode* l = parse_child("left");
     PlanNode* r = parse_child("right");
     n->join_type = parse_join_type(j.get_str("join_type", "Inner"));
-    n->partition_mode = smj ? std::string("Partitioned") : j.get_str("mode", "Partitioned");
+    n->partition_mode = smj ? std::string("Partitioned") : nlj ? std::string("CollectLeft") : j.get_str("mode", "Partitioned");
     n->null_equals_null = j.get_bool("null_equals_null", false);
-    const Json& on = j.at("on");
+    Json no_keys;
+    const Json& on = nlj ? (j.has("on") ? j.at("on") : no_keys) : j.at("on");
+    if (nlj && on.size() > 0) throw std::runtime_error("NestedLoopJoinExec has no equality keys");
     for (size_t i = 0; i < on.size(); i++) {
       ExprPtr le = parse_expr(on.at(i).at(0), l->schema);
       ExprPtr re = parse_expr(on.at(i).at(1), r->schema);

@@ -115,9 +115,12 @@ inline std::string dump_plan(const PlanNode& n) {
       break;
     }
     case PlanNode::HashJoin: {
-      o += std::string(",\"join_type\":\"") + join_types[(int)n.join_type] + "\",\"mode\":" + pbp::jstr(n.partition_mode) + ",\"on\":[";
-      for (size_t i = 0; i < n.on.size(); i++) o += std::string(i ? "," : "") + "[" + dump_expr(n.on[i].first) + "," + dump_expr(n.on[i].second) + "]";
-      o += "]";
+      o += std::string(",\"join_type\":\"") + join_types[(int)n.join_type] + "\"";
+      if (!n.nested_loop) {  // a nested-loop join has neither a partition mode of its own nor keys
+        o += ",\"mode\":" + pbp::jstr(n.partition_mode) + ",\"on\":[";
+        for (size_t i = 0; i < n.on.size(); i++) o += std::string(i ? "," : "") + "[" + dump_expr(n.on[i].first) + "," + dump_expr(n.on[i].second) + "]";
+        o += "]";
+      }
       if (n.join_filter) o += ",\"filter\":" + dump_expr(n.join_filter);
       if (n.has_projection) o += ",\"projection\":" + dump_ints(n.projection);
       if (!n.sort_keys.empty()) o += ",\"sort_keys\":" + dump_sort_keys(n.sort_keys);

@@ -465,15 +465,20 @@ inline std::string table_of_path(const std::string& path) {
 inline std::string plan_json(const Msg& n, const std::string& override_job = std::string());
 
 // JoinOn { left = 1, right = 2 } (:1198-1201); JoinFilter { expression = 1, column_indices = 2 { index = 1, side = 2 }, schema = 3 } (:1343-1352)
+// f_on = 0: the node has no equality keys (NestedLoopJoinExecNode) and no "on" key is written
 inline std::string join_common_json(const Msg& m, uint32_t f_on, uint32_t f_type, uint32_t f_filter) {
-  std::string o = ",\"on\":[";
-  bool first = true;
-  for (auto& on : m.subs(f_on)) {
-    if (!first) o += ",";
-    first = false;
-    o += "[" + expr_json(on.sub(1)) + "," + expr_json(on.sub(2)) + "]";
+  std::string o;
+  if (f_on) {
+    o = ",\"on\":[";
+    bool first = true;
+    for (auto& on : m.subs(f_on)) {
+      if (!first) o += ",";
+      first = false;
+      o += "[" + expr_json(on.sub(1)) + "," + expr_json(on.sub(2)) + "]";
+    }
+    o += "]";
   }
-  o += std::string("],\"join_type\":\"") + join_type_name(m.u64(f_type)) + "\"";
+  o += std::string(",\"join_type\":\"") + join_type_name(m.u64(f_type)) + "\"";
   if (m.has(f_filter)) {
     const Msg f = m.sub(f_filter);
     if (f.has(1)) {
@@ -606,6 +611,12 @@ inline std::string plan_json(const Msg& n, const std::string& override_job) {
       const Msg part = m.sub(5);  // Partitioning { round_robin = 1, hash = 2, unknown = 3 } (:1335-1341)
       if (part.has(2)) throw Unsupported("hash RepartitionExec inside a stage (the distributed planner cuts stages there)");
       return "{\"op\":\"RepartitionExec\",\"input\":" + in(1) + "}";
+    }
+    case 22: {  // NestedLoopJoinExecNode { left = 1, right = 2, join_type = 3, filter = 4, projection = 5 } (:1301-1307)
+      std::string o = "{\"op\":\"NestedLoopJoinExec\",\"left\":" + in(1) + ",\"right\":" + in(2) + join_common_json(m, 0, 3, 4);
+      const std::vector<uint64_t> proj = m.varints(5);
+      if (!proj.empty()) o += ",\"projection\":" + u32_list_json(proj);
+      return o + "}";
     }
     case 32: return in(1);                                                             // CooperativeExecNode: a scheduling wrapper (:1125-1127)
     case 18: {  // PhysicalExtensionNode { node = 1, inputs = 2 } (:845-848) -> BallistaPhysicalPlanNode (ballista.proto:47-54)

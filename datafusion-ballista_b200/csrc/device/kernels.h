@@ -255,6 +255,45 @@ void launch_select_indices(const uint32_t* flag01, const uint64_t* offs, int64_t
 void launch_counts_to_flag(const uint32_t* counts, uint8_t* flags, int64_t n, cudaStream_t st);
 void launch_mark_from_idx(const int64_t* idx, int64_t n, uint8_t* marks, cudaStream_t st);
 
+// ---- nested-loop join (nlj.cu) ------------------------------------------------------------------
+// The join filter as the kernels see it: a boolean program (AND / OR / NOT, Kleene logic) over at most NLJ_MAX_ATOMS
+// atoms.  An atom is a Bool column of one side (evaluated beforehand by the VM) or a comparison f(build) op g(probe)
+// of two columns, one per side.  Registers are bits of two words per pair: T (known true) and F (known false); NULL
+// is neither.  Atom k lands in register k, step s of the program writes register NLJ_MAX_ATOMS + s.
+static const int NLJ_MAX_ATOMS = 8;
+static const int NLJ_MAX_STEPS = 24;
+enum NljAtomKind : uint8_t { NLJ_BUILD_BOOL = 0, NLJ_PROBE_BOOL = 1, NLJ_CMP = 2 };
+enum NljValueKind : uint8_t {
+  NLJ_V_I64 = 0,   // integer-like columns (Int8..Int64, UInt8..UInt32, Date32, Timestamp, Bool), sign / zero extended
+  NLJ_V_U64,       // UInt64, compared unsigned
+  NLJ_V_F64,       // Float32 / Float64 in IEEE total order (-0.0 < +0.0, NaN above +inf)
+  NLJ_V_I128,      // Decimal128 of one scale
+  NLJ_V_STR        // 16-byte views: unsigned bytes, a proper prefix first
+};
+enum NljStepKind : uint8_t { NLJ_AND = 0, NLJ_OR = 1, NLJ_NOT = 2 };
+struct NljAtom {
+  KeyCol build, probe;  // NLJ_CMP: both operands; NLJ_BUILD_BOOL / NLJ_PROBE_BOOL: the Bool8 column in its side's slot
+  uint8_t kind;         // NljAtomKind
+  uint8_t cmp;          // NLJ_CMP: build op probe, 0 EQ 1 NE 2 LT 3 LE 4 GT 5 GE
+  uint8_t vk;           // NLJ_CMP: NljValueKind
+  uint8_t _pad[5];
+};
+struct NljStep {
+  uint8_t kind, a, b, dst;
+};
+struct NljSpec {
+  NljAtom atoms[NLJ_MAX_ATOMS];
+  NljStep steps[NLJ_MAX_STEPS];
+  int n_atoms, n_steps;
+  int result;   // register holding the filter's value; -1: no filter, every pair matches
+  int _pad;
+};
+// counts[j] = pairs of probe row j that pass; build_mark[i] / probe_mark[j] (optional) = 1 for rows with a pair
+void launch_nlj_count(const NljSpec& S, int64_t n_build, int64_t n_probe, uint32_t* counts, uint8_t* build_mark, uint8_t* probe_mark, cudaStream_t st);
+// the passing pairs in probe-row order, build-row order inside a probe row, at offsets = exclusive scan of counts
+void launch_nlj_write(const NljSpec& S, int64_t n_build, int64_t n_probe, const uint32_t* counts, const uint64_t* offsets, int64_t* out_build_idx,
+                      int64_t* out_probe_idx, cudaStream_t st);
+
 // ---- sort -------------------------------------------------------------------------------------
 struct SortWordArgs {
   const void* data;

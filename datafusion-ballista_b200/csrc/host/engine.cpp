@@ -118,6 +118,7 @@ struct b200_engine {
   std::mutex export_mu;                      // small-result export arena (pinned), one export at a time
   uint8_t* export_arena = nullptr;
   std::atomic<uint64_t> narrowed_bytes_saved{0};         // PCIe bytes not sent thanks to narrowing (b200_engine_counter)
+  std::atomic<uint64_t> nlj_pairs{0};                    // (build row, probe row) pairs the nested-loop join evaluated (b200_engine_counter)
 };
 
 struct b200_stage {
@@ -2354,7 +2355,7 @@ struct Runner {
         break;
       }
       case PlanNode::HashJoin:
-        out = exec_join(n, part, met);
+        out = n.nested_loop ? exec_nlj(n, part, met) : exec_join(n, part, met);
         if (!n.sort_keys.empty()) out = do_sort(n.sort_keys, -1, out, met);  // SortMergeJoinExec: ordered by the join keys
         break;
       case PlanNode::Sort: {
@@ -2589,6 +2590,12 @@ struct Runner {
     }
   }
 
+  // unmatched or semi / anti build rows: a join whose whole build side is read by every task (CollectLeft, nested loop)
+  // emits those rows once per task
+  static bool emits_build_rows(JoinType jt) {
+    return jt == JoinType::Left || jt == JoinType::Full || jt == JoinType::LeftSemi || jt == JoinType::LeftAnti;
+  }
+
   DevBatchPtr exec_join(const PlanNode& n, int part, OpMetrics* met) {
     const bool collect_left = n.partition_mode == "CollectLeft";
     std::vector<ExprPtr> lk, rk;
@@ -2602,8 +2609,7 @@ struct Runner {
     // (unmatched or semi/anti) would then emit them once per task.  DataFusion shares a visited bitmap across
     // the probe partitions of one process; tasks here are independent, so those shapes are only legal with a
     // single probe partition.
-    if (collect_left && (n.join_type == JoinType::Left || n.join_type == JoinType::Full || n.join_type == JoinType::LeftSemi || n.join_type == JoinType::LeftAnti) &&
-        n_partitions(*n.children[1]) > 1)
+    if (collect_left && emits_build_rows(n.join_type) && n_partitions(*n.children[1]) > 1)
       throw EngineError(B200_ERR_UNSUPPORTED, "CollectLeft hash join that emits build-side rows over more than one probe partition: plan it as Partitioned");
     // one integer-like key: the table is keyed by the key itself (no hash column, no second look at the keys)
     const bool exact = nk == 1 && exact_key(lk[0]->type) && lk[0]->type.id == rk[0]->type.id;
@@ -2719,6 +2725,18 @@ struct Runner {
       bidx = (const int64_t*)kept->cols[0].data;
       pidx = (const int64_t*)kept->cols[1].data;
     }
+    return join_output(n, Lp, Rp, bidx, pidx, n_pairs, bmark, pmark, t0, met);
+  }
+
+  // The join's output from its matching pairs (bidx[k], pidx[k]), k < n_pairs, shared by the hash join and the nested-loop
+  // join: semi / anti selection, outer rows (unmatched build rows, then unmatched probe rows, after the pairs) and the
+  // gather of the columns the projection keeps.  bmark / pmark: "has a pair" marks of build / probe rows when the caller
+  // already has them; otherwise they are derived from the pairs.
+  DevBatchPtr join_output(const PlanNode& n, const DevBatch& Lp, const DevBatch& Rp, const int64_t* bidx, const int64_t* pidx, int64_t n_pairs,
+                          const DevPtr& bmark, const DevPtr& pmark, std::chrono::steady_clock::time_point t0, OpMetrics* met) {
+    const JoinType jt = n.join_type;
+    const int64_t nb = Lp.n, np = Rp.n;
+    const bool left_outer = jt == JoinType::Left || jt == JoinType::Full, right_outer = jt == JoinType::Right || jt == JoinType::Full;
     auto flags_to_indices = [&](const uint8_t* marks, int64_t nrows, bool want, int64_t* n_sel) {
       DevPtr f = dev_alloc((size_t)(nrows + 1) * 4, x.st());
       DevPtr o = dev_alloc((size_t)(nrows + 2) * 8, x.st());
@@ -2733,7 +2751,7 @@ struct Runner {
       return idx;
     };
     auto marks_of = [&](const int64_t* idx, int64_t nrows, const DevPtr& from_probe) {
-      if (!has_filter && from_probe) return from_probe;  // the probe pass already marked them
+      if (from_probe) return from_probe;  // the probe pass already marked them
       DevPtr m = dev_alloc((size_t)std::max<int64_t>(nrows, 1), x.st());
       CUDA_CHECK(cudaMemsetAsync(m->ptr, 0, (size_t)std::max<int64_t>(nrows, 1), x.st()));
       if (n_pairs > 0) {
@@ -2839,6 +2857,182 @@ struct Runner {
       met->input_rows += (uint64_t)(nb + np);
     }
     return out;
+  }
+
+  // ---- nested-loop join -------------------------------------------------------------------------
+  // The join filter (over left ++ right) split into NljSpec's boolean program: AND / OR / NOT become steps, every other
+  // node is an atom -- a Bool expression over one side, or a comparison between an expression over the build side and
+  // one over the probe side.  The VM evaluates the atoms' side expressions as columns of their side.
+  struct NljLowered {
+    NljSpec S;
+    std::vector<ExprPtr> build_exprs, probe_exprs;  // probe expressions index the probe side's own schema
+    int build_at[NLJ_MAX_ATOMS], probe_at[NLJ_MAX_ATOMS];
+    int n_left = 0;
+  };
+  static int expr_sides(const Expr& e, int n_left) {  // bit 0: reads build columns, bit 1: reads probe columns
+    if (e.kind == Expr::Col) return e.col < n_left ? 1 : 2;
+    int s = 0;
+    for (auto& a : e.args) s |= expr_sides(*a, n_left);
+    return s;
+  }
+  static uint8_t nlj_value_kind(const DataType& b, const DataType& p, const Expr& e) {
+    auto refuse = [&](const std::string& why) {
+      return EngineError(B200_ERR_UNSUPPORTED, "nested-loop join filter " + dump_expr(std::make_shared<Expr>(e)) + ": " + why);
+    };
+    if (b.is_string() && p.is_string()) return NLJ_V_STR;
+    if (b.is_decimal() && p.is_decimal()) {
+      if (b.scale != p.scale) throw refuse("decimal operands of different scales (" + b.str() + " vs " + p.str() + "): the plan must cast one of them");
+      return NLJ_V_I128;
+    }
+    if (b.is_float() && p.is_float()) return NLJ_V_F64;
+    if (b.id == TypeId::UInt64 || p.id == TypeId::UInt64) {
+      if (b.id == p.id) return NLJ_V_U64;
+    } else if (b.pk() == p.pk() && (b.pk() == PK::I64 || b.pk() == PK::Bool)) {
+      return NLJ_V_I64;
+    }
+    throw refuse("cannot compare " + b.str() + " with " + p.str() + " without a cast");
+  }
+  int nlj_step(NljLowered& L, uint8_t kind, int a, int b) {
+    NljSpec& S = L.S;
+    if (S.n_steps == NLJ_MAX_STEPS) throw EngineError(B200_ERR_UNSUPPORTED, "nested-loop join filter has more than " + std::to_string(NLJ_MAX_STEPS) + " AND / OR / NOT nodes");
+    NljStep& s = S.steps[S.n_steps];
+    s.kind = kind;
+    s.a = (uint8_t)a;
+    s.b = (uint8_t)b;
+    s.dst = (uint8_t)(NLJ_MAX_ATOMS + S.n_steps);
+    return NLJ_MAX_ATOMS + S.n_steps++;
+  }
+  int nlj_lower(const ExprPtr& e, NljLowered& L) {
+    if (e->kind == Expr::Bin && is_logic(e->op)) {
+      const int a = nlj_lower(e->args[0], L), b = nlj_lower(e->args[1], L);
+      return nlj_step(L, e->op == BinOp::And ? NLJ_AND : NLJ_OR, a, b);
+    }
+    if (e->kind == Expr::Not) {
+      const int a = nlj_lower(e->args[0], L);
+      return nlj_step(L, NLJ_NOT, a, a);
+    }
+    NljSpec& S = L.S;
+    if (S.n_atoms == NLJ_MAX_ATOMS)
+      throw EngineError(B200_ERR_UNSUPPORTED, "nested-loop join filter has more than " + std::to_string(NLJ_MAX_ATOMS) + " comparisons or one-side conditions");
+    const int k = S.n_atoms++;
+    NljAtom& a = S.atoms[k];
+    L.build_at[k] = L.probe_at[k] = -1;
+    const int sides = expr_sides(*e, L.n_left);
+    if (sides != 3) {  // one side (or none: a constant, evaluated on the build side)
+      if (e->type.id != TypeId::Bool) throw EngineError(B200_ERR_UNSUPPORTED, "nested-loop join filter term is not boolean: " + dump_expr(e));
+      if (sides == 2) {
+        a.kind = NLJ_PROBE_BOOL;
+        L.probe_at[k] = (int)L.probe_exprs.size();
+        L.probe_exprs.push_back(shift_cols(e, -L.n_left));
+      } else {
+        a.kind = NLJ_BUILD_BOOL;
+        L.build_at[k] = (int)L.build_exprs.size();
+        L.build_exprs.push_back(e);
+      }
+      return k;
+    }
+    const int sl = e->kind == Expr::Bin && is_compare(e->op) ? expr_sides(*e->args[0], L.n_left) : 0;
+    const int sr = e->kind == Expr::Bin && is_compare(e->op) ? expr_sides(*e->args[1], L.n_left) : 0;
+    if (!((sl == 1 && sr == 2) || (sl == 2 && sr == 1)))
+      throw EngineError(B200_ERR_UNSUPPORTED, "nested-loop join filter term mixes both sides inside one operand, which the device does not evaluate: " + dump_expr(e));
+    static const uint8_t swapped[] = {0, 1, 4, 5, 2, 3};  // p op b == b op' p (codes 0 EQ 1 NE 2 LT 3 LE 4 GT 5 GE)
+    const int c = (int)e->op - (int)BinOp::Eq;
+    const ExprPtr& be = sl == 1 ? e->args[0] : e->args[1];
+    const ExprPtr& pe = sl == 1 ? e->args[1] : e->args[0];
+    a.kind = NLJ_CMP;
+    a.cmp = (uint8_t)(sl == 1 ? c : swapped[c]);
+    a.vk = nlj_value_kind(be->type, pe->type, *e);
+    L.build_at[k] = (int)L.build_exprs.size();
+    L.build_exprs.push_back(be);
+    L.probe_at[k] = (int)L.probe_exprs.size();
+    L.probe_exprs.push_back(shift_cols(pe, -L.n_left));
+    return k;
+  }
+  static KeyCol nlj_operand(const DevColumn& c, const NljAtom& a) {
+    bool ok;
+    if (a.kind != NLJ_CMP) ok = c.phys == PH_BOOL8;
+    else switch (a.vk) {
+      case NLJ_V_STR: ok = c.phys == PH_STRVIEW; break;
+      case NLJ_V_I128: ok = c.phys == PH_DEC128; break;
+      case NLJ_V_F64: ok = c.phys == PH_F64 || c.phys == PH_F32; break;
+      case NLJ_V_U64: ok = c.phys == PH_U64; break;
+      default: ok = c.phys <= PH_U32 || c.phys == PH_BOOL8;
+    }
+    if (!ok) throw EngineError(B200_ERR_EXECUTION, "nested-loop join: operand column " + c.name + " has an unexpected encoding");
+    return KeyCol{c.data, c.valid, (uint8_t)c.phys, (uint8_t)c.width()};
+  }
+
+  DevBatchPtr exec_nlj(const PlanNode& n, int part, OpMetrics* met) {
+    const JoinType jt = n.join_type;
+    // the build side is read whole by every task, as a CollectLeft hash join's
+    if (emits_build_rows(jt) && n_partitions(*n.children[1]) > 1)
+      throw EngineError(B200_ERR_UNSUPPORTED, "nested-loop join that emits build-side rows over more than one probe partition");
+    NljLowered L;
+    memset(&L.S, 0, sizeof L.S);
+    L.n_left = (int)n.children[0]->schema.size();
+    L.S.result = n.join_filter ? nlj_lower(n.join_filter, L) : -1;
+    JoinSide B = prepare_side(*n.children[0], part, true, L.build_exprs, false, met);
+    JoinSide P = prepare_side(*n.children[1], part, false, L.probe_exprs, false, met);
+    const int64_t nb = B.n, np = P.n;
+    if (nb >= ((int64_t)1 << 31)) throw EngineError(B200_ERR_UNSUPPORTED, "nested-loop join build side exceeds 2^31 rows");
+    auto t0 = std::chrono::steady_clock::now();
+    uint64_t w_b = 0, w_p = 0;
+    for (int k = 0; k < L.S.n_atoms; k++) {
+      NljAtom& a = L.S.atoms[k];
+      if (L.build_at[k] >= 0) {
+        a.build = nlj_operand(B.keys[(size_t)L.build_at[k]], a);
+        w_b += a.build.width;
+      }
+      if (L.probe_at[k] >= 0) {
+        a.probe = nlj_operand(P.keys[(size_t)L.probe_at[k]], a);
+        w_p += a.probe.width;
+      }
+    }
+    const bool want_bmark = emits_build_rows(jt);
+    const bool want_pmark = jt == JoinType::RightSemi || jt == JoinType::RightAnti || jt == JoinType::Right || jt == JoinType::Full;
+    DevPtr bmark, pmark;
+    if (want_bmark) {
+      bmark = dev_alloc((size_t)std::max<int64_t>(nb, 1), x.st());
+      CUDA_CHECK(cudaMemsetAsync(bmark->ptr, 0, (size_t)std::max<int64_t>(nb, 1), x.st()));
+    }
+    if (want_pmark) {
+      pmark = dev_alloc((size_t)std::max<int64_t>(np, 1), x.st());
+      CUDA_CHECK(cudaMemsetAsync(pmark->ptr, 0, (size_t)std::max<int64_t>(np, 1), x.st()));
+    }
+    x.check_cancel();
+    // algorithmic bytes: probe operands once, build operands once per 256-row probe tile
+    const uint64_t tiles = (uint64_t)(np + 255) / 256;
+    const uint64_t operand_bytes = (uint64_t)np * w_p + (uint64_t)nb * w_b * tiles;
+    DevPtr counts = dev_alloc((size_t)std::max<int64_t>(np, 1) * 4, x.st());
+    {
+      KernelTimer kt(x, "nlj_count", operand_bytes);
+      launch_nlj_count(L.S, nb, np, (uint32_t*)counts->ptr, bmark ? (uint8_t*)bmark->ptr : nullptr, pmark ? (uint8_t*)pmark->ptr : nullptr, x.st());
+      x.count();
+    }
+    x.e->nlj_pairs += (uint64_t)nb * (uint64_t)np;
+    x.check_cancel();
+    const bool semi_anti = jt == JoinType::LeftSemi || jt == JoinType::LeftAnti || jt == JoinType::RightSemi || jt == JoinType::RightAnti;
+    int64_t n_pairs = 0;
+    DevPtr bi, pi;
+    if (!semi_anti) {
+      DevPtr offs = dev_alloc((size_t)(np + 1) * 8, x.st());
+      DevPtr scratch = dev_alloc((size_t)(np / 1024 + 4) * 8, x.st());
+      if (np > 0) {
+        launch_scan_u32_to_u64((const uint32_t*)counts->ptr, (uint64_t*)offs->ptr, np, (uint64_t*)scratch->ptr, x.st());
+        x.count(3);
+        n_pairs = (int64_t)x.get<uint64_t>((const uint64_t*)offs->ptr + np);
+        x.check_cancel();
+      }
+      bi = dev_alloc((size_t)std::max<int64_t>(n_pairs, 1) * 8, x.st());
+      pi = dev_alloc((size_t)std::max<int64_t>(n_pairs, 1) * 8, x.st());
+      if (n_pairs > 0) {
+        KernelTimer kt(x, "nlj_write", operand_bytes + 16 * (uint64_t)n_pairs);
+        launch_nlj_write(L.S, nb, np, (const uint32_t*)counts->ptr, (const uint64_t*)offs->ptr, (int64_t*)bi->ptr, (int64_t*)pi->ptr, x.st());
+        x.count();
+      }
+      x.check_cancel();
+    }
+    return join_output(n, B.payload, P.payload, bi ? (const int64_t*)bi->ptr : nullptr, pi ? (const int64_t*)pi->ptr : nullptr, n_pairs, bmark, pmark, t0, met);
   }
 
   // ---- shuffle writer -----------------------------------------------------------------------------
@@ -4342,6 +4536,7 @@ uint64_t b200_engine_counter(b200_engine* e, const char* name) {
   if (n == "groupby") return e->n_groupby;
   if (n == "fastfilter") return e->n_fastfilter;
   if (n == "ingest_bytes_saved") return e->narrowed_bytes_saved;
+  if (n == "nlj_pairs") return e->nlj_pairs;
   return 0;
 }
 

@@ -37,7 +37,7 @@ def _probe_side_leaf(node: dict):
         return ("table", node["table"])
     if op in ("ShuffleReaderExec", "UnresolvedShuffleExec"):
         return ("stage", node["stage_id"])
-    if op in ("HashJoinExec", "SortMergeJoinExec"):
+    if op in ("HashJoinExec", "SortMergeJoinExec", "NestedLoopJoinExec"):
         return _probe_side_leaf(node["right"])
     return _probe_side_leaf(node["input"])
 

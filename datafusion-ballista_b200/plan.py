@@ -169,6 +169,18 @@ def hash_join(left: Json, right: Json, on: Sequence[Sequence[Json]], join_type: 
     return n
 
 
+def nested_loop_join(left: Json, right: Json, join_type: str = "Inner", filter: Optional[Json] = None,
+                     projection: Optional[List[int]] = None) -> Json:
+    """NestedLoopJoinExecNode (datafusion.proto:1301-1307): a join without equality keys.  The left input is the build
+    side, read whole by every task; `filter` indexes left ++ right."""
+    n: Json = {"op": "NestedLoopJoinExec", "left": left, "right": right, "join_type": join_type}
+    if filter is not None:
+        n["filter"] = filter
+    if projection is not None:
+        n["projection"] = projection
+    return n
+
+
 def sort_merge_join(left: Json, right: Json, on: Sequence[Sequence[Json]], join_type: str = "Inner",
                     filter: Optional[Json] = None, sort_options: Optional[Sequence[Json]] = None) -> Json:
     """SortMergeJoinExecNode (datafusion.proto:1433): Ballista's default join strategy (extension.rs:683).

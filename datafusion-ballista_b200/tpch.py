@@ -1003,6 +1003,39 @@ def q22(n_partitions: int = 4, codes=("13", "31", "23", "29", "30", "18", "17"))
     return [st1, st2, st3, st4, st5, st6, st7]
 
 
+# ---- q11 / q22 as DataFusion plans them: the scalar subquery's one row is the build side of a NestedLoopJoinExec ----
+# whose filter is the comparison (q11 / q22 above join it through an invented constant key instead)
+def q11_nlj(n_partitions: int = 4, nation: str = "GERMANY", fraction: float = 0.0001) -> List[Stage]:
+    c = P.col
+    stages = q11(n_partitions, nation, fraction)
+    s6 = P.aggregate("Final", [], [P.agg("sum", None, "total")], P.coalesce_partitions(P.shuffle_reader(5, [P.field("total[sum]", P.dec(38, 2), True)])))
+    s6 = P.project([(P.binop("*", P.cast(c(0), "f64"), P.lit_f64(fraction)), "thr")], s6)
+    pv = [P.field("ps_partkey", "i64", True), P.field("value", P.dec(36, 2), True)]
+    # filter columns: thr | ps_partkey, value
+    j = P.nested_loop_join(P.shuffle_reader(6, [P.field("thr", "f64", True)], broadcast=True), P.shuffle_reader(4, pv), "Inner",
+                           filter=P.binop(">", P.cast(c(2), "f64"), c(0)), projection=[1, 2])
+    keys = [P.sort_key(c(1), asc=False)]
+    stages[5] = Stage(6, P.shuffle_writer(s6, 6), n_tasks=1)
+    stages[6] = Stage(7, P.shuffle_writer(P.sort(keys, j, preserve_partitioning=True), 7))
+    return stages
+
+
+def q22_nlj(n_partitions: int = 4, codes=("13", "31", "23", "29", "30", "18", "17")) -> List[Stage]:
+    c, Pn = P.col, n_partitions
+    stages = q22(n_partitions, codes)
+    st_avg = [P.field("a[count]", "u64", True), P.field("a[sum]", P.dec(25, 2), True)]
+    s2 = P.aggregate("Final", [], [P.agg("avg", None, "a", D152)], P.coalesce_partitions(P.shuffle_reader(1, st_avg)))
+    code = P.fn("substr", c("c_phone"), P.lit_i64(1), P.lit_i64(2))
+    s3 = P.filter_(P.in_list(code, [P.lit_utf8(v) for v in codes]), table_scan("customer", Q22_TABLES["customer"]))
+    s3 = P.project([(c(0), "c_custkey"), (P.fn("substr", c(1), P.lit_i64(1), P.lit_i64(2)), "cntrycode"), (c(2), "c_acctbal")], s3)
+    # filter columns: a | c_custkey, cntrycode, c_acctbal ; c_acctbal > a compares as Decimal128(19, 6), AVG's result type
+    s3 = P.nested_loop_join(P.shuffle_reader(2, [P.field("a", P.dec(19, 6), True)], broadcast=True), s3, "Inner",
+                            filter=P.binop(">", P.cast(c(3), P.dec(19, 6)), c(0)), projection=[1, 2, 3])
+    stages[1] = Stage(2, P.shuffle_writer(s2, 2), n_tasks=1)
+    stages[2] = Stage(3, P.shuffle_writer(s3, 3, [c(0)], Pn))
+    return stages
+
+
 # ---- registry: query name -> (tables it scans with the columns it references, stage-plan builder) -------------
 QUERIES = {
     "q1": ({"lineitem": Q1_COLUMNS}, q1), "q3": (Q3_TABLES, q3), "q4": (Q4_TABLES, q4), "q5": (Q5_TABLES, q5),

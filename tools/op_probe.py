@@ -13,6 +13,8 @@ engine's own CUDA-event timing (b200_engine_kernel_stats) can be read for the sa
   minmax_str lineitem MIN/MAX(l_comment) GROUP BY l_returnflag, l_linestatus (4 groups)              -> pipeline_agg_reg
              and MAX(l_comment) GROUP BY l_orderkey (15 M groups at SF10)                             -> pipeline_agg_global
              (each result checked against the CPU oracle unless ORACLE=0)
+  nlj        NestedLoopJoinExec: lineitem against one build row (a scalar subquery) next to the same comparison
+             through fast_filter_kernel, and a band join of orders (msf 1000) against 10,000 build rows    -> nlj_count / nlj_write
 """
 import json
 import os
@@ -128,6 +130,79 @@ elif op == "minmax_str":
             assert_tables_equal(got, want)
             report[name]["matches_oracle"] = True
     print(json.dumps({op: report, "rows": n}, indent=1))
+elif op == "nlj":
+    # (a) scalar subquery: lineitem (msf 10000 = SF10) probed against ONE build row, l_extendedprice > avg, next to the same
+    #     comparison against a literal through fast_filter_kernel;
+    # (b) band join: orders (SF1) against a 10,000-row build side, o_totalprice BETWEEN lo AND hi.
+    # Every result is checked against the CPU oracle; (b) at SF0.01 with 1,000 build rows, where the oracle's pair list fits.
+    import decimal
+    import subprocess
+    import numpy as np
+    import pyarrow as pa
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    import oracle_ffi
+    from util import assert_tables_equal
+    from ballista_b200 import driver
+    smi = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
+    oracle = oracle_ffi.OracleEngine()
+    report = {"gpu": smi}
+
+    def both(table, batch):
+        for e in (eng, oracle):
+            e.drop_table(table)
+            e.register_batch(table, 0, batch)
+
+    def timed(st, nbytes, fams):
+        eng.kernel_stats(reset=True)
+        p0 = eng.counter("nlj_pairs")
+        run(st, [1])
+        ks = eng.kernel_stats(reset=True)
+        ms = {k: round(v["ms"] / reps, 3) for k, v in ks.items() if fams is None or k in fams}
+        pairs = (eng.counter("nlj_pairs") - p0) // reps
+        r = {"kernel_ms_per_run": ms, "bytes": nbytes, "GB_per_s": {k: round(nbytes / (v * 1e-3) / 1e9, 1) for k, v in ms.items() if v > 0}}
+        if pairs:
+            r["pairs"] = pairs
+            r["pairs_per_s"] = {k: float("%.3g" % (pairs / (v * 1e-3))) for k, v in ms.items() if v > 0 and k == "nlj_count"}
+        return r
+
+    li = ["l_orderkey", "l_extendedprice"]
+    n = eng.tpch_table_rows("lineitem", msf)
+    for e in (eng, oracle):
+        e.drop_table("lineitem")
+        e.tpch_generate("lineitem", msf, 0, 0, n, li)
+    avg = 3825000   # 38,250.00: about the mean l_extendedprice
+    both("nlj_avg", pa.RecordBatch.from_pydict({"a": pa.array([decimal.Decimal(avg).scaleb(-2)], pa.decimal128(15, 2))}))
+    scan = tpch.table_scan("lineitem", li)
+    nlj = P.nested_loop_join(P.scan("nlj_avg", [P.field("a", D152, True)]), scan, "Inner", filter=P.binop(">", c(2), c(0)), projection=[1, 2])
+    flt = P.filter_(P.binop(">", c(1), P.lit_dec(avg, 15, 2)), scan)
+    for name, plan, fams in (("a_scalar_nlj", nlj, ("nlj_count", "nlj_write")), ("a_fast_filter", flt, None)):
+        st = [P.Stage(1, P.shuffle_writer(plan, 1))]
+        report[name] = timed(st, 16 * n, fams)   # the comparison reads l_extendedprice (Decimal128, 16 B/row) once per pass
+        assert_tables_equal(driver.run_stages(eng, st, f"chk-{name}"), driver.run_stages(oracle, st, f"chk-{name}"), sort=False)
+        report[name]["matches_oracle"] = True
+    for e in (eng, oracle):
+        e.drop_table("lineitem")
+    rng = np.random.default_rng(1)
+
+    def band(n_build, m):
+        lo = rng.integers(100000, 50000000, n_build)
+        cents = lambda v: pa.array([decimal.Decimal(int(x)).scaleb(-2) for x in v], pa.decimal128(15, 2))  # noqa: E731
+        b = pa.RecordBatch.from_pydict({"lo": cents(lo), "hi": cents(lo + 1000)})
+        no = eng.tpch_table_rows("orders", m)
+        for e in (eng, oracle):
+            e.drop_table("orders")
+            e.tpch_generate("orders", m, 0, 0, no, ["o_orderkey", "o_totalprice"])
+        both("nlj_band", b)
+        j = P.nested_loop_join(P.scan("nlj_band", [P.field("lo", D152, True), P.field("hi", D152, True)]), tpch.table_scan("orders", ["o_orderkey", "o_totalprice"]),
+                               "Inner", filter=P.and_(P.binop(">=", c(3), c(0)), P.binop("<=", c(3), c(1))), projection=[2, 0])
+        return [P.Stage(1, P.shuffle_writer(j, 1))], no
+    st, no = band(10000, 1000)
+    report["b_band_join"] = timed(st, 16 * no + 32 * 10000 * ((no + 255) // 256), ("nlj_count", "nlj_write"))
+    st, _ = band(1000, 10)
+    assert_tables_equal(driver.run_stages(eng, st, "chk-band"), driver.run_stages(oracle, st, "chk-band"), sort=False)
+    report["b_band_join"]["matches_oracle_at_sf0.01_1000_build_rows"] = True
+    print(json.dumps({op: report, "lineitem_rows": n}, indent=1))
+    oracle.close()
 else:
     raise SystemExit(__doc__)
 print(json.dumps({op: eng.kernel_stats()}, indent=1))
