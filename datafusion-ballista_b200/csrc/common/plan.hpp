@@ -476,21 +476,40 @@ inline ExprPtr parse_expr(const Json& j, const Schema& in) {
 // ----------------------------------------------------------------------------------------------
 // Aggregates
 // ----------------------------------------------------------------------------------------------
-enum class AggFn : uint8_t { Sum, Min, Max, Count, Avg };
+enum class AggFn : uint8_t { Sum, Min, Max, Count, Avg, VarSamp, VarPop, StddevSamp, StddevPop, CovarSamp, CovarPop, Corr };
 enum class AggMode : uint8_t { Partial, Final, FinalPartitioned, Single, SinglePartitioned };
 
 inline bool agg_mode_consumes_states(AggMode m) { return m == AggMode::Final || m == AggMode::FinalPartitioned; }
 inline bool agg_mode_emits_states(AggMode m) { return m == AggMode::Partial; }
 
+// A plan the engine understands but does not run (e.g. statistical states laid out in an unknown way): B200_ERR_UNSUPPORTED
+struct PlanUnsupported : std::runtime_error {
+  explicit PlanUnsupported(const std::string& m) : std::runtime_error(m) {}
+};
+
+// The statistical aggregates: variance / standard deviation (one argument), covariance / correlation (two arguments)
+inline bool agg_is_stat(AggFn f) { return f >= AggFn::VarSamp; }
+inline bool agg_is_bivariate(AggFn f) { return f == AggFn::CovarSamp || f == AggFn::CovarPop || f == AggFn::Corr; }
+// [EXT] partial state columns, read by position and checked by suffix in Final modes:
+//  var / stddev:  [count] UInt64, [mean] Float64, [m2] Float64  (datafusion-functions-aggregate variance.rs)
+//  covar:         [count], [mean1], [mean2], [algo_const]        (covariance.rs)
+//  corr:          [count], [mean1], [m2_1], [mean2], [m2_2], [algo_const]  -- unpinned: no reference test fixes it
+inline std::vector<std::string> stat_state_suffixes(AggFn f) {
+  if (f == AggFn::Corr) return {"count", "mean1", "m2_1", "mean2", "m2_2", "algo_const"};
+  if (agg_is_bivariate(f)) return {"count", "mean1", "mean2", "algo_const"};
+  return {"count", "mean", "m2"};
+}
+
 struct AggExpr {
   AggFn fn = AggFn::Sum;
   ExprPtr arg;           // null for COUNT(*) and in Final modes
+  ExprPtr arg2;          // COVAR / CORR: the second argument (raw modes only)
   DataType input_type;   // type of arg (after AVG's integer->f64 coercion); for Final: taken from IR
   DataType sum_type;     // accumulator type for Sum/Avg
   DataType result_type;  // final value type
   bool distinct = false;
   std::string name;
-  int n_state_cols() const { return fn == AggFn::Avg ? 2 : 1; }
+  int n_state_cols() const { return agg_is_stat(fn) ? (int)stat_state_suffixes(fn).size() : fn == AggFn::Avg ? 2 : 1; }
 };
 
 // [EXT] datafusion-functions-aggregate 53: SUM(Decimal128(p,s)) -> Decimal128(min(38,p+10), s);
@@ -510,7 +529,35 @@ inline DataType avg_result_type(const DataType& t) {
   throw std::runtime_error("AVG does not support " + t.str());
 }
 
+// [EXT] VAR / STDDEV / COVAR / CORR take any integer, unsigned, float or Decimal128 argument, coerced to Float64, and return
+// a nullable Float64
+inline void check_stat_arg(const std::string& fn, const DataType& t) {
+  if (!(t.is_integer() || t.is_float() || t.is_decimal())) throw PlanUnsupported(fn + " does not support an argument of type " + t.str());
+}
+
+// The statistical aggregates are typed here for every consumer of the plan IR, but only a consumer built with
+// B200_PLAN_STAT_AGGREGATES=1 computes them (the device engine: Makefile NVFLAGS, for every translation unit of the
+// library alike).  Any other consumer -- the CPU oracle -- refuses such a plan instead of mis-evaluating it.
+#ifndef B200_PLAN_STAT_AGGREGATES
+#define B200_PLAN_STAT_AGGREGATES 0
+#endif
+inline AggFn parse_stat_aggfn(const std::string& s) {
+  // the lower-cased names and aliases the function registry resolves (datafusion-functions-aggregate)
+  if (s == "var" || s == "var_samp" || s == "var_sample") return AggFn::VarSamp;
+  if (s == "var_pop" || s == "var_population") return AggFn::VarPop;
+  if (s == "stddev" || s == "stddev_samp") return AggFn::StddevSamp;
+  if (s == "stddev_pop") return AggFn::StddevPop;
+  if (s == "covar" || s == "covar_samp") return AggFn::CovarSamp;
+  if (s == "covar_pop") return AggFn::CovarPop;
+  if (s == "corr") return AggFn::Corr;
+  return AggFn::Sum;
+}
 inline AggFn parse_aggfn(const std::string& s) {
+  const AggFn st = parse_stat_aggfn(s);
+  if (agg_is_stat(st)) {
+    if (!B200_PLAN_STAT_AGGREGATES) throw PlanUnsupported("aggregate '" + s + "' is not computed by this consumer of the plan IR");
+    return st;
+  }
   if (s == "sum") return AggFn::Sum;
   if (s == "min") return AggFn::Min;
   if (s == "max") return AggFn::Max;
@@ -712,7 +759,24 @@ inline PlanPtr parse_plan(const Json& j) {
       ae.distinct = a.get_bool("distinct", false);
       if (ae.distinct) throw std::runtime_error("DISTINCT aggregates must be lowered to two-level aggregation by the planner");
       ae.name = a.get_str("name", a.at("fn").str() + "_" + std::to_string(i));
-      if (from_states) {
+      if (from_states && agg_is_stat(ae.fn)) {
+        // states are read positionally; a column whose name does not end in the expected suffix means a layout this
+        // engine does not know, which is refused rather than misread
+        const std::vector<std::string> sfx = stat_state_suffixes(ae.fn);
+        for (size_t k = 0; k < sfx.size(); k++) {
+          if (state_col + k >= c->schema.size()) throw std::runtime_error("Final aggregate: missing state columns of " + ae.name);
+          const Field& f = c->schema[state_col + k];
+          const std::string want = "[" + sfx[k] + "]";
+          const bool name_ok = f.name.size() >= want.size() && f.name.compare(f.name.size() - want.size(), want.size(), want) == 0;
+          const bool type_ok = k == 0 ? f.type.is_integer() : f.type.id == TypeId::Float64;
+          if (!name_ok || !type_ok)
+            throw PlanUnsupported("Final " + a.at("fn").str() + ": state column '" + f.name + "' (" + f.type.str() + ") is not the expected '" + want + "'");
+        }
+        ae.input_type = DataType(TypeId::Float64);
+        ae.sum_type = ae.input_type;
+        ae.result_type = ae.input_type;
+        state_col += ae.n_state_cols();
+      } else if (from_states) {
         // states are read positionally: AVG -> (count:UInt64, sum), others -> one column
         if (ae.fn == AggFn::Avg) {
           if (state_col + 1 >= c->schema.size()) throw std::runtime_error("Final aggregate: missing AVG state columns");
@@ -741,6 +805,16 @@ inline PlanPtr parse_plan(const Json& j) {
         }
         if (!ae.arg && ae.fn != AggFn::Count) throw std::runtime_error("aggregate needs an argument");
         DataType it = ae.arg ? ae.arg->type : DataType(TypeId::Int64);
+        if (agg_is_stat(ae.fn)) {
+          const size_t want = agg_is_bivariate(ae.fn) ? 2 : 1;
+          if (a.at("args").size() != want) throw std::runtime_error(a.at("fn").str() + " takes " + std::to_string(want) + " argument(s)");
+          check_stat_arg(a.at("fn").str(), it);
+          if (want == 2) {
+            ae.arg2 = parse_expr(a.at("args").at(1), c->schema);
+            check_stat_arg(a.at("fn").str(), ae.arg2->type);
+          }
+          it = DataType(TypeId::Float64);
+        }
         switch (ae.fn) {
           case AggFn::Sum:
             ae.input_type = it;
@@ -766,7 +840,11 @@ inline PlanPtr parse_plan(const Json& j) {
       }
       n->aggs.push_back(ae);
       if (agg_mode_emits_states(n->agg_mode)) {
-        if (ae.fn == AggFn::Avg) {
+        if (agg_is_stat(ae.fn)) {
+          const std::vector<std::string> sfx = stat_state_suffixes(ae.fn);
+          for (size_t k = 0; k < sfx.size(); k++)
+            n->schema.push_back(Field{ae.name + "[" + sfx[k] + "]", DataType(k == 0 ? TypeId::UInt64 : TypeId::Float64), true});
+        } else if (ae.fn == AggFn::Avg) {
           n->schema.push_back(Field{ae.name + "[count]", DataType(TypeId::UInt64), true});
           n->schema.push_back(Field{ae.name + "[sum]", ae.sum_type, true});
         } else if (ae.fn == AggFn::Count) {

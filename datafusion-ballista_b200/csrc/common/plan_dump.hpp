@@ -83,7 +83,7 @@ inline std::string dump_sort_keys(const std::vector<SortKey>& ks) {
 inline std::string dump_plan(const PlanNode& n) {
   static const char* join_types[] = {"Inner", "Left", "Right", "Full", "LeftSemi", "RightSemi", "LeftAnti", "RightAnti"};
   static const char* agg_modes[] = {"Partial", "Final", "FinalPartitioned", "Single", "SinglePartitioned"};
-  static const char* agg_fns[] = {"sum", "min", "max", "count", "avg"};
+  static const char* agg_fns[] = {"sum", "min", "max", "count", "avg", "var_samp", "var_pop", "stddev_samp", "stddev_pop", "covar_samp", "covar_pop", "corr"};
   std::string o = "{\"op\":" + pbp::jstr(n.op_name);
   auto child = [&](size_t i) { return dump_plan(*n.children[i]); };
   switch (n.op) {
@@ -108,7 +108,7 @@ inline std::string dump_plan(const PlanNode& n) {
       o += "],\"aggr\":[";
       for (size_t i = 0; i < n.aggs.size(); i++) {
         const AggExpr& a = n.aggs[i];
-        o += std::string(i ? "," : "") + "{\"fn\":\"" + agg_fns[(int)a.fn] + "\",\"name\":" + pbp::jstr(a.name) + ",\"args\":[" + (a.arg ? dump_expr(a.arg) : std::string()) +
+        o += std::string(i ? "," : "") + "{\"fn\":\"" + agg_fns[(int)a.fn] + "\",\"name\":" + pbp::jstr(a.name) + ",\"args\":[" + (a.arg ? dump_expr(a.arg) : std::string()) + (a.arg2 ? "," + dump_expr(a.arg2) : std::string()) +
              "],\"input_type\":" + type_json(a.input_type) + ",\"sum_type\":" + type_json(a.sum_type) + ",\"result_type\":" + type_json(a.result_type) + "}";
       }
       o += "],\"input\":" + child(0);

@@ -73,6 +73,49 @@ __device__ void store_typed_i64(void* data, uint8_t phys, unsigned long long pos
   }
 }
 
+// VAR / STDDEV / COVAR / CORR of slot s from its count, f64 sums and co-moments (see StatOut); ok = false: NULL.  Takes
+// its inputs by value: a reference into the kernel parameters would copy them all to local memory.
+struct StatVal {
+  double v;
+  bool ok;
+};
+__device__ __noinline__ StatVal stat_value(const unsigned long long* acc, unsigned long long cap, unsigned long long s, int code, int c_n, int c_sx,
+                                           int c_sy, int c_xx, int c_yy, int c_xy) {
+  auto f64 = [&](int a) { return __longlong_as_double((long long)acc[((unsigned long long)a * cap + s) * 2]); };
+  const unsigned long long n = acc[((unsigned long long)c_n * cap + s) * 2];
+  const double dn = (double)n;
+  // a co-moment column c, corrected by its first-order sums (program.h, MomDesc)
+  auto mom = [&](int c) { return n ? f64(c) - f64(c + 1) * f64(c + 2) / dn : f64(c); };
+  switch (code) {
+    // the partial state's means: the pass-1 centre plus the pass-2 mean deviation from it (c_xy + 1 / + 2 hold
+    // Σw(x - mx) / Σw(y - my) around exactly these centres), which removes the rounding of the f64 sum to first order
+    case SO_MEAN_X: return StatVal{n ? f64(c_sx) / dn + f64(c_xy + 1) / dn : 0.0, true};
+    case SO_MEAN_Y: return StatVal{n ? f64(c_sy) / dn + f64(c_xy + 2) / dn : 0.0, true};
+    case SO_M2_X: return StatVal{mom(c_xx), true};
+    case SO_M2_Y: return StatVal{mom(c_yy), true};
+    case SO_CO: return StatVal{mom(c_xy), true};
+    case SO_VAR_SAMP:
+    case SO_STDDEV_SAMP:
+    case SO_COVAR_SAMP: {
+      if (n <= 1) return StatVal{0.0, false};
+      const double v = mom(code == SO_COVAR_SAMP ? c_xy : c_xx) / (dn - 1.0);
+      return StatVal{code == SO_STDDEV_SAMP ? sqrt(v) : v, true};
+    }
+    case SO_VAR_POP:
+    case SO_STDDEV_POP:
+    case SO_COVAR_POP: {
+      if (n == 0) return StatVal{0.0, false};
+      const double v = mom(code == SO_COVAR_POP ? c_xy : c_xx) / dn;
+      return StatVal{code == SO_STDDEV_POP ? sqrt(v) : v, true};
+    }
+    default: {  // SO_CORR; [EXT] NULL when either side has zero variance (unpinned: DataFusion releases differ)
+      const double mx = mom(c_xx), my = mom(c_yy);
+      if (n <= 1 || mx == 0.0 || my == 0.0) return StatVal{0.0, false};
+      return StatVal{mom(c_xy) / (sqrt(mx) * sqrt(my)), true};
+    }
+  }
+}
+
 __global__ void agg_extract_kernel(AggTable T, AggExtractArgs A) {
   for (unsigned long long s = blockIdx.x * (unsigned long long)blockDim.x + threadIdx.x; s < T.cap; s += (unsigned long long)gridDim.x * blockDim.x) {
     if (T.state[s] != 2) continue;
@@ -100,6 +143,12 @@ __global__ void agg_extract_kernel(AggTable T, AggExtractArgs A) {
           *dst = bytes;
           ((ulonglong2*)o.data)[pos] = make_ulonglong2(v ? (unsigned long long)dst : 0ull, v ? len : 0ull);
           if (o.valid) o.valid[pos] = v;
+          break;
+        }
+        case AO_STAT: {
+          const StatVal r = stat_value(T.acc, T.cap, s, o.imm, o.st[0], o.st[1], o.st[2], o.st[3], o.st[4], o.st[5]);
+          ((double*)o.data)[pos] = r.v;
+          if (o.valid) o.valid[pos] = r.ok ? 1 : 0;
           break;
         }
         default: {

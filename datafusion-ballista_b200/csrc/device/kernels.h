@@ -32,7 +32,15 @@ enum AggOutKind : uint8_t {
   AO_AVG_DEC,      // a: sum acc, b: count acc, imm: 10^k multiplier exponent
   AO_AVG_F64,      // a: sum acc (f64), b: count acc
   AO_KEY_PACKED,   // a: key index holding a packed short string (OP_STR_PACK8); imm: bit position of the length; aux: 8 B/row chars
-  AO_MINMAX_STR    // a: MIN_STR / MAX_STR acc -> string view (points at the input's characters); b count
+  AO_MINMAX_STR,   // a: MIN_STR / MAX_STR acc -> string view (points at the input's characters); b count
+  AO_STAT          // VAR / STDDEV / COVAR / CORR result or partial state (Float64); imm: StatOut; st: the cells it reads
+};
+// what an AO_STAT column holds.  n = count, mean = sum / n, m2 / co = the pass-2 co-moments.  [EXT] NULL rules: sample
+// variants n <= 1, population variants n = 0, CORR n < 2 or either m2 = 0; partial states are never NULL (an empty
+// group's mean and moments are 0, as DataFusion's accumulators start)
+enum StatOut : uint8_t {
+  SO_MEAN_X = 0, SO_MEAN_Y, SO_M2_X, SO_M2_Y, SO_CO,
+  SO_VAR_SAMP, SO_VAR_POP, SO_STDDEV_SAMP, SO_STDDEV_POP, SO_COVAR_SAMP, SO_COVAR_POP, SO_CORR
 };
 struct AggOut {
   void* data;
@@ -42,6 +50,8 @@ struct AggOut {
   uint8_t a, b;
   uint8_t phys;   // output encoding
   int32_t imm;
+  uint8_t st[6];  // AO_STAT: count acc, sum-x acc, sum-y acc, xx / yy / xy co-moment columns
+  uint8_t _pad[2];
 };
 struct AggExtractArgs {
   AggOut out[VM_MAX_OUT];

@@ -2248,9 +2248,182 @@ __device__ __forceinline__ uint32_t addsub128(bool minus, uint64_t llo, uint64_t
 }
 
 // ------------------------------------------------------------------------------------------------
+// Pass 2 of the statistical aggregates (VAR / STDDEV / COVAR / CORR): centred co-moments
+// The same lowered program runs twice over the same rows.  Pass 1 (the sinks above) fills each group's count and f64
+// sums; pass 2 adds w * (x - mx) * (y - my) + b per row into the co-moment columns (MomDesc), centred on the pass-1 mean
+// of the row's group.  Two passes keep the accuracy of a two-pass variance (no cancellation of power sums) without a
+// per-slot lock.  This code is compiled only into the pipeline_kernel variants with MOM = true, launched for pass 2.
+// ------------------------------------------------------------------------------------------------
+__device__ __forceinline__ uint32_t mom_valid(const Lane L, const MomDesc& md) {
+  return fetch_valid(L, md.x) & fetch_valid(L, md.y) & fetch_valid(L, md.w) & fetch_valid(L, md.b);
+}
+
+// one row's terms {w (x - mx) (y - my) + b, w (x - mx), w (y - my)}; a zero weight (an empty partial state) contributes its
+// b alone, so that an undefined centre never leaks
+struct MomTerm {
+  double co, dx, dy;
+};
+__device__ __noinline__ MomTerm mom_term(const Lane L, int m, int r, double mx, double my) {
+  const MomDesc md = PROG.mom[m];
+  const double b = md.b.kind == OPD_NONE ? 0.0 : ld1_f64(L, md.b, r);
+  const double w = md.w.kind == OPD_NONE ? 1.0 : ld1_f64(L, md.w, r);
+  if (w == 0.0) return MomTerm{b, 0.0, 0.0};
+  const double dx = w * (ld1_f64(L, md.x, r) - mx), ey = ld1_f64(L, md.y, r) - my;
+  return MomTerm{dx * ey + b, dx, w * ey};
+}
+
+// the pass-1 centres of co-moment m in table slot `slot`
+__device__ __forceinline__ void mom_centre(int m, unsigned long long slot, double& mx, double& my) {
+  const AggTable& T = PROG.table;
+  const MomDesc md = PROG.mom[m];
+  const double n = (double)T.acc[((unsigned long long)md.cnt * T.cap + slot) * 2];
+  mx = __longlong_as_double((long long)T.acc[((unsigned long long)md.sx * T.cap + slot) * 2]) / n;
+  my = __longlong_as_double((long long)T.acc[((unsigned long long)md.sy * T.cap + slot) * 2]) / n;
+}
+
+__device__ __noinline__ uint32_t sink_mom_global(const Lane L, uint32_t active) {
+  if (*(volatile unsigned int*)&PROG.status->overflow) return active;
+  const int n_keys = PROG.n_keys, n_mom = PROG.n_mom;
+  const AggTable& T = PROG.table;
+  uint32_t ok[VM_MAX_MOM];
+  for (int m = 0; m < n_mom; m++) ok[m] = mom_valid(L, PROG.mom[m]);
+#pragma unroll 1
+  for (int r = 0; r < VM_R; r++) {
+    if (!((active >> r) & 1)) continue;
+    KeyVal kv[VM_MAX_KEYS];
+    for (int k = 0; k < n_keys; k++) load_key(L, PROG.keys[k], r, &kv[k]);
+    const unsigned long long h = n_keys ? (unsigned long long)ld1_i64(L, PROG.key_hash, r) : 0ull;
+    const unsigned long long slot = table_upsert(n_keys, h, kv);  // pass 1 published every group: a lookup
+    if (slot == ~0ull) {
+      atomicExch(&PROG.status->overflow, 1u);
+      active &= ~(1u << r);
+      continue;
+    }
+    for (int m = 0; m < n_mom; m++) {
+      if (!((ok[m] >> r) & 1)) continue;
+      double mx, my;
+      mom_centre(m, slot, mx, my);
+      const MomTerm t = mom_term(L, m, r, mx, my);
+      const unsigned long long c0 = PROG.mom[m].col;
+      atomicAdd((double*)&T.acc[(c0 * T.cap + slot) * 2], t.co);
+      atomicAdd((double*)&T.acc[((c0 + 1) * T.cap + slot) * 2], t.dx);
+      atomicAdd((double*)&T.acc[((c0 + 2) * T.cap + slot) * 2], t.dy);
+    }
+  }
+  return active;
+}
+
+// register sink: each CTA looks a group up in the global table once, the first time one of its threads meets the group,
+// and keeps the slot and the centres here
+struct MomCentres {  // shared memory
+  unsigned int state[VM_REG_GROUPS];  // 0: not loaded, 1: loading, 2: ready
+  unsigned long long slot[VM_REG_GROUPS];
+  double mx[VM_REG_GROUPS][VM_MAX_MOM], my[VM_REG_GROUPS][VM_MAX_MOM];
+};
+__device__ __forceinline__ MomCentres* mom_centres() {
+  __shared__ MomCentres mc;
+  return &mc;
+}
+
+__device__ __noinline__ void mom_load_centres(RegGroupTable* gt, MomCentres* mc, int G, int g) {
+  unsigned int st = *(volatile unsigned int*)&mc->state[g];
+  if (st == 0 && atomicCAS(&mc->state[g], 0u, 1u) == 0u) {
+    const int n_keys = PROG.n_keys;
+    KeyVal kv[VM_MAX_KEYS];
+    unsigned long long h = 0;
+    if (G > 1) {
+      h = gt->hash[g];
+      for (int k = 0; k < n_keys; k++) {
+        kv[k].w0 = gt->key_w0[g][k];
+        kv[k].w1 = gt->key_w1[g][k];
+        kv[k].valid = gt->key_valid[g][k];
+        kv[k].vk = PROG.keys[k].vk;
+      }
+    }
+    const unsigned long long slot = table_upsert(n_keys, h, kv);
+    mc->slot[g] = slot;
+    if (slot == ~0ull) atomicExch(&PROG.status->overflow, 1u);
+    for (int m = 0; m < PROG.n_mom; m++) {
+      double mx = 0.0, my = 0.0;
+      if (slot != ~0ull) mom_centre(m, slot, mx, my);
+      mc->mx[g][m] = mx;
+      mc->my[g][m] = my;
+    }
+    __threadfence_block();
+    atomicExch(&mc->state[g], 2u);
+    return;
+  }
+  while (*(volatile unsigned int*)&mc->state[g] != 2u) {
+  }
+  __threadfence_block();
+}
+
+template <int G>
+__device__ __forceinline__ uint32_t sink_mom_reg(const Lane L, uint32_t active, double (&acc)[G][VM_MAX_MOM][3], RegGroupTable* gt, MomCentres* mc) {
+  uint32_t gid[VM_R];
+#pragma unroll
+  FOR_R gid[r] = 0;
+#pragma unroll 1
+  for (int r = 0; r < VM_R; r++) {
+    if (!((active >> r) & 1)) continue;
+    const int g = G > 1 ? reg_resolve_row(L, gt, G, r) : 0;
+    if (g < 0) {
+      atomicExch(&PROG.status->overflow, 1u);
+      active &= ~(1u << r);
+      continue;
+    }
+    gid[r] = (uint32_t)g;
+    if (*(volatile unsigned int*)&mc->state[g] != 2u) mom_load_centres(gt, mc, G, g);
+  }
+  __threadfence_block();  // acquire: the centres read below were published before their state became 2
+  const int n_mom = PROG.n_mom;
+#pragma unroll
+  for (int m = 0; m < VM_MAX_MOM; m++) {
+    if (m >= n_mom) break;
+    const uint32_t v = active & mom_valid(L, PROG.mom[m]);
+#pragma unroll
+    FOR_R {
+      if ((v >> r) & 1) {
+        const MomTerm t = mom_term(L, m, r, mc->mx[gid[r]][m], mc->my[gid[r]][m]);
+#pragma unroll
+        for (int g = 0; g < G; g++)
+          if (gid[r] == (uint32_t)g) {
+            acc[g][m][0] += t.co;
+            acc[g][m][1] += t.dx;
+            acc[g][m][2] += t.dy;
+          }
+      }
+    }
+  }
+  return active;
+}
+
+// end of pass 2 in the register sink: a warp reduction per (group, co-moment), then one f64 atomic per warp
+template <int G>
+__device__ __forceinline__ void mom_reg_flush(double (&acc)[G][VM_MAX_MOM][3], MomCentres* mc, int tid) {
+  const int n_mom = PROG.n_mom;
+  const AggTable& T = PROG.table;
+#pragma unroll
+  for (int g = 0; g < G; g++) {
+    const bool used = mc->state[g] == 2u && mc->slot[g] != ~0ull;
+#pragma unroll
+    for (int m = 0; m < VM_MAX_MOM; m++) {
+      if (m >= n_mom) break;
+#pragma unroll
+      for (int j = 0; j < 3; j++) {
+        double x = acc[g][m][j];
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) x += __shfl_xor_sync(0xFFFFFFFFu, x, o);
+        if (used && (tid & 31) == 0) atomicAdd((double*)&T.acc[((unsigned long long)(PROG.mom[m].col + j) * T.cap + mc->slot[g]) * 2], x);
+      }
+    }
+  }
+}
+
+// ------------------------------------------------------------------------------------------------
 // The kernel
 // ------------------------------------------------------------------------------------------------
-template <int SINK, int G, bool ADD_ONLY, bool SIDE>
+template <int SINK, int G, bool ADD_ONLY, bool SIDE, bool MOM = false>
 __global__ void __launch_bounds__(512, 1) pipeline_kernel() {
   extern __shared__ __align__(128) uint8_t smem[];
   __shared__ __align__(8) uint64_t full_bar[VM_MAX_STAGES];
@@ -2276,11 +2449,12 @@ __global__ void __launch_bounds__(512, 1) pipeline_kernel() {
   }
   const int n_instr = PROG.n_instr;
   for (int pc = tid; pc < n_instr; pc += B) decode_micro(pc, &mops[pc]);
-  if (SINK == SINK_AGG_REG && tid >= 64 && tid < 64 + PROG.n_acc) decode_acc(tid - 64, &accops[tid - 64]);
+  if (SINK == SINK_AGG_REG && !MOM && tid >= 64 && tid < 64 + PROG.n_acc) decode_acc(tid - 64, &accops[tid - 64]);
   if (SINK == SINK_AGG_REG && tid < VM_REG_GROUPS) {
     gtable.state[tid] = 0;
     gtable.hash[tid] = 0;
     if (tid == 0) gtable.n_groups = 0;
+    if (MOM) mom_centres()->state[tid] = 0;
   }
   __syncthreads();
 
@@ -2289,7 +2463,14 @@ __global__ void __launch_bounds__(512, 1) pipeline_kernel() {
   uint32_t dir_n = 0;
   unsigned long long* acc_hi = nullptr;
   unsigned long long* acc_side = nullptr;
-  if (SINK == SINK_AGG_REG) {
+  double macc[MOM ? G : 1][VM_MAX_MOM][3];
+  if (MOM) {
+#pragma unroll
+    for (int g = 0; g < (MOM ? G : 1); g++)
+#pragma unroll
+      for (int m = 0; m < VM_MAX_MOM; m++) macc[g][m][0] = macc[g][m][1] = macc[g][m][2] = 0.0;
+  }
+  if (SINK == SINK_AGG_REG && !MOM) {
     if (!ADD_ONLY) acc_hi = PROG.acc_hi + ((size_t)blockIdx.x * B + tid) * (VM_REG_GROUPS * VM_REG_ACC);
     reg_agg_init<G>(S_reg, acc_hi);
     if (SIDE) {
@@ -2347,7 +2528,11 @@ __global__ void __launch_bounds__(512, 1) pipeline_kernel() {
     {
       active = run_program(L, active, mops, n_instr);
     }
-    if (SINK == SINK_MATERIALIZE) {
+    if (MOM) {
+      if (SINK == SINK_AGG_GLOBAL) active = sink_mom_global(L, active);
+      else active = sink_mom_reg<(MOM ? G : 1)>(L, active, macc, &gtable, mom_centres());
+      live_rows += __popc(active);
+    } else if (SINK == SINK_MATERIALIZE) {
       sink_materialize(L, active, warp_tot, &tile_base_sh, t, n_tiles);
     } else if (SINK == SINK_AGG_GLOBAL) {
       active = sink_agg_global(L, active);
@@ -2379,7 +2564,10 @@ __global__ void __launch_bounds__(512, 1) pipeline_kernel() {
     KeyVal none[1];
     if (table_upsert(0, 0ull, none) == ~0ull) atomicExch(&PROG.status->overflow, 1u);
   }
-  if (SINK == SINK_AGG_REG) {
+  if (MOM && SINK == SINK_AGG_REG) {
+    __syncthreads();
+    mom_reg_flush<(MOM ? G : 1)>(macc, mom_centres(), tid);
+  } else if (SINK == SINK_AGG_REG) {
     __syncthreads();
     // scalar aggregates emit their single group even when no CTA saw a row: CTA 0 always flushes
     const bool has_rows = tile_of(0) < n_tiles;
@@ -2425,17 +2613,17 @@ struct GateLock {
   }
 };
 
-template <int SINK, int G, bool ADD_ONLY, bool SIDE = false>
+template <int SINK, int G, bool ADD_ONLY, bool SIDE = false, bool MOM = false>
 static cudaError_t launch_one(int grid, int block, size_t smem, cudaStream_t st) {
   // the opt-in to large dynamic shared memory is per (function, device) and sticky: raise it only when needed
   static size_t granted[64] = {0};
   const int dev = GateLock::current_device() & 63;
   if (smem > granted[dev]) {
-    cudaError_t e = cudaFuncSetAttribute(pipeline_kernel<SINK, G, ADD_ONLY, SIDE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    cudaError_t e = cudaFuncSetAttribute(pipeline_kernel<SINK, G, ADD_ONLY, SIDE, MOM>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
     granted[dev] = smem;
   }
-  pipeline_kernel<SINK, G, ADD_ONLY, SIDE><<<grid, block, smem, st>>>();
+  pipeline_kernel<SINK, G, ADD_ONLY, SIDE, MOM><<<grid, block, smem, st>>>();
   return cudaGetLastError();
 }
 
@@ -2455,6 +2643,11 @@ cudaError_t launch_pipeline(const Program& P, int reg_groups, int grid, int bloc
   cudaError_t e = cudaMemcpyToSymbolAsync(c_prog, &P, sizeof(Program), 0, cudaMemcpyHostToDevice, st);
   if (e != cudaSuccess) return e;
   const bool add_only = pipeline_add_only(P, grid, block);
+  if (P.mom_pass) {  // pass 2 of VAR / STDDEV / COVAR / CORR
+    if (P.sink == SINK_AGG_GLOBAL) return launch_one<SINK_AGG_GLOBAL, 1, true, false, true>(grid, block, smem, st);
+    return reg_groups <= 1 ? launch_one<SINK_AGG_REG, 1, false, false, true>(grid, block, smem, st)
+                           : launch_one<SINK_AGG_REG, VM_REG_GROUPS, false, false, true>(grid, block, smem, st);
+  }
   switch (P.sink) {
     case SINK_MATERIALIZE: return launch_one<SINK_MATERIALIZE, 1, true>(grid, block, smem, st);
     case SINK_AGG_GLOBAL: return launch_one<SINK_AGG_GLOBAL, 1, true>(grid, block, smem, st);

@@ -23,6 +23,7 @@ static const int VM_MAX_ACC = 16;     // physical accumulators of an aggregate s
 static const int VM_REG_ACC = 6;      // accumulators held in registers by the AGG_REG sink
 static const int VM_REG_GROUPS = 4;   // groups held in registers by the AGG_REG sink
 static const int VM_MAX_STAGES = 4;
+static const int VM_MAX_MOM = 6;      // centred co-moments of one aggregate sink (VAR / STDDEV / COVAR / CORR)
 
 // physical (in-HBM) column encodings
 enum Phys : uint8_t {
@@ -145,6 +146,21 @@ struct AccDesc {
 };
 
 // Global aggregate hash table (SoA), shared by both aggregate sinks and by the extraction kernel.
+// Centred co-moment of the statistical aggregates, filled by the second launch of an aggregate program ("pass 2"):
+//   table column `col`     += w * (x - mx) * (y - my) + b   over the rows where x, y (and w, b when present) are not NULL,
+//   table column `col` + 1 += w * (x - mx),  `col` + 2 += w * (y - my)
+// (the corrected two-pass algorithm: the extraction subtracts col+1 * col+2 / n, which removes the error of a rounded
+// centre to first order -- a plain f64 mean of values near 1e12 is off by far more than their spread allows),
+// where the centres mx = acc[sx] / acc[cnt] and my = acc[sy] / acc[cnt] are the group's cells of the first launch (pass 1:
+// a COUNT or an integer SUM of weights, and f64 SUMs of w * x and w * y).  Raw rows: w = 1 (OPD_NONE), no b.  Merging
+// partial states (Chan et al.): w = the state's count, x / y its means, b its m2 or co-moment.  x and y are f64 operands.
+struct MomDesc {
+  Operand x, y, w, b;   // w, b: OPD_NONE when absent
+  uint8_t cnt, sx, sy;  // pass-1 accumulator columns of the centres
+  uint8_t col;          // first of the three table accumulator columns of the co-moment
+  uint8_t _pad[4];
+};
+
 struct AggTable {
   unsigned long long* hash;   // [cap] 0 = empty
   unsigned int* state;        // [cap] 0 empty, 1 claimed, 2 keys published
@@ -199,6 +215,11 @@ struct Program {
   unsigned long long* tile_state;  // materialize sink: one look-back word per tile, zeroed before the launch
   int64_t n_rows;
   unsigned long long* acc_side; // register sink with has_side_acc: the side accumulators' 64-bit values, laid out as acc_hi
+  // statistical aggregates: the co-moments (all the fields above describe pass 1 and stay as they are for pass 2)
+  uint8_t n_mom;
+  uint8_t mom_pass;             // 1: this launch is pass 2 and folds rows into the co-moments only
+  uint8_t _pad2[6];
+  MomDesc mom[VM_MAX_MOM];
 };
 
 // ---- fused fast path (scan -> filter -> decimal products -> <=4-group SUM/COUNT aggregate) -----------

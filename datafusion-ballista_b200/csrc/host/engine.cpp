@@ -992,7 +992,9 @@ RunOutcome launch_program(const Exec& x, PipelineBuilder& pb, int reg_groups, co
   for (int i = 0; i < P.n_cols; i++) kt_bytes += (uint64_t)P.cols[i].width * (uint64_t)P.n_rows;
   if (P.sink == SINK_MATERIALIZE)
     for (int j = 0; j < P.n_out; j++) kt_bytes += (uint64_t)phys_width((Phys)P.out[j].phys) * (uint64_t)P.n_rows;  // upper bound: every row kept
-  KernelTimer kt(x, ff ? "filter_compact" : gb ? "groupby_hash_agg" : fused ? "pipeline_fused_agg" : P.sink == SINK_MATERIALIZE ? "pipeline_materialize" : P.sink == SINK_AGG_REG ? "pipeline_agg_reg" : "pipeline_agg_global", kt_bytes);
+  KernelTimer kt(x, ff ? "filter_compact" : gb ? "groupby_hash_agg" : fused ? "pipeline_fused_agg" : P.sink == SINK_MATERIALIZE ? "pipeline_materialize"
+                   : P.mom_pass ? (P.sink == SINK_AGG_REG ? "pipeline_agg_reg_pass2" : "pipeline_agg_global_pass2")
+                   : P.sink == SINK_AGG_REG ? "pipeline_agg_reg" : "pipeline_agg_global", kt_bytes);
   cudaEvent_t e0, e1;
   CUDA_CHECK(cudaEventCreate(&e0));
   CUDA_CHECK(cudaEventCreate(&e1));
@@ -1137,6 +1139,7 @@ struct AggLowered {
   ColRef combined;                   // valid when fast
   std::vector<AccDesc> accs;
   std::vector<ColRef> acc_src;
+  std::vector<MomDesc> moms;         // VAR / STDDEV / COVAR / CORR: co-moments of pass 2 (table columns after the accs)
   struct OutRecipe {
     uint8_t kind, a, b;
     Phys phys;
@@ -1145,6 +1148,7 @@ struct AggLowered {
     std::string name;
     bool with_valid;
     int key_idx;
+    uint8_t st[6];  // AO_STAT: count, sum x, sum y accumulators; xx, yy, xy co-moments (indices into `moms` until lowered)
   };
   std::vector<OutRecipe> outs;
 };
@@ -1174,6 +1178,26 @@ int add_acc(PipelineBuilder& pb, AggLowered& L, uint8_t kind, const ColRef* src)
     L.acc_src.push_back(*src);
   }
   return (int)L.accs.size() - 1;
+}
+
+// a co-moment sum w * (x - mx) * (y - my) + b of pass 2 (w, b optional); returns its index in L.moms
+int add_mom(PipelineBuilder& pb, AggLowered& L, const ColRef& x, const ColRef& y, const ColRef* w, const ColRef* b, int cnt, int sx, int sy) {
+  MomDesc m;
+  memset(&m, 0, sizeof m);
+  m.x = pb.resolve(x);
+  m.y = pb.resolve(y);
+  if (w) m.w = pb.resolve(*w);
+  if (b) m.b = pb.resolve(*b);
+  m.cnt = (uint8_t)cnt;
+  m.sx = (uint8_t)sx;
+  m.sy = (uint8_t)sy;
+  for (size_t i = 0; i < L.moms.size(); i++)
+    if (memcmp(&L.moms[i], &m, sizeof m) == 0) return (int)i;
+  if (L.moms.size() >= (size_t)VM_MAX_MOM) throw EngineError(B200_ERR_UNSUPPORTED, "too many VAR / STDDEV / COVAR / CORR co-moments in one AggregateExec");
+  for (const ColRef* c : {&x, &y, w, b})
+    if (c) pb.pin(*c);
+  L.moms.push_back(m);
+  return (int)L.moms.size() - 1;
 }
 
 static bool narrowable(const DataType& t) {
@@ -1278,9 +1302,157 @@ void lower_aggregate(PipelineBuilder& pb, const PlanNode& node, AggLowered& L, i
     push(s ? AO_MINMAX_STR : f ? AO_MINMAX_F64 : sum_out_kind(t), a, c, t, name, v.nullable || scalar);
     if (s) L.outs.back().phys = PH_STRVIEW;  // copied into a buffer of its own after the extraction
   };
+  // VAR / STDDEV / COVAR / CORR: the group's count and f64 sums (pass 1) and its centred co-moments (pass 2), then the
+  // result or the partial state columns computed from them at extraction
+  auto f64_expr = [](const ExprPtr& e) -> ExprPtr {
+    if (e->type.id == TypeId::Float64) return e;
+    auto c = std::make_shared<Expr>();
+    c->kind = Expr::Cast;
+    c->type = DataType(TypeId::Float64);
+    c->nullable = e->nullable;
+    c->args = {e};
+    return c;
+  };
+  auto col_expr = [&](size_t i) {
+    auto c = std::make_shared<Expr>();
+    c->kind = Expr::Col;
+    c->col = (int)i;
+    c->type = pb.cols.at(i).type;
+    c->nullable = pb.cols.at(i).nullable;
+    return c;
+  };
+  auto push_stat = [&](const AggExpr& ae, int cnt, int sx, int sy, int mxx, int myy, int mxy) {
+    const std::string& nm = ae.name;
+    const uint8_t st[6] = {(uint8_t)cnt, (uint8_t)sx, (uint8_t)sy, (uint8_t)mxx, (uint8_t)myy, (uint8_t)mxy};
+    auto out = [&](int code, const std::string& name) {
+      push(AO_STAT, 0, 0, DataType(TypeId::Float64), name, true, code);
+      memcpy(L.outs.back().st, st, sizeof st);
+    };
+    if (emit_states) {
+      push(AO_COUNT, cnt, 255, DataType(TypeId::UInt64), nm + "[count]", false);
+      if (ae.fn == AggFn::Corr) {
+        out(SO_MEAN_X, nm + "[mean1]");
+        out(SO_M2_X, nm + "[m2_1]");
+        out(SO_MEAN_Y, nm + "[mean2]");
+        out(SO_M2_Y, nm + "[m2_2]");
+        out(SO_CO, nm + "[algo_const]");
+      } else if (agg_is_bivariate(ae.fn)) {
+        out(SO_MEAN_X, nm + "[mean1]");
+        out(SO_MEAN_Y, nm + "[mean2]");
+        out(SO_CO, nm + "[algo_const]");
+      } else {
+        out(SO_MEAN_X, nm + "[mean]");
+        out(SO_M2_X, nm + "[m2]");
+      }
+      return;
+    }
+    switch (ae.fn) {
+      case AggFn::VarSamp: out(SO_VAR_SAMP, nm); break;
+      case AggFn::VarPop: out(SO_VAR_POP, nm); break;
+      case AggFn::StddevSamp: out(SO_STDDEV_SAMP, nm); break;
+      case AggFn::StddevPop: out(SO_STDDEV_POP, nm); break;
+      case AggFn::CovarSamp: out(SO_COVAR_SAMP, nm); break;
+      case AggFn::CovarPop: out(SO_COVAR_POP, nm); break;
+      default: out(SO_CORR, nm); break;
+    }
+  };
+  auto lower_stat_states = [&](const AggExpr& ae) {
+    // Chan's merge: n = sum n_i, mean = sum n_i * mean_i / n, m2 = sum (m2_i + n_i * (mean_i - mean)^2), and the same for the
+    // co-moment with both means.  Pass 1 sums n_i and n_i * mean_i, pass 2 the rest around the merged means.
+    const size_t c0 = state_col;
+    ColRef n_i = pb.cols.at(c0);
+    const int cnt = add_acc(pb, L, ACC_SUM_I128, &n_i);
+    ColRef w = pb.cast_to(n_i, DataType(TypeId::Float64));
+    pb.pin(w);
+    auto weighted = [&](size_t mean_col) {
+      auto e = std::make_shared<Expr>();
+      e->kind = Expr::Bin;
+      e->op = BinOp::Mul;
+      e->type = DataType(TypeId::Float64);
+      e->args = {f64_expr(col_expr(c0)), col_expr(mean_col)};
+      e->nullable = e->args[0]->nullable || e->args[1]->nullable;
+      ColRef v = pb.compile(*e);
+      return add_acc(pb, L, ACC_SUM_F64, &v);
+    };
+    if (!agg_is_bivariate(ae.fn)) {  // [count] [mean] [m2]
+      ColRef mean = pb.cols.at(c0 + 1), m2 = pb.cols.at(c0 + 2);
+      const int sx = weighted(c0 + 1);
+      const int mxx = add_mom(pb, L, mean, mean, &w, &m2, cnt, sx, sx);
+      push_stat(ae, cnt, sx, sx, mxx, mxx, mxx);
+      return;
+    }
+    const bool corr = ae.fn == AggFn::Corr;  // corr: [count] [mean1] [m2_1] [mean2] [m2_2] [algo_const]; covar: [count] [mean1] [mean2] [algo_const]
+    const size_t i_mean2 = corr ? c0 + 3 : c0 + 2, i_co = corr ? c0 + 5 : c0 + 3;
+    ColRef mean1 = pb.cols.at(c0 + 1), mean2 = pb.cols.at(i_mean2), co = pb.cols.at(i_co);
+    const int sx = weighted(c0 + 1), sy = weighted(i_mean2);
+    const int mxy = add_mom(pb, L, mean1, mean2, &w, &co, cnt, sx, sy);
+    int mxx = mxy, myy = mxy;
+    if (corr) {
+      ColRef m2_1 = pb.cols.at(c0 + 2), m2_2 = pb.cols.at(c0 + 4);
+      mxx = add_mom(pb, L, mean1, mean1, &w, &m2_1, cnt, sx, sx);
+      myy = add_mom(pb, L, mean2, mean2, &w, &m2_2, cnt, sy, sy);
+    }
+    push_stat(ae, cnt, sx, sy, mxx, myy, mxy);
+  };
+  // the Float64 argument values, compiled once per distinct argument (pair), so that e.g. VAR and STDDEV of one column, or
+  // COVAR and CORR of one pair, share their accumulators and co-moments
+  std::map<std::string, ColRef> stat_args;
+  auto lower_stat_rows = [&](const AggExpr& ae) {
+    // covar / corr count a row only when both arguments are non-NULL: each argument is masked by the other's validity
+    auto arg = [&](const ExprPtr& v, const ExprPtr& other) {
+      const bool mask = other && other->nullable;
+      const std::string key = dump_expr(v) + (mask ? "|" + dump_expr(other) : std::string());
+      auto it = stat_args.find(key);
+      if (it != stat_args.end()) return it->second;
+      ExprPtr e = f64_expr(v);
+      if (mask) {
+        auto nn = std::make_shared<Expr>();
+        nn->kind = Expr::IsNotNull;
+        nn->type = DataType(TypeId::Bool);
+        nn->nullable = false;
+        nn->args = {other};
+        auto c = std::make_shared<Expr>();
+        c->kind = Expr::Case;
+        c->type = DataType(TypeId::Float64);
+        c->nullable = true;
+        c->args = {nn, e};
+        e = c;
+      }
+      ColRef r = pb.compile(*e);
+      pb.pin(r);
+      stat_args.emplace(key, r);
+      return r;
+    };
+    const ColRef x = arg(ae.arg, ae.arg2);
+    const int cnt = x.nullable ? add_acc(pb, L, ACC_COUNT, &x) : star;
+    const int sx = add_acc(pb, L, ACC_SUM_F64, &x);
+    if (!ae.arg2) {
+      const int mxx = add_mom(pb, L, x, x, nullptr, nullptr, cnt, sx, sx);
+      push_stat(ae, cnt, sx, sx, mxx, mxx, mxx);
+      return;
+    }
+    const ColRef y = arg(ae.arg2, ae.arg);
+    const int sy = add_acc(pb, L, ACC_SUM_F64, &y);
+    const int mxy = add_mom(pb, L, x, y, nullptr, nullptr, cnt, sx, sy);
+    int mxx = mxy, myy = mxy;
+    if (ae.fn == AggFn::Corr) {
+      mxx = add_mom(pb, L, x, x, nullptr, nullptr, cnt, sx, sx);
+      myy = add_mom(pb, L, y, y, nullptr, nullptr, cnt, sy, sy);
+    }
+    push_stat(ae, cnt, sx, sy, mxx, myy, mxy);
+  };
   for (size_t ai = 0; ai < node.aggs.size(); ai++) {
     const AggExpr& ae = node.aggs[ai];
     const std::string& nm = ae.name;
+    if (agg_is_stat(ae.fn)) {
+      if (from_states) {
+        lower_stat_states(ae);
+        state_col += (size_t)ae.n_state_cols();
+      } else {
+        lower_stat_rows(ae);
+      }
+      continue;
+    }
     if (from_states) {
       ColRef s0 = pb.cols.at(state_col);
       switch (ae.fn) {
@@ -1310,6 +1482,7 @@ void lower_aggregate(PipelineBuilder& pb, const PlanNode& node, AggLowered& L, i
           else push(AO_AVG_DEC, a, c, ae.result_type, nm, true, ae.result_type.scale - ae.sum_type.scale);
           break;
         }
+        default: break;
       }
       state_col += (size_t)ae.n_state_cols();
       continue;
@@ -1354,8 +1527,15 @@ void lower_aggregate(PipelineBuilder& pb, const PlanNode& node, AggLowered& L, i
         }
         break;
       }
+      default: break;
     }
   }
+  // the co-moments occupy three table columns each after the accumulators
+  const size_t n_acc = L.accs.size();
+  for (size_t m = 0; m < L.moms.size(); m++) L.moms[m].col = (uint8_t)(n_acc + 3 * m);
+  for (auto& r : L.outs)
+    if (r.kind == AO_STAT)
+      for (int k = 3; k < 6; k++) r.st[k] = (uint8_t)(n_acc + 3 * r.st[k]);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1374,6 +1554,7 @@ bool match_fused(const Program& P, FusedPlan& FP) {
   FusedSpec& F = FP.spec;
   memset(&F, 0, sizeof F);
   if (P.sink != SINK_AGG_REG) return false;
+  if (P.n_mom) return false;  // VAR / STDDEV / COVAR / CORR need the second pass of the VM sinks
   if (getenv("B200_NO_FUSED")) return false;
   for (int a = 0; a < P.n_acc; a++)
     if (!(P.acc[a].kind == ACC_SUM_I128 || P.acc[a].kind == ACC_COUNT || P.acc[a].kind == ACC_COUNT_STAR)) return false;
@@ -1642,6 +1823,7 @@ bool match_fused(const Program& P, FusedPlan& FP) {
 bool match_groupby(const Program& P, GroupBySpec& S) {
   memset(&S, 0, sizeof S);
   if (getenv("B200_NO_GROUPBY")) return false;
+  if (P.n_mom) return false;  // VAR / STDDEV / COVAR / CORR need the second pass of the VM sinks
   if (P.n_keys < 1 || P.n_keys > 2 || P.n_acc > GB_MAX_ACC || P.n_cols > FUSED_MAX_COLS || P.n_cols == 0) return false;
   for (int c = 0; c < P.n_cols; c++) {
     const ColDesc& cd = P.cols[c];
@@ -1841,7 +2023,8 @@ struct TableMem {
   std::vector<DevPtr> keep;
 };
 
-TableMem alloc_table(const Exec& x, uint64_t cap, int n_keys, const std::vector<AccDesc>& accs) {
+// zero_cols: f64 sum columns after the accumulators (the co-moments of VAR / STDDEV / COVAR / CORR), zero-initialised
+TableMem alloc_table(const Exec& x, uint64_t cap, int n_keys, const std::vector<AccDesc>& accs, size_t zero_cols = 0) {
   TableMem tm;
   memset(&tm.T, 0, sizeof tm.T);
   auto A = [&](size_t bytes) {
@@ -1855,7 +2038,8 @@ TableMem alloc_table(const Exec& x, uint64_t cap, int n_keys, const std::vector<
   tm.T.lock = (unsigned int*)A(cap * 4);
   tm.T.keys = (unsigned long long*)A(std::max<size_t>(1, (size_t)n_keys) * cap * 16);
   tm.T.key_valid = (unsigned char*)A(std::max<size_t>(1, (size_t)n_keys) * cap);
-  tm.T.acc = (unsigned long long*)A(std::max<size_t>(1, accs.size()) * cap * 16);
+  tm.T.acc = (unsigned long long*)A(std::max<size_t>(1, accs.size() + zero_cols) * cap * 16);
+  if (zero_cols) CUDA_CHECK(cudaMemsetAsync(tm.T.acc + accs.size() * cap * 2, 0, zero_cols * cap * 16, x.st()));
   tm.T.n_groups = (unsigned int*)A(16);
   AccKinds k;
   memset(&k, 0, sizeof k);
@@ -1910,6 +2094,7 @@ DevBatchPtr run_aggregate(const Exec& x, const BuilderFactory& make_pb, const Pl
   TableMem tm;
   RunOutcome ro;
   unsigned int n_groups = 0;
+  int reg_groups = 0;
   bool gb_bailed = false, pf_off = false;
   for (;;) {
     x.check_cancel();
@@ -1923,6 +2108,8 @@ DevBatchPtr run_aggregate(const Exec& x, const BuilderFactory& make_pb, const Pl
     P.n_acc = (uint8_t)L.accs.size();
     for (int k = 0; k < n_keys; k++) P.keys[k] = pb.resolve(L.keys[(size_t)k]);
     for (size_t a = 0; a < L.accs.size(); a++) P.acc[a] = L.accs[a];
+    P.n_mom = (uint8_t)L.moms.size();
+    for (size_t m = 0; m < L.moms.size(); m++) P.mom[m] = L.moms[m];
     memset(&P.key_hash, 0, sizeof P.key_hash);
     P.keys_all_i64 = L.fast ? 1 : 0;
     if (n_keys) {
@@ -1939,7 +2126,7 @@ DevBatchPtr run_aggregate(const Exec& x, const BuilderFactory& make_pb, const Pl
     const bool small_input = src->n <= ((int64_t)1 << 22);
     if (level > 0 && small_input) level = 8;
     uint64_t cap;
-    int reg_groups = 0;
+    reg_groups = 0;
     if (level == 0) {
       P.sink = SINK_AGG_REG;
       reg_groups = n_keys ? VM_REG_GROUPS : 1;
@@ -1956,7 +2143,7 @@ DevBatchPtr run_aggregate(const Exec& x, const BuilderFactory& make_pb, const Pl
     }
     {
       ScopeTimer t_alloc("    agg: alloc_table");
-      tm = alloc_table(x, cap, n_keys, L.accs);
+      tm = alloc_table(x, cap, n_keys, L.accs, 3 * L.moms.size());
     }
     P.table = tm.T;
     pb.finalize_layout((size_t)VM_REG_ACC * 512 * 16 + 256);
@@ -2023,6 +2210,17 @@ DevBatchPtr run_aggregate(const Exec& x, const BuilderFactory& make_pb, const Pl
     }
     level++;
   }
+  if (!L.moms.empty()) {
+    // pass 2 of VAR / STDDEV / COVAR / CORR: the same program over the same rows folds the centred co-moments into the
+    // groups pass 1 published (an overflow of pass 1 has already restarted both passes above)
+    x.check_cancel();
+    Program& P = pbp->prog;
+    P.mom_pass = 1;
+    RunOutcome r2 = launch_program(x, *pbp, reg_groups, nullptr, true, met);
+    P.mom_pass = 0;
+    if (met) met->launches += 1;
+    if (r2.status.overflow) throw EngineError(B200_ERR_EXECUTION, "aggregate: a group of the first pass was not found by the second");
+  }
   {
     // remember the smallest table class that holds this many groups (not the level that happened to be used: a small
     // input jumps straight to a table sized for its row count)
@@ -2077,6 +2275,7 @@ DevBatchPtr run_aggregate(const Exec& x, const BuilderFactory& make_pb, const Pl
     o.b = r.b;
     o.phys = r.phys;
     o.imm = r.imm;
+    memcpy(o.st, r.st, sizeof o.st);
     wbytes += (uint64_t)oc.width() * n_groups;
     out->cols.push_back(oc);
   }
@@ -4308,6 +4507,9 @@ int guard(F&& f) {
   } catch (const EngineError& e) {
     g_err = e.what();
     return e.code;
+  } catch (const PlanUnsupported& e) {
+    g_err = e.what();
+    return B200_ERR_UNSUPPORTED;
   } catch (const std::bad_alloc&) {
     g_err = "host out of memory";
     return B200_ERR_OOM;

@@ -144,8 +144,9 @@ def project(exprs: Sequence, input: Json) -> Json:
     return {"op": "ProjectionExec", "exprs": [{"expr": e, "name": n} for e, n in exprs], "input": input}
 
 
-def agg(fn_: str, arg: Optional[Json], name: str, input_type=None) -> Json:
-    a: Json = {"fn": fn_, "name": name, "args": [] if arg is None else [arg]}
+def agg(fn_: str, arg: Optional[Json], name: str, input_type=None, arg2: Optional[Json] = None) -> Json:
+    """arg2: the second argument of covar / corr."""
+    a: Json = {"fn": fn_, "name": name, "args": ([] if arg is None else [arg]) + ([] if arg2 is None else [arg2])}
     if input_type is not None:
         a["input_type"] = input_type
     return a

@@ -13,6 +13,8 @@ engine's own CUDA-event timing (b200_engine_kernel_stats) can be read for the sa
   minmax_str lineitem MIN/MAX(l_comment) GROUP BY l_returnflag, l_linestatus (4 groups)              -> pipeline_agg_reg
              and MAX(l_comment) GROUP BY l_orderkey (15 M groups at SF10)                             -> pipeline_agg_global
              (each result checked against the CPU oracle unless ORACLE=0)
+  stats      STDDEV(l_extendedprice), CORR(l_quantity, l_extendedprice) and AVG of both, by (l_returnflag, l_linestatus)
+             (4 groups) and by l_suppkey (100 k groups at SF10)           -> pipeline_agg_* and pipeline_agg_*_pass2
   nlj        NestedLoopJoinExec: lineitem against one build row (a scalar subquery) next to the same comparison
              through fast_filter_kernel, and a band join of orders (msf 1000) against 10,000 build rows    -> nlj_count / nlj_write
 """
@@ -130,6 +132,69 @@ elif op == "minmax_str":
             assert_tables_equal(got, want)
             report[name]["matches_oracle"] = True
     print(json.dumps({op: report, "rows": n}, indent=1))
+elif op == "stats":
+    # STDDEV(l_extendedprice) and CORR(l_quantity, l_extendedprice) next to AVG of the same columns, by (l_returnflag,
+    # l_linestatus) (4 groups: register sink) and by l_suppkey (global sink).  Kernel ms per timer family: the statistical
+    # aggregates run a first pass (pipeline_agg_*) and a second (pipeline_agg_*_pass2) over the same rows.  Each result is
+    # checked against a numpy two-pass computation in float64 (the CPU oracle does not compute these functions) and AVG
+    # against the CPU oracle, unless ORACLE=0.  The card's name and power limit are read in the same run.
+    import subprocess
+    import numpy as np
+    cols = ["l_suppkey", "l_quantity", "l_extendedprice", "l_returnflag", "l_linestatus"]
+    n = load("lineitem", cols)
+    host = eng.export_table("lineitem", 0)
+    card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
+    scan = tpch.table_scan("lineitem", cols)
+    keys = {"reg_4_groups": ([(c(3), "l_returnflag"), (c(4), "l_linestatus")], 2 * (4 * (n + 1) + n)), "global_suppkey": ([(c(0), "l_suppkey")], 8 * n)}
+    funcs = {"stddev": ([P.agg("stddev", c(2), "r")], 16 * n), "corr": ([P.agg("corr", c(1), "r", arg2=c(2))], 32 * n),
+             "avg": ([P.agg("avg", c(1), "a"), P.agg("avg", c(2), "b")], 32 * n)}
+    import pyarrow as pa
+    import pyarrow.compute as pc
+    xq = pc.cast(host.column(1), pa.float64()).to_numpy()
+    xe = pc.cast(host.column(2), pa.float64()).to_numpy()
+    gid = {"reg_4_groups": pc.binary_join_element_wise(host.column(3), host.column(4), "").to_numpy(zero_copy_only=False),
+           "global_suppkey": host.column(0).to_numpy()}
+    check = os.environ.get("ORACLE", "1") != "0"
+    if check:
+        sys.path.insert(0, os.path.join(ROOT, "tests"))
+        import oracle_ffi
+        from util import assert_tables_equal
+        from ballista_b200 import driver
+        oracle = oracle_ffi.OracleEngine()
+        oracle.tpch_generate("lineitem", msf, 0, 0, n, cols)
+
+    def two_pass(g, x, y):
+        _, inv, cnt = np.unique(g, return_inverse=True, return_counts=True)
+        mx = np.bincount(inv, x) / cnt
+        my = np.bincount(inv, y) / cnt
+        dx, dy = x - mx[inv], y - my[inv]
+        return inv, cnt, np.bincount(inv, dx * dx), np.bincount(inv, dy * dy), np.bincount(inv, dx * dy)
+
+    report = {"card": card, "rows": n}
+    for kname, (gb, kbytes) in keys.items():
+        inv, cnt, sxx, syy, sxy = two_pass(gid[kname], xq, xe)
+        for fname, (aggs, abytes) in funcs.items():
+            st = [P.Stage(1, P.shuffle_writer(P.aggregate("Single", gb, aggs, scan), 1))]
+            eng.kernel_stats(reset=True)
+            run(st, [1])
+            ks = eng.kernel_stats(reset=True)
+            ms = {k: round(v["ms"] / reps, 3) for k, v in ks.items() if k.startswith("pipeline_") or k == "groupby_hash_agg"}
+            nbytes = kbytes + abytes
+            r = {"kernel_ms_per_run": ms, "arrow_bytes_read": nbytes, "GB_per_s": {k: round(nbytes / (v * 1e-3) / 1e9, 1) for k, v in ms.items() if v > 0}}
+            if check:
+                got = driver.run_stages(eng, st, f"chk-{kname}-{fname}")
+                if fname == "avg":
+                    assert_tables_equal(got, driver.run_stages(oracle, st, f"chk-{kname}-{fname}"))
+                else:
+                    gk = [a + b for a, b in zip(got.column(0).to_pylist(), got.column(1).to_pylist())] if len(gb) == 2 else got.column(0).to_pylist()
+                    order = {k: i for i, k in enumerate(np.unique(gid[kname]).tolist())}
+                    want = np.sqrt(syy / (cnt - 1)) if fname == "stddev" else sxy / np.sqrt(sxx * syy)
+                    for k, v in zip(gk, got.column("r").to_pylist()):
+                        w = want[order[k]]
+                        assert abs(v - w) <= 1e-9 * abs(w), (kname, fname, k, v, w)
+                r["matches_reference"] = True
+            report[f"{kname}/{fname}"] = r
+    print(json.dumps({op: report}, indent=1))
 elif op == "nlj":
     # (a) scalar subquery: lineitem (msf 10000 = SF10) probed against ONE build row, l_extendedprice > avg, next to the same
     #     comparison against a literal through fast_filter_kernel;
