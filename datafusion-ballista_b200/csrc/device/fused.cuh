@@ -811,13 +811,21 @@ constexpr FusedShapeDesc kShapeQ1 = {1, {4}, {3 /*LE*/}, 2, {1, 1}, {4, 4}, 1, 2
 // TPC-H q6 (benchmarks/queries/q6.sql): date range, discount BETWEEN, quantity <; count + sum(price*disc)
 constexpr FusedShapeDesc kShapeQ6 = {5, {4, 4, 16, 16, 16}, {5 /*GE*/, 2 /*LT*/, 5, 3 /*LE*/, 2}, 0, {0, 0}, {0, 0}, 0, 1, {2, 0}, {0, 0}, {16, 0}, {16, 0}, 2,
                                      {3, 1}, {0, 0}};
-// the same query when the two key columns carry pre-packed 4-byte images (registered tables, engine.cpp prepack_short_strings):
+// the same query when the two key columns carry pre-packed 4-byte images (registered tables, engine.cpp build_column_images):
 // the keys are plain 32-bit integer tile columns, no offsets / character gathers
 constexpr FusedShapeDesc kShapeQ1P = {1, {4}, {3 /*LE*/}, 2, {0, 0}, {4, 4}, 1, 2, {0, 1}, {0, 1}, {16, 0}, {16, 16}, 6,
                                       {3, 0, 0, 1, 2, 0}, {0, 16, 16, 0, 0, 16}};
+// q1 and q6 when the decimal columns carry their int32 images as well (registered tables whose values fit 32 bits, as
+// every TPC-H value does): 28 and 16 bytes per row instead of 76 and 52
+constexpr FusedShapeDesc kShapeQ1N = {1, {4}, {3 /*LE*/}, 2, {0, 0}, {4, 4}, 1, 2, {0, 1}, {0, 1}, {4, 0}, {4, 4}, 6,
+                                      {3, 0, 0, 1, 2, 0}, {0, 4, 4, 0, 0, 4}};
+constexpr FusedShapeDesc kShapeQ6N = {5, {4, 4, 4, 4, 4}, {5 /*GE*/, 2 /*LT*/, 5, 3 /*LE*/, 2}, 0, {0, 0}, {0, 0}, 0, 1, {2, 0}, {0, 0}, {4, 0}, {4, 0}, 2,
+                                      {3, 1}, {0, 0}};
 constexpr FusedShape kQ1P = fused_shape_encode(kShapeQ1P);
 constexpr FusedShape kQ1 = fused_shape_encode(kShapeQ1);
 constexpr FusedShape kQ6 = fused_shape_encode(kShapeQ6);
+constexpr FusedShape kQ1N = fused_shape_encode(kShapeQ1N);
+constexpr FusedShape kQ6N = fused_shape_encode(kShapeQ6N);
 
 // (rows per thread, launch bound) variants compiled for each shape
 template <int G, uint64_t SA, uint64_t SB>
@@ -842,6 +850,8 @@ static cudaError_t launch_fused(const FusedSpec& F, FusedShape shape, int reg_gr
   if (reg_groups > 1 && shape.a == kQ1.a && shape.b == kQ1.b) return launch_fused_variant<VM_REG_GROUPS, kQ1.a, kQ1.b>(R, grid, block, smem, st);
   if (reg_groups > 1 && shape.a == kQ1P.a && shape.b == kQ1P.b) return launch_fused_variant<VM_REG_GROUPS, kQ1P.a, kQ1P.b>(R, grid, block, smem, st);
   if (reg_groups <= 1 && shape.a == kQ6.a && shape.b == kQ6.b) return launch_fused_variant<1, kQ6.a, kQ6.b>(R, grid, block, smem, st);
+  if (reg_groups > 1 && shape.a == kQ1N.a && shape.b == kQ1N.b) return launch_fused_variant<VM_REG_GROUPS, kQ1N.a, kQ1N.b>(R, grid, block, smem, st);
+  if (reg_groups <= 1 && shape.a == kQ6N.a && shape.b == kQ6N.b) return launch_fused_variant<1, kQ6N.a, kQ6N.b>(R, grid, block, smem, st);
   *is_static = 0;
   if (reg_groups > 1) return launch_fused_variant<VM_REG_GROUPS, 0, 0>(R, grid, block, smem, st);
   return launch_fused_variant<1, 0, 0>(R, grid, block, smem, st);

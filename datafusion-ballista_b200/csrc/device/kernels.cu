@@ -445,6 +445,21 @@ __global__ void prepack3_kernel(const int32_t* offsets, const uint8_t* chars, in
 void launch_prepack3(const int32_t* offsets, const uint8_t* chars, int64_t n, uint32_t* out, unsigned int* too_long, cudaStream_t st) {
   prepack3_kernel<<<grid_for(n, 256, 4), 256, 0, st>>>(offsets, chars, n, out, too_long);
 }
+// 32-bit images of a Decimal128 column (the value as int32) -- the companion the fused aggregate kernel streams instead of
+// the 16-byte values; *too_wide is set when some value does not fit (the image is then unusable)
+__global__ void dec128_image_kernel(const ulonglong2* in, int64_t n, int32_t* out, unsigned int* too_wide) {
+  unsigned int wide = 0;
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+    const ulonglong2 v = in[i];
+    const int64_t lo = (int64_t)v.x;
+    wide |= (lo != (int64_t)(int32_t)lo || v.y != (unsigned long long)(lo >> 63)) ? 1u : 0u;
+    out[i] = (int32_t)lo;
+  }
+  if (wide) *too_wide = 1u;
+}
+void launch_dec128_image(const void* in, int64_t n, int32_t* out, unsigned int* too_wide, cudaStream_t st) {
+  dec128_image_kernel<<<grid_for(n, 256, 4), 256, 0, st>>>((const ulonglong2*)in, n, out, too_wide);
+}
 __global__ void view_lengths_kernel(const unsigned long long* views, const uint8_t* valid, uint32_t* lens, int64_t n) {
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
     lens[i] = (valid && !valid[i]) ? 0u : (uint32_t)views[2 * i + 1];

@@ -93,7 +93,7 @@ struct ColDesc {
   const void* data;        // values / offsets / views
   const uint8_t* valid;    // byte per row or nullptr
   const uint8_t* chars;    // PH_UTF8: character bytes
-  const void* packed32;    // PH_UTF8 whose strings are all <= 3 bytes: pre-packed images len<<24|bytes (4 B/row), else nullptr
+  const void* img32;       // 4-byte image per row (DevColumn::img32): PH_UTF8 len<<24|bytes, PH_DEC128 int32 value; else nullptr
   uint32_t smem_off;       // offset of this column's tile inside a stage buffer
   uint32_t valid_smem_off; // offset of the validity tile (if valid != nullptr)
   uint8_t phys;

@@ -135,7 +135,9 @@ struct DevColumn {
   const uint8_t* valid = nullptr;  // byte per row or nullptr
   const uint8_t* chars = nullptr;  // PH_UTF8 only
   int64_t chars_bytes = -1;        // PH_UTF8: bytes referenced by this column's rows (-1 unknown)
-  const uint32_t* pk32 = nullptr;  // PH_UTF8 with only <= 3-byte strings: pre-packed key images (kept alive through `keep`)
+  // 4-byte image of every row, or nullptr (build_column_images; kept alive through `keep`): PH_UTF8 with only <= 3-byte
+  // strings: len << 24 | bytes; PH_DEC128 whose values all fit int32: the value as int32
+  const uint32_t* img32 = nullptr;
   std::vector<DevPtr> keep;        // allocations that must outlive this column
   int width() const { return phys_width(phys); }
 };
@@ -152,7 +154,7 @@ inline DevColumn slice_column(const DevColumn& c, int64_t r0, int64_t r1) {
   o.n = r1 - r0;
   o.data = c.data ? c.data + r0 * c.width() : nullptr;
   o.valid = c.valid ? c.valid + r0 : nullptr;
-  o.pk32 = c.pk32 ? c.pk32 + r0 : nullptr;
+  o.img32 = c.img32 ? c.img32 + r0 : nullptr;
   o.chars_bytes = -1;
   return o;
 }

@@ -443,33 +443,41 @@ DevColumn as_utf8(const Exec& x, const DevColumn& c, int64_t known_total = -1) {
   return o;
 }
 
-// Registered tables: every Utf8 column whose strings are all at most 3 bytes long (TPC-H flags, status, ...) gets a
-// companion of 4-byte key images (len << 24 | bytes).  An aggregate that groups by such a column then streams 4 bytes per
-// row through the same TMA ring as its other operands instead of gathering characters behind the offsets.
-void prepack_short_strings(const Exec& x, DevBatch& b) {
-  struct Cand { size_t col; DevPtr img, flag; const unsigned int* h; };
-  std::vector<Cand> cands;
+// Registered tables get 4-byte companion images of the non-null columns that allow one, all or nothing per column:
+//  * Utf8 whose strings are all at most 3 bytes long (TPC-H flags, status, ...): key images len << 24 | bytes.  An
+//    aggregate that groups by such a column streams 4 bytes per row through the same TMA ring as its other operands
+//    instead of gathering characters behind the offsets.
+//  * Decimal128 whose values all fit int32 (TPC-H money and quantity columns): the value as int32.  The fused aggregate
+//    kernel streams 4 of the 16 bytes per row.
+// The table itself stays Arrow; the images cost 4 bytes per row and column of HBM.  One read-back for all columns.
+void build_column_images(const Exec& x, DevBatch& b) {
+  std::vector<size_t> cands;
   for (size_t ci = 0; ci < b.cols.size(); ci++) {
-    DevColumn& c = b.cols[ci];
-    if (c.phys != PH_UTF8 || c.valid || c.pk32 || c.n == 0) continue;
-    if (c.chars_bytes < 0 || c.chars_bytes > 3 * c.n) continue;  // some string must be longer
-    Cand cd;
-    cd.col = ci;
-    cd.img = dev_alloc((size_t)c.n * 4 + 64, x.st());
-    cd.flag = dev_alloc(16, x.st());
-    CUDA_CHECK(cudaMemsetAsync(cd.flag->ptr, 0, 16, x.st()));
-    launch_prepack3((const int32_t*)c.data, c.chars, c.n, (uint32_t*)cd.img->ptr, (unsigned int*)cd.flag->ptr, x.st());
-    x.count();
-    cd.h = x.fetch<unsigned int>(cd.flag->ptr);
-    cands.push_back(cd);
+    const DevColumn& c = b.cols[ci];
+    if (c.valid || c.img32 || c.n == 0) continue;
+    if (c.phys == PH_UTF8 && c.chars_bytes >= 0 && c.chars_bytes <= 3 * c.n) cands.push_back(ci);  // else some string is longer
+    if (c.phys == PH_DEC128) cands.push_back(ci);
   }
   if (cands.empty()) return;
+  DevPtr flags = dev_alloc(cands.size() * 4, x.st());
+  CUDA_CHECK(cudaMemsetAsync(flags->ptr, 0, cands.size() * 4, x.st()));
+  std::vector<DevPtr> imgs;
+  for (size_t k = 0; k < cands.size(); k++) {
+    const DevColumn& c = b.cols[cands[k]];
+    DevPtr img = dev_alloc((size_t)c.n * 4 + 64, x.st());  // slack: a TMA bulk copy of the last tile stays inside
+    unsigned int* flag = (unsigned int*)flags->ptr + k;
+    if (c.phys == PH_UTF8) launch_prepack3((const int32_t*)c.data, c.chars, c.n, (uint32_t*)img->ptr, flag, x.st());
+    else launch_dec128_image(c.data, c.n, (int32_t*)img->ptr, flag, x.st());
+    x.count();
+    imgs.push_back(img);
+  }
+  const unsigned int* h = (const unsigned int*)x.fetch_bytes(flags->ptr, cands.size() * 4);
   x.sync();
-  for (auto& cd : cands) {
-    if (*cd.h) continue;
-    DevColumn& c = b.cols[cd.col];
-    c.pk32 = (const uint32_t*)cd.img->ptr;
-    c.keep.push_back(cd.img);
+  for (size_t k = 0; k < cands.size(); k++) {
+    if (h[k]) continue;
+    DevColumn& c = b.cols[cands[k]];
+    c.img32 = (const uint32_t*)imgs[k]->ptr;
+    c.keep.push_back(imgs[k]);
   }
 }
 
@@ -989,7 +997,7 @@ RunOutcome launch_program(const Exec& x, PipelineBuilder& pb, int reg_groups, co
     for (int i = 0; i < P.n_regs; i++) fprintf(stderr, "[b200]   reg %d: vk=%d off=%u valid_off=%u\n", i, P.regs[i].vk, P.regs[i].smem_off, P.regs[i].valid_off);
   }
   uint64_t kt_bytes = 0;
-  for (int i = 0; i < P.n_cols; i++) kt_bytes += (uint64_t)P.cols[i].width * (uint64_t)P.n_rows;
+  for (int i = 0; i < P.n_cols; i++) kt_bytes += (uint64_t)(fused ? fused->spec.cols[i].width : P.cols[i].width) * (uint64_t)P.n_rows;  // fused: images when streamed
   if (P.sink == SINK_MATERIALIZE)
     for (int j = 0; j < P.n_out; j++) kt_bytes += (uint64_t)phys_width((Phys)P.out[j].phys) * (uint64_t)P.n_rows;  // upper bound: every row kept
   KernelTimer kt(x, ff ? "filter_compact" : gb ? "groupby_hash_agg" : fused ? "pipeline_fused_agg" : P.sink == SINK_MATERIALIZE ? "pipeline_materialize"
@@ -1562,32 +1570,40 @@ bool match_fused(const Program& P, FusedPlan& FP) {
   // 4 rows per thread amortise the per-tile work (claim, TMA issue, barrier wait); grouped shapes then fit
   // 8 warps of up to 255 registers next to their shared-memory partials, scalar shapes 12 warps.  On an
   // H100 SXM (700 W limit) stage 1 of q1 at SF10 took 1.62-1.73 ms at R=4 / 256 threads against
-  // 1.69-1.83 ms for R=4 / 384 and R=2 / 256, 384, 512
+  // 1.69-1.83 ms for R=4 / 384 and R=2 / 256, 384, 512 (Arrow widths, 76 B/row).
+  // With every column streamed as a 4-byte image (28 B/row) the kernel is no longer bandwidth-bound at 8 warps:
+  // on an H100 80GB HBM3 (700 W limit), median of 10 runs, stage 1 of q1 at SF10 took 1.09 ms at R=4 / 256
+  // threads (1.05-1.08 ms with 2-4 stages), 0.80 ms at R=4 / 384 (3 stages), 0.90 ms at R=8 / 256 (not kept), 1.39, 1.13
+  // and 1.01 ms at R=2 / 256, 384, 512.  So narrow tiles run 12 warps of R=4.
   const int R = env_int("B200_FUSED_R", 4);
   if (!(R == 2 || R == 4)) return false;
-  int block = env_int("B200_FUSED_B", (R == 4 && P.n_keys) ? 256 : 384);
-  if (block > (R == 4 ? 384 : 512) || block < 32 || (block & 31)) return false;
   const uint32_t TR = 32u * (uint32_t)R;
   if (P.n_cols > FUSED_MAX_COLS || P.n_cols == 0) return false;
   uint32_t fused_off[VM_MAX_COLS];
   uint32_t cur = 0, tx = 0, tx_utf8 = 0;
-  bool aligned = true;
-  // short-string keys with a pre-packed companion (prepack_short_strings) are read as 4-byte integer key columns
-  bool prepacked[VM_MAX_COLS] = {false};
-  if (!getenv("B200_NO_PREPACK"))
+  bool aligned = true, narrow = true;
+  // columns with a 4-byte companion image (build_column_images) stream the image: short-string keys are read as 4-byte
+  // integer key columns, decimals as int32 (every use of a decimal column in a matched program is a filter, a product
+  // operand or a SUM source, and all of them sign-extend 4-byte tile values)
+  bool imaged[VM_MAX_COLS] = {false};
+  if (!getenv("B200_NO_PREPACK")) {
     for (int i = 0; i < P.n_instr; i++) {
       const VInstr& v = P.code[i];
-      if (v.op == OP_STR_PACK8 && v.a.kind == OPD_COL && v.imm == 24 && v.aux <= 3 && P.cols[v.a.idx].phys == PH_UTF8 && P.cols[v.a.idx].packed32 &&
-          (((uintptr_t)P.cols[v.a.idx].packed32) & 15) == 0)
-        prepacked[v.a.idx] = true;
+      if (v.op == OP_STR_PACK8 && v.a.kind == OPD_COL && v.imm == 24 && v.aux <= 3 && P.cols[v.a.idx].phys == PH_UTF8 && P.cols[v.a.idx].img32)
+        imaged[v.a.idx] = true;
     }
+    for (int c = 0; c < P.n_cols; c++)
+      if (P.cols[c].phys == PH_DEC128 && P.cols[c].img32) imaged[c] = true;
+    for (int c = 0; c < P.n_cols; c++)
+      if (((uintptr_t)P.cols[c].img32) & 15) imaged[c] = false;  // the bulk copies need 16-byte aligned sources
+  }
   for (int c = 0; c < P.n_cols; c++) {
     const ColDesc& cd = P.cols[c];
     if (cd.valid) return false;
     FusedCol& fc = F.cols[c];
-    fc.data = prepacked[c] ? cd.packed32 : cd.data;
-    fc.width = prepacked[c] ? 4 : cd.width;
-    fc.utf8 = (cd.phys == PH_UTF8 && !prepacked[c]) ? 1u : 0u;
+    fc.data = imaged[c] ? cd.img32 : cd.data;
+    fc.width = imaged[c] ? 4 : cd.width;
+    fc.utf8 = (cd.phys == PH_UTF8 && !imaged[c]) ? 1u : 0u;
     fc.tile_bytes = TR * fc.width + (fc.utf8 ? 16u : 0u);
     if (fc.tile_bytes & 15u) return false;
     fc.off = cur;
@@ -1596,7 +1612,10 @@ bool match_fused(const Program& P, FusedPlan& FP) {
     if (fc.utf8) tx_utf8 += fc.tile_bytes;
     else tx += fc.tile_bytes;
     if (((uintptr_t)fc.data & 15) != 0) aligned = false;
+    narrow &= fc.width <= 4 && !fc.utf8;
   }
+  int block = env_int("B200_FUSED_B", (R == 4 && P.n_keys && !narrow) ? 256 : 384);
+  if (block > (R == 4 ? 384 : 512) || block < 32 || (block & 31)) return false;
   F.n_cols = P.n_cols;
   F.rows_per_thread = R;
   F.stage_bytes = (cur + 127u) & ~127u;
@@ -1632,11 +1651,9 @@ bool match_fused(const Program& P, FusedPlan& FP) {
     if (cd.valid) return false;
     if (!(cd.phys == PH_I32 || cd.phys == PH_I64 || cd.phys == PH_DEC128)) return false;
     if (want_i128 && o.vk == VK_I128 && cd.phys != PH_DEC128) return false;
-    if (o.vk != VK_I128 && cd.phys == PH_DEC128) {
-      // narrow view of a decimal: low word only
-    }
+    // the width the kernel streams: a decimal (also its narrow view, the low word) is 16 bytes, or 4 with its image
     *off = fused_off[o.idx];
-    *w = (o.vk == VK_I128) ? 16 : cd.width;
+    *w = (uint8_t)F.cols[o.idx].width;
     return true;
   };
   int prod_reg[2] = {-1, -1};
@@ -1662,7 +1679,6 @@ bool match_fused(const Program& P, FusedPlan& FP) {
         Operand c64 = col;
         c64.vk = VK_I64;
         if (!int_col(c64, &f.off, &f.w, false)) return false;
-        if (P.cols[col.idx].phys == PH_DEC128) f.w = 16;
         f.op = op;
         f.imm = (int64_t)P.imms[imm.idx].lo;
         F.n_filters++;
@@ -1691,7 +1707,7 @@ bool match_fused(const Program& P, FusedPlan& FP) {
         PackInfo pi;
         pi.reg = v.dst.idx;
         memset(&pi.k, 0, sizeof pi.k);
-        if (prepacked[v.a.idx]) {  // the image is already in the tile: an integer key column of width 4
+        if (imaged[v.a.idx]) {  // the image is already in the tile: an integer key column of width 4
           pi.k.kind = 0;
           pi.k.off = fused_off[v.a.idx];
           pi.k.w = 4;
@@ -4479,7 +4495,7 @@ DevBatchPtr scan_parquet(const Exec& x, const std::string& path, const std::vect
     }
     out->cols.push_back(col);
   }
-  prepack_short_strings(x, *out);
+  build_column_images(x, *out);
   x.sync();
   return out;
 }
@@ -4769,7 +4785,7 @@ int b200_engine_register_batch(b200_engine* e, const char* table, int partition,
     CUDA_CHECK(cudaSetDevice(e->device));
     DevBatchPtr b = import_batch(e, batch, schema);
     Exec x{e, nullptr, nullptr};
-    prepack_short_strings(x, *b);
+    build_column_images(x, *b);
     DevBatchPtr prev;
     {
       std::lock_guard<std::mutex> g(e->mu);
@@ -4782,6 +4798,9 @@ int b200_engine_register_batch(b200_engine* e, const char* table, int partition,
       Schema s;
       for (auto& c : prev->cols) s.push_back(Field{c.name, c.type, true});
       DevBatchPtr cat = r.concat({prev, b}, s);
+      // registered tables keep the canonical Arrow layout (concat leaves strings as views) and their companion images
+      for (auto& c : cat->cols) c = as_utf8(x, c);
+      build_column_images(x, *cat);
       CUDA_CHECK(cudaStreamSynchronize(e->stream));
       std::lock_guard<std::mutex> g(e->mu);
       e->tables[table][partition] = cat;
@@ -4866,7 +4885,7 @@ int b200_engine_tpch_generate(b200_engine* e, const char* table, int64_t msf, in
       }
       b->cols.push_back(col);
     }
-    prepack_short_strings(Exec{e, nullptr, nullptr}, *b);
+    build_column_images(Exec{e, nullptr, nullptr}, *b);
     CUDA_CHECK(cudaStreamSynchronize(st));
     std::lock_guard<std::mutex> g(e->mu);
     e->tables[table][partition] = b;

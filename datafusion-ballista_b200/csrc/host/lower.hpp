@@ -435,7 +435,7 @@ class PipelineBuilder {
       cd.data = sc.data;
       cd.valid = sc.valid;
       cd.chars = sc.chars;
-      cd.packed32 = sc.phys == PH_UTF8 ? (const void*)sc.pk32 : nullptr;
+      cd.img32 = sc.img32;
       cd.phys = sc.phys;
       cd.width = (uint8_t)sc.width();
       cd.in_tile = 1;

@@ -91,8 +91,18 @@ elif op == "parquet":
     for r in range(reps):
         eng.register_parquet("lineitem_pq", 0, path, tpch.Q1_COLUMNS)
 elif op == "q1":
-    load("lineitem", tpch.Q1_COLUMNS)
+    # the bytes are what the fused kernel streams (4-byte images where registered columns have them), against the H100 SXM
+    # data sheet's 3.35 TB/s; the card's name and power limit are read in the same run
+    import subprocess
+    n = load("lineitem", tpch.Q1_COLUMNS)
+    run([tpch.q1(1)[0]], [1])  # warm-up: the first launch of a kernel also loads it
+    eng.kernel_stats(reset=True)
     run([tpch.q1(1)[0]], [1])
+    f = eng.kernel_stats()["pipeline_fused_agg"]
+    card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
+    gbs = f["bytes"] / (f["ms"] * 1e-3) / 1e9
+    print(json.dumps({op: {"card": card, "rows": n, "kernel_ms_per_run": round(f["ms"] / reps, 3), "bytes_per_row": f["bytes"] / (n * reps),
+                           "GB_per_s": round(gbs, 1), "frac_of_datasheet_hbm_3350_GBps": round(gbs / 3350, 3)}}, indent=1))
 elif op == "minmax_str":
     cols = ["l_orderkey", "l_returnflag", "l_linestatus", "l_comment"]
     n = load("lineitem", cols)
