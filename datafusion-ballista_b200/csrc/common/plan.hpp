@@ -277,7 +277,7 @@ struct Expr {
   int col = -1;           // Col
   LitValue lit;           // Lit
   BinOp op = BinOp::Add;  // Bin
-  std::string fn;         // Fn: "date_part_year", "substr"
+  std::string fn;         // Fn: "date_part_<part>", "substr", "abs", "round", ... (type_scalar_fn)
   std::vector<ExprPtr> args;  // Bin: l,r; unary: x; Case: [w0,t0,w1,t1,...,(else)]; InList: x, items...; Fn args
   bool has_else = false;  // Case
   bool negated = false;   // InList / Like
@@ -346,6 +346,107 @@ inline DataType arith_result_type(BinOp op, DataType a, DataType b) {
 }
 
 ExprPtr parse_expr(const Json& j, const Schema& in);
+
+// A plan the engine understands but does not run (e.g. statistical states laid out in an unknown way): B200_ERR_UNSUPPORTED
+struct PlanUnsupported : std::runtime_error {
+  explicit PlanUnsupported(const std::string& m) : std::runtime_error(m) {}
+};
+
+// The date_part family: IR "date_part_<part>", parts in the order of DatePart (csrc/device/program.h); -1 for another name
+inline int date_part_index(const std::string& fn) {
+  static const char* const parts[] = {"year", "quarter", "month", "week", "day", "doy", "dow"};
+  if (fn.compare(0, 10, "date_part_") != 0) return -1;
+  for (int i = 0; i < 7; i++)
+    if (fn.compare(10, std::string::npos, parts[i]) == 0) return i;
+  return -1;
+}
+
+// Result type and nullability of a scalar function call (DESIGN.md §3, rules [EXT] in §6).  A known function over an
+// argument type it does not take is refused with PlanUnsupported naming the type; an unknown name or a wrong argument
+// count is a malformed plan.
+inline void type_scalar_fn(Expr& e) {
+  const std::string& f = e.fn;
+  const size_t n = e.args.size();
+  auto arity = [&](size_t lo, size_t hi) {
+    if (n < lo || n > hi) throw std::runtime_error("plan IR: " + f + " takes " + std::to_string(lo) + (hi > lo ? ".." + std::to_string(hi) : "") + " argument(s)");
+  };
+  auto arg_t = [&](size_t i) -> const DataType& { return e.args[i]->type; };
+  auto refuse = [&](size_t i) -> void { throw PlanUnsupported(f + " does not support an argument of type " + arg_t(i).str()); };
+  auto any_nullable = [&]() {
+    bool r = false;
+    for (auto& a : e.args) r = r || a->nullable;
+    return r;
+  };
+  auto need_utf8 = [&](size_t i) {
+    if (!arg_t(i).is_string() && arg_t(i).id != TypeId::Null) refuse(i);
+  };
+  if (date_part_index(f) >= 0) {
+    arity(1, 1);
+    // DataFusion: date_part(part, Date32) -> Int32 [EXT]
+    if (arg_t(0).id != TypeId::Date32 && arg_t(0).id != TypeId::Null) refuse(0);
+    e.type = DataType(TypeId::Int32);
+    e.nullable = e.args[0]->nullable;
+  } else if (f == "substr") {
+    e.type = DataType(TypeId::Utf8);
+    e.nullable = n ? e.args[0]->nullable : false;
+  } else if (f == "abs") {
+    arity(1, 1);
+    if (!arg_t(0).is_numeric()) refuse(0);
+    e.type = arg_t(0);
+    e.nullable = e.args[0]->nullable;
+  } else if (f == "round" || f == "floor" || f == "ceil") {
+    arity(1, f == "round" ? 2 : 1);
+    if (!arg_t(0).is_float()) refuse(0);
+    if (n == 2) {
+      if (!arg_t(1).is_integer()) refuse(1);
+      const Expr& d = *e.args[1];
+      // f = 10^|n| must be exact in binary64 for the result to be the one the formula defines
+      if (d.kind == Expr::Lit && !d.lit.is_null && (d.lit.i > 22 || d.lit.i < -22))
+        throw PlanUnsupported("round to " + std::to_string(d.lit.i) + " digits is not supported (|digits| <= 22)");
+    }
+    e.type = arg_t(0);
+    e.nullable = any_nullable();
+  } else if (f == "nullif") {
+    arity(2, 2);
+    if (arg_t(0) != arg_t(1) && arg_t(1).id != TypeId::Null)
+      throw PlanUnsupported("nullif of " + arg_t(0).str() + " and " + arg_t(1).str() + " (the arguments must have one type)");
+    e.type = arg_t(0);
+    e.nullable = true;
+  } else if (f == "coalesce") {
+    if (n == 0) throw std::runtime_error("plan IR: coalesce takes at least one argument");
+    DataType t;
+    bool all_nullable = true;
+    for (size_t i = 0; i < n; i++) {
+      if (arg_t(i).id != TypeId::Null) {
+        if (t.id != TypeId::Null && arg_t(i) != t)
+          throw PlanUnsupported("coalesce of " + t.str() + " and " + arg_t(i).str() + " (the arguments must have one type)");
+        t = arg_t(i);
+      }
+      all_nullable = all_nullable && e.args[i]->nullable;
+    }
+    e.type = t;
+    e.nullable = all_nullable;
+  } else if (f == "character_length" || f == "octet_length") {
+    arity(1, 1);
+    need_utf8(0);
+    e.type = DataType(TypeId::Int32);
+    e.nullable = e.args[0]->nullable;
+  } else if (f == "starts_with" || f == "ends_with") {
+    arity(2, 2);
+    need_utf8(0);
+    need_utf8(1);
+    e.type = DataType(TypeId::Bool);
+    e.nullable = any_nullable();
+  } else if (f == "btrim" || f == "ltrim" || f == "rtrim") {
+    arity(1, 2);
+    need_utf8(0);
+    if (n == 2) need_utf8(1);
+    e.type = DataType(TypeId::Utf8);
+    e.nullable = any_nullable();
+  } else {
+    throw std::runtime_error("plan IR: unknown scalar function '" + f + "'");
+  }
+}
 
 inline ExprPtr parse_expr(const Json& j, const Schema& in) {
   auto e = std::make_shared<Expr>();
@@ -459,15 +560,7 @@ inline ExprPtr parse_expr(const Json& j, const Schema& in) {
     e->fn = j.at("fn").str();
     const Json& as = j.at("args");
     for (size_t i = 0; i < as.size(); i++) e->args.push_back(parse_expr(as.at(i), in));
-    if (e->fn == "date_part_year") {
-      // DataFusion: date_part('year', Date32) -> Int32 [EXT]
-      e->type = DataType(TypeId::Int32);
-    } else if (e->fn == "substr") {
-      e->type = DataType(TypeId::Utf8);
-    } else {
-      throw std::runtime_error("plan IR: unknown scalar function '" + e->fn + "'");
-    }
-    e->nullable = e->args.empty() ? false : e->args[0]->nullable;
+    type_scalar_fn(*e);
     return e;
   }
   throw std::runtime_error("plan IR: unrecognised expression node");
@@ -481,11 +574,6 @@ enum class AggMode : uint8_t { Partial, Final, FinalPartitioned, Single, SingleP
 
 inline bool agg_mode_consumes_states(AggMode m) { return m == AggMode::Final || m == AggMode::FinalPartitioned; }
 inline bool agg_mode_emits_states(AggMode m) { return m == AggMode::Partial; }
-
-// A plan the engine understands but does not run (e.g. statistical states laid out in an unknown way): B200_ERR_UNSUPPORTED
-struct PlanUnsupported : std::runtime_error {
-  explicit PlanUnsupported(const std::string& m) : std::runtime_error(m) {}
-};
 
 // The statistical aggregates: variance / standard deviation (one argument), covariance / correlation (two arguments)
 inline bool agg_is_stat(AggFn f) { return f >= AggFn::VarSamp; }

@@ -392,10 +392,24 @@ inline std::string expr_json(const Msg& e) {
         std::string part;
         if (args.size() != 2 || !literal_utf8(args[0], part)) throw Unsupported("date_part with a non-literal part");
         for (auto& ch : part) ch = (char)tolower((unsigned char)ch);
-        if (part != "year") throw Unsupported("date_part('" + part + "', ..) is not supported by the device engine");
-        return "{\"fn\":\"date_part_year\",\"args\":[" + expr_json(args[1]) + "]}";
+        static const char* const parts[] = {"year", "quarter", "month", "week", "day", "doy", "dow"};
+        bool known = false;
+        for (const char* p : parts) known = known || part == p;
+        if (!known) throw Unsupported("date_part('" + part + "', ..) is not supported by the device engine");
+        return "{\"fn\":\"date_part_" + part + "\",\"args\":[" + expr_json(args[1]) + "]}";
       }
       if (name == "substr" || name == "substring") return "{\"fn\":\"substr\",\"args\":" + exprs_json(args) + "}";
+      // the scalar functions of DESIGN §3 that make no new string bytes, under the names the function registry resolves
+      static const std::pair<const char*, const char*> fns[] = {
+          {"abs", "abs"},         {"round", "round"},       {"floor", "floor"},
+          {"ceil", "ceil"},       {"nullif", "nullif"},     {"coalesce", "coalesce"},
+          {"character_length", "character_length"},         {"char_length", "character_length"},
+          {"length", "character_length"},                   {"octet_length", "octet_length"},
+          {"starts_with", "starts_with"},                   {"ends_with", "ends_with"},
+          {"btrim", "btrim"},     {"trim", "btrim"},        {"ltrim", "ltrim"},
+          {"rtrim", "rtrim"}};
+      for (auto& kv : fns)
+        if (name == kv.first) return "{\"fn\":\"" + std::string(kv.second) + "\",\"args\":" + exprs_json(args) + "}";
       throw Unsupported("scalar function " + name + " is not supported by the device engine");
     }
     case 18: {  // PhysicalLikeExprNode { negated = 1, case_insensitive = 2, expr = 3, pattern = 4 } (:969-974)

@@ -185,7 +185,8 @@ __device__ __noinline__ bool like_match_dev(const uint8_t* s, uint32_t sn, const
   while (pi < pn && p[pi] == '%') pi++;
   return pi == pn;
 }
-__device__ __noinline__ int64_t year_of_days_dev(int64_t z) {
+// proleptic Gregorian civil date of a day number (days since 1970-01-01), and back (H. Hinnant's algorithms)
+__device__ __forceinline__ int64_t civil_from_days_dev(int64_t z, int64_t* month, int64_t* day) {
   z += 719468;
   int64_t era = (z >= 0 ? z : z - 146096) / 146097;
   int64_t doe = z - era * 146097;
@@ -194,7 +195,35 @@ __device__ __noinline__ int64_t year_of_days_dev(int64_t z) {
   int64_t doy = doe - (365 * yoe + yoe / 4 - yoe / 100);
   int64_t mp = (5 * doy + 2) / 153;
   int64_t m = mp < 10 ? mp + 3 : mp - 9;
+  *month = m;
+  *day = doy - (153 * mp + 2) / 5 + 1;
   return y + (m <= 2);
+}
+__device__ __forceinline__ int64_t jan1_days_dev(int64_t y) {  // day number of January 1st of year y
+  y -= 1;
+  const int64_t era = (y >= 0 ? y : y - 399) / 400;
+  const int64_t yoe = y - era * 400;
+  return era * 146097 + yoe * 365 + yoe / 4 - yoe / 100 + 306 - 719468;
+}
+__device__ __forceinline__ int64_t floor_mod7(int64_t v) { return ((v % 7) + 7) % 7; }
+// date_part(part, Date32): week is the ISO 8601 week (that of the week's Thursday), dow 0 = Sunday, doy 1..366
+__device__ __noinline__ int64_t date_part_dev(int64_t z, int part) {
+  int64_t m, d;
+  const int64_t y = civil_from_days_dev(z, &m, &d);
+  switch (part) {
+    case DP_YEAR: return y;
+    case DP_QUARTER: return (m - 1) / 3 + 1;
+    case DP_MONTH: return m;
+    case DP_DAY: return d;
+    case DP_DOY: return z - jan1_days_dev(y) + 1;
+    case DP_DOW: return floor_mod7(z + 4);  // 1970-01-01 was a Thursday
+    default: {
+      const int64_t thu = z - floor_mod7(z + 3) + 3;  // floor_mod7(z + 3) = ISO weekday - 1 (Monday = 0)
+      int64_t tm, td;
+      const int64_t ty = civil_from_days_dev(thu, &tm, &td);
+      return (thu - jan1_days_dev(ty)) / 7 + 1;
+    }
+  }
 }
 __device__ __noinline__ uint64_t hash_bytes_dev(const uint8_t* p, uint32_t len) { return hash_bytes(p, len); }
 
@@ -469,9 +498,161 @@ __device__ __forceinline__ uint32_t cmp_mask(int op, uint32_t lt, uint32_t gt) {
 }
 
 // ------------------------------------------------------------------------------------------------
+// Scalar functions (OP_ABS and up): rolled like the cold operations, in functions of their own so that
+// cold_op and the interpreter do not grow.  String bytes are only read for live rows (a NULL or
+// filtered row's view may point anywhere).
+// ------------------------------------------------------------------------------------------------
+__device__ __forceinline__ uint32_t utf8_seq_len(uint8_t c) { return c < 0x80 ? 1u : (c >> 5) == 6 ? 2u : (c >> 4) == 14 ? 3u : 4u; }
+// is the code point p[0..n) one of the code points of the UTF-8 string set[0..sn)?
+__device__ __noinline__ bool in_code_point_set(const uint8_t* p, uint32_t n, const uint8_t* set, uint32_t sn) {
+  for (uint32_t i = 0; i < sn;) {
+    const uint32_t k = utf8_seq_len(set[i]);
+    bool eq = k == n && i + k <= sn;
+    for (uint32_t j = 0; eq && j < n; j++) eq = set[i + j] == p[j];
+    if (eq) return true;
+    i += k;
+  }
+  return false;
+}
+__device__ __noinline__ StrRef trim_dev(StrRef s, int side, const uint8_t* set, uint32_t sn) {
+  uint32_t b = 0, e = s.len;
+  if (side != TRIM_TRAILING) {
+    while (b < e) {
+      const uint32_t k = utf8_seq_len(s.p[b]);
+      if (b + k > e || !in_code_point_set(s.p + b, k, set, sn)) break;
+      b += k;
+    }
+  }
+  if (side != TRIM_LEADING) {
+    while (e > b) {
+      uint32_t q = e - 1;
+      while (q > b && (s.p[q] & 0xC0) == 0x80) q--;
+      if (!in_code_point_set(s.p + q, e - q, set, sn)) break;
+      e = q;
+    }
+  }
+  s.p += b;
+  s.len = e - b;
+  return s;
+}
+// abs / round / floor / ceil
+__device__ __noinline__ void scalar_num_op(const Lane L, const uint32_t active, const int pc) {
+  const VInstr ins = PROG.code[pc];
+  const uint32_t va = fetch_valid(L, ins.a);
+  const uint32_t live = active & va;
+#pragma unroll 1
+  for (int r = 0; r < VM_R; r++) {
+    const bool lv = (live >> r) & 1;
+    if (ins.op == OP_ABS) {
+      if (ins.t == VK_F64) {
+        st1_f64(L, ins.dst, r, fabs(ld1_f64(L, ins.a, r)));
+      } else if (ins.t == VK_I128) {
+        const i128 a = ld1_i128(L, ins.a, r);
+        if (a == make_i128(0, 0x8000000000000000ull) && lv) raise(1);
+        st1_i128(L, ins.dst, r, a < 0 ? (i128)((u128)0 - (u128)a) : a);
+      } else {
+        const int64_t a = ld1_i64(L, ins.a, r);
+        const int64_t mn = ins.aux == PH_I8 ? INT8_MIN : ins.aux == PH_I16 ? INT16_MIN : ins.aux == PH_I32 ? INT32_MIN : INT64_MIN;
+        if (a == mn && lv) raise(1);  // DataFusion's abs is checked [EXT]
+        st1_i64(L, ins.dst, r, a < 0 ? (int64_t)(0 - (uint64_t)a) : a);
+      }
+    } else if (ins.op == OP_ROUND) {  // round_half_away_from_zero(x * f) / f, each step rounded once (no contraction)
+      const double x = ld1_f64(L, ins.a, r), f = __longlong_as_double((long long)PROG.imms[ins.imm].lo);
+      double o = x;  // NaN: the input, bits included (the device would return its canonical NaN)
+      if (x != x) {
+      } else if (ins.aux == PH_F32) o = (double)__fdiv_rn(roundf(__fmul_rn((float)x, (float)f)), (float)f);
+      else o = __ddiv_rn(round(__dmul_rn(x, f)), f);
+      st1_f64(L, ins.dst, r, o);
+    } else {
+      const double x = ld1_f64(L, ins.a, r);
+      st1_f64(L, ins.dst, r, ins.op == OP_FLOOR ? floor(x) : ceil(x));
+    }
+  }
+  store_valid(L, ins.dst, va);
+}
+// nullif(a, b): a, NULL where b is not NULL and a = b by the engine's equality (floats: bitwise, i.e. total order)
+__device__ __noinline__ void scalar_nullif_op(const Lane L, const uint32_t active, const int pc) {
+  const VInstr ins = PROG.code[pc];
+  const uint32_t va = fetch_valid(L, ins.a), vb = fetch_valid(L, ins.b);
+  const uint32_t live = active & va & vb;
+  uint32_t vout = va, bmask = 0;
+#pragma unroll 1
+  for (int r = 0; r < VM_R; r++) {
+    bool eq = false;
+    if (ins.t == VK_STR) {
+      const StrRef a = ld1_str(L, ins.a, r);
+      if ((live >> r) & 1) eq = str_eq(a, ld1_str(L, ins.b, r));
+      st1_str(L, ins.dst, r, a);
+    } else if (ins.t == VK_I128) {
+      const i128 a = ld1_i128(L, ins.a, r);
+      eq = a == ld1_i128(L, ins.b, r);
+      st1_i128(L, ins.dst, r, a);
+    } else if (ins.t == VK_F64) {
+      const double a = ld1_f64(L, ins.a, r);
+      eq = __double_as_longlong(a) == __double_as_longlong(ld1_f64(L, ins.b, r));
+      st1_f64(L, ins.dst, r, a);
+    } else {
+      const int64_t a = ld1_i64(L, ins.a, r);
+      eq = a == ld1_i64(L, ins.b, r);
+      if (ins.t == VK_BOOL) bmask |= (a ? 1u : 0u) << r;
+      else st1_i64(L, ins.dst, r, a);
+    }
+    if (((vb >> r) & 1) && eq) vout &= ~(1u << r);
+  }
+  if (ins.t == VK_BOOL) store_bool(L, ins.dst, bmask);
+  store_valid(L, ins.dst, vout);
+}
+// character / octet length, starts / ends_with, the trims
+__device__ __noinline__ void scalar_str_op(const Lane L, const uint32_t active, const int pc) {
+  const VInstr ins = PROG.code[pc];
+  const uint32_t va = fetch_valid(L, ins.a);
+  const uint32_t vb = ins.b.kind != OPD_NONE ? fetch_valid(L, ins.b) : 0xFFFFFFFFu;
+  const uint32_t live = active & va & vb;
+  uint32_t bmask = 0;
+#pragma unroll 1
+  for (int r = 0; r < VM_R; r++) {
+    const bool lv = (live >> r) & 1;
+    StrRef a = ld1_str(L, ins.a, r);
+    if (ins.op == OP_CHAR_LENGTH || ins.op == OP_OCTET_LENGTH) {
+      int64_t n = a.len;
+      if (ins.op == OP_CHAR_LENGTH) {
+        n = 0;
+        if (lv)
+          for (uint32_t i = 0; i < a.len; i++) n += (a.p[i] & 0xC0) != 0x80;
+      }
+      st1_i64(L, ins.dst, r, n);
+    } else if (ins.op == OP_TRIM) {
+      if (lv) a = trim_dev(a, ins.aux, (const uint8_t*)PROG.imms[ins.imm].lo, (uint32_t)PROG.imms[ins.imm].hi);
+      st1_str(L, ins.dst, r, a);
+    } else {  // OP_STARTS_WITH / OP_ENDS_WITH
+      bool hit = false;
+      if (lv) {
+        const StrRef b = ld1_str(L, ins.b, r);
+        if (b.len <= a.len) {
+          const uint8_t* p = a.p + (ins.op == OP_ENDS_WITH ? a.len - b.len : 0);
+          hit = true;
+          for (uint32_t i = 0; hit && i < b.len; i++) hit = p[i] == b.p[i];
+        }
+      }
+      bmask |= (hit ? 1u : 0u) << r;
+    }
+  }
+  if (ins.op == OP_STARTS_WITH || ins.op == OP_ENDS_WITH) store_bool(L, ins.dst, bmask);
+  store_valid(L, ins.dst, va & vb);
+}
+
+// ------------------------------------------------------------------------------------------------
 // Cold operations: one rolled loop over the thread's rows; every body exists once in the binary.
 // ------------------------------------------------------------------------------------------------
+template <bool SFN>
 __device__ __noinline__ void cold_op(const Lane L, const uint32_t active, const int pc) {
+  if (SFN && PROG.code[pc].op >= OP_ABS) {  // the scalar functions (see run_generic)
+    const uint8_t op = PROG.code[pc].op;
+    if (op <= OP_CEIL) scalar_num_op(L, active, pc);
+    else if (op == OP_NULLIF) scalar_nullif_op(L, active, pc);
+    else scalar_str_op(L, active, pc);
+    return;
+  }
   const VInstr ins = PROG.code[pc];
   uint32_t va = 0xFFFFFFFFu, vb = 0xFFFFFFFFu;
   if (ins.flags & IF_NULLCHK) {
@@ -631,7 +812,7 @@ __device__ __noinline__ void cold_op(const Lane L, const uint32_t active, const 
         bmask |= ((ins.aux ? !hit : hit) ? 1u : 0u) << r;
         break;
       }
-      case OP_YEAR: st1_i64(L, ins.dst, r, year_of_days_dev(ld1_i64(L, ins.a, r))); break;
+      case OP_DATE_PART: st1_i64(L, ins.dst, r, date_part_dev(ld1_i64(L, ins.a, r), ins.aux)); break;
       case OP_SUBSTR: {
         StrRef a = ld1_str(L, ins.a, r);
         int64_t st = ld1_i64(L, ins.b, r);
@@ -1274,6 +1455,10 @@ __device__ __forceinline__ void mf_pack8(const Lane L, const uint32_t active, co
 // The interpreter: one pass over the expression program for the R rows this thread owns.
 // All branches are warp-uniform (driven by the program, not by data).
 // ------------------------------------------------------------------------------------------------
+// SFN: the program holds scalar-function ops (OP_ABS and up).  Only the kernel variants compiled with it reach their
+// functions, through a cold_op of their own, so every other variant's call graph -- and with it ptxas's register
+// allocation, which spans a kernel's whole call graph -- stays as without them.
+template <bool SFN>
 __device__ __noinline__ uint32_t run_generic(const Lane L, uint32_t active, const int pc) {
   const uint32_t head = *(const uint32_t*)&PROG.code[pc];  // op | t<<8 | flags<<16 | aux<<24
   const uint32_t op = head & 0xFF, t = (head >> 8) & 0xFF;
@@ -1296,7 +1481,7 @@ __device__ __noinline__ uint32_t run_generic(const Lane L, uint32_t active, cons
       if (t == VK_I64 || t == VK_BOOL) op_cmp_i64(L, active, pc);
       else if (t == VK_I128) op_cmp_i128(L, active, pc);
       else if (t == VK_F64) op_cmp_f64(L, active, pc);
-      else cold_op(L, active, pc);
+      else cold_op<SFN>(L, active, pc);
       if ((head >> 16) & IF_FILTER) {  // fused FilterExec conjunct evaluated through a scratch bool register
         const Operand d = PROG.code[pc].dst;
         active &= fetch_bool(L, d) & fetch_valid(L, d);
@@ -1316,7 +1501,7 @@ __device__ __noinline__ uint32_t run_generic(const Lane L, uint32_t active, cons
     case OP_STR_PACK8: {
       const Operand a = PROG.code[pc].a;
       if (a.kind == OPD_COL && PROG.cols[a.idx].phys == PH_UTF8) op_pack8_utf8(L, active, pc);
-      else cold_op(L, active, pc);
+      else cold_op<SFN>(L, active, pc);
       break;
     }
     case OP_HASH:
@@ -1327,11 +1512,12 @@ __device__ __noinline__ uint32_t run_generic(const Lane L, uint32_t active, cons
     case OP_SELECT:
     case OP_MOV: cold_move(L, pc); break;
     case OP_NOP: break;
-    default: cold_op(L, active, pc); break;
+    default: cold_op<SFN>(L, active, pc); break;
   }
   return active;
 }
 
+template <bool SFN>
 __device__ __forceinline__ uint32_t run_program(const Lane L, uint32_t active, const MicroOp* mops, int n_instr) {
   for (int pc = 0; pc < n_instr; pc++) {
     const MicroOp* m = &mops[pc];
@@ -1347,7 +1533,7 @@ __device__ __forceinline__ uint32_t run_program(const Lane L, uint32_t active, c
         ((uint32_t*)(L.regs + m->d_off))[L.tid] = m->op == OP_AND ? (x & y) : (x | y);
         break;
       }
-      default: active = run_generic(L, active, pc); break;
+      default: active = run_generic<SFN>(L, active, pc); break;
     }
   }
   return active;
@@ -2423,7 +2609,7 @@ __device__ __forceinline__ void mom_reg_flush(double (&acc)[G][VM_MAX_MOM][3], M
 // ------------------------------------------------------------------------------------------------
 // The kernel
 // ------------------------------------------------------------------------------------------------
-template <int SINK, int G, bool ADD_ONLY, bool SIDE, bool MOM = false>
+template <int SINK, int G, bool ADD_ONLY, bool SIDE, bool MOM = false, bool SFN = false>
 __global__ void __launch_bounds__(512, 1) pipeline_kernel() {
   extern __shared__ __align__(128) uint8_t smem[];
   __shared__ __align__(8) uint64_t full_bar[VM_MAX_STAGES];
@@ -2526,7 +2712,7 @@ __global__ void __launch_bounds__(512, 1) pipeline_kernel() {
 #pragma unroll
     FOR_R if (r * B + tid < rows) active |= 1u << r;
     {
-      active = run_program(L, active, mops, n_instr);
+      active = run_program<SFN>(L, active, mops, n_instr);
     }
     if (MOM) {
       if (SINK == SINK_AGG_GLOBAL) active = sink_mom_global(L, active);
@@ -2613,17 +2799,17 @@ struct GateLock {
   }
 };
 
-template <int SINK, int G, bool ADD_ONLY, bool SIDE = false, bool MOM = false>
+template <bool SFN, int SINK, int G, bool ADD_ONLY, bool SIDE = false, bool MOM = false>
 static cudaError_t launch_one(int grid, int block, size_t smem, cudaStream_t st) {
   // the opt-in to large dynamic shared memory is per (function, device) and sticky: raise it only when needed
   static size_t granted[64] = {0};
   const int dev = GateLock::current_device() & 63;
   if (smem > granted[dev]) {
-    cudaError_t e = cudaFuncSetAttribute(pipeline_kernel<SINK, G, ADD_ONLY, SIDE, MOM>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    cudaError_t e = cudaFuncSetAttribute(pipeline_kernel<SINK, G, ADD_ONLY, SIDE, MOM, SFN>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
     granted[dev] = smem;
   }
-  pipeline_kernel<SINK, G, ADD_ONLY, SIDE, MOM><<<grid, block, smem, st>>>();
+  pipeline_kernel<SINK, G, ADD_ONLY, SIDE, MOM, SFN><<<grid, block, smem, st>>>();
   return cudaGetLastError();
 }
 
@@ -2636,27 +2822,34 @@ bool pipeline_add_only(const Program& P, int grid, int block) {
   return add_only;
 }
 
+template <bool SFN>
+static cudaError_t launch_variant(const Program& P, int reg_groups, int grid, int block, size_t smem, cudaStream_t st) {
+  const bool add_only = pipeline_add_only(P, grid, block);
+  if (P.mom_pass) {  // pass 2 of VAR / STDDEV / COVAR / CORR
+    if (P.sink == SINK_AGG_GLOBAL) return launch_one<SFN, SINK_AGG_GLOBAL, 1, true, false, true>(grid, block, smem, st);
+    return reg_groups <= 1 ? launch_one<SFN, SINK_AGG_REG, 1, false, false, true>(grid, block, smem, st)
+                           : launch_one<SFN, SINK_AGG_REG, VM_REG_GROUPS, false, false, true>(grid, block, smem, st);
+  }
+  switch (P.sink) {
+    case SINK_MATERIALIZE: return launch_one<SFN, SINK_MATERIALIZE, 1, true>(grid, block, smem, st);
+    case SINK_AGG_GLOBAL: return launch_one<SFN, SINK_AGG_GLOBAL, 1, true>(grid, block, smem, st);
+    default:
+      // string / UInt64 MIN / MAX are never add-only
+      if (P.has_side_acc) return reg_groups <= 1 ? launch_one<SFN, SINK_AGG_REG, 1, false, true>(grid, block, smem, st) : launch_one<SFN, SINK_AGG_REG, VM_REG_GROUPS, false, true>(grid, block, smem, st);
+      if (reg_groups <= 1) return add_only ? launch_one<SFN, SINK_AGG_REG, 1, true>(grid, block, smem, st) : launch_one<SFN, SINK_AGG_REG, 1, false>(grid, block, smem, st);
+      return add_only ? launch_one<SFN, SINK_AGG_REG, VM_REG_GROUPS, true>(grid, block, smem, st) : launch_one<SFN, SINK_AGG_REG, VM_REG_GROUPS, false>(grid, block, smem, st);
+  }
+}
+
 cudaError_t launch_pipeline(const Program& P, int reg_groups, int grid, int block, size_t smem, cudaStream_t st) {
   GateLock gate(st);
   if (gate.err != cudaSuccess) return gate.err;
   // stream-ordered upload of the program into constant memory
   cudaError_t e = cudaMemcpyToSymbolAsync(c_prog, &P, sizeof(Program), 0, cudaMemcpyHostToDevice, st);
   if (e != cudaSuccess) return e;
-  const bool add_only = pipeline_add_only(P, grid, block);
-  if (P.mom_pass) {  // pass 2 of VAR / STDDEV / COVAR / CORR
-    if (P.sink == SINK_AGG_GLOBAL) return launch_one<SINK_AGG_GLOBAL, 1, true, false, true>(grid, block, smem, st);
-    return reg_groups <= 1 ? launch_one<SINK_AGG_REG, 1, false, false, true>(grid, block, smem, st)
-                           : launch_one<SINK_AGG_REG, VM_REG_GROUPS, false, false, true>(grid, block, smem, st);
-  }
-  switch (P.sink) {
-    case SINK_MATERIALIZE: return launch_one<SINK_MATERIALIZE, 1, true>(grid, block, smem, st);
-    case SINK_AGG_GLOBAL: return launch_one<SINK_AGG_GLOBAL, 1, true>(grid, block, smem, st);
-    default:
-      // string / UInt64 MIN / MAX are never add-only
-      if (P.has_side_acc) return reg_groups <= 1 ? launch_one<SINK_AGG_REG, 1, false, true>(grid, block, smem, st) : launch_one<SINK_AGG_REG, VM_REG_GROUPS, false, true>(grid, block, smem, st);
-      if (reg_groups <= 1) return add_only ? launch_one<SINK_AGG_REG, 1, true>(grid, block, smem, st) : launch_one<SINK_AGG_REG, 1, false>(grid, block, smem, st);
-      return add_only ? launch_one<SINK_AGG_REG, VM_REG_GROUPS, true>(grid, block, smem, st) : launch_one<SINK_AGG_REG, VM_REG_GROUPS, false>(grid, block, smem, st);
-  }
+  bool sfn = false;
+  for (int i = 0; i < P.n_instr; i++) sfn = sfn || P.code[i].op >= OP_ABS;
+  return sfn ? launch_variant<true>(P, reg_groups, grid, block, smem, st) : launch_variant<false>(P, reg_groups, grid, block, smem, st);
 }
 
 // exactness bound of the fused kernel's int64 partials: |addend| < 2^40 and (tiles are claimed

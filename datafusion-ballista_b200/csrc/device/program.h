@@ -62,7 +62,7 @@ enum VOp : uint8_t {
   OP_SELECT,                           // dst = a(bool) ? b : dst      (CASE lowering)
   OP_MOV,                              // dst = a
   OP_LIKE,                             // a: STR, imm: immediate index of pattern; aux: 1 = negated
-  OP_YEAR,                             // a: I64 days -> I64 year
+  OP_DATE_PART,                        // a: I64 days -> I64 field; aux = DatePart
   OP_SUBSTR,                           // a: STR, b: I64 start, imm: immediate idx of len or -1
   OP_HASH,                             // dst(I64) = hash(a)                 (first key column)
   OP_HASH_COMBINE,                     // dst(I64) = a valid ? combine(hash(a), dst) : dst
@@ -71,8 +71,19 @@ enum VOp : uint8_t {
   OP_DEC_MUL_LIT_MINUS,                // fused: dst = a * (imm - b)   [I128 x (I64-range)] checked
   OP_DEC_MUL_LIT_PLUS,                 // fused: dst = a * (imm + b)
   OP_MADD_I64,                         // dst = a + b * imm64 (imm = immediate index); wrapping
-  OP_STR_PACK8                         // dst(I64) = len<<imm | bytes of a string of <= aux bytes (imm = 56/aux = 7 or imm = 24/aux = 3); longer -> pack_overflow
+  OP_STR_PACK8,                        // dst(I64) = len<<imm | bytes of a string of <= aux bytes (imm = 56/aux = 7 or imm = 24/aux = 3); longer -> pack_overflow
+  // scalar functions (cold: scalar_num_op / scalar_nullif_op / scalar_str_op in pipeline.cu); every op from OP_ABS on is one
+  OP_ABS,                              // t = VK_I64 | VK_F64 | VK_I128; aux = Phys of a signed integer (its minimum raises overflow)
+  OP_ROUND,                            // t = VK_F64; imm = immediate idx of the factor f; aux = PH_F32 for f32 arithmetic
+  OP_FLOOR, OP_CEIL,                   // t = VK_F64
+  OP_NULLIF,                           // t = operand VK; dst = a, NULL where a = b (floats: bitwise, i.e. total order)
+  OP_CHAR_LENGTH, OP_OCTET_LENGTH,     // a: STR -> I64
+  OP_STARTS_WITH, OP_ENDS_WITH,        // a, b: STR -> BOOL
+  OP_TRIM                              // a: STR -> STR view; aux = TrimSide; imm = immediate idx of the set (" " by default)
 };
+
+enum DatePart : uint8_t { DP_YEAR = 0, DP_QUARTER, DP_MONTH, DP_WEEK, DP_DAY, DP_DOY, DP_DOW };
+enum TrimSide : uint8_t { TRIM_BOTH = 0, TRIM_LEADING, TRIM_TRAILING };
 
 enum InstrFlags : uint8_t {
   IF_NULLCHK = 1,   // some operand may be NULL: compute validity

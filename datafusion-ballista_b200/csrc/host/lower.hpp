@@ -195,17 +195,8 @@ class PipelineBuilder {
         return r;
       }
       case Expr::Fn: {
-        if (e.fn == "date_part_year") {
-          ColRef a = compile(*e.args[0]);
-          ColRef r = new_reg(e.type, a.nullable);
-          VInstr ins = blank(OP_YEAR, VK_I64);
-          ins.a = resolve(a);
-          ins.dst = r.op;
-          if (a.nullable) ins.flags |= IF_NULLCHK;
-          emit(ins);
-          release(a);
-          return r;
-        }
+        const int part = date_part_index(e.fn);
+        if (part >= 0) return unary_fn(e, OP_DATE_PART, VK_I64, (uint8_t)part, 0);
         if (e.fn == "substr") {
           ColRef a = compile(*e.args[0]);
           ColRef s = compile(*e.args[1]);
@@ -226,10 +217,137 @@ class PipelineBuilder {
           release(s);
           return r;
         }
-        throw EngineError(B200_ERR_UNSUPPORTED, "scalar function " + e.fn);
+        return compile_scalar_fn(e);
       }
     }
     throw EngineError(B200_ERR_UNSUPPORTED, "expression kind");
+  }
+
+  // one-operand function: dst = op(a); string results are views into a's bytes
+  ColRef unary_fn(const Expr& e, uint8_t op, uint8_t t, uint8_t aux, int32_t imm) {
+    ColRef a = compile(*e.args[0]);
+    ColRef r = new_reg(e.type, a.nullable);
+    r.keep = a.keep;
+    VInstr ins = blank(op, t);
+    ins.a = resolve(a);
+    ins.dst = r.op;
+    ins.aux = aux;
+    ins.imm = imm;
+    if (a.nullable) ins.flags |= IF_NULLCHK;
+    emit(ins);
+    release(a);
+    return r;
+  }
+  ColRef null_of(const DataType& t) {
+    LitValue l;
+    l.is_null = true;
+    return literal(t, l);
+  }
+  // a literal operand of a function, which travels as an immediate; NULL gives a NULL result
+  const Expr& literal_arg(const Expr& e, size_t i, const char* what) {
+    if (e.args[i]->kind != Expr::Lit) throw EngineError(B200_ERR_UNSUPPORTED, e.fn + ": " + what + " must be a literal");
+    return *e.args[i];
+  }
+
+  // the scalar functions of DESIGN.md §3 besides date_part and substr; typing (plan.hpp) has checked the argument types
+  ColRef compile_scalar_fn(const Expr& e) {
+    const std::string& f = e.fn;
+    if (f == "abs") {
+      const DataType& t = e.args[0]->type;
+      if (t.is_unsigned_int()) return compile(*e.args[0]);
+      return unary_fn(e, OP_ABS, vk_of(t), t.is_signed_int() ? phys_of(t) : 0, 0);
+    }
+    if (f == "floor" || f == "ceil") return unary_fn(e, f == "floor" ? OP_FLOOR : OP_CEIL, VK_F64, 0, 0);
+    if (f == "round") {
+      int64_t n = 0;
+      if (e.args.size() > 1) {
+        const Expr& d = literal_arg(e, 1, "the digit count");
+        if (d.lit.is_null) return null_of(e.type);
+        n = d.lit.i;
+      }
+      if (n > 22 || n < -22) throw EngineError(B200_ERR_UNSUPPORTED, "round to " + std::to_string(n) + " digits is not supported (|digits| <= 22)");
+      double p = 1;
+      for (int64_t i = 0; i < (n < 0 ? -n : n); i++) p *= 10;  // exact: 10^22 is the largest power of ten binary64 holds
+      const bool f32 = e.type.id == TypeId::Float32;
+      LitValue fl;
+      fl.f = f32 ? (n >= 0 ? (double)(float)p : (double)(1.0f / (float)p)) : (n >= 0 ? p : 1.0 / p);
+      const int fi = literal(DataType(TypeId::Float64), fl).op.idx;
+      return unary_fn(e, OP_ROUND, VK_F64, f32 ? PH_F32 : 0, fi);
+    }
+    if (f == "character_length" || f == "octet_length") return unary_fn(e, f == "octet_length" ? OP_OCTET_LENGTH : OP_CHAR_LENGTH, VK_STR, 0, 0);
+    if (f == "btrim" || f == "ltrim" || f == "rtrim") {
+      int set = -1;
+      if (e.args.size() > 1) {
+        const Expr& s = literal_arg(e, 1, "the character set");
+        if (s.lit.is_null) return null_of(e.type);
+        set = string_imm(s.lit.s);
+      } else {
+        set = string_imm(" ");  // DataFusion's default removes spaces only, not all whitespace [EXT]
+      }
+      return unary_fn(e, OP_TRIM, VK_STR, f == "btrim" ? TRIM_BOTH : f == "ltrim" ? TRIM_LEADING : TRIM_TRAILING, set);
+    }
+    if (f == "coalesce") {
+      // the CASE lowering's shape, CASE WHEN a0 IS NOT NULL THEN a0 ... ELSE a_last END, with every argument compiled
+      // once: dst = a_last, then from the back dst = a_i where a_i is not NULL (OP_SELECT)
+      if (e.args.size() == 1) return cast_to(compile(*e.args[0]), e.type);
+      ColRef dst = new_reg(e.type, true);
+      pin(dst);
+      {
+        ColRef v = cast_to(compile(*e.args.back()), e.type);
+        VInstr ins = blank(OP_MOV, vk_of(e.type));
+        ins.a = resolve(v);
+        ins.dst = dst.op;
+        ins.flags = IF_NULLCHK;
+        emit(ins);
+        dst.keep.insert(dst.keep.end(), v.keep.begin(), v.keep.end());
+        release(v);
+      }
+      for (size_t i = e.args.size() - 1; i-- > 0;) {
+        ColRef v = cast_to(compile(*e.args[i]), e.type);
+        pin(v);
+        ColRef c = new_reg(DataType(TypeId::Bool), false);
+        VInstr t = blank(OP_IS_NOT_NULL, VK_BOOL);
+        t.a = resolve(v);
+        t.dst = c.op;
+        emit(t);
+        unpin(v);
+        VInstr ins = blank(OP_SELECT, vk_of(e.type));
+        ins.a = c.op;
+        ins.b = resolve(v);
+        ins.dst = dst.op;
+        ins.flags = IF_NULLCHK;
+        emit(ins);
+        dst.keep.insert(dst.keep.end(), v.keep.begin(), v.keep.end());
+        release(c);
+        release(v);
+      }
+      unpin(dst);
+      return dst;
+    }
+    if (f == "nullif" || f == "starts_with" || f == "ends_with") {
+      ColRef a = compile(*e.args[0]);
+      pin(a);
+      ColRef b = compile(*e.args[1]);
+      unpin(a);
+      const bool nullif = f == "nullif";
+      if (nullif && (a.type.id == TypeId::Null || b.type.id == TypeId::Null)) {
+        release(b);
+        if (a.type.id == TypeId::Null) return null_of(e.type);
+        return a;  // nullif(a, NULL) = a
+      }
+      ColRef r = new_reg(e.type, nullif || a.nullable || b.nullable);
+      if (nullif) r.keep = a.keep;
+      VInstr ins = blank(nullif ? OP_NULLIF : f == "starts_with" ? OP_STARTS_WITH : OP_ENDS_WITH, nullif ? vk_of(a.type) : VK_STR);
+      ins.a = resolve(a);
+      ins.b = resolve(b);
+      ins.dst = r.op;
+      ins.flags = IF_NULLCHK;
+      emit(ins);
+      release(a);
+      release(b);
+      return r;
+    }
+    throw EngineError(B200_ERR_UNSUPPORTED, "scalar function " + f);
   }
 
   // hash of key columns in the structure of create_hashes (see csrc/common/hash.hpp)

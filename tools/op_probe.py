@@ -1,7 +1,7 @@
 """One big instance of one operator, so that `ncu -k regex:<kernel> -c 1` lands on a representative launch, and so that the
 engine's own CUDA-event timing (b200_engine_kernel_stats) can be read for the same launch without a profiler attached.
 
-  python tools/op_probe.py join|partition|groupby|groupby_small|filter|parquet|q1 [msf]
+  python tools/op_probe.py join|partition|groupby|groupby_small|filter|parquet|q1|minmax_str|stats|nlj|scalar [msf]
 
   join       orders (build, 15 M rows at SF10) |x| lineitem (probe, 60 M rows) on the order key      -> join_build2 / join_probe2
   partition  lineitem (4 columns, 48 B/row) hash-repartitioned on l_orderkey into 8 partitions       -> part_tile_hist / part_tile_scatter
@@ -15,6 +15,10 @@ engine's own CUDA-event timing (b200_engine_kernel_stats) can be read for the sa
              (each result checked against the CPU oracle unless ORACLE=0)
   stats      STDDEV(l_extendedprice), CORR(l_quantity, l_extendedprice) and AVG of both, by (l_returnflag, l_linestatus)
              (4 groups) and by l_suppkey (100 k groups at SF10)           -> pipeline_agg_* and pipeline_agg_*_pass2
+  scalar     ProjectionExec over lineitem of (a) date_part('year', l_shipdate), (b) date_part('month' / 'week', ..),
+             (c) character_length(l_shipinstruct) and btrim(l_shipmode), (d) round(CAST(l_extendedprice AS DOUBLE), 1)
+             -> pipeline_materialize; each result checked at SF1: (a) against the CPU oracle, the others (which the oracle
+             does not compute) against pyarrow.compute / numpy restatements of DESIGN §6 (vi)
   nlj        NestedLoopJoinExec: lineitem against one build row (a scalar subquery) next to the same comparison
              through fast_filter_kernel, and a band join of orders (msf 1000) against 10,000 build rows    -> nlj_count / nlj_write
 """
@@ -278,6 +282,59 @@ elif op == "nlj":
     report["b_band_join"]["matches_oracle_at_sf0.01_1000_build_rows"] = True
     print(json.dumps({op: report, "lineitem_rows": n}, indent=1))
     oracle.close()
+elif op == "scalar":
+    import subprocess
+    import numpy as np
+    import pyarrow.compute as pc
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    import oracle_ffi
+    from ballista_b200 import driver
+    smi = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
+    cols = ["l_extendedprice", "l_shipdate", "l_shipinstruct", "l_shipmode"]
+    scan = tpch.table_scan("lineitem", cols)
+    cases = {
+        "a_year": [(P.fn("date_part_year", c("l_shipdate")), "r")],
+        "b_month_week": [(P.fn("date_part_month", c("l_shipdate")), "m"), (P.fn("date_part_week", c("l_shipdate")), "w")],
+        "c_length_btrim": [(P.fn("character_length", c("l_shipinstruct")), "n"), (P.fn("btrim", c("l_shipmode")), "t")],
+        "d_round": [(P.fn("round", P.cast(c("l_extendedprice"), "f64"), P.lit_i64(1)), "r")],
+    }
+
+    def stages(exprs):
+        return [P.Stage(1, P.shuffle_writer(P.project(exprs, scan), 1))]
+
+    n = load("lineitem", cols)
+    report = {"gpu": smi, "lineitem_rows": n,
+              "bytes": "the kernel timer's count: values / offsets of the referenced columns and the materialised outputs "
+                       "(Utf8 results as 16-byte views); the Utf8 characters read by (c) come on top"}
+    for name, exprs in cases.items():
+        run(stages(exprs), [1])   # warm-up
+        eng.kernel_stats(reset=True)
+        run(stages(exprs), [1])
+        ks = {k: v for k, v in eng.kernel_stats(reset=True).items() if k.startswith("pipeline")}
+        report[name] = {k: {"kernel_ms_per_run": round(v["ms"] / reps, 3), "bytes_per_row": round(v["bytes"] / (reps * n), 2),
+                            "GB_per_s": round(v["bytes"] / (v["ms"] * 1e-3) / 1e9, 1)} for k, v in ks.items() if v["ms"] > 0}
+    # correctness at SF1
+    m1 = 1000
+    n1 = eng.tpch_table_rows("lineitem", m1)
+    eng.drop_table("lineitem")
+    eng.tpch_generate("lineitem", m1, 0, 0, n1, cols)
+    oracle = oracle_ffi.OracleEngine()
+    oracle.tpch_generate("lineitem", m1, 0, 0, n1, cols)
+    src = oracle.export_table("lineitem", 0)
+    got = {k: driver.run_stages(eng, stages(e), f"chk-{k}") for k, e in cases.items()}
+    assert got["a_year"].column("r").equals(driver.run_stages(oracle, stages(cases["a_year"]), "chk-year").column("r"))
+    d = src.column("l_shipdate")
+    assert got["b_month_week"].column("m").to_pylist() == pc.month(d).to_pylist()
+    assert got["b_month_week"].column("w").to_pylist() == pc.iso_week(d).to_pylist()
+    assert got["c_length_btrim"].column("n").to_pylist() == pc.utf8_length(src.column("l_shipinstruct")).to_pylist()
+    assert got["c_length_btrim"].column("t").to_pylist() == pc.utf8_trim(src.column("l_shipmode"), " ").to_pylist()
+    x = src.column("l_extendedprice").cast("float64").to_numpy() * 10.0   # round half away from zero, f = 10
+    t = np.trunc(x)
+    want = (t + np.where(np.abs(x - t) >= 0.5, np.sign(x), 0.0)) / 10.0
+    assert np.array_equal(got["d_round"].column("r").to_numpy().view(np.int64), want.view(np.int64))
+    report["checked_at_sf1"] = {"rows": n1, "a_year": "= CPU oracle", "others": "= pyarrow.compute / numpy, bit for bit"}
+    oracle.close()
+    print(json.dumps({op: report}, indent=1))
 else:
     raise SystemExit(__doc__)
 print(json.dumps({op: eng.kernel_stats()}, indent=1))
