@@ -75,7 +75,6 @@ struct b200_engine {
   std::mutex mu;
   std::map<std::string, std::map<int, DevBatchPtr>> tables;
   std::map<ShuffleKey, std::vector<Piece>> shuffle;
-  std::map<ShuffleKey, DevBatchPtr> packed_cache;  // b200_partition_device_buffers: exchange-layout copies handed out by pointer
   std::atomic<uint64_t> launches{0};
   std::atomic<uint64_t> n_fused{0}, n_fused_static{0}, n_vm{0}, n_groupby{0}, n_groupby_pf{0}, n_fastfilter{0};  // pipelines per kernel family (b200_engine_counter)
   int64_t batch_size = 8192;
@@ -4716,7 +4715,6 @@ void b200_engine_destroy(b200_engine* e) {
   cudaStreamSynchronize(e->stream);
   e->tables.clear();
   e->shuffle.clear();
-  e->packed_cache.clear();
   cudaStreamSynchronize(e->stream);
   for (auto& sl : e->nslot) {
     if (sl.pinned) cudaFreeHost(sl.pinned);
@@ -5339,120 +5337,6 @@ int64_t b200_partition_rows(b200_engine* e, const char* job_id, int64_t stage_id
   return n;
 }
 
-int b200_partition_device_buffers(b200_engine* e, const char* job_id, int64_t stage_id, int out_partition, b200_device_buffer* out, int cap, int* n_out,
-                                  int64_t* n_rows) {
-  return guard([&] {
-    CUDA_CHECK(cudaSetDevice(e->device));
-    std::vector<std::pair<DevBatchPtr, std::pair<int64_t, int64_t>>> pieces;
-    {
-      std::lock_guard<std::mutex> g(e->mu);
-      auto it = e->shuffle.find(ShuffleKey{job_id, stage_id, out_partition});
-      if (it == e->shuffle.end()) throw EngineError(B200_ERR_NOT_FOUND, "no such shuffle partition");
-      for (auto& p : it->second) pieces.push_back({p.batch, {p.r0, p.r1}});
-    }
-    Exec x{e, nullptr, nullptr};
-    Runner r{x, job_id};
-    Schema s;
-    for (auto& c : pieces[0].first->cols) s.push_back(Field{c.name, c.type, true});
-    DevBatchPtr cat = r.concat_slices(pieces, s);
-    // exchange layout per column: [validity bytes (n) or empty][values | offsets(n+1, rebased)][chars]
-    auto packed = std::make_shared<DevBatch>();
-    packed->n = cat->n;
-    int k = 0;
-    // Utf8 columns that are row slices of a larger column: rebase the offsets on the device and learn
-    // the chars range of every such column with ONE read-back (not a view round trip per column)
-    struct Pending { size_t col; int out_chars; };
-    std::vector<Pending> pending;
-    DevPtr fl = dev_alloc(8 * (cat->cols.size() + 1), x.st());
-    for (auto& c0 : cat->cols) {
-      DevColumn c = c0.phys == PH_STRVIEW ? as_utf8(x, c0) : c0;
-      if (k + 3 > cap) throw EngineError(B200_ERR_INVALID, "buffer array too small");
-      out[k++] = b200_device_buffer{(void*)c.valid, c.valid ? (uint64_t)c.n : 0};
-      if (c.phys == PH_UTF8) {
-        if (c.n == 0) {
-          DevColumn v = as_views(x, c);
-          c = as_utf8(x, v);
-        } else if (c0.phys != PH_STRVIEW) {  // as_utf8 output already starts at 0 and knows its length
-          DevPtr ro = dev_alloc((size_t)(c.n + 1) * 4 + 64, x.st());
-          launch_rebase_offsets((const int32_t*)c.data, c.n + 1, (int32_t*)ro->ptr, (int32_t*)fl->ptr + 2 * pending.size(), x.st());
-          x.count();
-          c.data = (const uint8_t*)ro->ptr;
-          c.keep.push_back(ro);
-          pending.push_back(Pending{packed->cols.size(), k + 1});
-        }
-        out[k++] = b200_device_buffer{(void*)c.data, (uint64_t)(c.n + 1) * 4};
-        out[k++] = b200_device_buffer{(void*)c.chars, (uint64_t)std::max<int64_t>(c.chars_bytes, 0)};
-      } else {
-        out[k++] = b200_device_buffer{(void*)c.data, (uint64_t)c.n * c.width()};
-        out[k++] = b200_device_buffer{nullptr, 0};
-      }
-      packed->cols.push_back(c);
-    }
-    if (!pending.empty()) {
-      std::vector<int32_t> h(2 * pending.size());
-      CUDA_CHECK(cudaMemcpyAsync(h.data(), fl->ptr, h.size() * 4, cudaMemcpyDeviceToHost, x.st()));
-      CUDA_CHECK(cudaStreamSynchronize(x.st()));
-      for (size_t i = 0; i < pending.size(); i++) {
-        DevColumn& c = packed->cols[pending[i].col];
-        c.chars = c.chars + h[2 * i];
-        c.chars_bytes = (int64_t)h[2 * i + 1] - (int64_t)h[2 * i];
-        out[pending[i].out_chars] = b200_device_buffer{(void*)c.chars, (uint64_t)c.chars_bytes};
-      }
-    }
-    CUDA_CHECK(cudaStreamSynchronize(x.st()));
-    // the packed form stays alive next to the partition (until its stage / job data is removed); the stored pieces,
-    // their file ids and anything a concurrent map task adds are left alone: this is a read-style call
-    {
-      std::lock_guard<std::mutex> g(e->mu);
-      e->packed_cache[ShuffleKey{job_id, stage_id, out_partition}] = packed;
-    }
-    *n_out = k;
-    *n_rows = packed->n;
-  });
-}
-
-int b200_partition_import_device(b200_engine* e, const char* job_id, int64_t stage_id, int out_partition, int64_t file_id, const char* schema_json,
-                                 const b200_device_buffer* bufs, int n_bufs, int64_t n_rows) {
-  return guard([&] {
-    CUDA_CHECK(cudaSetDevice(e->device));
-    Json j = parse_json(schema_json, strlen(schema_json));
-    Schema s = parse_schema(j);
-    if ((int)s.size() * 3 != n_bufs) throw EngineError(B200_ERR_INVALID, "expected 3 buffers per column");
-    cudaStream_t st = e->stream;
-    auto b = std::make_shared<DevBatch>();
-    b->n = n_rows;
-    for (size_t c = 0; c < s.size(); c++) {
-      const b200_device_buffer& bv = bufs[3 * c];
-      const b200_device_buffer& bd = bufs[3 * c + 1];
-      const b200_device_buffer& bc = bufs[3 * c + 2];
-      DevColumn col;
-      col.name = s[c].name;
-      col.type = s[c].type;
-      col.phys = phys_of(col.type);
-      col.n = n_rows;
-      auto copy_in = [&](const b200_device_buffer& src) -> const uint8_t* {
-        DevPtr d = dev_alloc((size_t)src.bytes + 64, st);
-        if (src.bytes) CUDA_CHECK(cudaMemcpyAsync(d->ptr, src.ptr, (size_t)src.bytes, cudaMemcpyDeviceToDevice, st));
-        col.keep.push_back(d);
-        return (const uint8_t*)d->ptr;
-      };
-      if (bv.bytes) col.valid = copy_in(bv);
-      col.nullable = bv.bytes != 0;
-      col.data = copy_in(bd);
-      if (col.phys == PH_UTF8) {
-        col.chars = copy_in(bc);
-        col.chars_bytes = (int64_t)bc.bytes;
-      }
-      b->cols.push_back(col);
-    }
-    CUDA_CHECK(cudaStreamSynchronize(st));
-    std::lock_guard<std::mutex> g(e->mu);
-    auto& v = e->shuffle[ShuffleKey{job_id, stage_id, out_partition}];
-    v.erase(std::remove_if(v.begin(), v.end(), [&](const Piece& pc) { return pc.file_id == file_id; }), v.end());
-    v.push_back(Piece{file_id, b, 0, n_rows});
-  });
-}
-
 int b200_remove_job_data(b200_engine* e, const char* job_id) {
   return guard([&] {
     CUDA_CHECK(cudaSetDevice(e->device));
@@ -5461,26 +5345,9 @@ int b200_remove_job_data(b200_engine* e, const char* job_id) {
       if (it->first.job == job_id) it = e->shuffle.erase(it);
       else ++it;
     }
-    for (auto it = e->packed_cache.begin(); it != e->packed_cache.end();) {
-      if (it->first.job == job_id) it = e->packed_cache.erase(it);
-      else ++it;
-    }
     // partitions that arrived through the fused shuffle live in the exchange window: it is recycled as a whole once no
     // stored partition can refer to it any more (peers write into it only inside a collective this executor takes part in)
     if (e->shuffle.empty()) e->win_used = 0;
-  });
-}
-
-int b200_device_gather(b200_engine* e, const b200_device_buffer* bufs, int n, void* dst, uint64_t dst_bytes) {
-  return guard([&] {
-    CUDA_CHECK(cudaSetDevice(e->device));
-    uint64_t pos = 0;
-    for (int i = 0; i < n; i++) {
-      if (!bufs[i].bytes) continue;
-      if (pos + bufs[i].bytes > dst_bytes) throw EngineError(B200_ERR_INVALID, "b200_device_gather: destination too small");
-      CUDA_CHECK(cudaMemcpyAsync((uint8_t*)dst + pos, bufs[i].ptr, (size_t)bufs[i].bytes, cudaMemcpyDeviceToDevice, e->stream));
-      pos += bufs[i].bytes;
-    }
   });
 }
 
@@ -5490,10 +5357,6 @@ int b200_remove_stage_data(b200_engine* e, const char* job_id, int64_t stage_id)
     std::lock_guard<std::mutex> g(e->mu);
     for (auto it = e->shuffle.begin(); it != e->shuffle.end();) {
       if (it->first.job == job_id && it->first.stage == stage_id) it = e->shuffle.erase(it);
-      else ++it;
-    }
-    for (auto it = e->packed_cache.begin(); it != e->packed_cache.end();) {
-      if (it->first.job == job_id && it->first.stage == stage_id) it = e->packed_cache.erase(it);
       else ++it;
     }
   });

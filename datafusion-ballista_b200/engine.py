@@ -52,10 +52,6 @@ EXCHANGE_HASH, EXCHANGE_GATHER, EXCHANGE_BROADCAST = 0, 1, 2
 NCCL_ID_BYTES = 128
 
 
-class DeviceBuffer(C.Structure):
-    _fields_ = [("ptr", C.c_void_p), ("bytes", C.c_uint64)]
-
-
 class ArrowSchema(C.Structure):
     _fields_ = [("format", C.c_char_p), ("name", C.c_char_p), ("metadata", C.c_char_p), ("flags", C.c_int64),
                 ("n_children", C.c_int64), ("children", C.c_void_p), ("dictionary", C.c_void_p),
@@ -74,8 +70,8 @@ EXPORTED_SYMBOLS = [
     "b200_engine_synchronize", "b200_engine_kernel_launches", "b200_engine_counter", "b200_engine_set_config",
     "b200_engine_register_batch", "b200_engine_register_parquet", "b200_parquet_describe", "b200_engine_drop_table", "b200_engine_tpch_generate",
     "b200_engine_export_table", "b200_tpch_table_rows", "b200_stage_prepare", "b200_stage_execute", "b200_stage_metrics",
-    "b200_stage_release", "b200_partition_export", "b200_partition_rows", "b200_partition_device_buffers",
-    "b200_partition_import_device", "b200_device_gather", "b200_remove_job_data", "b200_remove_stage_data", "b200_host_alloc_pinned", "b200_host_free_pinned",
+    "b200_stage_release", "b200_partition_export", "b200_partition_rows",
+    "b200_remove_job_data", "b200_remove_stage_data", "b200_host_alloc_pinned", "b200_host_free_pinned",
     "b200_comm_unique_id", "b200_engine_comm_init", "b200_exchange_stage", "b200_stage_execute_exchange", "b200_engine_kernel_stats",
     "b200_ipc_encode", "b200_ipc_free", "b200_ipc_decode", "b200_shuffle_write_files", "b200_shuffle_read_file",
     "b200_stage_prepare_proto", "b200_stage_prepare_task", "b200_task_status_encode", "b200_plan_proto_to_json", "b200_string_free", "b200_plan_typed_json",
@@ -130,11 +126,8 @@ def load_library():
     L.b200_partition_export.argtypes = [vp, cp, i64, ci, vp, vp]
     L.b200_partition_rows.argtypes = [vp, cp, i64, ci]
     L.b200_partition_rows.restype = i64
-    L.b200_partition_device_buffers.argtypes = [vp, cp, i64, ci, C.POINTER(DeviceBuffer), ci, C.POINTER(ci), C.POINTER(i64)]
-    L.b200_partition_import_device.argtypes = [vp, cp, i64, ci, i64, cp, C.POINTER(DeviceBuffer), ci, i64]
     L.b200_remove_job_data.argtypes = [vp, cp]
     L.b200_remove_stage_data.argtypes = [vp, cp, i64]
-    L.b200_device_gather.argtypes = [vp, C.POINTER(DeviceBuffer), ci, vp, u64]
     L.b200_engine_kernel_stats.argtypes = [vp, C.POINTER(KernelStat), ci, C.POINTER(ci), ci]
     L.b200_ipc_encode.argtypes = [vp, vp, ci, i64, C.POINTER(vp), C.POINTER(u64)]
     L.b200_ipc_free.argtypes = [vp]
@@ -441,32 +434,6 @@ class GpuExecutionEngine:
 
     def partition_rows(self, job_id: str, stage_id: int, out_partition: int) -> int:
         return load_library().b200_partition_rows(self.h, job_id.encode(), stage_id, out_partition)
-
-    def partition_device_buffers(self, job_id: str, stage_id: int, out_partition: int):
-        cap = 3 * 64
-        out = (DeviceBuffer * cap)()
-        n = C.c_int(0)
-        rows = C.c_int64(0)
-        _check(load_library().b200_partition_device_buffers(self.h, job_id.encode(), stage_id, out_partition, out, cap,
-                                                            C.byref(n), C.byref(rows)))
-        return [(out[i].ptr or 0, out[i].bytes) for i in range(n.value)], rows.value
-
-    def partition_import_device(self, job_id: str, stage_id: int, out_partition: int, file_id: int, schema_json: str,
-                                bufs, n_rows: int) -> None:
-        arr = (DeviceBuffer * len(bufs))()
-        for i, (p, b) in enumerate(bufs):
-            arr[i].ptr = p
-            arr[i].bytes = b
-        _check(load_library().b200_partition_import_device(self.h, job_id.encode(), stage_id, out_partition, file_id,
-                                                           schema_json.encode(), arr, len(bufs), n_rows))
-
-    def device_gather(self, bufs, dst_ptr: int, dst_bytes: int) -> None:
-        """Pack device buffers [(ptr, bytes), ...] back to back into dst (b200_device_gather)."""
-        arr = (DeviceBuffer * max(len(bufs), 1))()
-        for i, (p, b) in enumerate(bufs):
-            arr[i].ptr = p
-            arr[i].bytes = b
-        _check(load_library().b200_device_gather(self.h, arr, len(bufs), dst_ptr, dst_bytes))
 
     # -- exchange between the box's GPU executors (NCCL inside the library) -------------------------
     @staticmethod

@@ -192,29 +192,10 @@ int b200_partition_export(b200_engine* e, const char* job_id, int64_t stage_id, 
                           struct ArrowArray* out, struct ArrowSchema* out_schema);
 /* Rows currently stored for (job, stage, out_partition); -1 if absent. */
 int64_t b200_partition_rows(b200_engine* e, const char* job_id, int64_t stage_id, int out_partition);
-/* Device-resident exchange descriptor for peer pulls / NCCL all-to-all: fills device pointers and
- * byte sizes of the partition's column buffers (see DESIGN.md "Exchange"). */
-typedef struct b200_device_buffer {
-  void* ptr;
-  uint64_t bytes;
-} b200_device_buffer;
-int b200_partition_device_buffers(b200_engine* e, const char* job_id, int64_t stage_id, int out_partition,
-                                  b200_device_buffer* out, int cap, int* n_out, int64_t* n_rows);
-/* Install a partition received from a peer GPU (buffers already in this GPU's HBM, laid out as
- * b200_partition_device_buffers describes; the engine takes ownership via copy on its stream). */
-int b200_partition_import_device(b200_engine* e, const char* job_id, int64_t stage_id, int out_partition,
-                                 int64_t file_id, const char* schema_json, const b200_device_buffer* bufs,
-                                 int n_bufs, int64_t n_rows);
-/* Pack `n` device buffers back to back into `dst` (device memory of this GPU, >= the sum of their
- * sizes) on the engine's stream: the send side of the exchange builds one contiguous message per
- * peer this way (the reference's counterpart is the IPC writer appending batches to one shuffle file,
- * ballista/core/src/execution_plans/shuffle_writer.rs:262-330).  Returns after the copies are
- * enqueued; call b200_engine_synchronize (or use the same stream) before reading `dst`. */
-int b200_device_gather(b200_engine* e, const b200_device_buffer* bufs, int n, void* dst, uint64_t dst_bytes);
 /* RemoveJobData RPC (ballista/executor/src/executor_server.rs:921-932). */
 int b200_remove_job_data(b200_engine* e, const char* job_id);
-/* Drop every stored partition of one stage (used by the exchange step once the pieces have been
- * handed to their owning GPUs; the reference deletes map outputs the same way on stage rollback). */
+/* Drop every stored partition of one stage, all its map tasks' pieces included; the engine's other
+ * stages and jobs are left alone (the reference deletes map outputs the same way on stage rollback). */
 int b200_remove_stage_data(b200_engine* e, const char* job_id, int64_t stage_id);
 
 /* ---- exchange between the box's GPU executors ------------------------------------------------
@@ -231,7 +212,8 @@ int b200_remove_stage_data(b200_engine* e, const char* job_id, int64_t stage_id)
  *       B200_EXCHANGE_GATHER     every partition -> executor `root`       (CoalescePartitions / SortPreservingMerge)
  *       B200_EXCHANGE_BROADCAST  every partition -> every executor        (broadcast join build side,
  *                                                                          planner.rs:142-183, shuffle_reader.rs:121-144)
- *     schema_json: the stage's output schema (same JSON as b200_partition_import_device). */
+ *     schema_json: the stage's output schema as a JSON list of fields {"name", "type", "nullable"}, with the plan IR's
+ *       type names ("i64", "utf8", {"dec": [precision, scale]}, ...); "nullable" is optional and defaults to true. */
 #define B200_NCCL_ID_BYTES 128
 enum { B200_EXCHANGE_HASH = 0, B200_EXCHANGE_GATHER = 1, B200_EXCHANGE_BROADCAST = 2 };
 typedef struct b200_exchange_stats {

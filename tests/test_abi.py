@@ -33,7 +33,6 @@ def test_struct_layouts_match_header():
     import ctypes as C
     assert C.sizeof(bb.engine.ShuffleWritePartition) == 48   # 4*u64 + i64 + 2*i32
     assert C.sizeof(bb.engine.OperatorMetrics) == 48 + 6 * 8
-    assert C.sizeof(bb.engine.DeviceBuffer) == 16
 
 
 def test_engine_requires_a_gpu_no_cpu_fallback():
