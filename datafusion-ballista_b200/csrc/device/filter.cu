@@ -254,7 +254,7 @@ cudaError_t launch_fast_filter(const FastFilterSpec& S, int sm_count, cudaStream
     per_sm = v > 4 ? 4 : v;
   }
   int64_t g = n_tiles < (int64_t)sm_count * per_sm ? n_tiles : (int64_t)sm_count * per_sm;
-  fast_filter_kernel<<<(unsigned)g, FF_BLOCK, 0, st>>>(S);
+  launch_kernel(fast_filter_kernel, (unsigned)g, FF_BLOCK, 0, st, S);
   return cudaGetLastError();
 }
 

@@ -799,7 +799,7 @@ static cudaError_t launch_fused_one(int grid, int block, size_t smem, cudaStream
   if (block > BT) return cudaErrorInvalidValue;
   cudaError_t e = cudaFuncSetAttribute(fused_kernel<G, R, BT, SA, SB>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return e;
-  fused_kernel<G, R, BT, SA, SB><<<grid, block, smem, st>>>();
+  launch_kernel(fused_kernel<G, R, BT, SA, SB>, grid, block, smem, st);
   return cudaGetLastError();
 }
 

@@ -270,7 +270,7 @@ __global__ void groupby_plan_kernel(const unsigned long long* __restrict__ count
 
 cudaError_t launch_groupby_plan(const unsigned long long* counts, int K, unsigned long long* row_start, unsigned int* cta_start, cudaStream_t st) {
   static_assert(GROUPBY_ROWS_PER_CTA == GB_BLOCK * GB_R, "one tile per CTA in partition-first mode");
-  groupby_plan_kernel<<<1, 32, 0, st>>>(counts, K, row_start, cta_start);
+  launch_kernel(groupby_plan_kernel, 1, 32, 0, st, counts, K, row_start, cta_start);
   return cudaGetLastError();
 }
 
@@ -278,13 +278,13 @@ cudaError_t launch_groupby(const GroupBySpec& S, int sm_count, cudaStream_t st) 
   if (S.pf_K > 0) {
     // upper bound of sum_b ceil(rows_b / tile): the CTAs past cta_start[K] exit at once
     const int64_t g = (S.n_rows + GROUPBY_ROWS_PER_CTA - 1) / GROUPBY_ROWS_PER_CTA + S.pf_K;
-    groupby_kernel<<<(unsigned)g, GB_BLOCK, 0, st>>>(S);
+    launch_kernel(groupby_kernel, (unsigned)g, GB_BLOCK, 0, st, S);
     return cudaGetLastError();
   }
   int64_t g = (S.n_rows + (int64_t)GB_BLOCK * GB_R - 1) / ((int64_t)GB_BLOCK * GB_R);
   if (g < 1) g = 1;
   if (g > (int64_t)sm_count * 8) g = (int64_t)sm_count * 8;  // 8 resident CTAs of 256 threads per SM
-  groupby_kernel<<<(unsigned)g, GB_BLOCK, 0, st>>>(S);
+  launch_kernel(groupby_kernel, (unsigned)g, GB_BLOCK, 0, st, S);
   return cudaGetLastError();
 }
 

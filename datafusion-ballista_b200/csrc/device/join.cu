@@ -142,7 +142,7 @@ template <bool EXACT>
 static void launch_probe_mode(int mode, int grid, const JoinKeys& K, const JoinNode* nodes, const int32_t* heads, uint64_t mask, const uint64_t* probe_hash, int64_t n_probe,
                               unsigned long long* counter, uint64_t cap, int64_t* out_b, int64_t* out_p, uint8_t* probe_mark, uint8_t* build_mark, cudaStream_t st) {
 #define JP_CASE(M)                                                                                                                                        \
-  case M: join_probe2_kernel<EXACT, M><<<grid, JP_BLOCK, 0, st>>>(K, nodes, heads, mask, probe_hash, n_probe, counter, cap, out_b, out_p, probe_mark, build_mark); break;
+  case M: launch_kernel(join_probe2_kernel<EXACT, M>, grid, JP_BLOCK, 0, st, K, nodes, heads, mask, probe_hash, n_probe, counter, cap, out_b, out_p, probe_mark, build_mark); break;
   switch (mode) {
     JP_CASE(1)
     JP_CASE(2)
@@ -159,8 +159,8 @@ static void launch_probe_mode(int mode, int grid, const JoinKeys& K, const JoinN
 void launch_join_build2(const JoinKeys& K, bool exact, const uint64_t* build_hash, int64_t n_build, int32_t* heads, uint64_t n_buckets, JoinNode* nodes, cudaStream_t st) {
   if (n_build <= 0) return;
   const int g = join_grid(n_build, 256, 4);
-  if (exact) join_build2_kernel<true><<<g, 256, 0, st>>>(K, build_hash, n_build, heads, n_buckets - 1, nodes);
-  else join_build2_kernel<false><<<g, 256, 0, st>>>(K, build_hash, n_build, heads, n_buckets - 1, nodes);
+  if (exact) launch_kernel(join_build2_kernel<true>, g, 256, 0, st, K, build_hash, n_build, heads, n_buckets - 1, nodes);
+  else launch_kernel(join_build2_kernel<false>, g, 256, 0, st, K, build_hash, n_build, heads, n_buckets - 1, nodes);
 }
 
 void launch_join_probe2(const JoinKeys& K, bool exact, int mode, const JoinNode* nodes, const int32_t* heads, uint64_t n_buckets, const uint64_t* probe_hash, int64_t n_probe,

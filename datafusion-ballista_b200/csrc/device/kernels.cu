@@ -18,6 +18,10 @@ namespace b200 {
 typedef __int128 i128;
 typedef unsigned __int128 u128;
 
+static thread_local uint64_t t_launches = 0;
+uint64_t launches_on_thread() { return t_launches; }
+void count_launches(uint64_t n) { t_launches += n; }
+
 static inline int grid_for(int64_t n, int block, int per_thread = 1) {
   int64_t g = (n + (int64_t)block * per_thread - 1) / ((int64_t)block * per_thread);
   if (g < 1) g = 1;
@@ -51,7 +55,7 @@ __global__ void agg_table_init_kernel(AggTable T, AccKinds kinds) {
   if (blockIdx.x == 0 && threadIdx.x == 0) *T.n_groups = 0;
 }
 void launch_agg_table_init(const AggTable& T, const AccKinds& kinds, cudaStream_t st) {
-  agg_table_init_kernel<<<grid_for((int64_t)T.cap, 256), 256, 0, st>>>(T, kinds);
+  launch_kernel(agg_table_init_kernel, grid_for((int64_t)T.cap, 256), 256, 0, st, T, kinds);
 }
 
 __device__ __forceinline__ i128 mk128(unsigned long long lo, unsigned long long hi) { return (i128)(((u128)hi << 64) | lo); }
@@ -197,7 +201,7 @@ __global__ void agg_extract_kernel(AggTable T, AggExtractArgs A) {
   }
 }
 void launch_agg_extract(const AggTable& T, const AggExtractArgs& A, cudaStream_t st) {
-  agg_extract_kernel<<<grid_for((int64_t)T.cap, 256), 256, 0, st>>>(T, A);
+  launch_kernel(agg_extract_kernel, grid_for((int64_t)T.cap, 256), 256, 0, st, T, A);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -277,9 +281,9 @@ __global__ void scan_add_kernel(uint64_t* out, int64_t n, const uint64_t* block_
 void launch_scan_u32_to_u64(const uint32_t* in, uint64_t* out, int64_t n, uint64_t* scratch, cudaStream_t st) {
   int64_t nb = (n + SCAN_TILE - 1) / SCAN_TILE;
   if (nb < 1) nb = 1;
-  scan_block_kernel<<<(unsigned)nb, SCAN_BLOCK, 0, st>>>(in, out, n, scratch);
-  scan_sums_kernel<<<1, 256, 0, st>>>(scratch, nb, scratch + nb);
-  scan_add_kernel<<<(unsigned)nb, SCAN_BLOCK, 0, st>>>(out, n, scratch, scratch + nb);
+  launch_kernel(scan_block_kernel, (unsigned)nb, SCAN_BLOCK, 0, st, in, out, n, scratch);
+  launch_kernel(scan_sums_kernel, 1, 256, 0, st, scratch, nb, scratch + nb);
+  launch_kernel(scan_add_kernel, (unsigned)nb, SCAN_BLOCK, 0, st, out, n, scratch, scratch + nb);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -304,7 +308,7 @@ __global__ void histogram_kernel(const uint32_t* ids, int64_t n, uint32_t n_bins
 }
 void launch_histogram_u32(const uint32_t* ids, int64_t n, uint32_t n_bins, unsigned long long* counts, cudaStream_t st) {
   size_t sm = n_bins <= 8192 ? n_bins * sizeof(unsigned int) : 0;
-  histogram_kernel<<<grid_for(n, 256, 8), 256, sm, st>>>(ids, n, n_bins, counts);
+  launch_kernel(histogram_kernel, grid_for(n, 256, 8), 256, sm, st, ids, n, n_bins, counts);
 }
 
 template <typename T>
@@ -314,11 +318,11 @@ __global__ void scatter_kernel(const T* in, T* out, const uint32_t* dest, int64_
 void launch_scatter_fixed(const void* in, void* out, const uint32_t* dest, int64_t n, int width, cudaStream_t st) {
   int g = grid_for(n, 256, 4);
   switch (width) {
-    case 1: scatter_kernel<uint8_t><<<g, 256, 0, st>>>((const uint8_t*)in, (uint8_t*)out, dest, n); break;
-    case 2: scatter_kernel<uint16_t><<<g, 256, 0, st>>>((const uint16_t*)in, (uint16_t*)out, dest, n); break;
-    case 4: scatter_kernel<uint32_t><<<g, 256, 0, st>>>((const uint32_t*)in, (uint32_t*)out, dest, n); break;
-    case 8: scatter_kernel<uint64_t><<<g, 256, 0, st>>>((const uint64_t*)in, (uint64_t*)out, dest, n); break;
-    default: scatter_kernel<ulonglong2><<<g, 256, 0, st>>>((const ulonglong2*)in, (ulonglong2*)out, dest, n); break;
+    case 1: launch_kernel(scatter_kernel<uint8_t>, g, 256, 0, st, (const uint8_t*)in, (uint8_t*)out, dest, n); break;
+    case 2: launch_kernel(scatter_kernel<uint16_t>, g, 256, 0, st, (const uint16_t*)in, (uint16_t*)out, dest, n); break;
+    case 4: launch_kernel(scatter_kernel<uint32_t>, g, 256, 0, st, (const uint32_t*)in, (uint32_t*)out, dest, n); break;
+    case 8: launch_kernel(scatter_kernel<uint64_t>, g, 256, 0, st, (const uint64_t*)in, (uint64_t*)out, dest, n); break;
+    default: launch_kernel(scatter_kernel<ulonglong2>, g, 256, 0, st, (const ulonglong2*)in, (ulonglong2*)out, dest, n); break;
   }
 }
 
@@ -335,11 +339,11 @@ __global__ void gather_kernel(const T* in, const uint8_t* valid_in, T* out, uint
 void launch_gather_fixed(const void* in, const uint8_t* valid_in, void* out, uint8_t* valid_out, const int64_t* idx, int64_t n, int width, cudaStream_t st) {
   int g = grid_for(n, 256, 4);
   switch (width) {
-    case 1: gather_kernel<uint8_t><<<g, 256, 0, st>>>((const uint8_t*)in, valid_in, (uint8_t*)out, valid_out, idx, n); break;
-    case 2: gather_kernel<uint16_t><<<g, 256, 0, st>>>((const uint16_t*)in, valid_in, (uint16_t*)out, valid_out, idx, n); break;
-    case 4: gather_kernel<uint32_t><<<g, 256, 0, st>>>((const uint32_t*)in, valid_in, (uint32_t*)out, valid_out, idx, n); break;
-    case 8: gather_kernel<uint64_t><<<g, 256, 0, st>>>((const uint64_t*)in, valid_in, (uint64_t*)out, valid_out, idx, n); break;
-    default: gather_kernel<ulonglong2><<<g, 256, 0, st>>>((const ulonglong2*)in, valid_in, (ulonglong2*)out, valid_out, idx, n); break;
+    case 1: launch_kernel(gather_kernel<uint8_t>, g, 256, 0, st, (const uint8_t*)in, valid_in, (uint8_t*)out, valid_out, idx, n); break;
+    case 2: launch_kernel(gather_kernel<uint16_t>, g, 256, 0, st, (const uint16_t*)in, valid_in, (uint16_t*)out, valid_out, idx, n); break;
+    case 4: launch_kernel(gather_kernel<uint32_t>, g, 256, 0, st, (const uint32_t*)in, valid_in, (uint32_t*)out, valid_out, idx, n); break;
+    case 8: launch_kernel(gather_kernel<uint64_t>, g, 256, 0, st, (const uint64_t*)in, valid_in, (uint64_t*)out, valid_out, idx, n); break;
+    default: launch_kernel(gather_kernel<ulonglong2>, g, 256, 0, st, (const ulonglong2*)in, valid_in, (ulonglong2*)out, valid_out, idx, n); break;
   }
 }
 // ingest: sign-extend host-narrowed Decimal128 values (int32 / int64) back to 16 bytes
@@ -352,8 +356,8 @@ __global__ void widen_to_i128_kernel(const T* in, ulonglong2* out, int64_t n) {
 }
 void launch_widen_to_i128(const void* in, int width, void* out, int64_t n, cudaStream_t st) {
   if (n <= 0) return;
-  if (width == 4) widen_to_i128_kernel<int32_t><<<grid_for(n, 256, 4), 256, 0, st>>>((const int32_t*)in, (ulonglong2*)out, n);
-  else widen_to_i128_kernel<int64_t><<<grid_for(n, 256, 4), 256, 0, st>>>((const int64_t*)in, (ulonglong2*)out, n);
+  if (width == 4) launch_kernel(widen_to_i128_kernel<int32_t>, grid_for(n, 256, 4), 256, 0, st, (const int32_t*)in, (ulonglong2*)out, n);
+  else launch_kernel(widen_to_i128_kernel<int64_t>, grid_for(n, 256, 4), 256, 0, st, (const int64_t*)in, (ulonglong2*)out, n);
 }
 
 // Arrow offsets of a row slice -> offsets starting at 0; also reports the slice's first/last offset
@@ -367,7 +371,7 @@ __global__ void rebase_offsets_kernel(const int32_t* in, int64_t n_plus_1, int32
   }
 }
 void launch_rebase_offsets(const int32_t* in, int64_t n_plus_1, int32_t* out, int32_t* first_last, cudaStream_t st) {
-  rebase_offsets_kernel<<<grid_for(n_plus_1, 256, 4), 256, 0, st>>>(in, n_plus_1, out, first_last);
+  launch_kernel(rebase_offsets_kernel, grid_for(n_plus_1, 256, 4), 256, 0, st, in, n_plus_1, out, first_last);
 }
 
 // every column of a batch in one launch (blockIdx.y = column): the tail of a query handles a few rows
@@ -398,20 +402,20 @@ __global__ void gather_multi_kernel(const GatherCols cols, const int64_t* idx, i
 void launch_gather_multi(const GatherCols& cols, const int64_t* idx, int64_t n, cudaStream_t st) {
   if (cols.n <= 0) return;
   dim3 grid((unsigned)grid_for(n, 256, 4), (unsigned)cols.n);
-  gather_multi_kernel<<<grid, 256, 0, st>>>(cols, idx, n);
+  launch_kernel(gather_multi_kernel, grid, 256, 0, st, cols, idx, n);
 }
 __global__ void iota_i64_kernel(int64_t* out, int64_t n) {
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) out[i] = i;
 }
-void launch_iota_i64(int64_t* out, int64_t n, cudaStream_t st) { iota_i64_kernel<<<grid_for(n, 256, 4), 256, 0, st>>>(out, n); }
+void launch_iota_i64(int64_t* out, int64_t n, cudaStream_t st) { launch_kernel(iota_i64_kernel, grid_for(n, 256, 4), 256, 0, st, out, n); }
 __global__ void iota_u32_kernel(uint32_t* out, int64_t n) {
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) out[i] = (uint32_t)i;
 }
-void launch_iota_u32(uint32_t* out, int64_t n, cudaStream_t st) { iota_u32_kernel<<<grid_for(n, 256, 4), 256, 0, st>>>(out, n); }
+void launch_iota_u32(uint32_t* out, int64_t n, cudaStream_t st) { launch_kernel(iota_u32_kernel, grid_for(n, 256, 4), 256, 0, st, out, n); }
 __global__ void u32_to_i64_kernel(const uint32_t* in, int64_t* out, int64_t n) {
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) out[i] = in[i];
 }
-void launch_u32_to_i64(const uint32_t* in, int64_t* out, int64_t n, cudaStream_t st) { u32_to_i64_kernel<<<grid_for(n, 256, 4), 256, 0, st>>>(in, out, n); }
+void launch_u32_to_i64(const uint32_t* in, int64_t* out, int64_t n, cudaStream_t st) { launch_kernel(u32_to_i64_kernel, grid_for(n, 256, 4), 256, 0, st, in, out, n); }
 
 // ------------------------------------------------------------------------------------------------
 // Strings and validity
@@ -424,7 +428,7 @@ __global__ void utf8_to_views_kernel(const int32_t* offsets, const uint8_t* char
   }
 }
 void launch_utf8_to_views(const int32_t* offsets, const uint8_t* chars, unsigned long long* views, int64_t n, cudaStream_t st) {
-  utf8_to_views_kernel<<<grid_for(n, 256, 4), 256, 0, st>>>(offsets, chars, views, n);
+  launch_kernel(utf8_to_views_kernel, grid_for(n, 256, 4), 256, 0, st, offsets, chars, views, n);
 }
 // 32-bit images (len << 24 | up to 3 bytes, first character in the low byte: the OP_STR_PACK8 image) of a Utf8 column whose
 // strings are all at most 3 bytes long -- the companion the fused aggregate kernel reads instead of offsets + characters
@@ -443,7 +447,7 @@ __global__ void prepack3_kernel(const int32_t* offsets, const uint8_t* chars, in
   }
 }
 void launch_prepack3(const int32_t* offsets, const uint8_t* chars, int64_t n, uint32_t* out, unsigned int* too_long, cudaStream_t st) {
-  prepack3_kernel<<<grid_for(n, 256, 4), 256, 0, st>>>(offsets, chars, n, out, too_long);
+  launch_kernel(prepack3_kernel, grid_for(n, 256, 4), 256, 0, st, offsets, chars, n, out, too_long);
 }
 // 32-bit images of a Decimal128 column (the value as int32) -- the companion the fused aggregate kernel streams instead of
 // the 16-byte values; *too_wide is set when some value does not fit (the image is then unusable)
@@ -458,14 +462,14 @@ __global__ void dec128_image_kernel(const ulonglong2* in, int64_t n, int32_t* ou
   if (wide) *too_wide = 1u;
 }
 void launch_dec128_image(const void* in, int64_t n, int32_t* out, unsigned int* too_wide, cudaStream_t st) {
-  dec128_image_kernel<<<grid_for(n, 256, 4), 256, 0, st>>>((const ulonglong2*)in, n, out, too_wide);
+  launch_kernel(dec128_image_kernel, grid_for(n, 256, 4), 256, 0, st, (const ulonglong2*)in, n, out, too_wide);
 }
 __global__ void view_lengths_kernel(const unsigned long long* views, const uint8_t* valid, uint32_t* lens, int64_t n) {
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
     lens[i] = (valid && !valid[i]) ? 0u : (uint32_t)views[2 * i + 1];
 }
 void launch_view_lengths(const unsigned long long* views, const uint8_t* valid, uint32_t* lens, int64_t n, cudaStream_t st) {
-  view_lengths_kernel<<<grid_for(n, 256, 4), 256, 0, st>>>(views, valid, lens, n);
+  launch_kernel(view_lengths_kernel, grid_for(n, 256, 4), 256, 0, st, views, valid, lens, n);
 }
 __global__ void views_to_utf8_kernel(const unsigned long long* views, const uint8_t* valid, const uint64_t* offs64, int32_t* offsets_out,
                                      uint8_t* chars_out, int64_t n) {
@@ -481,7 +485,7 @@ __global__ void views_to_utf8_kernel(const unsigned long long* views, const uint
 }
 void launch_views_to_utf8(const unsigned long long* views, const uint8_t* valid, const uint64_t* offs64, int32_t* offsets_out, uint8_t* chars_out,
                           int64_t n, cudaStream_t st) {
-  views_to_utf8_kernel<<<grid_for(n + 1, 256, 2), 256, 0, st>>>(views, valid, offs64, offsets_out, chars_out, n);
+  launch_kernel(views_to_utf8_kernel, grid_for(n + 1, 256, 2), 256, 0, st, views, valid, offs64, offsets_out, chars_out, n);
 }
 __global__ void bitmap_to_bytes_kernel(const uint8_t* bitmap, int64_t bit_offset, uint8_t* bytes, int64_t n) {
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
@@ -490,7 +494,7 @@ __global__ void bitmap_to_bytes_kernel(const uint8_t* bitmap, int64_t bit_offset
   }
 }
 void launch_bitmap_to_bytes(const uint8_t* bitmap, int64_t bit_offset, uint8_t* bytes, int64_t n, cudaStream_t st) {
-  bitmap_to_bytes_kernel<<<grid_for(n, 256, 4), 256, 0, st>>>(bitmap, bit_offset, bytes, n);
+  launch_kernel(bitmap_to_bytes_kernel, grid_for(n, 256, 4), 256, 0, st, bitmap, bit_offset, bytes, n);
 }
 __global__ void bytes_to_bitmap_kernel(const uint8_t* bytes, uint8_t* bitmap, int64_t n, unsigned long long* null_count) {
   // one thread per output byte
@@ -510,7 +514,7 @@ __global__ void bytes_to_bitmap_kernel(const uint8_t* bytes, uint8_t* bitmap, in
   if (null_count && nulls) atomicAdd(null_count, nulls);
 }
 void launch_bytes_to_bitmap(const uint8_t* bytes, uint8_t* bitmap, int64_t n, unsigned long long* null_count, cudaStream_t st) {
-  bytes_to_bitmap_kernel<<<grid_for((n + 7) / 8, 256, 1), 256, 0, st>>>(bytes, bitmap, n, null_count);
+  launch_kernel(bytes_to_bitmap_kernel, grid_for((n + 7) / 8, 256, 1), 256, 0, st, bytes, bitmap, n, null_count);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -528,7 +532,7 @@ __global__ void join_build_kernel(const uint64_t* build_hash, const uint8_t* bui
 }
 void launch_join_build(const uint64_t* build_hash, const uint8_t* build_ok, int64_t n_build, int32_t* heads, uint64_t n_buckets, int32_t* next,
                        cudaStream_t st) {
-  join_build_kernel<<<grid_for(n_build, 256, 4), 256, 0, st>>>(build_hash, build_ok, n_build, heads, n_buckets - 1, next);
+  launch_kernel(join_build_kernel, grid_for(n_build, 256, 4), 256, 0, st, build_hash, build_ok, n_build, heads, n_buckets - 1, next);
 }
 
 __device__ __forceinline__ bool key_cols_equal(const JoinKeys& K, int64_t bi, int64_t pi) {
@@ -602,40 +606,40 @@ __global__ void join_probe_kernel(JoinKeys K, const uint64_t* build_hash, const 
 void launch_join_probe_count(const JoinKeys& K, const uint64_t* build_hash, const int32_t* heads, uint64_t n_buckets, const int32_t* next,
                              const uint64_t* probe_hash, const uint8_t* probe_ok, int64_t n_probe, uint32_t* counts, uint8_t* build_mark,
                              cudaStream_t st) {
-  join_probe_kernel<false><<<grid_for(n_probe, 256, 2), 256, 0, st>>>(K, build_hash, heads, n_buckets - 1, next, probe_hash, probe_ok, n_probe, counts,
+  launch_kernel(join_probe_kernel<false>, grid_for(n_probe, 256, 2), 256, 0, st, K, build_hash, heads, n_buckets - 1, next, probe_hash, probe_ok, n_probe, counts,
                                                                        build_mark, nullptr, nullptr, nullptr);
 }
 void launch_join_probe_write(const JoinKeys& K, const uint64_t* build_hash, const int32_t* heads, uint64_t n_buckets, const int32_t* next,
                              const uint64_t* probe_hash, const uint8_t* probe_ok, int64_t n_probe, const uint64_t* offsets, int64_t* out_build_idx,
                              int64_t* out_probe_idx, cudaStream_t st) {
-  join_probe_kernel<true><<<grid_for(n_probe, 256, 2), 256, 0, st>>>(K, build_hash, heads, n_buckets - 1, next, probe_hash, probe_ok, n_probe, nullptr,
+  launch_kernel(join_probe_kernel<true>, grid_for(n_probe, 256, 2), 256, 0, st, K, build_hash, heads, n_buckets - 1, next, probe_hash, probe_ok, n_probe, nullptr,
                                                                       nullptr, offsets, out_build_idx, out_probe_idx);
 }
 __global__ void flag_to_u32_kernel(const uint8_t* flags, uint8_t want, uint32_t* out, int64_t n) {
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) out[i] = (flags[i] != 0) == (want != 0);
 }
 void launch_flag_to_u32(const uint8_t* flags, uint8_t want, uint32_t* out, int64_t n, cudaStream_t st) {
-  flag_to_u32_kernel<<<grid_for(n, 256, 4), 256, 0, st>>>(flags, want, out, n);
+  launch_kernel(flag_to_u32_kernel, grid_for(n, 256, 4), 256, 0, st, flags, want, out, n);
 }
 __global__ void select_indices_kernel(const uint32_t* flag01, const uint64_t* offs, int64_t* out_idx, int64_t n) {
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
     if (flag01[i]) out_idx[offs[i]] = i;
 }
 void launch_select_indices(const uint32_t* flag01, const uint64_t* offs, int64_t* out_idx, int64_t n, cudaStream_t st) {
-  select_indices_kernel<<<grid_for(n, 256, 4), 256, 0, st>>>(flag01, offs, out_idx, n);
+  launch_kernel(select_indices_kernel, grid_for(n, 256, 4), 256, 0, st, flag01, offs, out_idx, n);
 }
 __global__ void counts_to_flag_kernel(const uint32_t* counts, uint8_t* flags, int64_t n) {
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) flags[i] = counts[i] ? 1 : 0;
 }
 void launch_counts_to_flag(const uint32_t* counts, uint8_t* flags, int64_t n, cudaStream_t st) {
-  counts_to_flag_kernel<<<grid_for(n, 256, 4), 256, 0, st>>>(counts, flags, n);
+  launch_kernel(counts_to_flag_kernel, grid_for(n, 256, 4), 256, 0, st, counts, flags, n);
 }
 __global__ void mark_from_idx_kernel(const int64_t* idx, int64_t n, uint8_t* marks) {
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
     if (idx[i] >= 0) marks[idx[i]] = 1;
 }
 void launch_mark_from_idx(const int64_t* idx, int64_t n, uint8_t* marks, cudaStream_t st) {
-  mark_from_idx_kernel<<<grid_for(n, 256, 4), 256, 0, st>>>(idx, n, marks);
+  launch_kernel(mark_from_idx_kernel, grid_for(n, 256, 4), 256, 0, st, idx, n, marks);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -699,7 +703,7 @@ __global__ void sort_word_kernel(SortWordArgs A, const uint32_t* perm, uint64_t*
   }
 }
 void launch_sort_word(const SortWordArgs& A, const uint32_t* perm, uint64_t* out, int64_t n, cudaStream_t st) {
-  sort_word_kernel<<<grid_for(n, 256, 4), 256, 0, st>>>(A, perm, out, n);
+  launch_kernel(sort_word_kernel, grid_for(n, 256, 4), 256, 0, st, A, perm, out, n);
 }
 // ---- small-n comparison sort ---------------------------------------------------------------------
 // three-way compare of rows i and j under one key; mirrors the word encoding of sort_word_kernel
@@ -766,7 +770,7 @@ __global__ void small_sort_kernel(const SmallSortKeys K, int64_t* perm_out, int6
 }
 void launch_small_sort(const SmallSortKeys& K, int64_t* perm_out, int64_t n, cudaStream_t st) {
   if (n <= 0) return;
-  small_sort_kernel<<<1, 256, 0, st>>>(K, perm_out, n);
+  launch_kernel(small_sort_kernel, 1, 256, 0, st, K, perm_out, n);
 }
 
 __global__ void max_view_len_kernel(const unsigned long long* views, const uint8_t* valid, int64_t n, unsigned int* out_max) {
@@ -777,7 +781,7 @@ __global__ void max_view_len_kernel(const unsigned long long* views, const uint8
   if ((threadIdx.x & 31) == 0 && m) atomicMax(out_max, m);
 }
 void launch_max_view_len(const unsigned long long* views, const uint8_t* valid, int64_t n, unsigned int* out_max, cudaStream_t st) {
-  max_view_len_kernel<<<grid_for(n, 256, 4), 256, 0, st>>>(views, valid, n, out_max);
+  launch_kernel(max_view_len_kernel, grid_for(n, 256, 4), 256, 0, st, views, valid, n, out_max);
 }
 
 static const int RS_BLOCK = 256, RS_ROUNDS = 8, RS_TILE = RS_BLOCK * RS_ROUNDS;
@@ -862,11 +866,10 @@ __global__ void rank_sort_kernel(const uint64_t* keys, const uint32_t* vals, uin
 }
 
 void radix_sort_pairs_u64(uint64_t* keys_a, uint32_t* vals_a, uint64_t* keys_b, uint32_t* vals_b, int64_t n, uint32_t* hist_scratch,
-                          uint64_t* scan_scratch, cudaStream_t st, bool* result_in_a, uint64_t* launches) {
+                          uint64_t* scan_scratch, cudaStream_t st, bool* result_in_a) {
   // hist_scratch: 256*n_blocks u32 ; scan_scratch: 256*n_blocks+1 u64 offsets + scan temp
   if (n <= 4096) {
-    rank_sort_kernel<<<(unsigned)((n + 127) / 128), 128, 0, st>>>(keys_a, vals_a, keys_b, vals_b, (int)n);
-    if (launches) *launches += 1;
+    launch_kernel(rank_sort_kernel, (unsigned)((n + 127) / 128), 128, 0, st, keys_a, vals_a, keys_b, vals_b, (int)n);
     *result_in_a = false;
     return;
   }
@@ -881,10 +884,9 @@ void radix_sort_pairs_u64(uint64_t* keys_a, uint32_t* vals_a, uint64_t* keys_b, 
     uint32_t* vin = in_a ? vals_a : vals_b;
     uint64_t* kout = in_a ? keys_b : keys_a;
     uint32_t* vout = in_a ? vals_b : vals_a;
-    radix_hist_kernel<<<n_blocks, RS_BLOCK, 0, st>>>(kin, n, shift, hist_scratch, n_blocks);
+    launch_kernel(radix_hist_kernel, n_blocks, RS_BLOCK, 0, st, kin, n, shift, hist_scratch, n_blocks);
     launch_scan_u32_to_u64(hist_scratch, offsets, (int64_t)256 * n_blocks, scan_tmp, st);
-    radix_scatter_kernel<<<n_blocks, RS_BLOCK, 0, st>>>(kin, vin, kout, vout, n, shift, offsets, n_blocks);
-    if (launches) *launches += 5;
+    launch_kernel(radix_scatter_kernel, n_blocks, RS_BLOCK, 0, st, kin, vin, kout, vout, n, shift, offsets, n_blocks);
     in_a = !in_a;
   }
   *result_in_a = in_a;
@@ -914,15 +916,14 @@ __global__ void partition_keys_kernel(const uint32_t* ids, int64_t n, uint64_t* 
 __global__ void invert_perm_kernel(const uint32_t* perm, int64_t n, uint32_t* dest) {
   for (int64_t k = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; k < n; k += (int64_t)gridDim.x * blockDim.x) dest[perm[k]] = (uint32_t)k;
 }
-uint64_t launch_partition_dest_stable(const uint32_t* ids, int64_t n, uint32_t n_bins, uint32_t* dest, uint64_t* keys_a, uint32_t* vals_a, uint64_t* keys_b,
-                                      uint32_t* vals_b, uint32_t* hist_scratch, uint64_t* scan_scratch, cudaStream_t st) {
-  if (n <= 0) return 0;
+void launch_partition_dest_stable(const uint32_t* ids, int64_t n, uint32_t n_bins, uint32_t* dest, uint64_t* keys_a, uint32_t* vals_a, uint64_t* keys_b,
+                                  uint32_t* vals_b, uint32_t* hist_scratch, uint64_t* scan_scratch, cudaStream_t st) {
+  if (n <= 0) return;
   if (n <= 4096) {
-    partition_dest_small_kernel<<<(unsigned)((n + 127) / 128), 128, 0, st>>>(ids, (int)n, dest);
-    return 1;
+    launch_kernel(partition_dest_small_kernel, (unsigned)((n + 127) / 128), 128, 0, st, ids, (int)n, dest);
+    return;
   }
-  partition_keys_kernel<<<grid_for(n, 256, 4), 256, 0, st>>>(ids, n, keys_a, vals_a);
-  uint64_t launches = 1;
+  launch_kernel(partition_keys_kernel, grid_for(n, 256, 4), 256, 0, st, ids, n, keys_a, vals_a);
   const int passes = n_bins <= 256 ? 1 : n_bins <= 65536 ? 2 : 4;
   uint32_t n_blocks = (uint32_t)((n + RS_TILE - 1) / RS_TILE);
   uint64_t* offsets = scan_scratch;
@@ -933,14 +934,12 @@ uint64_t launch_partition_dest_stable(const uint32_t* ids, int64_t n, uint32_t n
     uint32_t* vin = in_a ? vals_a : vals_b;
     uint64_t* kout = in_a ? keys_b : keys_a;
     uint32_t* vout = in_a ? vals_b : vals_a;
-    radix_hist_kernel<<<n_blocks, RS_BLOCK, 0, st>>>(kin, n, pass * 8, hist_scratch, n_blocks);
+    launch_kernel(radix_hist_kernel, n_blocks, RS_BLOCK, 0, st, kin, n, pass * 8, hist_scratch, n_blocks);
     launch_scan_u32_to_u64(hist_scratch, offsets, (int64_t)256 * n_blocks, scan_tmp, st);
-    radix_scatter_kernel<<<n_blocks, RS_BLOCK, 0, st>>>(kin, vin, kout, vout, n, pass * 8, offsets, n_blocks);
-    launches += 5;
+    launch_kernel(radix_scatter_kernel, n_blocks, RS_BLOCK, 0, st, kin, vin, kout, vout, n, pass * 8, offsets, n_blocks);
     in_a = !in_a;
   }
-  invert_perm_kernel<<<grid_for(n, 256, 4), 256, 0, st>>>(in_a ? vals_a : vals_b, n, dest);
-  return launches + 1;
+  launch_kernel(invert_perm_kernel, grid_for(n, 256, 4), 256, 0, st, in_a ? vals_a : vals_b, n, dest);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -958,7 +957,7 @@ __global__ void tpch_fixed_kernel(int table, int col, int kind, int64_t msf, int
   }
 }
 void launch_tpch_fixed(int table, int col, int kind, int64_t msf, int64_t row0, int64_t n, void* out, cudaStream_t st) {
-  tpch_fixed_kernel<<<grid_for(n, 256, 4), 256, 0, st>>>(table, col, kind, msf, row0, n, out);
+  launch_kernel(tpch_fixed_kernel, grid_for(n, 256, 4), 256, 0, st, table, col, kind, msf, row0, n, out);
 }
 __global__ void tpch_str_len_kernel(int table, int col, int64_t msf, int64_t row0, int64_t n, uint32_t* lens) {
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
@@ -967,7 +966,7 @@ __global__ void tpch_str_len_kernel(int table, int col, int64_t msf, int64_t row
   }
 }
 void launch_tpch_str_len(int table, int col, int64_t msf, int64_t row0, int64_t n, uint32_t* lens, cudaStream_t st) {
-  tpch_str_len_kernel<<<grid_for(n, 256, 4), 256, 0, st>>>(table, col, msf, row0, n, lens);
+  launch_kernel(tpch_str_len_kernel, grid_for(n, 256, 4), 256, 0, st, table, col, msf, row0, n, lens);
 }
 __global__ void tpch_str_fill_kernel(int table, int col, int64_t msf, int64_t row0, int64_t n, const uint64_t* offs64, int32_t* offsets, uint8_t* chars) {
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i <= n; i += (int64_t)gridDim.x * blockDim.x) {
@@ -981,7 +980,7 @@ __global__ void tpch_str_fill_kernel(int table, int col, int64_t msf, int64_t ro
 }
 void launch_tpch_str_fill(int table, int col, int64_t msf, int64_t row0, int64_t n, const uint64_t* offs64, int32_t* offsets, uint8_t* chars,
                           cudaStream_t st) {
-  tpch_str_fill_kernel<<<grid_for(n + 1, 256, 2), 256, 0, st>>>(table, col, msf, row0, n, offs64, offsets, chars);
+  launch_kernel(tpch_str_fill_kernel, grid_for(n + 1, 256, 2), 256, 0, st, table, col, msf, row0, n, offs64, offsets, chars);
 }
 
 }  // namespace b200

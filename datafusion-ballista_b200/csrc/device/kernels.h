@@ -7,6 +7,21 @@
 
 namespace b200 {
 
+// ---- launch accounting (kernels.cu) -------------------------------------------------------------
+// Kernels the calling host thread has enqueued so far.  Per thread because several tasks, on one engine or several, run
+// at once in one process: the launches of some piece of work are the difference of two readings around it.
+uint64_t launches_on_thread();
+// Adds n to the calling thread's count: launch_kernel below, and work enqueued by other libraries (an NCCL group).
+void count_launches(uint64_t n = 1);
+#ifdef __CUDACC__
+// The one place the device module launches a kernel (every launcher calls it), so that every launch is counted.
+template <class... P, class... A>
+inline void launch_kernel(void (*kernel)(P...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, const A&... args) {
+  count_launches();
+  kernel<<<grid, block, smem, st>>>(args...);
+}
+#endif
+
 // ---- fused pipeline (pipeline.cu) ---------------------------------------------------------------
 cudaError_t launch_pipeline(const Program& P, int reg_groups, int grid, int block, size_t smem, cudaStream_t st);
 // fused scan->filter->project->aggregate kernel (fused.cuh); *is_static: 1 when an ahead-of-time shape ran
@@ -69,8 +84,8 @@ void launch_histogram_u32(const uint32_t* ids, int64_t n, uint32_t n_bins, unsig
 // dest[i] = cursor[ids[i]]++  (cursor pre-seeded with the exclusive scan of counts)
 // stable placement of rows into hash partitions: dest[i] = rows of lower partitions + earlier rows of the same
 // partition (input order kept inside a partition, like the reference's BatchPartitioner).  Scratch as for
-// radix_sort_pairs_u64; returns the number of launches.
-uint64_t launch_partition_dest_stable(const uint32_t* ids, int64_t n, uint32_t n_bins, uint32_t* dest, uint64_t* keys_a, uint32_t* vals_a, uint64_t* keys_b,
+// radix_sort_pairs_u64.
+void launch_partition_dest_stable(const uint32_t* ids, int64_t n, uint32_t n_bins, uint32_t* dest, uint64_t* keys_a, uint32_t* vals_a, uint64_t* keys_b,
                                       uint32_t* vals_b, uint32_t* hist_scratch, uint64_t* scan_scratch, cudaStream_t st);
 void launch_scatter_fixed(const void* in, void* out, const uint32_t* dest, int64_t n, int width, cudaStream_t st);
 // out[i] = idx[i] >= 0 ? in[idx[i]] : 0 ; valid_out (optional) = idx>=0 && valid_in
@@ -328,7 +343,7 @@ void launch_small_sort(const SmallSortKeys& K, int64_t* perm_out, int64_t n, cud
 void launch_max_view_len(const unsigned long long* views, const uint8_t* valid, int64_t n, unsigned int* out_max, cudaStream_t st);
 // stable LSD radix sort of (key, val) pairs on 64-bit keys; ping-pong buffers; returns via *result_in_a
 void radix_sort_pairs_u64(uint64_t* keys_a, uint32_t* vals_a, uint64_t* keys_b, uint32_t* vals_b, int64_t n, uint32_t* hist_scratch,
-                          uint64_t* scan_scratch, cudaStream_t st, bool* result_in_a, uint64_t* launches);
+                          uint64_t* scan_scratch, cudaStream_t st, bool* result_in_a);
 void launch_iota_u32(uint32_t* out, int64_t n, cudaStream_t st);
 void launch_u32_to_i64(const uint32_t* in, int64_t* out, int64_t n, cudaStream_t st);
 

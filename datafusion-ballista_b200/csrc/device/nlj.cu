@@ -200,14 +200,14 @@ __global__ void __launch_bounds__(NLJ_BLOCK) nlj_kernel(const __grid_constant__ 
 void launch_nlj_count(const NljSpec& S, int64_t n_build, int64_t n_probe, uint32_t* counts, uint8_t* build_mark, uint8_t* probe_mark, cudaStream_t st) {
   if (n_probe <= 0) return;
   const int64_t g = (n_probe + NLJ_BLOCK - 1) / NLJ_BLOCK;
-  nlj_kernel<0><<<(unsigned)g, NLJ_BLOCK, 0, st>>>(S, n_build, n_probe, counts, build_mark, probe_mark, nullptr, nullptr, nullptr);
+  launch_kernel(nlj_kernel<0>, (unsigned)g, NLJ_BLOCK, 0, st, S, n_build, n_probe, counts, build_mark, probe_mark, nullptr, nullptr, nullptr);
 }
 
 void launch_nlj_write(const NljSpec& S, int64_t n_build, int64_t n_probe, const uint32_t* counts, const uint64_t* offsets, int64_t* out_build_idx,
                       int64_t* out_probe_idx, cudaStream_t st) {
   if (n_probe <= 0 || n_build <= 0) return;
   const int64_t g = (n_probe + NLJ_BLOCK - 1) / NLJ_BLOCK;
-  nlj_kernel<1><<<(unsigned)g, NLJ_BLOCK, 0, st>>>(S, n_build, n_probe, const_cast<uint32_t*>(counts), nullptr, nullptr, offsets, out_build_idx, out_probe_idx);
+  launch_kernel(nlj_kernel<1>, (unsigned)g, NLJ_BLOCK, 0, st, S, n_build, n_probe, const_cast<uint32_t*>(counts), nullptr, nullptr, offsets, out_build_idx, out_probe_idx);
 }
 
 }  // namespace b200

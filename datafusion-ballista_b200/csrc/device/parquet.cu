@@ -1179,38 +1179,38 @@ done:
 
 static inline unsigned pq_grid(int n_warps) { return (unsigned)((n_warps * 32 + 127) / 128); }
 void launch_pq_snappy(const PqDecompJob* jobs, int n_jobs, unsigned int* error, cudaStream_t st) {
-  if (n_jobs > 0) pq_snappy_kernel<<<pq_grid(n_jobs), 128, 0, st>>>(jobs, n_jobs, error);
+  if (n_jobs > 0) launch_kernel(pq_snappy_kernel, pq_grid(n_jobs), 128, 0, st, jobs, n_jobs, error);
 }
 void launch_pq_inflate(const PqDecompJob* jobs, int n_jobs, unsigned int* error, cudaStream_t st) {
-  if (n_jobs > 0) pq_inflate_kernel<<<pq_grid(n_jobs), 128, 0, st>>>(jobs, n_jobs, error);
+  if (n_jobs > 0) launch_kernel(pq_inflate_kernel, pq_grid(n_jobs), 128, 0, st, jobs, n_jobs, error);
 }
 void launch_pq_lz4(const PqDecompJob* jobs, int n_jobs, unsigned int* error, cudaStream_t st) {
-  if (n_jobs > 0) pq_lz4_kernel<<<pq_grid(n_jobs), 128, 0, st>>>(jobs, n_jobs, error);
+  if (n_jobs > 0) launch_kernel(pq_lz4_kernel, pq_grid(n_jobs), 128, 0, st, jobs, n_jobs, error);
 }
 
 void launch_pq_levels(const PqPage* pages, int n_pages, uint8_t* valid, uint32_t* nonnull, unsigned long long* total_nonnull, cudaStream_t st) {
-  if (n_pages > 0) pq_levels_kernel<<<pq_grid(n_pages), 128, 0, st>>>(pages, n_pages, valid, nonnull, total_nonnull);
+  if (n_pages > 0) launch_kernel(pq_levels_kernel, pq_grid(n_pages), 128, 0, st, pages, n_pages, valid, nonnull, total_nonnull);
 }
 void launch_pq_page_scan(const uint32_t* nonnull, int n_pages, unsigned long long* dense_base, cudaStream_t st) {
-  if (n_pages > 0) pq_page_scan_kernel<<<1, 1024, 0, st>>>(nonnull, n_pages, dense_base);
+  if (n_pages > 0) launch_kernel(pq_page_scan_kernel, 1, 1024, 0, st, nonnull, n_pages, dense_base);
 }
 void launch_pq_dict(const PqColumn& C, const PqPage* dict_pages, int n_dicts, cudaStream_t st) {
-  if (n_dicts > 0) pq_dict_kernel<<<pq_grid(n_dicts), 128, 0, st>>>(C, dict_pages, n_dicts);
+  if (n_dicts > 0) launch_kernel(pq_dict_kernel, pq_grid(n_dicts), 128, 0, st, C, dict_pages, n_dicts);
 }
 void launch_pq_values(const PqColumn& C, const PqPage* pages, int n_pages, const unsigned long long* dense_base, const uint32_t* nonnull, void* out, cudaStream_t st) {
-  if (n_pages > 0) pq_values_kernel<<<pq_grid(n_pages), 128, 0, st>>>(C, pages, n_pages, dense_base, nonnull, out);
+  if (n_pages > 0) launch_kernel(pq_values_kernel, pq_grid(n_pages), 128, 0, st, C, pages, n_pages, dense_base, nonnull, out);
 }
 void launch_pq_expand(const PqPage* pages, int n_pages, const unsigned long long* dense_base, const uint8_t* valid, const void* dense, void* out, int width,
                       cudaStream_t st) {
-  if (n_pages > 0) pq_expand_kernel<<<pq_grid(n_pages), 128, 0, st>>>(pages, n_pages, dense_base, valid, dense, out, width);
+  if (n_pages > 0) launch_kernel(pq_expand_kernel, pq_grid(n_pages), 128, 0, st, pages, n_pages, dense_base, valid, dense, out, width);
 }
 void launch_pq_delta_prepare(const PqColumn& C, const PqPage* pages, int n_pages, const unsigned long long* dense_base, const uint32_t* nonnull, const PqDeltaAux& A,
                              cudaStream_t st) {
-  if (n_pages > 0) pq_delta_prepare_kernel<<<pq_grid(n_pages), 128, 0, st>>>(C, pages, n_pages, dense_base, nonnull, A);
+  if (n_pages > 0) launch_kernel(pq_delta_prepare_kernel, pq_grid(n_pages), 128, 0, st, C, pages, n_pages, dense_base, nonnull, A);
 }
 void launch_pq_values_delta(const PqColumn& C, const PqPage* pages, int n_pages, const unsigned long long* dense_base, const uint32_t* nonnull, void* out,
                             const PqDeltaAux& A, cudaStream_t st) {
-  if (n_pages > 0) pq_values_delta_kernel<<<pq_grid(n_pages), 128, 0, st>>>(C, pages, n_pages, dense_base, nonnull, out, A);
+  if (n_pages > 0) launch_kernel(pq_values_delta_kernel, pq_grid(n_pages), 128, 0, st, C, pages, n_pages, dense_base, nonnull, out, A);
 }
 
 }  // namespace b200

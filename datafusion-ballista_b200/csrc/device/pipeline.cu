@@ -2809,7 +2809,7 @@ static cudaError_t launch_one(int grid, int block, size_t smem, cudaStream_t st)
     if (e != cudaSuccess) return e;
     granted[dev] = smem;
   }
-  pipeline_kernel<SINK, G, ADD_ONLY, SIDE, MOM, SFN><<<grid, block, smem, st>>>();
+  launch_kernel(pipeline_kernel<SINK, G, ADD_ONLY, SIDE, MOM, SFN>, grid, block, smem, st);
   return cudaGetLastError();
 }
 

@@ -385,7 +385,7 @@ cudaError_t launch_partition_hist(const PidSrc& pid, int64_t n, uint32_t P, uint
     cudaError_t e = cudaFuncSetAttribute(part_tile_hist_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm);
     if (e != cudaSuccess) return e;
   }
-  part_tile_hist_kernel<<<nt, PT_BLOCK, sm, st>>>(pid, n, P, nt, tile_hist, counts, sc, str_bytes);
+  launch_kernel(part_tile_hist_kernel, nt, PT_BLOCK, sm, st, pid, n, P, nt, tile_hist, counts, sc, str_bytes);
   return cudaGetLastError();
 }
 
@@ -397,7 +397,7 @@ cudaError_t launch_partition_scatter(const PidSrc& pid, int64_t n, uint32_t P, c
   for (int c = 0; c < cols.n; c++) peer = peer || cols.c[c].part_base != nullptr;
   static const int force_staged = getenv("B200_SCATTER_STAGED") ? atoi(getenv("B200_SCATTER_STAGED")) : -1;  // measurement switch
   if (!dest_out && P <= 32 && (force_staged == 1 || (force_staged != 0 && peer))) {
-    part_tile_scatter_wstaged_kernel<<<nt, PT_BLOCK, 0, st>>>(pid, n, P, nt, offsets, cols);
+    launch_kernel(part_tile_scatter_wstaged_kernel, nt, PT_BLOCK, 0, st, pid, n, P, nt, offsets, cols);
     return cudaGetLastError();
   }
   if (!dest_out && P <= PT_STAGED_MAX_P && (force_staged == 1 || (force_staged != 0 && peer))) {
@@ -408,7 +408,7 @@ cudaError_t launch_partition_scatter(const PidSrc& pid, int64_t n, uint32_t P, c
       if (e != cudaSuccess) return e;
       attr_set = true;
     }
-    part_tile_scatter_staged_kernel<<<nt, PT_BLOCK, sm, st>>>(pid, n, P, nt, offsets, cols);
+    launch_kernel(part_tile_scatter_staged_kernel, nt, PT_BLOCK, sm, st, pid, n, P, nt, offsets, cols);
     return cudaGetLastError();
   }
   const size_t sm = partition_scatter_smem(P);
@@ -416,7 +416,7 @@ cudaError_t launch_partition_scatter(const PidSrc& pid, int64_t n, uint32_t P, c
     cudaError_t e = cudaFuncSetAttribute(part_tile_scatter_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm);
     if (e != cudaSuccess) return e;
   }
-  part_tile_scatter_kernel<<<nt, PT_BLOCK, sm, st>>>(pid, n, P, nt, offsets, cols, dest_out);
+  launch_kernel(part_tile_scatter_kernel, nt, PT_BLOCK, sm, st, pid, n, P, nt, offsets, cols, dest_out);
   return cudaGetLastError();
 }
 
@@ -526,7 +526,7 @@ __global__ void __launch_bounds__(256) pack_jobs_kernel(const PackJob* __restric
 
 void launch_pack_jobs(const PackJob* jobs_dev, int n_jobs, cudaStream_t st) {
   if (n_jobs <= 0) return;
-  pack_jobs_kernel<<<n_jobs, 256, 0, st>>>(jobs_dev, n_jobs);
+  launch_kernel(pack_jobs_kernel, n_jobs, 256, 0, st, jobs_dev, n_jobs);
 }
 
 }  // namespace b200

@@ -51,6 +51,11 @@ struct ArenaChunk {
 };
 static const size_t ARENA_CHUNK_BYTES = (size_t)2 << 20;
 static const size_t ARENA_MAX_ALLOC = (size_t)64 << 10;
+// the chunk the calling thread carves new small allocations from
+inline std::shared_ptr<ArenaChunk>& arena_chunk() {
+  static thread_local std::shared_ptr<ArenaChunk> cur;
+  return cur;
+}
 
 struct DevAlloc {
   void* ptr = nullptr;
@@ -60,7 +65,7 @@ struct DevAlloc {
   DevAlloc(size_t n, cudaStream_t st) : bytes(n), stream(st) {
     const size_t padded = ((n + 255) & ~(size_t)255) + 256;
     if (padded <= ARENA_MAX_ALLOC) {
-      static thread_local std::shared_ptr<ArenaChunk> cur;
+      std::shared_ptr<ArenaChunk>& cur = arena_chunk();
       if (!cur || cur->stream != st || cur->used + padded > cur->cap) {
         auto c = std::make_shared<ArenaChunk>();
         void* p = nullptr;

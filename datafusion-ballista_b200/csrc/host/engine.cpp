@@ -169,7 +169,6 @@ struct Exec {
   void check_cancel() const {
     if (cancel && *cancel) throw EngineError(B200_ERR_CANCELLED, "task cancelled");
   }
-  void count(uint64_t n = 1) const { e->launches.fetch_add(n, std::memory_order_relaxed); }
   OpMetrics* m(const PlanNode* n) const {
     if (!s) return nullptr;
     auto it = s->metric_index.find(n);
@@ -366,7 +365,6 @@ struct PackList {
       CUDA_CHECK(cudaMemcpyAsync(d->ptr, jobs.data(), bytes, cudaMemcpyHostToDevice, x.st()));  // pageable: staged by the driver before returning
     }
     launch_pack_jobs((const PackJob*)d->ptr, (int)jobs.size(), x.st());
-    x.count();
     if (keep) keep->push_back(d);
     jobs.clear();
   }
@@ -378,7 +376,6 @@ DevColumn as_views(const Exec& x, const DevColumn& c) {
   DevColumn o = c;
   DevPtr v = dev_alloc((size_t)std::max<int64_t>(c.n, 1) * 16, x.st());
   launch_utf8_to_views((const int32_t*)c.data, c.chars, (unsigned long long*)v->ptr, c.n, x.st());
-  x.count();
   o.phys = PH_STRVIEW;
   o.data = (const uint8_t*)v->ptr;
   o.chars = nullptr;
@@ -418,13 +415,11 @@ DevColumn as_utf8(const Exec& x, const DevColumn& c, int64_t known_total = -1) {
   DevPtr scratch = dev_alloc((size_t)(n / 1024 + 4) * 8, x.st());
   launch_view_lengths((const unsigned long long*)c.data, c.valid, (uint32_t*)lens->ptr, n, x.st());
   launch_scan_u32_to_u64((const uint32_t*)lens->ptr, (uint64_t*)offs64->ptr, n, (uint64_t*)scratch->ptr, x.st());
-  x.count(4);
   uint64_t total = known_total >= 0 ? (uint64_t)known_total : x.get<uint64_t>((const uint64_t*)offs64->ptr + n);
   if (total > 0x7FFFFFFFull) throw EngineError(B200_ERR_UNSUPPORTED, "string column exceeds 2 GiB (LargeUtf8 not supported)");
   DevPtr offsets = dev_alloc((size_t)(n + 1) * 4, x.st());
   DevPtr chars = dev_alloc((size_t)total + 16, x.st());
   launch_views_to_utf8((const unsigned long long*)c.data, c.valid, (const uint64_t*)offs64->ptr, (int32_t*)offsets->ptr, (uint8_t*)chars->ptr, n, x.st());
-  x.count();
   DevColumn o;
   o.name = c.name;
   o.type = c.type;
@@ -467,7 +462,6 @@ void build_column_images(const Exec& x, DevBatch& b) {
     unsigned int* flag = (unsigned int*)flags->ptr + k;
     if (c.phys == PH_UTF8) launch_prepack3((const int32_t*)c.data, c.chars, c.n, (uint32_t*)img->ptr, flag, x.st());
     else launch_dec128_image(c.data, c.n, (int32_t*)img->ptr, flag, x.st());
-    x.count();
     imgs.push_back(img);
   }
   const unsigned int* h = (const unsigned int*)x.fetch_bytes(flags->ptr, cands.size() * 4);
@@ -491,7 +485,6 @@ DevBatchPtr gather_batch(const Exec& x, const DevBatch& in, const int64_t* idx, 
       for (int k = 0; k < gc.n; k++) b += 2ull * (uint64_t)gc.c[k].width;
       KernelTimer kt(x, "gather", (uint64_t)n_out * b);
       launch_gather_multi(gc, idx, n_out, x.st());
-      x.count();
       gc.n = 0;
     }
   };
@@ -591,7 +584,6 @@ void ingest_decimal_narrowed(b200_engine* e, const uint8_t* src, uint8_t* dst, i
     }
     CUDA_CHECK(cudaMemcpyAsync(sl.dev, sl.pinned, (size_t)rows * width, cudaMemcpyHostToDevice, st));
     launch_widen_to_i128(sl.dev, width, dst + r0 * 16, rows, st);
-    e->launches++;
     CUDA_CHECK(cudaEventRecord(sl.done, st));
     sl.used = true;
     e->narrowed_bytes_saved += (uint64_t)rows * (uint64_t)(16 - width);
@@ -643,7 +635,6 @@ DevBatchPtr import_batch_impl(b200_engine* e, ArrowArray* arr, ArrowSchema* sch)
       CUDA_CHECK(cudaMemcpyAsync(bm->ptr, ic.validity + b0, (size_t)(b1 - b0), cudaMemcpyHostToDevice, st));
       DevPtr v = dev_alloc((size_t)n + 16, st);
       launch_bitmap_to_bytes((const uint8_t*)bm->ptr, ic.offset & 7, (uint8_t*)v->ptr, n, st);
-      e->launches++;
       c.valid = (const uint8_t*)v->ptr;
       c.keep.push_back(v);
       c.keep.push_back(bm);
@@ -654,7 +645,6 @@ DevBatchPtr import_batch_impl(b200_engine* e, ArrowArray* arr, ArrowSchema* sch)
       CUDA_CHECK(cudaMemcpyAsync(bm->ptr, ic.data + b0, (size_t)(b1 - b0), cudaMemcpyHostToDevice, st));
       DevPtr v = dev_alloc((size_t)n + 16, st);
       launch_bitmap_to_bytes((const uint8_t*)bm->ptr, ic.offset & 7, (uint8_t*)v->ptr, n, st);
-      e->launches++;
       c.data = (const uint8_t*)v->ptr;
       c.keep.push_back(v);
       c.keep.push_back(bm);
@@ -813,7 +803,6 @@ std::vector<HostCol> download_batch(const Exec& x, const DevBatch& b, int64_t r0
       DevPtr cnt = dev_alloc(8, st);
       CUDA_CHECK(cudaMemsetAsync(cnt->ptr, 0, 8, st));
       launch_bytes_to_bitmap(c.valid, (uint8_t*)bm->ptr, n, (unsigned long long*)cnt->ptr, st);
-      x.count();
       h.validity.resize((size_t)(n + 7) / 8);
       CUDA_CHECK(cudaMemcpyAsync(h.validity.data(), bm->ptr, h.validity.size(), cudaMemcpyDeviceToHost, st));
       h.null_count = (int64_t)x.get<unsigned long long>(cnt->ptr);
@@ -824,7 +813,6 @@ std::vector<HostCol> download_batch(const Exec& x, const DevBatch& b, int64_t r0
       if (n) {
         DevPtr bm = dev_alloc((size_t)(n + 7) / 8 + 16, st);
         launch_bytes_to_bitmap(c.data, (uint8_t*)bm->ptr, n, nullptr, st);
-        x.count();
         CUDA_CHECK(cudaMemcpyAsync(h.data.data(), bm->ptr, h.data.size(), cudaMemcpyDeviceToHost, st));
         CUDA_CHECK(cudaStreamSynchronize(st));
       }
@@ -941,7 +929,6 @@ bool partition_for_groupby(const Exec& x, GroupBySpec& S, std::vector<DevPtr>& k
   CUDA_CHECK(launch_partition_scatter(ps, n, K, (const uint64_t*)offs->ptr, gc, nullptr, x.st()));
   DevPtr row_start = dev_alloc((size_t)(K + 1) * 8 + 64, x.st()), cta_start = dev_alloc((size_t)(K + 1) * 4 + 64, x.st());
   CUDA_CHECK(launch_groupby_plan((const unsigned long long*)acc->ptr, (int)K, (unsigned long long*)row_start->ptr, (unsigned int*)cta_start->ptr, x.st()));
-  x.count(6);
   S.pf_K = (int)K;
   S.pf_slots = S.table.cap / K;
   S.pf_row_start = (const unsigned long long*)row_start->ptr;
@@ -1049,7 +1036,6 @@ RunOutcome launch_program(const Exec& x, PipelineBuilder& pb, int reg_groups, co
     CUDA_CHECK(le);
   }
   CUDA_CHECK(cudaEventRecord(e1, x.st()));
-  x.count();
   RunOutcome o;
   const RunStatus* hs = x.fetch<RunStatus>(dstat->ptr);
   const unsigned int* he = extra_fetch ? x.fetch<unsigned int>(extra_fetch) : nullptr;
@@ -1133,7 +1119,6 @@ DevBatchPtr run_materialize(const Exec& x, PipelineBuilder& pb, const std::vecto
   if (met) {
     met->bytes_read += source_bytes(pb);
     met->bytes_written += wbytes;
-    met->launches += 1;
   }
   return out;
 }
@@ -2061,7 +2046,6 @@ TableMem alloc_table(const Exec& x, uint64_t cap, int n_keys, const std::vector<
   k.n = (int)accs.size();
   for (size_t i = 0; i < accs.size(); i++) k.kind[i] = accs[i].kind;
   launch_agg_table_init(tm.T, k, x.st());
-  x.count();
   return tm;
 }
 
@@ -2206,7 +2190,6 @@ DevBatchPtr run_aggregate(const Exec& x, const BuilderFactory& make_pb, const Pl
       ScopeTimer t_l("    agg: launch_program (incl. sync)");
       ro = launch_program(x, pb, reg_groups, use_fused ? &fspec : nullptr, true, met, tm.T.n_groups, &n_groups, use_gb ? &gspec : nullptr);
     }
-    if (met) met->launches += 2;
     if (ro.status.pack_overflow && use_gb) {
       gb_bailed = true;  // operands outside the dedicated kernel's ranges: same table size on the general sink
       continue;
@@ -2233,7 +2216,6 @@ DevBatchPtr run_aggregate(const Exec& x, const BuilderFactory& make_pb, const Pl
     P.mom_pass = 1;
     RunOutcome r2 = launch_program(x, *pbp, reg_groups, nullptr, true, met);
     P.mom_pass = 0;
-    if (met) met->launches += 1;
     if (r2.status.overflow) throw EngineError(B200_ERR_EXECUTION, "aggregate: a group of the first pass was not found by the second");
   }
   {
@@ -2295,7 +2277,6 @@ DevBatchPtr run_aggregate(const Exec& x, const BuilderFactory& make_pb, const Pl
     out->cols.push_back(oc);
   }
   launch_agg_extract(tm.T, A, x.st());
-  x.count();
   // string MIN / MAX results are views of the input's characters (or of a literal of the pipeline): copy them into a
   // buffer of their own, so that the result outlives the input and a few strings do not pin a multi-GB character buffer.
   // The character total is not known on the host: each such column costs three launches and one read-back of it.
@@ -2478,17 +2459,32 @@ struct Runner {
     return outs;
   }
 
-  // B200_TIMING=1: inclusive host wall time per operator (launch + synchronisation overheads)
+  // Runs operator n and charges it (its kernel_launches metric) the kernels it launched itself: what this thread enqueued
+  // meanwhile, less what the operators it ran through exec() enqueued -- they are charged their own.  Filter / projection
+  // nodes fused into a parent's chain run inside the parent and are charged to it.  Returns the operator's own launches.
+  uint64_t nested_launches = 0;  // kernels enqueued inside the charged calls of this Runner so far
+  template <class F>
+  uint64_t charge_launches(const PlanNode& n, F&& run) {
+    const uint64_t l0 = launches_on_thread(), n0 = nested_launches;
+    run();
+    const uint64_t all = launches_on_thread() - l0, own = all - (nested_launches - n0);
+    nested_launches = n0 + all;
+    if (OpMetrics* m = x.m(&n)) m->launches += own;
+    return own;
+  }
+
+  // B200_TIMING=1: inclusive host wall time per operator (launch + synchronisation overheads) and its own launches
   DevBatchPtr exec(const PlanNode& n, int part) {
     static const bool timing = getenv("B200_TIMING") != nullptr;
-    if (!timing) return exec_impl(n, part);
     const auto t0 = std::chrono::steady_clock::now();
-    const uint64_t l0 = x.e->launches;
-    DevBatchPtr out = exec_impl(n, part);
-    cudaStreamSynchronize(x.st());
-    const double ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
-    fprintf(stderr, "[b200-time] op=%d part=%d rows_out=%lld host_ms=%.3f launches=%llu\n", (int)n.op, part, (long long)(out ? out->n : -1), ms,
-            (unsigned long long)(x.e->launches - l0));
+    DevBatchPtr out;
+    const uint64_t own = charge_launches(n, [&] { out = exec_impl(n, part); });
+    if (timing) {
+      cudaStreamSynchronize(x.st());
+      const double ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
+      fprintf(stderr, "[b200-time] op=%d part=%d rows_out=%lld host_ms=%.3f launches=%llu\n", (int)n.op, part, (long long)(out ? out->n : -1), ms,
+              (unsigned long long)own);
+    }
     return out;
   }
   DevBatchPtr exec_impl(const PlanNode& n, int part) {
@@ -2649,7 +2645,6 @@ struct Runner {
       }
       DevPtr idx = dev_alloc((size_t)n * 8, x.st());
       launch_small_sort(K, (int64_t*)idx->ptr, n, x.st());
-      x.count();
       const int64_t m = fetch >= 0 ? std::min<int64_t>(fetch, n) : n;
       DevBatch proj;
       proj.n = n;
@@ -2669,7 +2664,6 @@ struct Runner {
     uint32_t* perm = (uint32_t*)va->ptr;
     uint32_t* perm_alt = (uint32_t*)vb->ptr;
     launch_iota_u32(perm, n, x.st());
-    x.count();
     for (size_t ki = keys.size(); ki-- > 0;) {
       DevColumn kc = as_views(x, kcols[ki]);
       int n_words = 1;
@@ -2678,7 +2672,6 @@ struct Runner {
         DevPtr mx = dev_alloc(16, x.st());
         CUDA_CHECK(cudaMemsetAsync(mx->ptr, 0, 16, x.st()));
         launch_max_view_len((const unsigned long long*)kc.data, kc.valid, n, (unsigned int*)mx->ptr, x.st());
-        x.count();
         unsigned int maxlen = x.get<unsigned int>(mx->ptr);
         n_words = (int)(maxlen / 7) + 1;
       }
@@ -2694,25 +2687,21 @@ struct Runner {
         A.word = w;
         uint64_t* kin = (uint64_t*)ka->ptr;
         launch_sort_word(A, perm, kin, n, x.st());
-        x.count();
         bool in_a;
-        uint64_t ln = 0;
         if (perm == (uint32_t*)va->ptr) {
-          radix_sort_pairs_u64((uint64_t*)ka->ptr, (uint32_t*)va->ptr, (uint64_t*)kb->ptr, (uint32_t*)vb->ptr, n, (uint32_t*)hist->ptr, (uint64_t*)scan->ptr, x.st(), &in_a, &ln);
+          radix_sort_pairs_u64((uint64_t*)ka->ptr, (uint32_t*)va->ptr, (uint64_t*)kb->ptr, (uint32_t*)vb->ptr, n, (uint32_t*)hist->ptr, (uint64_t*)scan->ptr, x.st(), &in_a);
           perm = in_a ? (uint32_t*)va->ptr : (uint32_t*)vb->ptr;
         } else {
           // current permutation lives in vb: sort with roles swapped (keys were written to ka)
-          radix_sort_pairs_u64((uint64_t*)ka->ptr, (uint32_t*)vb->ptr, (uint64_t*)kb->ptr, (uint32_t*)va->ptr, n, (uint32_t*)hist->ptr, (uint64_t*)scan->ptr, x.st(), &in_a, &ln);
+          radix_sort_pairs_u64((uint64_t*)ka->ptr, (uint32_t*)vb->ptr, (uint64_t*)kb->ptr, (uint32_t*)va->ptr, n, (uint32_t*)hist->ptr, (uint64_t*)scan->ptr, x.st(), &in_a);
           perm = in_a ? (uint32_t*)vb->ptr : (uint32_t*)va->ptr;
         }
-        x.count(ln);
         (void)perm_alt;
       }
     }
     int64_t m = fetch >= 0 ? std::min<int64_t>(fetch, n) : n;
     DevPtr idx = dev_alloc((size_t)std::max<int64_t>(m, 1) * 8, x.st());
     launch_u32_to_i64(perm, (int64_t*)idx->ptr, m, x.st());
-    x.count();
     DevBatch proj;
     proj.n = n;
     for (size_t c = 0; c < n_in_cols; c++) proj.cols.push_back(in->cols[c]);
@@ -2856,7 +2845,6 @@ struct Runner {
       KernelTimer kt(x, "join_build", (uint64_t)nb * (key_bytes_b + sizeof(JoinNode)) + n_buckets * 4);
       CUDA_CHECK(cudaMemsetAsync(heads->ptr, 0xFF, (size_t)n_buckets * 4, x.st()));
       launch_join_build2(K, exact, L.hash, nb, (int32_t*)heads->ptr, n_buckets, (JoinNode*)nodes->ptr, x.st());
-      x.count();
     }
     x.check_cancel();
     const bool has_filter = n.join_filter != nullptr;
@@ -2895,7 +2883,6 @@ struct Runner {
           launch_join_probe2(K, exact, mode, (const JoinNode*)nodes->ptr, (const int32_t*)heads->ptr, n_buckets, R.hash, np, (unsigned long long*)counter->ptr, cap,
                              need_pairs ? (int64_t*)bi->ptr : nullptr, need_pairs ? (int64_t*)pi->ptr : nullptr, pmark ? (uint8_t*)pmark->ptr : nullptr,
                              bmark ? (uint8_t*)bmark->ptr : nullptr, x.st());
-          x.count();
         }
         if (!need_pairs) break;
         n_pairs = (int64_t)x.get<unsigned long long>(counter->ptr);
@@ -2957,11 +2944,9 @@ struct Runner {
       DevPtr sc = dev_alloc((size_t)(nrows / 1024 + 4) * 8, x.st());
       launch_flag_to_u32(marks, want ? 1 : 0, (uint32_t*)f->ptr, nrows, x.st());
       launch_scan_u32_to_u64((const uint32_t*)f->ptr, (uint64_t*)o->ptr, nrows, (uint64_t*)sc->ptr, x.st());
-      x.count(4);
       *n_sel = (int64_t)x.get<uint64_t>((const uint64_t*)o->ptr + nrows);
       DevPtr idx = dev_alloc((size_t)std::max<int64_t>(*n_sel, 1) * 8, x.st());
       launch_select_indices((const uint32_t*)f->ptr, (const uint64_t*)o->ptr, (int64_t*)idx->ptr, nrows, x.st());
-      x.count();
       return idx;
     };
     auto marks_of = [&](const int64_t* idx, int64_t nrows, const DevPtr& from_probe) {
@@ -2970,7 +2955,6 @@ struct Runner {
       CUDA_CHECK(cudaMemsetAsync(m->ptr, 0, (size_t)std::max<int64_t>(nrows, 1), x.st()));
       if (n_pairs > 0) {
         launch_mark_from_idx(idx, n_pairs, (uint8_t*)m->ptr, x.st());
-        x.count();
       }
       return m;
     };
@@ -3221,7 +3205,6 @@ struct Runner {
     {
       KernelTimer kt(x, "nlj_count", operand_bytes);
       launch_nlj_count(L.S, nb, np, (uint32_t*)counts->ptr, bmark ? (uint8_t*)bmark->ptr : nullptr, pmark ? (uint8_t*)pmark->ptr : nullptr, x.st());
-      x.count();
     }
     x.e->nlj_pairs += (uint64_t)nb * (uint64_t)np;
     x.check_cancel();
@@ -3233,7 +3216,6 @@ struct Runner {
       DevPtr scratch = dev_alloc((size_t)(np / 1024 + 4) * 8, x.st());
       if (np > 0) {
         launch_scan_u32_to_u64((const uint32_t*)counts->ptr, (uint64_t*)offs->ptr, np, (uint64_t*)scratch->ptr, x.st());
-        x.count(3);
         n_pairs = (int64_t)x.get<uint64_t>((const uint64_t*)offs->ptr + np);
         x.check_cancel();
       }
@@ -3242,7 +3224,6 @@ struct Runner {
       if (n_pairs > 0) {
         KernelTimer kt(x, "nlj_write", operand_bytes + 16 * (uint64_t)n_pairs);
         launch_nlj_write(L.S, nb, np, (const uint32_t*)counts->ptr, (const uint64_t*)offs->ptr, (int64_t*)bi->ptr, (int64_t*)pi->ptr, x.st());
-        x.count();
       }
       x.check_cancel();
     }
@@ -3288,7 +3269,6 @@ struct Runner {
       PidSrc none;
       memset(&none, 0, sizeof none);
       CUDA_CHECK(launch_partition_hist(none, b.n, 1, nullptr, (unsigned long long*)acc->ptr, sc, (unsigned long long*)acc->ptr + 1, x.st()));
-      x.count();
       const unsigned long long* h = (const unsigned long long*)x.fetch_bytes((const unsigned long long*)acc->ptr + 1, (size_t)sc.n * 8);
       x.sync();
       for (size_t k = 0; k < unknown.size(); k++) out[unknown[k]] = (int64_t)h[k];
@@ -3337,7 +3317,7 @@ struct Runner {
       NCCL_CHECK(N.Recv(mrows + mrow * (size_t)d, mrow * 8, kNcclUint8, d, e->comm, x.st()));
     }
     NCCL_CHECK(N.GroupEnd());
-    x.count(1);
+    count_launches();
     // (the matrix and the base table below can exceed the task's pinned arena at large fan-outs: plain host vectors)
     std::vector<unsigned long long> Mv(mrow * (size_t)W);
     CUDA_CHECK(cudaMemcpyAsync(Mv.data(), mat->ptr, Mv.size() * 8, cudaMemcpyDeviceToHost, x.st()));
@@ -3348,7 +3328,6 @@ struct Runner {
     DevPtr scratch = dev_alloc((size_t)(hn / 1024 + 4) * 8, x.st());
     if (hn > 0) {
       launch_scan_u32_to_u64((const uint32_t*)tile_hist->ptr, (uint64_t*)offs->ptr, hn, (uint64_t*)scratch->ptr, x.st());
-      x.count(3);
     }
     x.sync();
     auto cnt = [&](int s, uint32_t p) { return (uint64_t)M[mrow * (size_t)s + p]; };
@@ -3404,7 +3383,6 @@ struct Runner {
           for (int k = 0; k < gc.n; k++) b += (uint64_t)gc.c[k].width;
           KernelTimer kt(x, "partition_scatter_peer", (uint64_t)n * (2 * b + 4));
           CUDA_CHECK(launch_partition_scatter(pid, n, P, (const uint64_t*)offs->ptr, gc, nullptr, x.st()));
-          x.count();
         }
         gc.n = 0;
       };
@@ -3442,7 +3420,7 @@ struct Runner {
         NCCL_CHECK(N.Recv((uint8_t*)bar->ptr + 8 * (size_t)d, 8, kNcclUint8, d, e->comm, x.st()));
       }
       NCCL_CHECK(N.GroupEnd());
-      x.count(1);
+      count_launches();
     }
     e->win_used = cursor[(size_t)me];
     // the reduce side's view: one batch per owned partition, one piece per map task
@@ -3509,6 +3487,11 @@ struct Runner {
   }
 
   std::vector<b200_shuffle_write_partition> execute_stage(const PlanNode& root, int input_partition, FusedExchange* fx = nullptr) {
+    std::vector<b200_shuffle_write_partition> res;
+    charge_launches(root, [&] { res = write_stage(root, input_partition, fx); });
+    return res;
+  }
+  std::vector<b200_shuffle_write_partition> write_stage(const PlanNode& root, int input_partition, FusedExchange* fx) {
     if (root.op != PlanNode::ShuffleWriter) throw EngineError(B200_ERR_INVALID, "stage plan root must be a ShuffleWriterExec");
     OpMetrics* met = x.m(&root);
     const PlanNode& child = *root.children[0];
@@ -3648,7 +3631,6 @@ struct Runner {
       for (int k = 0; k < pid.n_keys; k++) kb += pid.keys[k].width;
       KernelTimer kt(x, "partition_hist", (uint64_t)n * kb);
       CUDA_CHECK(launch_partition_hist(pid, n, P, (uint32_t*)tile_hist->ptr, acc_ptr, sc, acc_ptr + P, x.st()));
-      x.count();
     }
     if (fuse) {
       std::vector<b200_shuffle_write_partition> fr;
@@ -3661,7 +3643,6 @@ struct Runner {
     DevPtr scratch = dev_alloc((size_t)(hn / 1024 + 4) * 8, x.st());
     if (hn > 0) {
       launch_scan_u32_to_u64((const uint32_t*)tile_hist->ptr, (uint64_t*)offs->ptr, hn, (uint64_t*)scratch->ptr, x.st());
-      x.count(3);
     }
     auto st = std::make_shared<DevBatch>();
     st->n = n;
@@ -3674,7 +3655,6 @@ struct Runner {
           for (int k = 0; k < gc.n; k++) b += (uint64_t)gc.c[k].width;
           KernelTimer kt(x, "partition_scatter", (uint64_t)n * (2 * b + 4));
           CUDA_CHECK(launch_partition_scatter(pid, n, P, (const uint64_t*)offs->ptr, gc, nullptr, x.st()));
-          x.count();
         }
         gc.n = 0;
       };
@@ -3951,7 +3931,6 @@ struct Exchange {
                 DevPtr ro = dev_alloc((size_t)(u.n + 1) * 4 + 64, x.st());
                 DevPtr fl = dev_alloc(16, x.st());
                 launch_rebase_offsets((const int32_t*)u.data, u.n + 1, (int32_t*)ro->ptr, (int32_t*)fl->ptr, x.st());
-                x.count();
                 // first offset of the slice: needed on the host to position the chars pointer
                 const int32_t first = x.get<int32_t>(fl->ptr);
                 chars = u.chars + first;
@@ -3979,7 +3958,7 @@ struct Exchange {
       NCCL_CHECK(N.Recv((uint8_t*)recvbuf->ptr + (size_t)d * slot, slot, kNcclUint8, d, e->comm, x.st()));
     }
     NCCL_CHECK(N.GroupEnd());
-    x.count(1);
+    count_launches();
     // incoming headers: every peer used hdr_bytes(me)
     const size_t hb = hdr_bytes(me);
     std::vector<const uint64_t*> rh((size_t)W, nullptr);
@@ -4055,7 +4034,7 @@ struct Exchange {
       for (auto& so : sends) NCCL_CHECK(N.Send(so.ptr, so.bytes, kNcclUint8, so.peer, e->comm, x.st()));
       for (auto& ro : recvs) NCCL_CHECK(N.Recv(ro.ptr, ro.bytes, kNcclUint8, ro.peer, e->comm, x.st()));
       NCCL_CHECK(N.GroupEnd());
-      x.count(1);
+      count_launches();
     }
     // ---- install ---------------------------------------------------------------------------------------------
     {
@@ -4324,15 +4303,12 @@ DevBatchPtr scan_parquet(const Exec& x, const std::string& path, const std::vect
         if (codec == pq::C_SNAPPY) {
           KernelTimer kt(x, "parquet_snappy", bytes);
           launch_pq_snappy(jobs, (int)(j1 - j0), e, st);
-          x.count();
         } else if (codec == pq::C_GZIP) {
           KernelTimer kt(x, "parquet_gzip", bytes);
           launch_pq_inflate(jobs, (int)(j1 - j0), e, st);
-          x.count();
         } else {
           KernelTimer kt(x, "parquet_lz4", bytes);
           launch_pq_lz4(jobs, (int)(j1 - j0), e, st);
-          x.count();
         }
         j0 = j1;
       }
@@ -4383,7 +4359,6 @@ DevBatchPtr scan_parquet(const Exec& x, const std::string& path, const std::vect
       w.dict = dev_alloc((size_t)c.dict_entries * (size_t)w.width + 64, st);
       w.pc.dict = w.dict->ptr;
       launch_pq_dict(w.pc, (const PqPage*)w.d_dicts->ptr, (int)c.dicts.size(), st);
-      x.count();
     }
     if (c.optional) {
       w.valid = dev_alloc((size_t)std::max<int64_t>(n_rows, 1) + 64, st);
@@ -4393,7 +4368,6 @@ DevBatchPtr scan_parquet(const Exec& x, const std::string& path, const std::vect
       CUDA_CHECK(cudaMemsetAsync(w.total->ptr, 0, 16, st));
       launch_pq_levels((const PqPage*)w.d_pages->ptr, (int)c.pages.size(), (uint8_t*)w.valid->ptr, (uint32_t*)w.nonnull->ptr, (unsigned long long*)w.total->ptr, st);
       launch_pq_page_scan((const uint32_t*)w.nonnull->ptr, (int)c.pages.size(), (unsigned long long*)w.dense_base->ptr, st);
-      x.count(2);
       w.h_total = x.fetch<unsigned long long>(w.total->ptr);
     }
     if (c.delta_pages) {
@@ -4422,10 +4396,8 @@ DevBatchPtr scan_parquet(const Exec& x, const std::string& path, const std::vect
         KernelTimer kt(x, "parquet_delta_prepare", c.delta_bytes + (c.dba_pages ? (uint64_t)n_rows * 8 : 0));
         launch_pq_delta_prepare(w.pc, (const PqPage*)w.d_pages->ptr, (int)c.pages.size(), c.optional ? (const unsigned long long*)w.dense_base->ptr : nullptr,
                                 c.optional ? (const uint32_t*)w.nonnull->ptr : nullptr, w.aux, st);
-        x.count();
         if (dba_strings) {
           launch_pq_page_scan((const uint32_t*)w.page_bytes->ptr, (int)c.pages.size(), (unsigned long long*)w.char_base->ptr, st);
-          x.count();
         }
       }
       w.h_err = x.fetch<unsigned int>(w.d_err->ptr);
@@ -4453,10 +4425,8 @@ DevBatchPtr scan_parquet(const Exec& x, const std::string& path, const std::vect
       KernelTimer kt(x, "parquet_decode_values", (uint64_t)n_rows * (uint64_t)w.width);
       if (!has_nulls) {
         launch_pq_values(w.pc, (const PqPage*)w.d_pages->ptr, (int)c.pages.size(), nullptr, nullptr, w.out->ptr, st);
-        x.count();
         if (c.delta_pages) {
           launch_pq_values_delta(w.pc, (const PqPage*)w.d_pages->ptr, (int)c.pages.size(), nullptr, nullptr, w.out->ptr, w.aux, st);
-          x.count();
         }
       } else {
         DevPtr dense = dev_alloc((size_t)std::max<int64_t>(n_rows, 1) * (size_t)w.width + 64, st);
@@ -4464,11 +4434,9 @@ DevBatchPtr scan_parquet(const Exec& x, const std::string& path, const std::vect
         if (c.delta_pages) {
           launch_pq_values_delta(w.pc, (const PqPage*)w.d_pages->ptr, (int)c.pages.size(), (const unsigned long long*)w.dense_base->ptr, (const uint32_t*)w.nonnull->ptr,
                                  dense->ptr, w.aux, st);
-          x.count();
         }
         launch_pq_expand((const PqPage*)w.d_pages->ptr, (int)c.pages.size(), (const unsigned long long*)w.dense_base->ptr, (const uint8_t*)w.valid->ptr, dense->ptr,
                          w.out->ptr, w.width, st);
-        x.count(2);
       }
     }
     DevColumn col;
@@ -4535,6 +4503,16 @@ int guard(F&& f) {
     g_err = "unknown error";
     return B200_ERR_INVALID;
   }
+}
+
+// guard() for an entry point that launches kernels for engine e: what this thread enqueued during the call, whether it
+// succeeds or fails, goes to e's count (b200_engine_kernel_launches)
+template <class F>
+int guard(b200_engine* e, F&& f) {
+  const uint64_t l0 = launches_on_thread();
+  const int rc = guard(std::forward<F>(f));
+  if (e) e->launches += launches_on_thread() - l0;
+  return rc;
 }
 
 }  // namespace
@@ -4724,6 +4702,8 @@ void b200_engine_destroy(b200_engine* e) {
   release_window(e);
   if (e->comm && NcclApi::get().ok()) NcclApi::get().CommDestroy(e->comm);
   if (e->export_arena) cudaFreeHost(e->export_arena);
+  // the calling thread's arena chunk is freed on the stream it was carved for: not after that stream is gone (at exit)
+  if (arena_chunk() && arena_chunk()->stream == e->own_stream) arena_chunk().reset();
   if (e->own_stream) cudaStreamDestroy(e->own_stream);
   delete e;
 }
@@ -4779,7 +4759,7 @@ int b200_engine_set_config(b200_engine* e, const char* key, const char* value) {
 }
 
 int b200_engine_register_batch(b200_engine* e, const char* table, int partition, struct ArrowArray* batch, struct ArrowSchema* schema) {
-  return guard([&] {
+  return guard(e, [&] {
     CUDA_CHECK(cudaSetDevice(e->device));
     DevBatchPtr b = import_batch(e, batch, schema);
     Exec x{e, nullptr, nullptr};
@@ -4815,7 +4795,7 @@ int b200_engine_drop_table(b200_engine* e, const char* table) {
 }
 
 int b200_engine_tpch_generate(b200_engine* e, const char* table, int64_t msf, int partition, int64_t row_begin, int64_t row_end, const char* columns_csv) {
-  return guard([&] {
+  return guard(e, [&] {
     CUDA_CHECK(cudaSetDevice(e->device));
     int t = table_id(table);
     if (t < 0) throw EngineError(B200_ERR_INVALID, std::string("unknown TPC-H table ") + table);
@@ -4862,13 +4842,11 @@ int b200_engine_tpch_generate(b200_engine* e, const char* table, int64_t msf, in
         DevPtr scratch = dev_alloc((size_t)(n / 1024 + 4) * 8, st);
         launch_tpch_str_len(t, c, msf, row_begin, n, (uint32_t*)lens->ptr, st);
         launch_scan_u32_to_u64((const uint32_t*)lens->ptr, (uint64_t*)offs64->ptr, n, (uint64_t*)scratch->ptr, st);
-        e->launches += 4;
         uint64_t total = Exec{e, nullptr, nullptr}.get<uint64_t>((const uint64_t*)offs64->ptr + n);
         if (total > 0x7FFFFFFFull) throw EngineError(B200_ERR_UNSUPPORTED, "generated string column exceeds 2 GiB; use more partitions");
         DevPtr offsets = dev_alloc((size_t)(n + 1) * 4 + 64, st);
         DevPtr chars = dev_alloc((size_t)total + 64, st);
         launch_tpch_str_fill(t, c, msf, row_begin, n, (const uint64_t*)offs64->ptr, (int32_t*)offsets->ptr, (uint8_t*)chars->ptr, st);
-        e->launches++;
         col.data = (const uint8_t*)offsets->ptr;
         col.chars = (const uint8_t*)chars->ptr;
         col.chars_bytes = (int64_t)total;
@@ -4877,7 +4855,6 @@ int b200_engine_tpch_generate(b200_engine* e, const char* table, int64_t msf, in
       } else {
         DevPtr d = dev_alloc((size_t)std::max<int64_t>(n, 1) * col.width() + 64, st);
         launch_tpch_fixed(t, c, cd.kind, msf, row_begin, n, d->ptr, st);
-        e->launches++;
         col.data = (const uint8_t*)d->ptr;
         col.keep.push_back(d);
       }
@@ -4967,7 +4944,7 @@ int b200_parquet_describe(const char* path, char* out, uint64_t cap) {
 }
 
 int b200_engine_register_parquet(b200_engine* e, const char* table, int partition, const char* path, const char* columns_csv) {
-  return guard([&] {
+  return guard(e, [&] {
     if (!e || !table || !path) throw EngineError(B200_ERR_INVALID, "null argument");
     CUDA_CHECK(cudaSetDevice(e->device));
     std::vector<std::string> cols;
@@ -5001,7 +4978,7 @@ int64_t b200_tpch_table_rows(const char* table, int64_t msf) {
 }
 
 int b200_engine_export_table(b200_engine* e, const char* table, int partition, struct ArrowArray* out, struct ArrowSchema* out_schema) {
-  return guard([&] {
+  return guard(e, [&] {
     CUDA_CHECK(cudaSetDevice(e->device));
     DevBatchPtr b;
     {
@@ -5209,7 +5186,7 @@ int b200_task_status_encode(const char* job_id, const char* executor_id, const b
 
 int b200_stage_execute(b200_stage* s, int input_partition, const volatile int32_t* cancel_flag, b200_shuffle_write_partition* out, int cap, int* n_out) {
   ScopeTimer tm("stage_execute");
-  return guard([&] {
+  return guard(s ? s->eng : nullptr, [&] {
     if (!s || !n_out) throw EngineError(B200_ERR_INVALID, "null argument");
     CUDA_CHECK(cudaSetDevice(s->eng->device));
     Exec x{s->eng, s, cancel_flag};
@@ -5247,7 +5224,7 @@ int b200_stage_execute(b200_stage* s, int input_partition, const volatile int32_
 int b200_stage_execute_exchange(b200_stage* s, int input_partition, const volatile int32_t* cancel_flag, b200_shuffle_write_partition* out, int cap,
                                 int* n_out, b200_exchange_stats* stats) {
   ScopeTimer tm("stage_execute_exchange");
-  return guard([&] {
+  return guard(s ? s->eng : nullptr, [&] {
     if (!s || !n_out) throw EngineError(B200_ERR_INVALID, "null argument");
     b200_engine* e = s->eng;
     if (s->plan->op != PlanNode::ShuffleWriter || s->plan->n_out_partitions < 1)
@@ -5306,7 +5283,7 @@ void b200_stage_release(b200_stage* s) { delete s; }
 
 int b200_partition_export(b200_engine* e, const char* job_id, int64_t stage_id, int out_partition, struct ArrowArray* out, struct ArrowSchema* out_schema) {
   ScopeTimer tm("partition_export");
-  return guard([&] {
+  return guard(e, [&] {
     CUDA_CHECK(cudaSetDevice(e->device));
     std::vector<std::pair<DevBatchPtr, std::pair<int64_t, int64_t>>> pieces;
     {
@@ -5429,7 +5406,7 @@ int b200_engine_comm_init(b200_engine* e, const void* nccl_id, uint64_t id_bytes
 
 int b200_exchange_stage(b200_engine* e, const char* job_id, int64_t stage_id, int n_out_partitions, int mode, int root, const char* schema_json,
                         b200_exchange_stats* stats) {
-  return guard([&] {
+  return guard(e, [&] {
     if (!e || !job_id || !schema_json) throw EngineError(B200_ERR_INVALID, "null argument");
     if (mode < 0 || mode > 2 || n_out_partitions < 0 || root < 0 || root >= std::max(e->world, 1)) throw EngineError(B200_ERR_INVALID, "b200_exchange_stage: bad mode / root");
     CUDA_CHECK(cudaSetDevice(e->device));
@@ -5574,7 +5551,7 @@ int b200_ipc_decode(const uint8_t* buf, uint64_t len, struct ArrowArray* out, st
 // readable by the reference's own readers (a CPU executor's ShuffleReaderExec, the Flight service).
 int b200_shuffle_write_files(b200_engine* e, const char* job_id, int64_t stage_id, const char* work_dir, int n_out_partitions, int sort_layout,
                              uint64_t* files_written, uint64_t* bytes_written) {
-  return guard([&] {
+  return guard(e, [&] {
     if (!e || !job_id || !work_dir) throw EngineError(B200_ERR_INVALID, "null argument");
     CUDA_CHECK(cudaSetDevice(e->device));
     Exec x{e, nullptr, nullptr};
@@ -5649,7 +5626,7 @@ int b200_shuffle_write_files(b200_engine* e, const char* job_id, int64_t stage_i
 // use_index != 0: `path` is a sort-shuffle data file, the range of `out_partition` is taken from `path` + ".index".
 int b200_shuffle_read_file(b200_engine* e, const char* job_id, int64_t stage_id, int out_partition, int64_t file_id, const char* path, uint64_t byte_offset,
                            uint64_t byte_length, int use_index) {
-  return guard([&] {
+  return guard(e, [&] {
     if (!e || !job_id || !path) throw EngineError(B200_ERR_INVALID, "null argument");
     CUDA_CHECK(cudaSetDevice(e->device));
     std::vector<HostCol> cols;
