@@ -205,7 +205,7 @@ inline DataType int_as_decimal(const DataType& t) {
   }
 }
 
-enum class BinOp : uint8_t { Add, Sub, Mul, Div, Mod, Eq, Ne, Lt, Le, Gt, Ge, And, Or };
+enum class BinOp : uint8_t { Add, Sub, Mul, Div, Mod, Eq, Ne, Lt, Le, Gt, Ge, And, Or, BitAnd, BitOr, BitXor, Shl, Shr };
 
 inline BinOp parse_binop(const std::string& s) {
   static const std::pair<const char*, BinOp> tab[] = {
@@ -213,7 +213,8 @@ inline BinOp parse_binop(const std::string& s) {
       {"%", BinOp::Mod},  {"=", BinOp::Eq},   {"==", BinOp::Eq},  {"!=", BinOp::Ne},
       {"<>", BinOp::Ne},  {"<", BinOp::Lt},   {"<=", BinOp::Le},  {">", BinOp::Gt},
       {">=", BinOp::Ge},  {"and", BinOp::And}, {"or", BinOp::Or},  {"AND", BinOp::And},
-      {"OR", BinOp::Or}};
+      {"OR", BinOp::Or},  {"&", BinOp::BitAnd}, {"|", BinOp::BitOr}, {"^", BinOp::BitXor},
+      {"<<", BinOp::Shl}, {">>", BinOp::Shr}};
   for (auto& kv : tab)
     if (s == kv.first) return kv.second;
   throw std::runtime_error("plan IR: unknown binary operator '" + s + "'");
@@ -221,6 +222,28 @@ inline BinOp parse_binop(const std::string& s) {
 inline bool is_arith(BinOp o) { return o <= BinOp::Mod; }
 inline bool is_compare(BinOp o) { return o >= BinOp::Eq && o <= BinOp::Ge; }
 inline bool is_logic(BinOp o) { return o == BinOp::And || o == BinOp::Or; }
+inline bool is_bitwise(BinOp o) { return o >= BinOp::BitAnd; }
+
+// Grouping sets (ROLLUP / CUBE / GROUPING SETS) and the bitwise operators DataFusion rewrites GROUPING() into are typed
+// here for every consumer of the plan IR, but only a consumer built with B200_PLAN_GROUPING_SETS=1 computes them (the
+// device engine: Makefile NVFLAGS).  Any other consumer -- the CPU oracle -- refuses such a plan instead of mis-evaluating it.
+#ifndef B200_PLAN_GROUPING_SETS
+#define B200_PLAN_GROUPING_SETS 0
+#endif
+// the grouping-set id occupies one more group key of the device table (VM_MAX_KEYS = 8, csrc/device/program.h)
+static const size_t kMaxGroupingSetKeys = 7;
+static const size_t kMaxGroupingSets = 32;
+// [EXT] DataFusion 53 PhysicalGroupBy: the keys are folded from first to last, id = id << 1 | is_null, so the first key is
+// the most significant bit; `mask` has bit k set when key k is replaced by NULL in the set
+inline uint64_t grouping_id(uint32_t mask, size_t n_keys) {
+  uint64_t id = 0;
+  for (size_t k = 0; k < n_keys; k++) id = id << 1 | ((mask >> k) & 1u);
+  return id;
+}
+// [EXT] the type of __grouping_id: the narrowest unsigned integer with a bit per key
+inline DataType grouping_id_type(size_t n_keys) {
+  return DataType(n_keys <= 8 ? TypeId::UInt8 : n_keys <= 16 ? TypeId::UInt16 : n_keys <= 32 ? TypeId::UInt32 : TypeId::UInt64);
+}
 
 // Result type of decimal (op) decimal, following arrow-arith 58 `decimal_op` [EXT]:
 //   add/sub: scale = max(s1,s2); precision = min(38, max(p1-s1,p2-s2) + scale + 1)
@@ -476,6 +499,14 @@ inline ExprPtr parse_expr(const Json& j, const Schema& in) {
     e->args.push_back(parse_expr(j.at("r"), in));
     const DataType& a = e->args[0]->type;
     const DataType& b = e->args[1]->type;
+    if (is_bitwise(e->op)) {
+      // [EXT] arrow-rs bitwise kernels: integer operands of one type, the result has that type (DESIGN.md §6)
+      if (!B200_PLAN_GROUPING_SETS) throw PlanUnsupported("bitwise operators are not computed by this consumer of the plan IR");
+      if (!a.is_integer() || a != b) throw PlanUnsupported("bitwise operator between " + a.str() + " and " + b.str() + " (integer operands of one type only)");
+      e->type = a;
+      e->nullable = e->args[0]->nullable || e->args[1]->nullable;
+      return e;
+    }
     if (is_arith(e->op)) e->type = arith_result_type(e->op, a, b);
     else e->type = DataType(TypeId::Bool);
     if (is_logic(e->op) && (a.id != TypeId::Bool || b.id != TypeId::Bool) && a.id != TypeId::Null && b.id != TypeId::Null)
@@ -715,6 +746,7 @@ struct PlanNode {
   AggMode agg_mode = AggMode::Single;
   std::vector<NamedExpr> group_by;
   std::vector<AggExpr> aggs;
+  std::vector<uint32_t> grouping_sets;  // empty: a plain GROUP BY; else one mask per set, bit k = key k replaced by NULL
   // HashJoin
   JoinType join_type = JoinType::Inner;
   std::string partition_mode;  // CollectLeft | Partitioned
@@ -838,6 +870,33 @@ inline PlanPtr parse_plan(const Json& j) {
       f.nullable = ne.expr->nullable;
       n->schema.push_back(f);
     }
+    if (j.has("grouping_sets")) {
+      // every row is aggregated once per set; the output holds the keys (all nullable), then __grouping_id (DESIGN.md §6)
+      if (!B200_PLAN_GROUPING_SETS) throw PlanUnsupported("grouping sets are not computed by this consumer of the plan IR");
+      if (from_states) throw std::runtime_error("AggregateExec: a Final-mode aggregate carries no grouping sets");
+      const Json& sets = j.at("grouping_sets");
+      const size_t nk = gs.size();
+      if (sets.size() == 0) throw std::runtime_error("AggregateExec: empty grouping_sets");
+      for (size_t s = 0; s < sets.size(); s++) {
+        const Json& set = sets.at(s);
+        if (set.size() != nk) throw std::runtime_error("AggregateExec: grouping set " + std::to_string(s) + " has " + std::to_string(set.size()) + " entries for " + std::to_string(nk) + " keys");
+        uint32_t mask = 0;
+        for (size_t k = 0; k < nk && k < 32; k++) mask |= (set.at(k).as_bool() ? 1u : 0u) << k;
+        n->grouping_sets.push_back(mask);
+      }
+      if (nk == 0) throw PlanUnsupported("grouping sets without a group key are not supported");
+      if (nk > kMaxGroupingSetKeys)
+        throw PlanUnsupported("grouping sets over " + std::to_string(nk) + " keys are not supported (at most " + std::to_string(kMaxGroupingSetKeys) + ")");
+      if (sets.size() > kMaxGroupingSets)
+        throw PlanUnsupported(std::to_string(sets.size()) + " grouping sets are not supported (at most " + std::to_string(kMaxGroupingSets) + ")");
+      for (size_t s = 0; s < n->grouping_sets.size(); s++)
+        for (size_t t = 0; t < s; t++)
+          if (n->grouping_sets[s] == n->grouping_sets[t])
+            throw PlanUnsupported("duplicate grouping set " + std::to_string(s) + " (same as set " + std::to_string(t) + ", __grouping_id " +
+                                  std::to_string(grouping_id(n->grouping_sets[s], nk)) + ")");
+      for (auto& f : n->schema) f.nullable = true;
+      n->schema.push_back(Field{"__grouping_id", grouping_id_type(nk), false});
+    }
     const Json& as = j.at("aggr");
     size_t state_col = gs.size();
     for (size_t i = 0; i < as.size(); i++) {
@@ -945,6 +1004,8 @@ inline PlanPtr parse_plan(const Json& j) {
       } else {
         n->schema.push_back(Field{ae.name, ae.result_type, ae.fn != AggFn::Count});
       }
+      if (!n->grouping_sets.empty() && agg_is_stat(ae.fn))
+        throw PlanUnsupported(a.at("fn").str() + " (" + ae.name + ") alongside grouping sets is not supported");
     }
   } else if (op == "HashJoinExec" || op == "SortMergeJoinExec" || op == "NestedLoopJoinExec") {
     // SortMergeJoinExec (datafusion.proto:1433, Ballista's default join, extension.rs:683): same matching

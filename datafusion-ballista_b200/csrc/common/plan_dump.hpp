@@ -19,7 +19,7 @@ inline std::string dump_schema(const Schema& s) {
 }
 
 inline std::string dump_expr(const ExprPtr& e) {
-  static const char* ops[] = {"+", "-", "*", "/", "%", "=", "!=", "<", "<=", ">", ">=", "and", "or"};
+  static const char* ops[] = {"+", "-", "*", "/", "%", "=", "!=", "<", "<=", ">", ">=", "and", "or", "&", "|", "^", "<<", ">>"};
   auto list = [&](size_t from) {
     std::string o = "[";
     for (size_t i = from; i < e->args.size(); i++) o += (i > from ? "," : "") + dump_expr(e->args[i]);
@@ -105,6 +105,14 @@ inline std::string dump_plan(const PlanNode& n) {
       o += std::string(",\"mode\":\"") + agg_modes[(int)n.agg_mode] + "\",\"group_by\":[";
       for (size_t i = 0; i < n.group_by.size(); i++)
         o += std::string(i ? "," : "") + "{\"expr\":" + dump_expr(n.group_by[i].expr) + ",\"name\":" + pbp::jstr(n.group_by[i].name) + "}";
+      if (!n.grouping_sets.empty()) {
+        o += "],\"grouping_sets\":[";
+        for (size_t s = 0; s < n.grouping_sets.size(); s++) {
+          o += s ? ",[" : "[";
+          for (size_t k = 0; k < n.group_by.size(); k++) o += std::string(k ? "," : "") + (((n.grouping_sets[s] >> k) & 1u) ? "true" : "false");
+          o += "]";
+        }
+      }
       o += "],\"aggr\":[";
       for (size_t i = 0; i < n.aggs.size(); i++) {
         const AggExpr& a = n.aggs[i];

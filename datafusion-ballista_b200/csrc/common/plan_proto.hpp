@@ -325,7 +325,8 @@ inline std::string binop_symbol(const std::string& op) {
   // BinaryExpr.op is the Debug name of datafusion_expr::Operator [EXT, datafusion-proto to_proto]
   static const std::pair<const char*, const char*> tab[] = {
       {"Eq", "="},     {"NotEq", "!="},   {"Lt", "<"},       {"LtEq", "<="},  {"Gt", ">"},   {"GtEq", ">="}, {"Plus", "+"},
-      {"Minus", "-"},  {"Multiply", "*"}, {"Divide", "/"},   {"Modulo", "%"}, {"And", "and"}, {"Or", "or"}};
+      {"Minus", "-"},  {"Multiply", "*"}, {"Divide", "/"},   {"Modulo", "%"}, {"And", "and"}, {"Or", "or"},
+      {"BitwiseAnd", "&"}, {"BitwiseOr", "|"}, {"BitwiseXor", "^"}, {"BitwiseShiftLeft", "<<"}, {"BitwiseShiftRight", ">>"}};
   for (auto& kv : tab)
     if (op == kv.first) return kv.second;
   throw Unsupported("binary operator " + op + " is not supported by the device engine");
@@ -570,9 +571,6 @@ inline std::string plan_json(const Msg& n, const std::string& override_job) {
       static const char* modes[] = {"Partial", "Final", "FinalPartitioned", "Single", "SinglePartitioned"};
       const uint64_t mode = m.u64(3);
       if (mode > 4) throw Unsupported("aggregate mode PartialReduce is not supported by the device engine");
-      if (m.boolean(12)) throw Unsupported("grouping sets are not supported by the device engine");
-      for (uint64_t g : m.varints(9))
-        if (g) throw Unsupported("grouping sets are not supported by the device engine");
       for (auto& f : m.subs(10))
         if (f.has(1)) throw Unsupported("aggregate FILTER clauses are not supported by the device engine");
       const std::vector<Msg> gs = m.subs(1), as = m.subs(2);
@@ -580,6 +578,32 @@ inline std::string plan_json(const Msg& n, const std::string& override_job) {
       if (gn.size() != gs.size() || an.size() != as.size()) throw std::runtime_error("plan proto: aggregate names do not match its expressions");
       std::string o = std::string("{\"op\":\"AggregateExec\",\"mode\":\"") + modes[mode] + "\",\"group_by\":[";
       for (size_t i = 0; i < gs.size(); i++) o += std::string(i ? "," : "") + "{\"expr\":" + expr_json(gs[i]) + ",\"name\":" + jstr(gn[i]) + "}";
+      // grouping sets: groups = 9 (S x n bools, row-major; true = the key is NULL in that set), null_expr = 8 (n NULL
+      // literals), has_grouping_set = 12.  A node is a grouping-set node iff has_grouping_set is set or some entry of
+      // groups is true [EXT]: a plain GROUP BY carries one all-false set and decodes as before, whatever null_expr holds.
+      const std::vector<uint64_t> groups = m.varints(9);
+      bool gsets = m.boolean(12);
+      for (uint64_t g : groups) gsets = gsets || g != 0;
+      if (gsets) {
+        const size_t nk = gs.size();
+        if (groups.empty() || nk == 0 || groups.size() % nk != 0)
+          throw std::runtime_error("plan proto: " + std::to_string(groups.size()) + " grouping-set entries for " + std::to_string(nk) + " group keys");
+        const std::vector<Msg> nulls = m.subs(8);
+        if (nulls.size() != nk) throw std::runtime_error("plan proto: " + std::to_string(nulls.size()) + " null_expr for " + std::to_string(nk) + " group keys");
+        static const std::string lit_head = "{\"lit\":", null_tail = ",\"v\":null}}";
+        for (auto& ne : nulls) {
+          const std::string lj = expr_json(ne);
+          if (lj.compare(0, lit_head.size(), lit_head) != 0 || lj.size() < null_tail.size() ||
+              lj.compare(lj.size() - null_tail.size(), null_tail.size(), null_tail) != 0)
+            throw std::runtime_error("plan proto: a grouping-set null_expr is not a NULL literal");
+        }
+        o += "],\"grouping_sets\":[";
+        for (size_t s = 0; s < groups.size() / nk; s++) {
+          o += s ? ",[" : "[";
+          for (size_t k = 0; k < nk; k++) o += std::string(k ? "," : "") + (groups[s * nk + k] ? "true" : "false");
+          o += "]";
+        }
+      }
       o += "],\"aggr\":[";
       for (size_t i = 0; i < as.size(); i++) {
         const Entry* ax = as[i].last(4);  // PhysicalExprNode.aggregate_expr

@@ -641,6 +641,33 @@ __device__ __noinline__ void scalar_str_op(const Lane L, const uint32_t active, 
   store_valid(L, ins.dst, va & vb);
 }
 
+// & | ^ << >> over integers of one type (aux = its Phys).  The values sit sign- or zero-extended in 64 bits, so & | ^ and
+// an arithmetic (signed) or logical (unsigned) >> stay in range; the lowering narrows << to the width.  Shift counts are
+// taken modulo the bit width, as Rust's wrapping_shl / wrapping_shr do in arrow-rs [EXT].
+__device__ __noinline__ void scalar_bit_op(const Lane L, const uint32_t active, const int pc) {
+  (void)active;
+  const VInstr ins = PROG.code[pc];
+  const uint32_t va = fetch_valid(L, ins.a), vb = fetch_valid(L, ins.b);
+  const uint8_t ph = ins.aux;
+  const uint64_t bits = (ph == PH_I8 || ph == PH_U8) ? 8 : (ph == PH_I16 || ph == PH_U16) ? 16 : (ph == PH_I32 || ph == PH_U32) ? 32 : 64;
+  const bool is_unsigned = ph >= PH_U8 && ph <= PH_U64;
+#pragma unroll 1
+  for (int r = 0; r < VM_R; r++) {
+    const int64_t a = ld1_i64(L, ins.a, r), b = ld1_i64(L, ins.b, r);
+    const uint32_t c = (uint32_t)((uint64_t)b & (bits - 1));
+    int64_t o;
+    switch (ins.op) {
+      case OP_BIT_AND: o = a & b; break;
+      case OP_BIT_OR: o = a | b; break;
+      case OP_BIT_XOR: o = a ^ b; break;
+      case OP_SHL: o = (int64_t)((uint64_t)a << c); break;
+      default: o = is_unsigned ? (int64_t)((uint64_t)a >> c) : (a >> c); break;
+    }
+    st1_i64(L, ins.dst, r, o);
+  }
+  store_valid(L, ins.dst, va & vb);
+}
+
 // ------------------------------------------------------------------------------------------------
 // Cold operations: one rolled loop over the thread's rows; every body exists once in the binary.
 // ------------------------------------------------------------------------------------------------
@@ -650,6 +677,7 @@ __device__ __noinline__ void cold_op(const Lane L, const uint32_t active, const 
     const uint8_t op = PROG.code[pc].op;
     if (op <= OP_CEIL) scalar_num_op(L, active, pc);
     else if (op == OP_NULLIF) scalar_nullif_op(L, active, pc);
+    else if (op >= OP_BIT_AND) scalar_bit_op(L, active, pc);
     else scalar_str_op(L, active, pc);
     return;
   }
@@ -1949,6 +1977,100 @@ __device__ __noinline__ uint32_t sink_agg_global(const Lane L, uint32_t active) 
   return active;
 }
 
+// 128-bit MIN / MAX of a table cell without the slot lock: a compare-and-swap of the whole 16-byte cell, as
+// table_merge_str does for strings.  The coarse grouping sets (ROLLUP's () above all) send every row into a handful of
+// cells, and most rows do not beat the value they read, so they issue no atomic.  Every write to such a cell in the
+// grouping-set kernel is this 16-byte CAS (table_merge's locked path, which stores the two halves separately, is not
+// used there), so the 16-byte load never sees a torn value.
+__device__ __noinline__ void table_minmax_i128_cas(int kind, unsigned long long slot, int a, Acc128 x) {
+  const AggTable& T = PROG.table;
+  unsigned long long* cell = T.acc + ((unsigned long long)a * T.cap + slot) * 2;
+  const i128 v = make_i128(x.lo, x.hi);
+  const ulonglong2 val = make_ulonglong2(x.lo, x.hi);
+  ulonglong2 cur = ld_relaxed_b128(cell);
+  for (;;) {
+    const i128 c = make_i128(cur.x, cur.y);
+    if (kind == ACC_MIN_I128 ? !(v < c) : !(v > c)) return;
+    const ulonglong2 seen = atom_cas_b128(cell, cur, val);
+    if (seen.x == cur.x && seen.y == cur.y) return;
+    cur = seen;
+  }
+}
+
+// Grouping sets (ROLLUP / CUBE / GROUPING SETS): one pass over the input for all PROG.n_sets sets.  A live row loads its
+// keys, key hashes and accumulator arguments once, then upserts once per set: the keys masked in the set are NULL, the
+// set's __grouping_id is key n_keys, and the table hash combines the id with the hashes of the present keys (the mask is a
+// function of the id, so equal groups hash equally).  Compiled only into the pipeline_kernel variant with GSETS = true.
+__device__ __noinline__ uint32_t sink_agg_global_gsets(const Lane L, uint32_t active) {
+  if (*(volatile unsigned int*)&PROG.status->overflow) return active;
+  const int n_keys = PROG.n_keys, n_acc = PROG.n_acc, n_sets = PROG.n_sets;
+#pragma unroll 1
+  for (int r = 0; r < VM_R; r++) {
+    if (!((active >> r) & 1)) continue;
+    KeyVal row[VM_MAX_KEYS], kv[VM_MAX_KEYS];
+    unsigned long long kh[VM_MAX_KEYS];
+    for (int k = 0; k < n_keys; k++) {
+      load_key(L, PROG.keys[k], r, &row[k]);
+      kh[k] = (unsigned long long)ld1_i64(L, PROG.key_hashes[k], r);
+    }
+    Acc128 x[VM_MAX_ACC];
+    uint32_t present = 0;  // accumulators with a (non-NULL) contribution of this row
+    for (int a = 0; a < n_acc; a++) {
+      const AccDesc ad = PROG.acc[a];
+      if (ad.kind != ACC_COUNT_STAR && ad.nullable && !((fetch_valid(L, ad.src) >> r) & 1)) continue;
+      present |= 1u << a;
+      x[a].lo = 1;
+      x[a].hi = 0;
+      if (ad.kind == ACC_SUM_I128 || ad.kind == ACC_MIN_I128 || ad.kind == ACC_MAX_I128) {
+        i128 v = ld1_i128(L, ad.src, r);
+        x[a].lo = lo64(v);
+        x[a].hi = ad.zext ? 0ull : hi64(v);
+      } else if (ad.kind == ACC_MIN_STR || ad.kind == ACC_MAX_STR) {
+        const StrRef s = ld1_str(L, ad.src, r);
+        x[a].lo = (uint64_t)s.p;
+        x[a].hi = s.len;
+      } else if (ad.kind == ACC_SUM_F64) {
+        x[a].lo = (uint64_t)__double_as_longlong(ld1_f64(L, ad.src, r));
+      } else if (ad.kind == ACC_MIN_F64 || ad.kind == ACC_MAX_F64) {
+        x[a].lo = (uint64_t)f64_order_key(ld1_f64(L, ad.src, r));
+      }
+    }
+    for (int s = 0; s < n_sets; s++) {
+      const uint32_t mask = PROG.set_mask[s];
+      const unsigned long long id = PROG.set_id[s];
+      unsigned long long h = hash_i64((int64_t)id);
+      for (int k = 0; k < n_keys; k++) {
+        if ((mask >> k) & 1) {
+          kv[k].w0 = kv[k].w1 = 0;
+          kv[k].valid = 0;
+          kv[k].vk = row[k].vk;
+        } else {
+          kv[k] = row[k];
+          h = combine_hashes(kh[k], h);
+        }
+      }
+      kv[n_keys].w0 = id;
+      kv[n_keys].w1 = 0;
+      kv[n_keys].valid = 1;
+      kv[n_keys].vk = VK_I64;
+      const unsigned long long slot = table_upsert(n_keys + 1, h, kv);
+      if (slot == ~0ull) {
+        atomicExch(&PROG.status->overflow, 1u);
+        active &= ~(1u << r);
+        break;
+      }
+      for (int a = 0; a < n_acc; a++) {
+        if (!((present >> a) & 1)) continue;
+        const uint8_t kind = PROG.acc[a].kind;
+        if (kind == ACC_MIN_I128 || kind == ACC_MAX_I128) table_minmax_i128_cas(kind, slot, a, x[a]);
+        else if (kind == ACC_MIN_STR || kind == ACC_MAX_STR) table_merge_str(kind, slot, a, x[a]);
+        else table_merge(kind, slot, a, x[a]);
+      }
+    }
+  }
+  return active;
+}
+
 // ------------------------------------------------------------------------------------------------
 // Register-resident aggregate sink: <= VM_REG_GROUPS groups, <= VM_REG_ACC accumulators.
 // Every thread keeps the full (group x accumulator) matrix in registers: no atomics and no shared
@@ -2609,7 +2731,7 @@ __device__ __forceinline__ void mom_reg_flush(double (&acc)[G][VM_MAX_MOM][3], M
 // ------------------------------------------------------------------------------------------------
 // The kernel
 // ------------------------------------------------------------------------------------------------
-template <int SINK, int G, bool ADD_ONLY, bool SIDE, bool MOM = false, bool SFN = false>
+template <int SINK, int G, bool ADD_ONLY, bool SIDE, bool MOM = false, bool SFN = false, bool GSETS = false>
 __global__ void __launch_bounds__(512, 1) pipeline_kernel() {
   extern __shared__ __align__(128) uint8_t smem[];
   __shared__ __align__(8) uint64_t full_bar[VM_MAX_STAGES];
@@ -2721,7 +2843,7 @@ __global__ void __launch_bounds__(512, 1) pipeline_kernel() {
     } else if (SINK == SINK_MATERIALIZE) {
       sink_materialize(L, active, warp_tot, &tile_base_sh, t, n_tiles);
     } else if (SINK == SINK_AGG_GLOBAL) {
-      active = sink_agg_global(L, active);
+      active = GSETS ? sink_agg_global_gsets(L, active) : sink_agg_global(L, active);
       live_rows += __popc(active);
     } else {
       active = sink_agg_reg<G, ADD_ONLY, SIDE>(L, active, S_reg, acc_hi, acc_side, &gtable, dir, dir_n, accops);
@@ -2799,17 +2921,17 @@ struct GateLock {
   }
 };
 
-template <bool SFN, int SINK, int G, bool ADD_ONLY, bool SIDE = false, bool MOM = false>
+template <bool SFN, int SINK, int G, bool ADD_ONLY, bool SIDE = false, bool MOM = false, bool GSETS = false>
 static cudaError_t launch_one(int grid, int block, size_t smem, cudaStream_t st) {
   // the opt-in to large dynamic shared memory is per (function, device) and sticky: raise it only when needed
   static size_t granted[64] = {0};
   const int dev = GateLock::current_device() & 63;
   if (smem > granted[dev]) {
-    cudaError_t e = cudaFuncSetAttribute(pipeline_kernel<SINK, G, ADD_ONLY, SIDE, MOM, SFN>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    cudaError_t e = cudaFuncSetAttribute(pipeline_kernel<SINK, G, ADD_ONLY, SIDE, MOM, SFN, GSETS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
     granted[dev] = smem;
   }
-  launch_kernel(pipeline_kernel<SINK, G, ADD_ONLY, SIDE, MOM, SFN>, grid, block, smem, st);
+  launch_kernel(pipeline_kernel<SINK, G, ADD_ONLY, SIDE, MOM, SFN, GSETS>, grid, block, smem, st);
   return cudaGetLastError();
 }
 
@@ -2830,6 +2952,8 @@ static cudaError_t launch_variant(const Program& P, int reg_groups, int grid, in
     return reg_groups <= 1 ? launch_one<SFN, SINK_AGG_REG, 1, false, false, true>(grid, block, smem, st)
                            : launch_one<SFN, SINK_AGG_REG, VM_REG_GROUPS, false, false, true>(grid, block, smem, st);
   }
+  // grouping sets: the global sink's variant that upserts every row once per set (run_aggregate never gives them another sink)
+  if (P.n_sets) return launch_one<SFN, SINK_AGG_GLOBAL, 1, true, false, false, true>(grid, block, smem, st);
   switch (P.sink) {
     case SINK_MATERIALIZE: return launch_one<SFN, SINK_MATERIALIZE, 1, true>(grid, block, smem, st);
     case SINK_AGG_GLOBAL: return launch_one<SFN, SINK_AGG_GLOBAL, 1, true>(grid, block, smem, st);

@@ -79,7 +79,10 @@ enum VOp : uint8_t {
   OP_NULLIF,                           // t = operand VK; dst = a, NULL where a = b (floats: bitwise, i.e. total order)
   OP_CHAR_LENGTH, OP_OCTET_LENGTH,     // a: STR -> I64
   OP_STARTS_WITH, OP_ENDS_WITH,        // a, b: STR -> BOOL
-  OP_TRIM                              // a: STR -> STR view; aux = TrimSide; imm = immediate idx of the set (" " by default)
+  OP_TRIM,                             // a: STR -> STR view; aux = TrimSide; imm = immediate idx of the set (" " by default)
+  // bitwise operators (scalar_bit_op): t = VK_I64, a and b of one integer type; aux = Phys of that type (shift counts are
+  // taken modulo its bit width; >> is arithmetic for signed types, logical for unsigned ones)
+  OP_BIT_AND, OP_BIT_OR, OP_BIT_XOR, OP_SHL, OP_SHR
 };
 
 enum DatePart : uint8_t { DP_YEAR = 0, DP_QUARTER, DP_MONTH, DP_WEEK, DP_DAY, DP_DOY, DP_DOW };
@@ -231,6 +234,14 @@ struct Program {
   uint8_t mom_pass;             // 1: this launch is pass 2 and folds rows into the co-moments only
   uint8_t _pad2[6];
   MomDesc mom[VM_MAX_MOM];
+  // grouping sets (global sink only): every live row is upserted once per set s, with the keys whose bit is set in
+  // set_mask[s] replaced by NULL and set_id[s] as one more VK_I64 key (index n_keys).  key_hashes[k] is the I64
+  // register holding the hash of key k (0 for NULL); the table hash of a set combines those of its present keys.
+  uint8_t n_sets;               // 0: a plain aggregate
+  uint8_t _pad3[7];
+  uint8_t set_mask[32];
+  uint64_t set_id[32];
+  Operand key_hashes[VM_MAX_KEYS];
 };
 
 // ---- fused fast path (scan -> filter -> decimal products -> <=4-group SUM/COUNT aggregate) -----------

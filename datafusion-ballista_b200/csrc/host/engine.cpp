@@ -988,7 +988,7 @@ RunOutcome launch_program(const Exec& x, PipelineBuilder& pb, int reg_groups, co
     for (int j = 0; j < P.n_out; j++) kt_bytes += (uint64_t)phys_width((Phys)P.out[j].phys) * (uint64_t)P.n_rows;  // upper bound: every row kept
   KernelTimer kt(x, ff ? "filter_compact" : gb ? "groupby_hash_agg" : fused ? "pipeline_fused_agg" : P.sink == SINK_MATERIALIZE ? "pipeline_materialize"
                    : P.mom_pass ? (P.sink == SINK_AGG_REG ? "pipeline_agg_reg_pass2" : "pipeline_agg_global_pass2")
-                   : P.sink == SINK_AGG_REG ? "pipeline_agg_reg" : "pipeline_agg_global", kt_bytes);
+                   : P.sink == SINK_AGG_REG ? "pipeline_agg_reg" : P.n_sets ? "pipeline_agg_gsets" : "pipeline_agg_global", kt_bytes);
   cudaEvent_t e0, e1;
   CUDA_CHECK(cudaEventCreate(&e0));
   CUDA_CHECK(cudaEventCreate(&e1));
@@ -1132,6 +1132,7 @@ struct AggLowered {
   std::vector<AccDesc> accs;
   std::vector<ColRef> acc_src;
   std::vector<MomDesc> moms;         // VAR / STDDEV / COVAR / CORR: co-moments of pass 2 (table columns after the accs)
+  std::vector<ColRef> key_hashes;    // grouping sets: the hash of each key on its own
   struct OutRecipe {
     uint8_t kind, a, b;
     Phys phys;
@@ -1215,6 +1216,7 @@ void lower_aggregate(PipelineBuilder& pb, const PlanNode& node, AggLowered& L, i
   const bool from_states = agg_mode_consumes_states(node.agg_mode);
   const bool emit_states = agg_mode_emits_states(node.agg_mode);
   const bool scalar = node.group_by.empty();
+  const bool gsets = !node.grouping_sets.empty();
   std::vector<ColRef> narrow32;  // pack_mode 2: non-negative 32-bit images of the keys
   for (size_t g = 0; g < node.group_by.size(); g++) {
     ColRef k0 = pb.compile(*node.group_by[g].expr);
@@ -1244,10 +1246,25 @@ void lower_aggregate(PipelineBuilder& pb, const PlanNode& node, AggLowered& L, i
     r.type = k0.type;
     r.phys = k0.type.id == TypeId::Utf8 ? PH_STRVIEW : phys_of(k0.type);
     r.name = k.name;
-    r.with_valid = k0.nullable;
+    r.with_valid = k0.nullable || gsets;
     r.key_idx = (int)g;
     r.imm = shift;
     L.outs.push_back(r);
+  }
+  if (gsets) {
+    // __grouping_id: table key n_keys (written by the grouping-set sink), narrowed to its type by the extraction
+    AggLowered::OutRecipe r{};
+    r.kind = AO_KEY;
+    r.a = (uint8_t)node.group_by.size();
+    r.b = 255;
+    r.type = grouping_id_type(node.group_by.size());
+    r.phys = phys_of(r.type);
+    r.name = "__grouping_id";
+    r.with_valid = false;
+    r.key_idx = -1;
+    L.outs.push_back(r);
+    // the sink hashes each set's keys itself, from one hash register per key
+    for (auto& k : L.keys) L.key_hashes.push_back(pb.hash_of({k}));
   }
   // injective 64-bit key image => the register-cached group directory can be used
   {
@@ -1256,7 +1273,7 @@ void lower_aggregate(PipelineBuilder& pb, const PlanNode& node, AggLowered& L, i
       all_i64 &= (k.type.pk() == PK::I64 || k.type.pk() == PK::Bool);
       any_null |= k.nullable;
     }
-    if (all_i64 && !any_null) {
+    if (all_i64 && !any_null && !gsets) {
       if (L.keys.size() == 1) {
         L.fast = true;
         L.combined = L.keys[0];
@@ -1547,6 +1564,7 @@ bool match_fused(const Program& P, FusedPlan& FP) {
   memset(&F, 0, sizeof F);
   if (P.sink != SINK_AGG_REG) return false;
   if (P.n_mom) return false;  // VAR / STDDEV / COVAR / CORR need the second pass of the VM sinks
+  if (P.n_sets) return false;  // grouping sets run on the global sink's grouping-set variant only
   if (getenv("B200_NO_FUSED")) return false;
   for (int a = 0; a < P.n_acc; a++)
     if (!(P.acc[a].kind == ACC_SUM_I128 || P.acc[a].kind == ACC_COUNT || P.acc[a].kind == ACC_COUNT_STAR)) return false;
@@ -1824,6 +1842,7 @@ bool match_groupby(const Program& P, GroupBySpec& S) {
   memset(&S, 0, sizeof S);
   if (getenv("B200_NO_GROUPBY")) return false;
   if (P.n_mom) return false;  // VAR / STDDEV / COVAR / CORR need the second pass of the VM sinks
+  if (P.n_sets) return false;  // grouping sets run on the global sink's grouping-set variant only
   if (P.n_keys < 1 || P.n_keys > 2 || P.n_acc > GB_MAX_ACC || P.n_cols > FUSED_MAX_COLS || P.n_cols == 0) return false;
   for (int c = 0; c < P.n_cols; c++) {
     const ColDesc& cd = P.cols[c];
@@ -2054,6 +2073,12 @@ typedef std::function<std::unique_ptr<PipelineBuilder>()> BuilderFactory;
 DevBatchPtr run_aggregate(const Exec& x, const BuilderFactory& make_pb, const PlanNode& node, const DevBatchPtr& src, OpMetrics* met) {
   const int n_keys = (int)node.group_by.size();
   if (n_keys > VM_MAX_KEYS) throw EngineError(B200_ERR_UNSUPPORTED, "too many group-by columns");
+  // grouping sets: every row lands in up to n_sets groups, all on the global table's grouping-set sink (the register sink
+  // holds 4 groups: a ROLLUP of two flags already has more)
+  const int n_sets = (int)node.grouping_sets.size();
+  static_assert(kMaxGroupingSetKeys + 1 <= (size_t)VM_MAX_KEYS && kMaxGroupingSets <= sizeof(Program::set_mask), "grouping-set limits");
+  const int table_keys = n_keys + (n_sets ? 1 : 0);
+  const int64_t max_groups = std::max<int64_t>(src->n, 1) * std::max(n_sets, 1);
   // initial optimism about the keys
   int pack_mode = 0;
   {
@@ -2062,7 +2087,7 @@ DevBatchPtr run_aggregate(const Exec& x, const BuilderFactory& make_pb, const Pl
       any_str |= g.expr->type.id == TypeId::Utf8;
       all_narrow &= narrowable(g.expr->type);
     }
-    if (n_keys == 2 && all_narrow) pack_mode = 2;
+    if (n_keys == 2 && all_narrow && !n_sets) pack_mode = 2;
     else if (any_str) pack_mode = 1;
   }
   int node_idx = -1;
@@ -2094,7 +2119,7 @@ DevBatchPtr run_aggregate(const Exec& x, const BuilderFactory& make_pb, const Pl
   RunOutcome ro;
   unsigned int n_groups = 0;
   int reg_groups = 0;
-  bool gb_bailed = false, pf_off = false;
+  bool gb_bailed = false, pf_off = false, gs_grown = false;
   for (;;) {
     x.check_cancel();
     ScopeTimer t_iter("  agg: lower+alloc+launch+sync");
@@ -2111,7 +2136,13 @@ DevBatchPtr run_aggregate(const Exec& x, const BuilderFactory& make_pb, const Pl
     for (size_t m = 0; m < L.moms.size(); m++) P.mom[m] = L.moms[m];
     memset(&P.key_hash, 0, sizeof P.key_hash);
     P.keys_all_i64 = L.fast ? 1 : 0;
-    if (n_keys) {
+    P.n_sets = (uint8_t)n_sets;
+    for (int s = 0; s < n_sets; s++) {
+      P.set_mask[s] = (uint8_t)node.grouping_sets[(size_t)s];
+      P.set_id[s] = grouping_id(node.grouping_sets[(size_t)s], (size_t)n_keys);
+    }
+    for (size_t k = 0; k < L.key_hashes.size(); k++) P.key_hashes[k] = pb.resolve(L.key_hashes[k]);
+    if (n_keys && !n_sets) {
       if (L.fast) {
         P.key_hash = pb.resolve(L.combined);
       } else {
@@ -2119,11 +2150,14 @@ DevBatchPtr run_aggregate(const Exec& x, const BuilderFactory& make_pb, const Pl
         P.key_hash = h.op;
       }
     }
-    const bool reg_ok = (int)L.accs.size() <= VM_REG_ACC;
+    const bool reg_ok = (int)L.accs.size() <= VM_REG_ACC && !n_sets;
     if (!reg_ok && level == 0) level = 1;
-    // up to a few million input rows a table sized for "every row its own group" is cheap: no capacity ladder
+    // up to a few million input rows a table sized for "every row its own group" is cheap: no capacity ladder.  Grouping
+    // sets first get that size too (the finest set holds at most one group per row and the coarser ones usually few);
+    // the table for every row in every set only after that overflows
     const bool small_input = src->n <= ((int64_t)1 << 22);
     if (level > 0 && small_input) level = 8;
+    const bool gs_rows_first = n_sets && small_input && !gs_grown;
     uint64_t cap;
     reg_groups = 0;
     if (level == 0) {
@@ -2133,7 +2167,7 @@ DevBatchPtr run_aggregate(const Exec& x, const BuilderFactory& make_pb, const Pl
     } else {
       P.sink = SINK_AGG_GLOBAL;
       if (!n_keys) cap = 2;
-      else cap = std::min<uint64_t>(next_pow2((uint64_t)std::max<int64_t>(src->n, 1) * 2), (uint64_t)1 << std::min(40, 12 + 4 * level));
+      else cap = std::min<uint64_t>(next_pow2((uint64_t)(gs_rows_first ? std::max<int64_t>(src->n, 1) : max_groups) * 2), (uint64_t)1 << std::min(40, 12 + 4 * level));
       // a plan shape seen before: size the table for the groups its tasks produced (x2.5: load factor <= 0.4 with room for a
       // somewhat larger sibling task) instead of the whole class -- the classes are 16x apart, and every slot costs ~80 bytes
       // of memset and of extraction scan.  An overflow falls back to the class size (level++ below leaves hinted_level).
@@ -2142,7 +2176,7 @@ DevBatchPtr run_aggregate(const Exec& x, const BuilderFactory& make_pb, const Pl
     }
     {
       ScopeTimer t_alloc("    agg: alloc_table");
-      tm = alloc_table(x, cap, n_keys, L.accs, 3 * L.moms.size());
+      tm = alloc_table(x, cap, table_keys, L.accs, 3 * L.moms.size());
     }
     P.table = tm.T;
     pb.finalize_layout((size_t)VM_REG_ACC * 512 * 16 + 256);
@@ -2199,7 +2233,11 @@ DevBatchPtr run_aggregate(const Exec& x, const BuilderFactory& make_pb, const Pl
       continue;
     }
     if (!ro.status.overflow) break;
-    if (level > 0 && cap >= next_pow2((uint64_t)std::max<int64_t>(src->n, 1) * 2)) {
+    if (gs_rows_first) {
+      gs_grown = true;  // more groups than input rows over all sets: the table for every row in every set
+      continue;
+    }
+    if (level > 0 && cap >= next_pow2((uint64_t)max_groups * 2)) {
       if (use_gb && !pf_off) {
         pf_off = true;  // a bucket's region of the partitioned table filled up (skewed buckets): same table, unpartitioned
         continue;
@@ -2240,7 +2278,7 @@ DevBatchPtr run_aggregate(const Exec& x, const BuilderFactory& make_pb, const Pl
   memset(&A, 0, sizeof A);
   if (L.outs.size() > (size_t)VM_MAX_OUT) throw EngineError(B200_ERR_UNSUPPORTED, "too many aggregate output columns");
   A.n_out = (int)L.outs.size();
-  A.n_keys = n_keys;
+  A.n_keys = table_keys;
   DevPtr counter = dev_alloc(16, x.st());
   CUDA_CHECK(cudaMemsetAsync(counter->ptr, 0, 16, x.st()));
   A.counter = (unsigned long long*)counter->ptr;

@@ -779,6 +779,25 @@ class PipelineBuilder {
       release(b);
       return r;
     }
+    if (is_bitwise(e.op)) {
+      // integer operands of the result's type (plan.hpp); only << can leave the type's range
+      ColRef a = compile(*e.args[0]);
+      pin(a);
+      ColRef b = compile(*e.args[1]);
+      unpin(a);
+      static const uint8_t vops[] = {OP_BIT_AND, OP_BIT_OR, OP_BIT_XOR, OP_SHL, OP_SHR};
+      ColRef r = new_reg(e.type, a.nullable || b.nullable);
+      VInstr ins = blank(vops[(int)e.op - (int)BinOp::BitAnd], VK_I64);
+      ins.a = resolve(a);
+      ins.b = resolve(b);
+      ins.dst = r.op;
+      ins.aux = phys_of(e.type);
+      if (a.nullable || b.nullable) ins.flags |= IF_NULLCHK;
+      emit(ins);
+      release(a);
+      release(b);
+      return e.op == BinOp::Shl ? wrap_int(r, e.type) : r;
+    }
     const DataType rt = e.type;
     // fused decimal shape  a * (lit +/- b)
     if (rt.is_decimal() && e.op == BinOp::Mul) {

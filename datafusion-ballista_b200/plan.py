@@ -152,10 +152,34 @@ def agg(fn_: str, arg: Optional[Json], name: str, input_type=None, arg2: Optiona
     return a
 
 
-def aggregate(mode: str, group_by: Sequence, aggr: Sequence[Json], input: Json) -> Json:
-    """group_by: list of (expr, name)."""
-    return {"op": "AggregateExec", "mode": mode,
-            "group_by": [{"expr": e, "name": n} for e, n in group_by], "aggr": list(aggr), "input": input}
+def aggregate(mode: str, group_by: Sequence, aggr: Sequence[Json], input: Json,
+              grouping_sets: Optional[Sequence[Sequence[bool]]] = None) -> Json:
+    """group_by: list of (expr, name).  grouping_sets (Partial / Single / SinglePartitioned only): one list of len(group_by)
+    bools per set, True where that key is replaced by NULL; the output then holds the keys, `__grouping_id`, then the
+    aggregates (DESIGN.md §6)."""
+    n: Json = {"op": "AggregateExec", "mode": mode,
+               "group_by": [{"expr": e, "name": n} for e, n in group_by], "aggr": list(aggr), "input": input}
+    if grouping_sets is not None:
+        n["grouping_sets"] = [[bool(b) for b in s] for s in grouping_sets]
+    return n
+
+
+def rollup_sets(n_keys: int) -> List[List[bool]]:
+    """ROLLUP(k0, ..., k{n-1}): (k0..k{n-1}), (k0..k{n-2}), ..., ()."""
+    return [[k >= n_keys - d for k in range(n_keys)] for d in range(n_keys + 1)]
+
+
+def cube_sets(n_keys: int) -> List[List[bool]]:
+    """CUBE(k0, ..., k{n-1}): every subset of the keys (the order of the sets does not change the result)."""
+    return [[bool((m >> (n_keys - 1 - k)) & 1) for k in range(n_keys)] for m in range(1 << n_keys)]
+
+
+def grouping_id(mask: Sequence[bool]) -> int:
+    """__grouping_id of a set: the keys folded first to last, id = id << 1 | is_null [EXT]."""
+    v = 0
+    for b in mask:
+        v = v << 1 | int(bool(b))
+    return v
 
 
 def hash_join(left: Json, right: Json, on: Sequence[Sequence[Json]], join_type: str = "Inner",

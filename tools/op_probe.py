@@ -1,7 +1,7 @@
 """One big instance of one operator, so that `ncu -k regex:<kernel> -c 1` lands on a representative launch, and so that the
 engine's own CUDA-event timing (b200_engine_kernel_stats) can be read for the same launch without a profiler attached.
 
-  python tools/op_probe.py join|partition|groupby|groupby_small|filter|parquet|q1|minmax_str|stats|nlj|scalar [msf]
+  python tools/op_probe.py join|partition|groupby|groupby_small|filter|parquet|q1|minmax_str|stats|nlj|scalar|rollup [msf]
 
   join       orders (build, 15 M rows at SF10) |x| lineitem (probe, 60 M rows) on the order key      -> join_build2 / join_probe2
   partition  lineitem (4 columns, 48 B/row) hash-repartitioned on l_orderkey into 8 partitions       -> part_tile_hist / part_tile_scatter
@@ -19,6 +19,9 @@ engine's own CUDA-event timing (b200_engine_kernel_stats) can be read for the sa
              (c) character_length(l_shipinstruct) and btrim(l_shipmode), (d) round(CAST(l_extendedprice AS DOUBLE), 1)
              -> pipeline_materialize; each result checked at SF1: (a) against the CPU oracle, the others (which the oracle
              does not compute) against pyarrow.compute / numpy restatements of DESIGN §6 (vi)
+  rollup     Single-mode ROLLUP / CUBE over lineitem, SUM(l_extendedprice), COUNT(*), MIN(l_shipdate): (a) ROLLUP(l_returnflag,
+             l_linestatus), (b) ROLLUP(l_suppkey, l_returnflag), (c) CUBE(l_returnflag, l_linestatus, l_shipmode), each in one
+             pass (-> pipeline_agg_gsets) and as one ordinary aggregate per set; results checked at SF1 against the oracle
   nlj        NestedLoopJoinExec: lineitem against one build row (a scalar subquery) next to the same comparison
              through fast_filter_kernel, and a band join of orders (msf 1000) against 10,000 build rows    -> nlj_count / nlj_write
 """
@@ -335,6 +338,91 @@ elif op == "scalar":
     report["checked_at_sf1"] = {"rows": n1, "a_year": "= CPU oracle", "others": "= pyarrow.compute / numpy, bit for bit"}
     oracle.close()
     print(json.dumps({op: report}, indent=1))
+elif op == "rollup":
+    # one grouping-set aggregate against the same result computed as S ordinary aggregates (the UNION ALL rewrite), Single
+    # mode over lineitem, SUM(l_extendedprice), COUNT(*), MIN(l_shipdate).  The two forms are timed alternately, ROUNDS
+    # times in one process, and every round is reported.  Every result is checked at SF1 against the oracle.
+    import subprocess
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    import grouping_set_cases as GC
+    import oracle_ffi
+    from util import assert_tables_equal
+    from ballista_b200 import driver
+    rounds = int(os.environ.get("ROUNDS", "3"))
+    smi = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
+    cols = ["l_suppkey", "l_extendedprice", "l_shipdate", "l_returnflag", "l_linestatus", "l_shipmode"]
+    scan = tpch.table_scan("lineitem", cols)
+    aggs = [P.agg("sum", c("l_extendedprice"), "s"), P.agg("count", None, "n"), P.agg("min", c("l_shipdate"), "d")]
+    cases = {"a_rollup_flag_status": (["l_returnflag", "l_linestatus"], P.rollup_sets(2)),
+             "b_rollup_suppkey_flag": (["l_suppkey", "l_returnflag"], P.rollup_sets(2)),
+             "c_cube_flag_status_mode": (["l_returnflag", "l_linestatus", "l_shipmode"], P.cube_sets(3))}
+
+    def log(*a):
+        print(*a, file=sys.stderr, flush=True)
+
+    def one_pass(keys, sets, a=aggs):
+        return GC.single_stages(scan, [(c(k), k) for k in keys], a, sets)
+
+    def per_set(keys, sets, a=aggs):
+        return [[P.Stage(1, P.shuffle_writer(P.aggregate("Single", [(c(k), k) for k, m in zip(keys, mask) if not m], a, scan), 1))]
+                for mask in sets]
+
+    def device_ms(stage_lists):
+        eng.kernel_stats(reset=True)
+        for sl in stage_lists:
+            run(sl, [1])
+        ks = eng.kernel_stats(reset=True)
+        return {k: round(v["ms"] / reps, 3) for k, v in ks.items() if v["ms"] > 0}, round(sum(v["ms"] for v in ks.values()) / reps, 3)
+
+    report = {"gpu": smi, "reps_per_round": reps, "rounds": rounds}
+    n = load("lineitem", cols)
+    report["lineitem_rows"] = n
+    for name, (keys, sets) in cases.items():
+        # per-set form of (c) at SF10: see c_per_set_cause below; it is measured at a smaller scale there
+        forms = {"one_pass": [one_pass(keys, sets)]}
+        if name != "c_cube_flag_status_mode":
+            forms["per_set"] = per_set(keys, sets)
+        for sl in forms.values():   # warm-up (and the table-size hint of every plan)
+            for st in sl:
+                run(st, [1])
+        r = {"sets": len(sets)}
+        for rd in range(rounds):
+            for form, sl in forms.items():
+                fam, tot = device_ms(sl)
+                r.setdefault(form + "_total_ms", []).append(tot)
+                r[form + "_kernel_ms_last_round"] = fam
+                log(name, form, "round", rd, tot, "ms")
+        report[name] = r
+    # The per-set form of (c) has sets of 5 to 42 groups: more than the register sink's 4, so they run on the plain global
+    # sink, where a 128-bit MIN takes the slot lock for every row.  Measured at SF0.1 with and without MIN(l_shipdate).
+    m01 = 100
+    n01 = eng.tpch_table_rows("lineitem", m01)
+    eng.drop_table("lineitem")
+    eng.tpch_generate("lineitem", m01, 0, 0, n01, cols)
+    keys, sets = cases["c_cube_flag_status_mode"]
+    cause = {"lineitem_rows": n01}
+    for label, a in (("with_min", aggs), ("without_min", aggs[:2])):
+        for form, sl in (("one_pass", [one_pass(keys, sets, a)]), ("per_set", per_set(keys, sets, a))):
+            for st in sl:
+                run(st, [1])
+            fam, tot = device_ms(sl)
+            cause[f"{label}/{form}_total_ms"] = tot
+            cause[f"{label}/{form}_kernel_ms"] = fam
+            log("c_per_set_cause", label, form, tot, "ms")
+    report["c_per_set_cause_sf0.1"] = cause
+    print(json.dumps({op: report}, indent=1), flush=True)
+    m1 = 1000
+    n1 = eng.tpch_table_rows("lineitem", m1)
+    eng.drop_table("lineitem")
+    eng.tpch_generate("lineitem", m1, 0, 0, n1, cols)
+    oracle = oracle_ffi.OracleEngine()
+    oracle.tpch_generate("lineitem", m1, 0, 0, n1, cols)
+    for name, (keys, sets) in cases.items():
+        got = driver.run_stages(eng, one_pass(keys, sets), f"chk-{name}")
+        assert_tables_equal(got, GC.expected(oracle, scan, [(c(k), k) for k in keys], aggs, sets, f"chk-{name}"))
+        log(name, "matches the oracle at SF1 (", n1, "rows )")
+    oracle.close()
+    print(json.dumps({op: {"checked_at_sf1": {"rows": n1, "cases": list(cases), "result": "= CPU oracle (UNION ALL form)"}}}), flush=True)
 else:
     raise SystemExit(__doc__)
 print(json.dumps({op: eng.kernel_stats()}, indent=1))
