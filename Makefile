@@ -6,8 +6,9 @@ SRC       := $(PKG)/csrc
 OUT       := $(PKG)/lib
 # B200_PLAN_STAT_AGGREGATES: this library computes VAR / STDDEV / COVAR / CORR (plan.hpp); set for every unit alike
 # B200_PLAN_GROUPING_SETS: ... and grouping sets and the bitwise operators (plan.hpp)
-NVFLAGS   := $(ARCH) -lineinfo -O3 -std=c++17 -Xcompiler -fPIC -Xcompiler -Wno-unused-function -DB200_PLAN_STAT_AGGREGATES=1 -DB200_PLAN_GROUPING_SETS=1
-OBJS      := $(OUT)/pipeline.o $(OUT)/kernels.o $(OUT)/shuffle.o $(OUT)/join.o $(OUT)/nlj.o $(OUT)/groupby.o $(OUT)/parquet.o $(OUT)/filter.o $(OUT)/engine.o $(OUT)/host_narrow.o
+# B200_PLAN_WINDOW: ... and window functions (plan.hpp)
+NVFLAGS   := $(ARCH) -lineinfo -O3 -std=c++17 -Xcompiler -fPIC -Xcompiler -Wno-unused-function -DB200_PLAN_STAT_AGGREGATES=1 -DB200_PLAN_GROUPING_SETS=1 -DB200_PLAN_WINDOW=1
+OBJS      := $(OUT)/pipeline.o $(OUT)/kernels.o $(OUT)/shuffle.o $(OUT)/join.o $(OUT)/nlj.o $(OUT)/groupby.o $(OUT)/parquet.o $(OUT)/filter.o $(OUT)/window.o $(OUT)/engine.o $(OUT)/host_narrow.o
 CXX       ?= g++
 COMMON    := $(wildcard $(SRC)/common/*.hpp) $(wildcard $(SRC)/device/*.h) $(wildcard $(SRC)/device/*.cuh) $(wildcard $(SRC)/host/*.hpp) include/b200exec.h include/b200_arrow_abi.h
 
@@ -35,6 +36,9 @@ $(OUT)/nlj.o: $(SRC)/device/nlj.cu $(COMMON)
 	@mkdir -p $(OUT)
 	$(NVCC) $(NVFLAGS) -c $< -o $@
 $(OUT)/shuffle.o: $(SRC)/device/shuffle.cu $(COMMON)
+	@mkdir -p $(OUT)
+	$(NVCC) $(NVFLAGS) -c $< -o $@
+$(OUT)/window.o: $(SRC)/device/window.cu $(COMMON)
 	@mkdir -p $(OUT)
 	$(NVCC) $(NVFLAGS) -c $< -o $@
 $(OUT)/engine.o: $(SRC)/host/engine.cpp $(COMMON)

@@ -14,6 +14,8 @@
 // This header is shared by the product (csrc/host) and by the CPU oracle (oracle/): it contains
 // parsing and *typing* only -- no arithmetic on data.
 #pragma once
+#include <climits>
+#include <cstdint>
 #include <memory>
 #include <string>
 #include <vector>
@@ -718,13 +720,111 @@ struct NamedExpr {
   std::string name;
 };
 
+// ----------------------------------------------------------------------------------------------
+// Window functions (WindowAggExec / BoundedWindowAggExec): typed here for every consumer of the plan IR, computed only
+// by a consumer built with B200_PLAN_WINDOW=1 (the device engine: Makefile NVFLAGS).  Semantics: DESIGN.md §6 (viii).
+// ----------------------------------------------------------------------------------------------
+#ifndef B200_PLAN_WINDOW
+#define B200_PLAN_WINDOW 0
+#endif
+enum class WinFn : uint8_t {
+  RowNumber, Rank, DenseRank, PercentRank, CumeDist, Ntile, Lag, Lead, FirstValue, LastValue, NthValue, Count, Sum, Avg, Min, Max
+};
+inline bool win_fn_is_agg(WinFn f) { return f >= WinFn::Count; }
+inline bool win_fn_uses_frame(WinFn f) { return f >= WinFn::FirstValue; }
+// one frame bound; kind follows csrc/device/kernels.h WinBound: 0 UNBOUNDED PRECEDING, 1 n PRECEDING, 2 CURRENT ROW,
+// 3 n FOLLOWING, 4 UNBOUNDED FOLLOWING
+struct WindowBound {
+  uint8_t kind = 0;
+  uint64_t n = 0;
+};
+struct WindowFrame {
+  bool range = true;  // RANGE (the default with and without ORDER BY) or ROWS
+  WindowBound start, end;
+};
+struct WindowExpr {
+  WinFn fn = WinFn::RowNumber;
+  std::string fn_name;      // as written in the plan (aliases kept for the dump)
+  std::string name;         // output column
+  std::vector<ExprPtr> args;
+  int64_t n = 0;            // ntile / nth_value: n; lag / lead: the offset (lead +k, lag -k after the sign of k)
+  ExprPtr default_value;    // lag / lead: a literal of the argument's type, or null
+  WindowFrame frame;
+  DataType result_type;
+  bool nullable = true;
+};
+
+// Offsets and positions beyond any partition (the operator takes < 2^32 rows) are clamped to this, which keeps every row
+// index the kernels form from them far inside int64
+static const int64_t kWindowMaxOffset = (int64_t)1 << 40;
+
+// The LAG / LEAD default `d` (a non-NULL literal) as a literal of type `to`, or null when `to` cannot hold it exactly.
+// Integers, Date32 and Timestamp take integers in range; Float64 / Float32 take numbers; Decimal128 takes integers and
+// decimals of a scale not above its own, within its precision.
+inline ExprPtr window_default_as(const ExprPtr& d, const DataType& to) {
+  if (d->type == to) return d;
+  auto out = std::make_shared<Expr>(*d);
+  out->type = to;
+  out->nullable = false;
+  const DataType& from = d->type;
+  const bool from_int = from.is_integer();
+  if (to.is_integer() || to.id == TypeId::Date32 || to.id == TypeId::Timestamp) {
+    if (!from_int) return nullptr;
+    const int64_t v = d->lit.i;
+    if (from.id == TypeId::UInt64 && v < 0) return nullptr;  // above INT64_MAX
+    static const std::pair<TypeId, std::pair<int64_t, int64_t>> range[] = {
+        {TypeId::Int8, {-128, 127}}, {TypeId::Int16, {-32768, 32767}}, {TypeId::Int32, {INT32_MIN, INT32_MAX}},
+        {TypeId::UInt8, {0, 255}},   {TypeId::UInt16, {0, 65535}},     {TypeId::UInt32, {0, (int64_t)UINT32_MAX}},
+        {TypeId::UInt64, {0, INT64_MAX}}, {TypeId::Date32, {INT32_MIN, INT32_MAX}}};
+    for (auto& r : range)
+      if (to.id == r.first && (v < r.second.first || v > r.second.second)) return nullptr;
+    return out;
+  }
+  if (to.is_float()) {
+    if (from.is_float()) out->lit.f = d->lit.f;
+    else if (from_int) out->lit.f = from.id == TypeId::UInt64 ? (double)(uint64_t)d->lit.i : (double)d->lit.i;
+    else return nullptr;
+    return out;
+  }
+  if (to.is_decimal()) {
+    i128 v;
+    if (from_int) {
+      if (from.id == TypeId::UInt64 && d->lit.i < 0) return nullptr;
+      v = (i128)d->lit.i * pow10_i128(to.scale);
+    } else if (from.is_decimal() && from.scale <= to.scale) {
+      v = d->lit.d * pow10_i128(to.scale - from.scale);
+    } else {
+      return nullptr;
+    }
+    const i128 lim = pow10_i128(to.precision);
+    if (v >= lim || v <= -lim) return nullptr;
+    out->lit.d = v;
+    return out;
+  }
+  return nullptr;  // Utf8 / Bool arguments take a default of their own type only
+}
+
+// structural equality of two typed expressions (window PARTITION BY / ORDER BY against the node's and the sort's keys)
+inline bool expr_equal(const ExprPtr& a, const ExprPtr& b) {
+  if (!a || !b) return a == b;
+  if (a->kind != b->kind || a->type != b->type || a->col != b->col || a->op != b->op || a->fn != b->fn || a->negated != b->negated ||
+      a->has_else != b->has_else || a->pattern != b->pattern || a->args.size() != b->args.size())
+    return false;
+  if (a->kind == Expr::Lit && (a->lit.is_null != b->lit.is_null || a->lit.i != b->lit.i || a->lit.d != b->lit.d || a->lit.s != b->lit.s ||
+                               !(a->lit.f == b->lit.f || (a->lit.f != a->lit.f && b->lit.f != b->lit.f))))
+    return false;
+  for (size_t k = 0; k < a->args.size(); k++)
+    if (!expr_equal(a->args[k], b->args[k])) return false;
+  return true;
+}
+
 struct PlanNode;
 typedef std::unique_ptr<PlanNode> PlanPtr;
 
 struct PlanNode {
   enum Op {
     Scan, ShuffleReader, Filter, Projection, Aggregate, HashJoin, Sort, SortPreservingMerge,
-    Passthrough /* CoalesceBatches, CoalescePartitions, round-robin Repartition */, Limit, ShuffleWriter
+    Passthrough /* CoalesceBatches, CoalescePartitions, round-robin Repartition */, Limit, ShuffleWriter, Window
   } op = Scan;
   std::string op_name;
   std::vector<PlanPtr> children;
@@ -765,6 +865,11 @@ struct PlanNode {
   std::vector<ExprPtr> part_exprs;
   int64_t n_out_partitions = 0;  // 0 => no repartitioning ("None" branch, shuffle_writer.rs:221-268)
   bool sort_shuffle = true;
+  // Window: the input's columns, then one column per expression.  All expressions share the partition keys and ORDER BY.
+  bool window_sorted = false;        // BoundedWindowAggExec (input_order_mode sorted); false: WindowAggExec
+  std::vector<ExprPtr> window_partition;
+  std::vector<SortKey> window_order;
+  std::vector<WindowExpr> window_exprs;
 };
 
 // deep copy of an expression with every column reference moved by `delta` positions
@@ -1107,6 +1212,182 @@ inline PlanPtr parse_plan(const Json& j) {
     n->op = PlanNode::Passthrough;
     PlanNode* c = parse_child("input");
     n->schema = c->schema;
+  } else if (op == "WindowAggExec" || op == "BoundedWindowAggExec") {
+    n->op = PlanNode::Window;
+    PlanNode* c = parse_child("input");
+    if (!B200_PLAN_WINDOW) throw PlanUnsupported("window functions are not computed by this consumer of the plan IR");
+    if (j.has("mode") && !j.at("mode").is_null()) {
+      const std::string m = j.at("mode").str();
+      if (m == "linear" || m == "partially_sorted") throw PlanUnsupported("window input order mode " + m + " is not supported");
+      if (m != "sorted") throw std::runtime_error("WindowAggExec: unknown input order mode '" + m + "'");
+      n->window_sorted = true;
+    }
+    if (op == "BoundedWindowAggExec") n->window_sorted = true;
+    if (j.has("partition_keys"))
+      for (size_t i = 0; i < j.at("partition_keys").size(); i++) n->window_partition.push_back(parse_expr(j.at("partition_keys").at(i), c->schema));
+    n->schema = c->schema;
+    const Json& ws = j.at("window_expr");
+    if (ws.size() == 0) throw std::runtime_error("WindowAggExec without window expressions");
+    for (size_t i = 0; i < ws.size(); i++) {
+      const Json& w = ws.at(i);
+      WindowExpr we;
+      we.fn_name = w.at("fn").str();
+      we.name = w.get_str("name", we.fn_name + "_" + std::to_string(i));
+      const std::string& f = we.fn_name;
+      const std::string who = f + " (" + we.name + ")";
+      if (w.get_bool("ignore_nulls", false)) throw PlanUnsupported("IGNORE NULLS in window function " + who + " is not supported");
+      if (w.get_bool("distinct", false)) throw PlanUnsupported("DISTINCT window function " + who + " is not supported");
+      static const std::pair<const char*, WinFn> fns[] = {
+          {"row_number", WinFn::RowNumber}, {"rank", WinFn::Rank},         {"dense_rank", WinFn::DenseRank}, {"percent_rank", WinFn::PercentRank},
+          {"cume_dist", WinFn::CumeDist},   {"ntile", WinFn::Ntile},       {"lag", WinFn::Lag},              {"lead", WinFn::Lead},
+          {"first_value", WinFn::FirstValue}, {"last_value", WinFn::LastValue}, {"nth_value", WinFn::NthValue}, {"count", WinFn::Count},
+          {"sum", WinFn::Sum},              {"avg", WinFn::Avg},           {"mean", WinFn::Avg},             {"min", WinFn::Min},
+          {"max", WinFn::Max}};
+      bool known = false;
+      for (auto& kv : fns)
+        if (f == kv.first) {
+          we.fn = kv.second;
+          known = true;
+        }
+      if (!known) throw PlanUnsupported("window function " + who + " is not supported");
+      std::vector<ExprPtr> part;
+      if (w.has("partition_by"))
+        for (size_t k = 0; k < w.at("partition_by").size(); k++) part.push_back(parse_expr(w.at("partition_by").at(k), c->schema));
+      bool same_part = part.size() == n->window_partition.size();
+      for (size_t k = 0; k < part.size() && same_part; k++) {
+        bool found = false;
+        for (auto& pk : n->window_partition) found = found || expr_equal(part[k], pk);
+        same_part = found;
+      }
+      if (!same_part) throw PlanUnsupported("window function " + who + ": its PARTITION BY differs from the node's partition keys");
+      std::vector<SortKey> order = w.has("order_by") ? parse_sort_keys(w.at("order_by"), c->schema) : std::vector<SortKey>();
+      if (i == 0) {
+        n->window_order = order;
+      } else {
+        bool same = order.size() == n->window_order.size();
+        for (size_t k = 0; k < order.size() && same; k++)
+          same = expr_equal(order[k].expr, n->window_order[k].expr) && order[k].asc == n->window_order[k].asc && order[k].nulls_first == n->window_order[k].nulls_first;
+        if (!same) throw PlanUnsupported("window function " + who + ": its ORDER BY differs from that of the node's other expressions");
+      }
+      if (w.has("frame") && !w.at("frame").is_null()) {
+        const Json& fr = w.at("frame");
+        const std::string units = fr.get_str("units", "range");
+        if (units == "groups") throw PlanUnsupported("GROUPS window frame of " + who + " is not supported");
+        if (units != "rows" && units != "range") throw std::runtime_error("window frame units '" + units + "'");
+        we.frame.range = units == "range";
+        auto bound = [&](const Json& b, const char* side) {
+          static const char* kinds[] = {"unbounded_preceding", "preceding", "current_row", "following", "unbounded_following"};
+          WindowBound wb;
+          const std::string k = b.at("kind").str();
+          bool ok = false;
+          for (uint8_t t = 0; t < 5; t++)
+            if (k == kinds[t]) {
+              wb.kind = t;
+              ok = true;
+            }
+          if (!ok) throw std::runtime_error("window frame bound '" + k + "'");
+          if (wb.kind == 1 || wb.kind == 3) {
+            if (we.frame.range) throw PlanUnsupported("RANGE window frame with an offset bound (" + std::string(side) + " of " + who + ") is not supported");
+            const Json& v = b.at("n");
+            if (!v.is_int || v.i < 0) throw PlanUnsupported("ROWS frame offset of " + who + " must be a non-negative integer literal");
+            wb.n = (uint64_t)v.i;
+          }
+          return wb;
+        };
+        we.frame.start = bound(fr.at("start"), "start");
+        we.frame.end = bound(fr.at("end"), "end");
+        if (we.frame.start.kind == 4) throw std::runtime_error("window frame of " + who + " starts at UNBOUNDED FOLLOWING");
+        if (we.frame.end.kind == 0) throw std::runtime_error("window frame of " + who + " ends at UNBOUNDED PRECEDING");
+      } else {
+        we.frame.range = true;
+        we.frame.start.kind = 0;
+        we.frame.end.kind = 2;
+      }
+      const Json no_args;
+      const Json& as = w.has("args") ? w.at("args") : no_args;
+      for (size_t k = 0; k < as.size(); k++) we.args.push_back(parse_expr(as.at(k), c->schema));
+      auto int_literal = [&](size_t k, const char* what) -> int64_t {
+        const ExprPtr& e = we.args[k];
+        if (e->kind != Expr::Lit || e->lit.is_null || !(e->type.is_integer()))
+          throw PlanUnsupported(std::string(what) + " of " + who + " must be an integer literal");
+        return e->lit.i;
+      };
+      auto want_args = [&](size_t lo, size_t hi) {
+        if (we.args.size() < lo || we.args.size() > hi) throw std::runtime_error(who + " takes " + std::to_string(lo) + ".." + std::to_string(hi) + " arguments");
+      };
+      switch (we.fn) {
+        case WinFn::RowNumber:
+        case WinFn::Rank:
+        case WinFn::DenseRank:
+          want_args(0, 0);
+          we.result_type = DataType(TypeId::UInt64);
+          we.nullable = false;
+          break;
+        case WinFn::PercentRank:
+        case WinFn::CumeDist:
+          want_args(0, 0);
+          we.result_type = DataType(TypeId::Float64);
+          we.nullable = false;
+          break;
+        case WinFn::Ntile:
+          want_args(1, 1);
+          we.n = int_literal(0, "the bucket count");
+          if (we.n < 1) throw std::runtime_error("ntile of " + who + " needs n >= 1, got " + std::to_string(we.n));
+          we.args.clear();
+          we.result_type = DataType(TypeId::UInt64);
+          break;
+        case WinFn::Lag:
+        case WinFn::Lead: {
+          want_args(1, 3);
+          int64_t k = we.args.size() > 1 ? int_literal(1, "the offset") : 1;
+          k = std::max<int64_t>(-kWindowMaxOffset, std::min<int64_t>(k, kWindowMaxOffset));  // past any partition: the default
+          we.n = we.fn == WinFn::Lead ? k : -k;
+          if (we.args.size() > 2) {
+            const ExprPtr& d = we.args[2];
+            if (d->kind != Expr::Lit) throw PlanUnsupported("the default of " + who + " must be a literal");
+            if (!d->lit.is_null) {
+              // [EXT] DataFusion casts the default to the argument's type; a value the type cannot hold exactly is refused
+              we.default_value = window_default_as(d, we.args[0]->type);
+              if (!we.default_value)
+                throw PlanUnsupported("the default of " + who + " has type " + d->type.str() + " and does not cast exactly to the argument's " + we.args[0]->type.str());
+            }
+          }
+          we.args.resize(1);
+          we.result_type = we.args[0]->type;
+          break;
+        }
+        case WinFn::FirstValue:
+        case WinFn::LastValue:
+          want_args(1, 1);
+          we.result_type = we.args[0]->type;
+          break;
+        case WinFn::NthValue:
+          want_args(2, 2);
+          we.n = int_literal(1, "the position");
+          if (we.n < 1) throw std::runtime_error("nth_value of " + who + " needs n >= 1, got " + std::to_string(we.n));
+          we.n = std::min<int64_t>(we.n, kWindowMaxOffset);  // past any frame (< 2^32 rows): NULL, and no overflow in fs + n
+          we.args.resize(1);
+          we.result_type = we.args[0]->type;
+          break;
+        case WinFn::Count:
+          want_args(0, 1);
+          if (!we.args.empty() && we.args[0]->kind == Expr::Lit && !we.args[0]->lit.is_null) we.args.clear();  // COUNT(<literal>) is COUNT(*)
+          we.result_type = DataType(TypeId::Int64);
+          we.nullable = false;
+          break;
+        default: {  // Sum, Avg, Min, Max
+          want_args(1, 1);
+          const DataType& t = we.args[0]->type;
+          const bool ok = we.fn == WinFn::Sum || we.fn == WinFn::Avg
+                              ? t.is_numeric()
+                              : (t.is_numeric() || t.id == TypeId::Date32 || t.id == TypeId::Timestamp || t.id == TypeId::Bool);
+          if (!ok) throw PlanUnsupported("window function " + who + " does not support an argument of type " + t.str());
+          we.result_type = we.fn == WinFn::Sum ? sum_result_type(t) : we.fn == WinFn::Avg ? avg_result_type(t) : t;
+        }
+      }
+      n->schema.push_back(Field{we.name, we.result_type, we.nullable});
+      n->window_exprs.push_back(we);
+    }
   } else if (op == "GlobalLimitExec" || op == "LocalLimitExec") {
     n->op = PlanNode::Limit;
     PlanNode* c = parse_child("input");

@@ -142,6 +142,26 @@ inline std::string dump_plan(const PlanNode& n) {
       o += ",\"input\":" + child(0);
       break;
     case PlanNode::Passthrough: o += ",\"input\":" + child(0); break;
+    case PlanNode::Window: {
+      static const char* bounds[] = {"unbounded_preceding", "preceding", "current_row", "following", "unbounded_following"};
+      auto bound = [&](const WindowBound& b) {
+        return std::string("{\"kind\":\"") + bounds[b.kind] + "\"" + (b.kind == 1 || b.kind == 3 ? ",\"n\":" + std::to_string(b.n) : std::string()) + "}";
+      };
+      o += std::string(",\"mode\":") + (n.window_sorted ? "\"sorted\"" : "null") + ",\"partition_keys\":[";
+      for (size_t i = 0; i < n.window_partition.size(); i++) o += (i ? "," : "") + dump_expr(n.window_partition[i]);
+      o += "],\"order_by\":" + dump_sort_keys(n.window_order) + ",\"window_expr\":[";
+      for (size_t i = 0; i < n.window_exprs.size(); i++) {
+        const WindowExpr& w = n.window_exprs[i];
+        o += std::string(i ? "," : "") + "{\"fn\":" + pbp::jstr(w.fn_name) + ",\"name\":" + pbp::jstr(w.name) + ",\"args\":[";
+        for (size_t k = 0; k < w.args.size(); k++) o += (k ? "," : "") + dump_expr(w.args[k]);
+        o += "],\"n\":" + std::to_string(w.n);
+        if (w.default_value) o += ",\"default\":" + dump_expr(w.default_value);
+        o += std::string(",\"frame\":{\"units\":\"") + (w.frame.range ? "range" : "rows") + "\",\"start\":" + bound(w.frame.start) + ",\"end\":" + bound(w.frame.end) + "}";
+        o += ",\"result_type\":" + type_json(w.result_type) + "}";
+      }
+      o += "],\"input\":" + child(0);
+      break;
+    }
     case PlanNode::Limit: o += ",\"fetch\":" + std::to_string(n.fetch) + ",\"skip\":" + std::to_string(n.skip) + ",\"input\":" + child(0); break;
     case PlanNode::ShuffleWriter: {
       o += ",\"job_id\":" + pbp::jstr(n.job_id) + ",\"stage_id\":" + std::to_string(n.stage_id) + ",\"sort_shuffle\":" + (n.sort_shuffle ? "true" : "false");

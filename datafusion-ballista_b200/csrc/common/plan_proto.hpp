@@ -423,17 +423,43 @@ inline std::string expr_json(const Msg& e) {
   }
 }
 
-// PhysicalSortExprNode { expr = 1, asc = 2, nulls_first = 3 } wrapped in PhysicalExprNode.sort = 10 (:976-980)
+// PhysicalSortExprNode { expr = 1, asc = 2, nulls_first = 3 } (:976-980)
+inline std::string sort_expr_json(const Msg& s) {
+  return "{\"expr\":" + expr_json(s.sub(1)) + ",\"asc\":" + (s.boolean(2) ? "true" : "false") + ",\"nulls_first\":" + (s.boolean(3) ? "true" : "false") + "}";
+}
+// ... wrapped in PhysicalExprNode.sort = 10 (SortExec, SortPreservingMergeExec)
 inline std::string sort_exprs_json(const std::vector<Msg>& v) {
   std::string o = "[";
   for (size_t i = 0; i < v.size(); i++) {
     const Entry* x = v[i].last(10);
     if (!x) throw std::runtime_error("plan proto: sort expression expected");
-    const Msg s(x->b);
-    o += std::string(i ? "," : "") + "{\"expr\":" + expr_json(s.sub(1)) + ",\"asc\":" + (s.boolean(2) ? "true" : "false") + ",\"nulls_first\":" +
-         (s.boolean(3) ? "true" : "false") + "}";
+    o += std::string(i ? "," : "") + sort_expr_json(Msg(x->b));
   }
   return o + "]";
+}
+
+// WindowFrameBound { window_frame_bound_type = 1 (CURRENT_ROW 0, PRECEDING 1, FOLLOWING 2), bound_value = 2 } (:627-635).
+// [EXT] datafusion-proto writes UNBOUNDED as a NULL bound value (ScalarValue.null_value = 33); an absent value means the same.
+// An integer value becomes "n"; any other value (an interval, a float) becomes "n": null, which the typing refuses.
+inline std::string window_bound_json(const Msg& b) {
+  const uint64_t t = b.u64(1);
+  if (t == 0) return "{\"kind\":\"current_row\"}";
+  if (t > 2) throw std::runtime_error("plan proto: window frame bound type " + std::to_string(t));
+  const char* side = t == 1 ? "preceding" : "following";
+  const Msg v = b.sub(2);
+  const Entry* x = v.e.empty() ? nullptr : &v.e.back();
+  if (!x || x->field == 33) return std::string("{\"kind\":\"unbounded_") + side + "\"}";
+  std::string n = "null";
+  if (x->field >= 4 && x->field <= 7) n = std::to_string((int64_t)x->v);        // int8 .. int64 values
+  else if (x->field >= 8 && x->field <= 11) n = std::to_string((uint64_t)x->v);  // uint8 .. uint64 values
+  return std::string("{\"kind\":\"") + side + "\",\"n\":" + n + "}";
+}
+// WindowFrame { window_frame_units = 1 (ROWS 0, RANGE 1, GROUPS 2), start_bound = 2, bound = 3 (the end) } (:610-625)
+inline std::string window_frame_json(const Msg& f) {
+  static const char* units[] = {"rows", "range", "groups"};
+  const uint64_t u = f.u64(1);
+  if (u > 2) throw std::runtime_error("plan proto: window frame units " + std::to_string(u));
+  return std::string("{\"units\":\"") + units[u] + "\",\"start\":" + window_bound_json(f.sub(2)) + ",\"end\":" + window_bound_json(f.sub(3)) + "}";
 }
 
 inline std::string u32_list_json(const std::vector<uint64_t>& v) {
@@ -721,6 +747,31 @@ inline std::string plan_json(const Msg& n, const std::string& override_job) {
         first = false;
       }
       return o + "]}";
+    }
+    case 15: {  // WindowAggExecNode { input = 1, window_expr = 2, partition_keys = 5, linear = 7 | partially_sorted = 8 | sorted = 9 } (:1230-1240)
+      // no input order mode: WindowAggExec; sorted: BoundedWindowAggExec; the other two modes are refused by the typing
+      const char* mode = m.has(9) ? "\"sorted\"" : m.has(8) ? "\"partially_sorted\"" : m.has(7) ? "\"linear\"" : "null";
+      std::string o = std::string("{\"op\":\"WindowAggExec\",\"mode\":") + mode + ",\"partition_keys\":" + exprs_json(m.subs(5)) + ",\"window_expr\":[";
+      const std::vector<Msg> ws = m.subs(2);
+      for (size_t i = 0; i < ws.size(); i++) {
+        // PhysicalWindowExprNode { user_defined_aggr_function = 3 | user_defined_window_function = 10, args = 4, partition_by = 5,
+        // order_by = 6, window_frame = 7, name = 8, ignore_nulls = 11, distinct = 12 } (:924-938); fun_definition = 9 is
+        // ignored, as the aggregate decoder ignores UDAF payloads
+        const Msg& w = ws[i];
+        std::string fn = w.has(10) ? w.str(10) : w.str(3);
+        if (fn.empty()) throw std::runtime_error("plan proto: window expression without a function name");
+        for (auto& ch : fn) ch = (char)tolower((unsigned char)ch);
+        o += std::string(i ? "," : "") + "{\"fn\":" + jstr(fn) + ",\"name\":" + jstr(w.str(8)) + ",\"args\":" + exprs_json(w.subs(4)) +
+             ",\"partition_by\":" + exprs_json(w.subs(5)) + ",\"order_by\":[";
+        const std::vector<Msg> ob = w.subs(6);
+        for (size_t k = 0; k < ob.size(); k++) o += std::string(k ? "," : "") + sort_expr_json(ob[k]);
+        o += "]";
+        if (w.has(7)) o += ",\"frame\":" + window_frame_json(w.sub(7));
+        if (w.boolean(11)) o += ",\"ignore_nulls\":true";
+        if (w.boolean(12)) o += ",\"distinct\":true";
+        o += "}";
+      }
+      return o + "],\"input\":" + in(1) + "}";
     }
     default: throw Unsupported("physical plan node variant " + std::to_string(x->field) + " is not supported by the device engine");
   }

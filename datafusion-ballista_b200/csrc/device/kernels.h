@@ -410,6 +410,85 @@ void launch_pq_delta_prepare(const PqColumn& C, const PqPage* pages, int n_pages
 void launch_pq_values_delta(const PqColumn& C, const PqPage* pages, int n_pages, const unsigned long long* dense_base, const uint32_t* nonnull, void* out,
                             const PqDeltaAux& A, cudaStream_t st);
 
+// ---- window functions (window.cu) ---------------------------------------------------------------
+// Kernels work on sorted positions i; perm[i] is the input row there (nullptr: the input already is in sorted order).
+static const int WIN_MAX_KEYS = 16;
+struct WinKeys {
+  KeyCol k[WIN_MAX_KEYS];  // partition keys, then order keys (strings as views)
+  int n_part, n_order;
+};
+// part_flag / peer_flag[i] = 1 where sorted row i starts a partition / a peer group (a partition start is also a peer start)
+void launch_window_flags(const WinKeys& K, const int64_t* perm, int64_t n, uint32_t* part_flag, uint32_t* peer_flag, cudaStream_t st);
+struct WinBounds {
+  uint32_t* pid;              // [n] partition of each sorted row
+  uint32_t* gid;              // [n] peer group of each sorted row
+  uint32_t* part_start;       // [partitions + 1] first sorted row of each partition, then n
+  uint32_t* peer_start;       // [peer groups + 1] first sorted row of each peer group, then n
+  uint32_t* part_first_peer;  // [partitions] peer group of each partition's first row
+};
+// part_ex / peer_ex: exclusive scans of the flags (launch_scan_u32_to_u64)
+void launch_window_segments(const uint32_t* part_flag, const uint32_t* peer_flag, const uint64_t* part_ex, const uint64_t* peer_ex, int64_t n,
+                            const WinBounds& B, cudaStream_t st);
+// accumulator value types and their argument conversions
+enum WinAcc : uint8_t { WACC_I64 = 0, WACC_F64 = 1, WACC_I128 = 2 };
+enum WinConv : uint8_t {
+  WCV_I64 = 0,     // integers, Date32, Bool: sign / zero extended (WACC_I64)
+  WCV_U64_KEY,     // UInt64 with the sign bit flipped: signed order = unsigned order (MIN / MAX)
+  WCV_F64,         // any number as double (float SUM / AVG, integer AVG)
+  WCV_F64_KEY,     // Float32 / Float64 as an IEEE total-order key (MIN / MAX)
+  WCV_I128,        // Decimal128
+  WCV_VALID,       // COUNT(x): only the validity
+  WCV_ONE          // COUNT(*): every row counts
+};
+struct WinLoad {
+  const void* data;
+  const uint8_t* valid;
+  uint8_t phys, conv;
+  void* out;           // [n] accumulator values in sorted order
+  uint8_t* out_valid;  // [n]
+};
+void launch_window_load(const WinLoad& L, const int64_t* perm, int64_t n, cudaStream_t st);
+enum WinOp : uint8_t { WOP_SUM = 0, WOP_MIN, WOP_MAX };
+enum WinSeg : uint8_t { WSEG_PART = 0, WSEG_PEER, WSEG_BLOCK };
+// segmented inclusive scan of (value, non-NULL count) over sorted rows; dir 1 runs from the last row to the first
+struct WinScan {
+  const void* vals;
+  const uint8_t* valid;
+  void* out_v;
+  uint32_t* out_c;
+  void* tiles;  // window_scan_tile_bytes(n)
+  int64_t n, w;  // w: WSEG_BLOCK block length
+  uint8_t acc, op, dir, seg;
+};
+int64_t window_scan_tile_bytes(int64_t n);
+void launch_window_scan(const WinScan& S, const WinBounds& B, cudaStream_t st);
+enum WinFnKind : uint8_t { WF_ROW_NUMBER = 0, WF_RANK, WF_DENSE_RANK, WF_PERCENT_RANK, WF_CUME_DIST, WF_NTILE, WF_OFFSET, WF_FIRST, WF_LAST, WF_NTH, WF_AGG };
+enum WinBound : uint8_t { WB_UNBOUNDED_PRECEDING = 0, WB_PRECEDING, WB_CURRENT_ROW, WB_FOLLOWING, WB_UNBOUNDED_FOLLOWING };
+enum WinUnits : uint8_t { WUNITS_ROWS = 0, WUNITS_RANGE };
+// how WF_AGG reads a frame [fs, fe): the forward scan at fe - 1, the backward scan at fs, or both over blocks of w rows
+enum WinRead : uint8_t { WRD_FWD = 0, WRD_BWD, WRD_BLOCKS };
+enum WinFinish : uint8_t { WFIN_VALUE = 0, WFIN_COUNT, WFIN_AVG, WFIN_MINMAX_U64, WFIN_MINMAX_F64 };
+struct WinEval {
+  uint8_t fn, units, s_kind, e_kind;
+  uint8_t acc, op, read, fin;
+  uint8_t out_phys;
+  int32_t imm;          // WFIN_AVG over Decimal128: result scale - input scale
+  int64_t s_off, e_off;
+  int64_t arg;          // WF_NTILE: n; WF_NTH: n; WF_OFFSET: signed distance (LEAD +k, LAG -k)
+  int64_t w;
+  const void* fwd_v;
+  const uint32_t* fwd_c;
+  const void* bwd_v;
+  const uint32_t* bwd_c;
+  void* out;            // result per input row
+  uint8_t* out_valid;
+  int64_t* idx_out;     // WF_OFFSET / WF_FIRST / WF_LAST / WF_NTH: input row to take per input row, -1 = none
+  unsigned int* error;  // WFIN_AVG over Decimal128: overflow
+};
+void launch_window_eval(const WinEval& E, const WinBounds& B, const int64_t* perm, int64_t n, cudaStream_t st);
+// LAG / LEAD default: rows with idx < 0 get the 16-byte literal image (its first `width` bytes) and valid = 1
+void launch_window_fill(const int64_t* idx, int64_t n, void* out, uint8_t* valid, int width, const void* lit16, cudaStream_t st);
+
 // ---- synthetic TPC-H input ----------------------------------------------------------------------
 void launch_tpch_fixed(int table, int col, int kind, int64_t msf, int64_t row0, int64_t n, void* out, cudaStream_t st);
 void launch_tpch_str_len(int table, int col, int64_t msf, int64_t row0, int64_t n, uint32_t* lens, cudaStream_t st);

@@ -117,6 +117,7 @@ struct b200_engine {
   std::mutex export_mu;                      // small-result export arena (pinned), one export at a time
   uint8_t* export_arena = nullptr;
   std::atomic<uint64_t> narrowed_bytes_saved{0};         // PCIe bytes not sent thanks to narrowing (b200_engine_counter)
+  std::atomic<uint64_t> n_window_sorts{0};               // sorts the window operator ran itself (b200_engine_counter)
   std::atomic<uint64_t> nlj_pairs{0};                    // (build row, probe row) pairs the nested-loop join evaluated (b200_engine_counter)
 };
 
@@ -2628,6 +2629,7 @@ struct Runner {
         for (auto& c : in->cols) out->cols.push_back(slice_column(c, r0, r1));
         break;
       }
+      case PlanNode::Window: out = exec_window(n, part, met); break;
       case PlanNode::ShuffleWriter: throw EngineError(B200_ERR_INVALID, "nested ShuffleWriterExec");
     }
     if (met) met->output_rows += (uint64_t)out->n;
@@ -2664,6 +2666,350 @@ struct Runner {
       for (size_t c = 0; c < n_in_cols; c++) out->cols.push_back(slice_column(in->cols[c], 0, m));
       return out;
     }
+    const int64_t m = fetch >= 0 ? std::min<int64_t>(fetch, n) : n;
+    DevPtr idx = sort_permutation(keys, kcols, n, m);
+    DevBatch proj;
+    proj.n = n;
+    for (size_t c = 0; c < n_in_cols; c++) proj.cols.push_back(in->cols[c]);
+    DevBatchPtr out = gather_batch(x, proj, (const int64_t*)idx->ptr, m, false);
+    if (n > SMALL_SORT_MAX_ROWS || keys.size() > (size_t)SMALL_SORT_MAX_KEYS) CUDA_CHECK(cudaStreamSynchronize(x.st()));
+    if (met) {
+      met->elapsed_ns += (uint64_t)std::chrono::duration_cast<std::chrono::nanoseconds>(std::chrono::steady_clock::now() - t0).count();
+      met->input_rows += (uint64_t)n;
+    }
+    return out;
+  }
+
+  // ---- window functions (WindowAggExec / BoundedWindowAggExec) ---------------------------------------------------------
+  // True when the input is a sort (through CoalesceBatchesExec) by the partition keys, in any order and direction, then
+  // exactly the window's ORDER BY: its rows already are in the window's order and the operator sorts nothing.
+  static bool window_input_sorted(const PlanNode& n) {
+    const PlanNode* c = n.children[0].get();
+    while (c->op == PlanNode::Passthrough && c->op_name == "CoalesceBatchesExec") c = c->children[0].get();
+    if (c->op != PlanNode::Sort && c->op != PlanNode::SortPreservingMerge) return false;
+    const size_t np = n.window_partition.size(), no = n.window_order.size();
+    if (c->sort_keys.size() != np + no) return false;
+    auto in_sort_prefix = [&](const ExprPtr& e) {
+      for (size_t k = 0; k < np; k++)
+        if (expr_equal(c->sort_keys[k].expr, e)) return true;
+      return false;
+    };
+    for (size_t k = 0; k < np; k++) {
+      bool found = false;
+      for (auto& pk : n.window_partition) found = found || expr_equal(c->sort_keys[k].expr, pk);
+      if (!found || !in_sort_prefix(n.window_partition[k])) return false;
+    }
+    for (size_t k = 0; k < no; k++) {
+      const SortKey &a = c->sort_keys[np + k], &b = n.window_order[k];
+      if (!expr_equal(a.expr, b.expr) || a.asc != b.asc || a.nulls_first != b.nulls_first) return false;
+    }
+    return true;
+  }
+
+  DevBatchPtr exec_window(const PlanNode& n, int part, OpMetrics* met) {
+    DevBatchPtr in = exec(*n.children[0], part);
+    const auto t0 = std::chrono::steady_clock::now();
+    const int64_t N = in->n;
+    if (N >= ((int64_t)1 << 32)) throw EngineError(B200_ERR_UNSUPPORTED, "window over " + std::to_string(N) + " rows (the sort takes at most 2^32)");
+    const size_t np = n.window_partition.size(), no = n.window_order.size(), nw = n.window_exprs.size();
+    if (np + no > (size_t)WIN_MAX_KEYS) throw EngineError(B200_ERR_UNSUPPORTED, "window with more than " + std::to_string(WIN_MAX_KEYS) + " partition and order keys");
+    auto out = std::make_shared<DevBatch>();
+    out->n = N;
+    out->cols = in->cols;
+    const size_t n_in = in->cols.size();
+    if (met) met->input_rows += (uint64_t)N;
+    if (N == 0) {
+      for (size_t w = 0; w < nw; w++) {
+        const Field& f = n.schema[n_in + w];
+        DevColumn c = make_out_column(f.name, f.type, f.type.id == TypeId::Utf8 ? PH_STRVIEW : phys_of(f.type), 0, f.nullable, x.st());
+        c.n = 0;
+        out->cols.push_back(c);
+      }
+      return out;
+    }
+    // the columns the kernels read: partition keys, order keys, then the first argument of each function
+    std::vector<ExprPtr> exprs(n.window_partition);
+    for (auto& k : n.window_order) exprs.push_back(k.expr);
+    std::vector<size_t> arg_at(nw, 0);
+    for (size_t w = 0; w < nw; w++)
+      if (!n.window_exprs[w].args.empty()) {
+        arg_at[w] = exprs.size();
+        exprs.push_back(n.window_exprs[w].args[0]);
+      }
+    std::vector<DevColumn> cols;
+    bool need_eval = false;
+    for (auto& e : exprs) need_eval |= e->kind != Expr::Col;
+    if (need_eval) {
+      PipelineBuilder pb(*in, x.st());
+      std::vector<ColRef> outs;
+      for (auto& e : exprs) {
+        ColRef c = pb.compile(*e);
+        pb.pin(c);
+        outs.push_back(c);
+      }
+      cols = run_materialize(x, pb, outs, in, met)->cols;
+    } else {
+      for (auto& e : exprs) cols.push_back(in->cols.at((size_t)e->col));
+    }
+    // the order: the input's own when a matching sort feeds the window, else the device sort's permutation
+    DevPtr perm_buf;
+    const int64_t* perm = nullptr;
+    if (np + no > 0 && N > 1 && !window_input_sorted(n)) {
+      x.check_cancel();
+      std::vector<SortKey> keys;
+      std::vector<DevColumn> kcols;
+      for (size_t k = 0; k < np + no; k++) {
+        SortKey sk;
+        if (k < np) sk.expr = n.window_partition[k];  // any direction groups a partition's rows
+        else sk = n.window_order[k - np];
+        keys.push_back(sk);
+        kcols.push_back(cols[k]);
+      }
+      KernelTimer kt(x, "window_sort", (uint64_t)N * 8 * 2 * (np + no));
+      perm_buf = sort_permutation(keys, kcols, N, N);
+      perm = (const int64_t*)perm_buf->ptr;
+      x.e->n_window_sorts++;
+    }
+    // partition and peer-group boundaries
+    x.check_cancel();
+    WinKeys K;
+    memset(&K, 0, sizeof K);
+    K.n_part = (int)np;
+    K.n_order = (int)no;
+    std::vector<DevColumn> kviews;
+    uint64_t key_bytes = 0;
+    for (size_t k = 0; k < np + no; k++) kviews.push_back(as_views(x, cols[k]));
+    for (size_t k = 0; k < np + no; k++) {
+      const DevColumn& c = kviews[k];
+      K.k[k] = KeyCol{c.data, c.valid, (uint8_t)c.phys, (uint8_t)c.width()};
+      key_bytes += 2ull * ((uint64_t)c.width() + (c.valid ? 1 : 0));
+    }
+    const size_t N1 = (size_t)N + 1;
+    DevPtr part_flag = dev_alloc((size_t)N * 4, x.st()), peer_flag = dev_alloc((size_t)N * 4, x.st());
+    DevPtr part_ex = dev_alloc(N1 * 8, x.st()), peer_ex = dev_alloc(N1 * 8, x.st()), scan_scratch = dev_alloc(((size_t)N / 1024 + 4) * 8, x.st());
+    DevPtr pid = dev_alloc((size_t)N * 4, x.st()), gid = dev_alloc((size_t)N * 4, x.st());
+    DevPtr part_start = dev_alloc(N1 * 4, x.st()), peer_start = dev_alloc(N1 * 4, x.st()), first_peer = dev_alloc((size_t)N * 4, x.st());
+    WinBounds B;
+    B.pid = (uint32_t*)pid->ptr;
+    B.gid = (uint32_t*)gid->ptr;
+    B.part_start = (uint32_t*)part_start->ptr;
+    B.peer_start = (uint32_t*)peer_start->ptr;
+    B.part_first_peer = (uint32_t*)first_peer->ptr;
+    {
+      // flags (keys of two rows, two flags), two scans (flag in, offset out, and back), segments (flags, offsets, ids, starts)
+      KernelTimer kt(x, "window_bounds", (uint64_t)N * (key_bytes + (perm ? 16 : 0) + 8 + 2 * (4 + 16) + (16 + 16 + 8 + 12)));
+      launch_window_flags(K, perm, N, (uint32_t*)part_flag->ptr, (uint32_t*)peer_flag->ptr, x.st());
+      launch_scan_u32_to_u64((const uint32_t*)part_flag->ptr, (uint64_t*)part_ex->ptr, N, (uint64_t*)scan_scratch->ptr, x.st());
+      launch_scan_u32_to_u64((const uint32_t*)peer_flag->ptr, (uint64_t*)peer_ex->ptr, N, (uint64_t*)scan_scratch->ptr, x.st());
+      launch_window_segments((const uint32_t*)part_flag->ptr, (const uint32_t*)peer_flag->ptr, (const uint64_t*)part_ex->ptr, (const uint64_t*)peer_ex->ptr, N, B,
+                             x.st());
+    }
+    DevPtr error;
+    for (size_t w = 0; w < nw; w++) {
+      x.check_cancel();
+      const WindowExpr& we = n.window_exprs[w];
+      const Field& f = n.schema[n_in + w];
+      WinEval E;
+      memset(&E, 0, sizeof E);
+      const int64_t kMaxOff = (int64_t)1 << 40;  // beyond any partition (< 2^32 rows): no overflow in the frame arithmetic
+      E.units = we.frame.range ? WUNITS_RANGE : WUNITS_ROWS;
+      E.s_kind = we.frame.start.kind;
+      E.e_kind = we.frame.end.kind;
+      E.s_off = (int64_t)std::min<uint64_t>(we.frame.start.n, (uint64_t)kMaxOff);
+      E.e_off = (int64_t)std::min<uint64_t>(we.frame.end.n, (uint64_t)kMaxOff);
+      E.arg = we.n;
+      E.acc = WACC_I64;
+      static const uint8_t fn_kind[] = {WF_ROW_NUMBER, WF_RANK, WF_DENSE_RANK, WF_PERCENT_RANK, WF_CUME_DIST, WF_NTILE, WF_OFFSET, WF_OFFSET,
+                                        WF_FIRST,      WF_LAST, WF_NTH,        WF_AGG,          WF_AGG,       WF_AGG,   WF_AGG,    WF_AGG};
+      E.fn = fn_kind[(int)we.fn];
+      if (E.fn == WF_OFFSET || E.fn == WF_FIRST || E.fn == WF_LAST || E.fn == WF_NTH) {
+        DevPtr idx = dev_alloc((size_t)N * 8, x.st());
+        E.idx_out = (int64_t*)idx->ptr;
+        {
+          KernelTimer kt(x, "window_frames", (uint64_t)N * (8 + 8 + 16 + (perm ? 16 : 0)));
+          launch_window_eval(E, B, perm, N, x.st());
+        }
+        DevBatch one;
+        one.n = N;
+        one.cols.push_back(cols[arg_at[w]]);
+        DevColumn oc = gather_batch(x, one, (const int64_t*)idx->ptr, N, true)->cols[0];
+        if (we.default_value) {
+          const LitValue& l = we.default_value->lit;
+          uint64_t lit[2] = {0, 0};
+          switch (we.result_type.pk()) {
+            case PK::F64:
+              if (we.result_type.id == TypeId::Float32) {
+                const float v = (float)l.f;
+                memcpy(lit, &v, 4);
+              } else {
+                memcpy(lit, &l.f, 8);
+              }
+              break;
+            case PK::I128: memcpy(lit, &l.d, 16); break;
+            case PK::Str: {
+              DevPtr chars = dev_alloc(l.s.size() + 1, x.st());
+              if (!l.s.empty()) CUDA_CHECK(cudaMemcpyAsync(chars->ptr, l.s.data(), l.s.size(), cudaMemcpyHostToDevice, x.st()));
+              lit[0] = (uint64_t)(uintptr_t)chars->ptr;
+              lit[1] = (uint64_t)l.s.size();
+              oc.keep.push_back(chars);
+              break;
+            }
+            default: memcpy(lit, &l.i, 8); break;  // little-endian: the low bytes are the narrower integer
+          }
+          launch_window_fill((const int64_t*)idx->ptr, N, (void*)oc.data, (uint8_t*)oc.valid, oc.width(), lit, x.st());
+        }
+        oc.name = f.name;
+        out->cols.push_back(oc);
+        continue;
+      }
+      const Phys out_phys = phys_of(f.type);
+      // only the aggregates write a validity (ntile is typed nullable but never NULL)
+      DevColumn oc = make_out_column(f.name, f.type, out_phys, N, f.nullable && E.fn == WF_AGG, x.st());
+      oc.n = N;
+      E.out = (void*)oc.data;
+      E.out_valid = (uint8_t*)oc.valid;
+      E.out_phys = out_phys;
+      if (E.fn != WF_AGG) {
+        KernelTimer kt(x, "window_frames", (uint64_t)N * (8 + 16 + (perm ? 8 : 0)));
+        launch_window_eval(E, B, perm, N, x.st());
+        out->cols.push_back(oc);
+        continue;
+      }
+      // framed aggregates: the argument in sorted order, then forward / backward segmented scans by frame kind
+      const DevColumn* arg = we.args.empty() ? nullptr : &cols[arg_at[w]];
+      const DataType at = arg ? arg->type : DataType(TypeId::Int64);
+      WinLoad L;
+      memset(&L, 0, sizeof L);
+      if (arg) {
+        L.data = arg->data;
+        L.valid = arg->valid;
+        L.phys = (uint8_t)arg->phys;
+      }
+      E.op = WOP_SUM;
+      E.fin = WFIN_VALUE;
+      switch (we.fn) {
+        case WinFn::Count:
+          L.conv = arg ? WCV_VALID : WCV_ONE;
+          E.fin = WFIN_COUNT;
+          break;
+        case WinFn::Sum:
+        case WinFn::Avg:
+          if (at.is_decimal()) {
+            E.acc = WACC_I128;
+            L.conv = WCV_I128;
+          } else if (we.fn == WinFn::Avg || at.is_float()) {
+            E.acc = WACC_F64;
+            L.conv = WCV_F64;
+          } else {
+            L.conv = WCV_I64;
+          }
+          if (we.fn == WinFn::Avg) {
+            E.fin = WFIN_AVG;
+            E.imm = we.result_type.scale - at.scale;
+          }
+          break;
+        default:  // Min, Max
+          E.op = we.fn == WinFn::Min ? WOP_MIN : WOP_MAX;
+          if (at.is_decimal()) {
+            E.acc = WACC_I128;
+            L.conv = WCV_I128;
+          } else if (at.is_float()) {
+            L.conv = WCV_F64_KEY;
+            E.fin = WFIN_MINMAX_F64;
+          } else if (at.id == TypeId::UInt64) {
+            L.conv = WCV_U64_KEY;
+            E.fin = WFIN_MINMAX_U64;
+          } else {
+            L.conv = WCV_I64;
+          }
+      }
+      if (arg && arg->phys == PH_UTF8 && L.conv != WCV_VALID) throw EngineError(B200_ERR_UNSUPPORTED, "window " + we.fn_name + " over Utf8");
+      const size_t vw = E.acc == WACC_I128 ? 16 : 8;
+      DevPtr vals = dev_alloc((size_t)N * vw, x.st()), valid = dev_alloc((size_t)N, x.st());
+      L.out = vals->ptr;
+      L.out_valid = (uint8_t*)valid->ptr;
+      // which scans the frame needs (the frame kinds of DESIGN.md §4.8)
+      const uint8_t sk = we.frame.start.kind, ek = we.frame.end.kind;
+      bool fwd = false, bwd = false;
+      uint8_t seg = WSEG_PART;
+      if (sk == WB_UNBOUNDED_PRECEDING) {
+        fwd = true;
+        E.read = WRD_FWD;
+      } else if (ek == WB_UNBOUNDED_FOLLOWING) {
+        bwd = true;
+        E.read = WRD_BWD;
+      } else if (we.frame.range) {  // RANGE CURRENT ROW .. CURRENT ROW: the peer group
+        fwd = true;
+        seg = WSEG_PEER;
+        E.read = WRD_FWD;
+      } else {  // ROWS bounded on both sides: a fixed width
+        const int64_t so = sk == WB_PRECEDING ? -E.s_off : sk == WB_CURRENT_ROW ? 0 : E.s_off;
+        const int64_t eo = ek == WB_PRECEDING ? -E.e_off : ek == WB_CURRENT_ROW ? 0 : E.e_off;
+        E.w = std::min<int64_t>(eo - so + 1, N);
+        fwd = bwd = E.w > 0;  // w <= 0: every frame is empty, nothing to scan
+        seg = WSEG_BLOCK;
+        E.read = WRD_BLOCKS;
+      }
+      DevPtr fv, fc, bv, bc, tiles;
+      {
+        KernelTimer kt(x, "window_scan", (uint64_t)N * ((arg ? (uint64_t)arg->width() + 1 : 0) + (perm ? 8 : 0) + vw + 1) +
+                                             (uint64_t)N * (fwd + bwd) * 2 * (vw + 1 + 8 + vw + 4));
+        launch_window_load(L, perm, N, x.st());
+        WinScan S;
+        memset(&S, 0, sizeof S);
+        S.vals = vals->ptr;
+        S.valid = (const uint8_t*)valid->ptr;
+        S.n = N;
+        S.w = std::max<int64_t>(E.w, 1);
+        S.acc = E.acc;
+        S.op = E.op;
+        S.seg = seg;
+        if (fwd || bwd) tiles = dev_alloc((size_t)window_scan_tile_bytes(N), x.st());
+        S.tiles = tiles ? tiles->ptr : nullptr;
+        if (fwd) {
+          fv = dev_alloc((size_t)N * vw, x.st());
+          fc = dev_alloc((size_t)N * 4, x.st());
+          S.out_v = fv->ptr;
+          S.out_c = (uint32_t*)fc->ptr;
+          S.dir = 0;
+          launch_window_scan(S, B, x.st());
+          E.fwd_v = fv->ptr;
+          E.fwd_c = (const uint32_t*)fc->ptr;
+        }
+        x.check_cancel();
+        if (bwd) {
+          bv = dev_alloc((size_t)N * vw, x.st());
+          bc = dev_alloc((size_t)N * 4, x.st());
+          S.out_v = bv->ptr;
+          S.out_c = (uint32_t*)bc->ptr;
+          S.dir = 1;
+          launch_window_scan(S, B, x.st());
+          E.bwd_v = bv->ptr;
+          E.bwd_c = (const uint32_t*)bc->ptr;
+        }
+      }
+      if (E.fin == WFIN_AVG && E.acc == WACC_I128) {
+        if (!error) {
+          error = dev_alloc(16, x.st());
+          CUDA_CHECK(cudaMemsetAsync(error->ptr, 0, 16, x.st()));
+        }
+        E.error = (unsigned int*)error->ptr;
+      }
+      {
+        KernelTimer kt(x, "window_frames", (uint64_t)N * (32 + 2 * (vw + 4) + (perm ? 8 : 0) + (uint64_t)oc.width() + 1));
+        launch_window_eval(E, B, perm, N, x.st());
+      }
+      out->cols.push_back(oc);
+    }
+    if (error && x.get<unsigned int>(error->ptr)) throw EngineError(B200_ERR_EXECUTION, "Arithmetic overflow in a window AVG over Decimal128");
+    CUDA_CHECK(cudaStreamSynchronize(x.st()));  // the temporaries above are freed stream-ordered; the metrics take the device time
+    if (met) met->elapsed_ns += (uint64_t)std::chrono::duration_cast<std::chrono::nanoseconds>(std::chrono::steady_clock::now() - t0).count();
+    return out;
+  }
+
+  // The stable sort permutation of n >= 2 rows by `keys`, evaluated in `kcols`: the input rows of sorted positions
+  // [0, m) as int64 indices.  Rows with equal keys keep their input order.  SortExec and the window operator share it.
+  DevPtr sort_permutation(const std::vector<SortKey>& keys, const std::vector<DevColumn>& kcols, int64_t n, int64_t m) {
     if (n >= ((int64_t)1 << 32)) throw EngineError(B200_ERR_UNSUPPORTED, "sort of more than 2^32 rows");
     if (n <= SMALL_SORT_MAX_ROWS && keys.size() <= (size_t)SMALL_SORT_MAX_KEYS) {
       // the tail of a query (ORDER BY over a few groups): one comparison-sort launch, no length read-backs
@@ -2683,16 +3029,7 @@ struct Runner {
       }
       DevPtr idx = dev_alloc((size_t)n * 8, x.st());
       launch_small_sort(K, (int64_t*)idx->ptr, n, x.st());
-      const int64_t m = fetch >= 0 ? std::min<int64_t>(fetch, n) : n;
-      DevBatch proj;
-      proj.n = n;
-      for (size_t c = 0; c < n_in_cols; c++) proj.cols.push_back(in->cols[c]);
-      DevBatchPtr out = gather_batch(x, proj, (const int64_t*)idx->ptr, m, false);
-      if (met) {
-        met->elapsed_ns += (uint64_t)std::chrono::duration_cast<std::chrono::nanoseconds>(std::chrono::steady_clock::now() - t0).count();
-        met->input_rows += (uint64_t)n;
-      }
-      return out;
+      return idx;
     }
     const uint32_t n_blocks = (uint32_t)((n + 2047) / 2048);
     DevPtr ka = dev_alloc((size_t)n * 8, x.st()), kb = dev_alloc((size_t)n * 8, x.st());
@@ -2700,7 +3037,6 @@ struct Runner {
     DevPtr hist = dev_alloc((size_t)256 * n_blocks * 4 + 64, x.st());
     DevPtr scan = dev_alloc(((size_t)256 * n_blocks + 1 + (size_t)(256 * n_blocks) / 1024 + 8) * 8, x.st());
     uint32_t* perm = (uint32_t*)va->ptr;
-    uint32_t* perm_alt = (uint32_t*)vb->ptr;
     launch_iota_u32(perm, n, x.st());
     for (size_t ki = keys.size(); ki-- > 0;) {
       DevColumn kc = as_views(x, kcols[ki]);
@@ -2734,22 +3070,11 @@ struct Runner {
           radix_sort_pairs_u64((uint64_t*)ka->ptr, (uint32_t*)vb->ptr, (uint64_t*)kb->ptr, (uint32_t*)va->ptr, n, (uint32_t*)hist->ptr, (uint64_t*)scan->ptr, x.st(), &in_a);
           perm = in_a ? (uint32_t*)vb->ptr : (uint32_t*)va->ptr;
         }
-        (void)perm_alt;
       }
     }
-    int64_t m = fetch >= 0 ? std::min<int64_t>(fetch, n) : n;
     DevPtr idx = dev_alloc((size_t)std::max<int64_t>(m, 1) * 8, x.st());
     launch_u32_to_i64(perm, (int64_t*)idx->ptr, m, x.st());
-    DevBatch proj;
-    proj.n = n;
-    for (size_t c = 0; c < n_in_cols; c++) proj.cols.push_back(in->cols[c]);
-    DevBatchPtr out = gather_batch(x, proj, (const int64_t*)idx->ptr, m, false);
-    CUDA_CHECK(cudaStreamSynchronize(x.st()));
-    if (met) {
-      met->elapsed_ns += (uint64_t)std::chrono::duration_cast<std::chrono::nanoseconds>(std::chrono::steady_clock::now() - t0).count();
-      met->input_rows += (uint64_t)n;
-    }
-    return out;
+    return idx;
   }
 
   // ---- hash join --------------------------------------------------------------------------------
@@ -4771,6 +5096,7 @@ uint64_t b200_engine_counter(b200_engine* e, const char* name) {
   if (n == "fastfilter") return e->n_fastfilter;
   if (n == "ingest_bytes_saved") return e->narrowed_bytes_saved;
   if (n == "nlj_pairs") return e->nlj_pairs;
+  if (n == "window_sorts") return e->n_window_sorts;
   return 0;
 }
 

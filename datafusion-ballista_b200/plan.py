@@ -236,6 +236,46 @@ def sort_preserving_merge(keys: Sequence[Json], input: Json, fetch: Optional[int
     return n
 
 
+UNBOUNDED_PRECEDING: Json = {"kind": "unbounded_preceding"}
+CURRENT_ROW: Json = {"kind": "current_row"}
+UNBOUNDED_FOLLOWING: Json = {"kind": "unbounded_following"}
+
+
+def preceding(n: int) -> Json:
+    return {"kind": "preceding", "n": int(n)}
+
+
+def following(n: int) -> Json:
+    return {"kind": "following", "n": int(n)}
+
+
+def rows(start: Json, end: Json) -> Json:
+    """ROWS BETWEEN start AND end (bounds: UNBOUNDED_PRECEDING, preceding(n), CURRENT_ROW, following(n), UNBOUNDED_FOLLOWING)."""
+    return {"units": "rows", "start": start, "end": end}
+
+
+def range_(start: Json, end: Json) -> Json:
+    """RANGE BETWEEN start AND end; the device takes UNBOUNDED and CURRENT ROW bounds (CURRENT ROW = the row's peers)."""
+    return {"units": "range", "start": start, "end": end}
+
+
+def win(fn_: str, name: str, args: Sequence[Json] = (), partition_by: Sequence[Json] = (), order_by: Sequence[Json] = (),
+        frame: Optional[Json] = None) -> Json:
+    """One window expression.  frame=None: DataFusion's default, RANGE BETWEEN UNBOUNDED PRECEDING AND CURRENT ROW (the whole
+    partition without ORDER BY).  order_by: sort_key(...) entries."""
+    w: Json = {"fn": fn_, "name": name, "args": list(args), "partition_by": list(partition_by), "order_by": list(order_by)}
+    if frame is not None:
+        w["frame"] = frame
+    return w
+
+
+def window(exprs: Sequence[Json], input: Json, partition_keys: Optional[Sequence[Json]] = None, mode: Optional[str] = "sorted") -> Json:
+    """WindowAggExec (mode None) / BoundedWindowAggExec (mode "sorted").  The output is the input's columns, then one column
+    per expression, named by its name (DESIGN.md §6 (viii)).  partition_keys default to the first expression's."""
+    pk = list(exprs[0]["partition_by"]) if partition_keys is None else list(partition_keys)
+    return {"op": "WindowAggExec", "mode": mode, "partition_keys": pk, "window_expr": list(exprs), "input": input}
+
+
 def coalesce_batches(input: Json) -> Json:
     return {"op": "CoalesceBatchesExec", "input": input}
 

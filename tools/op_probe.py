@@ -1,7 +1,7 @@
 """One big instance of one operator, so that `ncu -k regex:<kernel> -c 1` lands on a representative launch, and so that the
 engine's own CUDA-event timing (b200_engine_kernel_stats) can be read for the same launch without a profiler attached.
 
-  python tools/op_probe.py join|partition|groupby|groupby_small|filter|parquet|q1|minmax_str|stats|nlj|scalar|rollup [msf]
+  python tools/op_probe.py join|partition|groupby|groupby_small|filter|parquet|q1|minmax_str|stats|nlj|scalar|rollup|window [msf]
 
   join       orders (build, 15 M rows at SF10) |x| lineitem (probe, 60 M rows) on the order key      -> join_build2 / join_probe2
   partition  lineitem (4 columns, 48 B/row) hash-repartitioned on l_orderkey into 8 partitions       -> part_tile_hist / part_tile_scatter
@@ -22,6 +22,11 @@ engine's own CUDA-event timing (b200_engine_kernel_stats) can be read for the sa
   rollup     Single-mode ROLLUP / CUBE over lineitem, SUM(l_extendedprice), COUNT(*), MIN(l_shipdate): (a) ROLLUP(l_returnflag,
              l_linestatus), (b) ROLLUP(l_suppkey, l_returnflag), (c) CUBE(l_returnflag, l_linestatus, l_shipmode), each in one
              pass (-> pipeline_agg_gsets) and as one ordinary aggregate per set; results checked at SF1 against the oracle
+  window     WindowAggExec over lineitem: (a) row_number() by l_suppkey ORDER BY l_extendedprice DESC, (b) sum(l_quantity)
+             by l_orderkey ORDER BY l_linenumber ROWS 2 PRECEDING..CURRENT ROW, (c) avg(CAST(l_extendedprice AS DOUBLE)) by
+             (l_returnflag, l_linestatus) ORDER BY l_shipdate ROWS 99 PRECEDING..100 FOLLOWING, (d) lag(l_extendedprice)
+             and a running sum(l_extendedprice) by l_suppkey ORDER BY l_shipdate -> window_sort / window_bounds /
+             window_scan / window_frames; every result checked at SF1 against numpy
   nlj        NestedLoopJoinExec: lineitem against one build row (a scalar subquery) next to the same comparison
              through fast_filter_kernel, and a band join of orders (msf 1000) against 10,000 build rows    -> nlj_count / nlj_write
 """
@@ -423,6 +428,105 @@ elif op == "rollup":
         log(name, "matches the oracle at SF1 (", n1, "rows )")
     oracle.close()
     print(json.dumps({op: {"checked_at_sf1": {"rows": n1, "cases": list(cases), "result": "= CPU oracle (UNION ALL form)"}}}), flush=True)
+elif op == "window":
+    # device time per kernel family (the sort apart from the window's own kernels), bytes per row as the kernel timers count
+    # them, and every result checked at SF1 against numpy (integer cents for the decimal columns: exact)
+    import subprocess
+    import numpy as np
+    import pyarrow as pa
+    import pyarrow.compute as pc
+    from ballista_b200 import driver
+    smi = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
+    cols = ["l_orderkey", "l_suppkey", "l_linenumber", "l_quantity", "l_extendedprice", "l_returnflag", "l_linestatus", "l_shipdate"]
+    scan = tpch.table_scan("lineitem", cols)
+    desc = P.sort_key(c("l_extendedprice"), False, False)
+    cases = {
+        "a_row_number_by_suppkey": ([c("l_suppkey")], [desc], [P.win("row_number", "rn")]),
+        "b_sum_rows_2p_by_orderkey": ([c("l_orderkey")], [P.sort_key(c("l_linenumber"))],
+                                      [P.win("sum", "s", [c("l_quantity")], frame=P.rows(P.preceding(2), P.CURRENT_ROW))]),
+        "c_avg_rows_99p_100f_by_flag_status": ([c("l_returnflag"), c("l_linestatus")], [P.sort_key(c("l_shipdate"))],
+                                               [P.win("avg", "a", [P.cast(c("l_extendedprice"), "f64")], frame=P.rows(P.preceding(99), P.following(100)))]),
+        "d_lag_and_running_sum_by_suppkey": ([c("l_suppkey")], [P.sort_key(c("l_shipdate"))],
+                                             [P.win("lag", "lg", [c("l_extendedprice")]), P.win("sum", "rs", [c("l_extendedprice")])]),
+    }
+
+    def stages(pk, ob, ws):
+        return [P.Stage(1, P.shuffle_writer(P.window([dict(w, partition_by=pk, order_by=ob) for w in ws], scan, pk), 1))]
+
+    n = load("lineitem", cols)
+    report = {"gpu": smi, "lineitem_rows": n, "reps": reps,
+              "bytes": "the kernel timers' algorithmic bytes: keys, flags, ids, scan values and counts, results, the permutation"}
+    for name, (pk, ob, ws) in cases.items():
+        run(stages(pk, ob, ws), [1])   # warm-up
+        eng.kernel_stats(reset=True)
+        run(stages(pk, ob, ws), [1])
+        ks = eng.kernel_stats(reset=True)
+        fam = {k: {"ms_per_run": round(v["ms"] / reps, 3), "bytes_per_row": round(v["bytes"] / (reps * n), 1),
+                   "GB_per_s": round(v["bytes"] / (v["ms"] * 1e-3) / 1e9, 1)} for k, v in ks.items() if v["ms"] > 0}
+        own = [k for k in fam if k.startswith("window_") and k != "window_sort"]
+        report[name] = {"families": fam, "window_kernels_ms": round(sum(fam[k]["ms_per_run"] for k in own), 3),
+                        "sort_ms": fam.get("window_sort", {}).get("ms_per_run", 0.0)}
+        print(name, json.dumps(report[name]), file=sys.stderr, flush=True)
+    print(json.dumps({op: report}, indent=1), flush=True)
+    # correctness at SF1 against numpy
+    m1 = 1000
+    n1 = eng.tpch_table_rows("lineitem", m1)
+    eng.drop_table("lineitem")
+    eng.tpch_generate("lineitem", m1, 0, 0, n1, cols)
+    src = pa.Table.from_batches([eng.export_table("lineitem", 0)])
+    cents = lambda a: np.rint(pc.cast(a, pa.float64()).to_numpy(zero_copy_only=False) * 100).astype(np.int64)
+    supp, okey, line = (src.column(k).to_numpy() for k in ("l_suppkey", "l_orderkey", "l_linenumber"))
+    price, qty = cents(src.column("l_extendedprice")), cents(src.column("l_quantity"))
+    ship = src.column("l_shipdate").cast(pa.int32()).to_numpy()
+    fs = pc.binary_join_element_wise(src.column("l_returnflag"), src.column("l_linestatus"), "").to_numpy(zero_copy_only=False)
+    rid = np.arange(n1)
+    got = {name: driver.run_stages(eng, stages(*case), f"chk-{name}") for name, case in cases.items()}
+
+    def starts(order, *keys):
+        brk = np.ones(n1, bool)
+        brk[1:] = np.any([k[order][1:] != k[order][:-1] for k in keys], axis=0)
+        return np.maximum.accumulate(np.where(brk, np.arange(n1), 0)), brk
+
+    # (a)
+    o = np.lexsort((rid, -price, supp))
+    ps, _ = starts(o, supp)
+    want = np.empty(n1, np.int64)
+    want[o] = np.arange(n1) - ps + 1
+    assert np.array_equal(got["a_row_number_by_suppkey"].column("rn").to_numpy(), want)
+    # (b)
+    o = np.lexsort((rid, line, okey))
+    ps, _ = starts(o, okey)
+    x = qty[o]
+    s = x.copy()
+    idx = np.arange(n1)
+    for k in (1, 2):
+        s[k:] += np.where(idx[k:] - k >= ps[k:], x[:-k], 0)
+    want = np.empty(n1, np.int64)
+    want[o] = s
+    assert np.array_equal(cents(got["b_sum_rows_2p_by_orderkey"].column("s")), want)
+    # (c) exact frame sums in integer cents over [max(ps, i - 99), min(pe, i + 101))
+    o = np.lexsort((rid, ship, fs))
+    ps, brk = starts(o, fs)
+    pe = np.minimum.accumulate(np.where(np.append(brk[1:], True), np.arange(1, n1 + 1), n1)[::-1])[::-1]
+    pre = np.concatenate([[0], np.cumsum(price[o])])
+    lo, hi = np.maximum(ps, idx - 99), np.minimum(pe, idx + 101)
+    want = np.empty(n1)
+    want[o] = (pre[hi] - pre[lo]) / 100.0 / (hi - lo)
+    assert np.allclose(got["c_avg_rows_99p_100f_by_flag_status"].column("a").to_numpy(), want, rtol=1e-12, atol=0)
+    # (d) lag within the partition; running sum up to the last peer (same l_shipdate)
+    o = np.lexsort((rid, ship, supp))
+    ps, _ = starts(o, supp)
+    qs, qbrk = starts(o, supp, ship)
+    lag = np.where(idx > ps, np.roll(price[o], 1), -1)
+    run_ = np.concatenate([[0], np.cumsum(price[o])])
+    qe = np.minimum.accumulate(np.where(np.append(qbrk[1:], True), np.arange(1, n1 + 1), n1)[::-1])[::-1]
+    want_lag, want_rs = np.empty(n1, np.int64), np.empty(n1, np.int64)
+    want_lag[o] = lag
+    want_rs[o] = run_[qe] - run_[ps]
+    g = got["d_lag_and_running_sum_by_suppkey"]
+    assert np.array_equal(np.where(g.column("lg").is_null().to_numpy(zero_copy_only=False), -1, cents(g.column("lg").fill_null(0))), want_lag)
+    assert np.array_equal(cents(g.column("rs")), want_rs)
+    print(json.dumps({op: {"checked_at_sf1": {"rows": n1, "cases": list(cases), "result": "= numpy (integer cents; (c) within 1e-12 relative)"}}}), flush=True)
 else:
     raise SystemExit(__doc__)
 print(json.dumps({op: eng.kernel_stats()}, indent=1))
