@@ -119,13 +119,17 @@ struct b200_engine {
   std::atomic<uint64_t> narrowed_bytes_saved{0};         // PCIe bytes not sent thanks to narrowing (b200_engine_counter)
   std::atomic<uint64_t> n_window_sorts{0};               // sorts the window operator ran itself (b200_engine_counter)
   std::atomic<uint64_t> nlj_pairs{0};                    // (build row, probe row) pairs the nested-loop join evaluated (b200_engine_counter)
+  std::atomic<uint64_t> host_syncs{0};                   // host waits on the stream inside tasks, exchanges and exports (host_wait)
+  // parsed stage plans by plan text with the job id taken out (b200_stage_prepare): the next job that runs the same stage
+  // plan shares the parsed tree instead of parsing and typing the JSON again.  Plans are read-only once parsed.
+  std::map<std::string, std::shared_ptr<const PlanNode>> plan_cache;
 };
 
 struct b200_stage {
   b200_engine* eng = nullptr;
   std::string job_id;
   int64_t stage_id = 0;
-  PlanPtr plan;
+  std::shared_ptr<const PlanNode> plan;  // possibly shared with other stages of the same plan text (b200_engine::plan_cache)
   std::string fingerprint;
   std::vector<OpMetrics> metrics;  // pre-order
   std::map<const PlanNode*, int> metric_index;
@@ -160,6 +164,13 @@ inline TaskCtx& task_ctx() {
   static thread_local TaskCtx t;
   if (!t.arena && cudaHostAlloc((void**)&t.arena, TASK_ARENA_BYTES, cudaHostAllocDefault) != cudaSuccess) t.arena = nullptr;
   return t;
+}
+
+// Blocks the host until the stream has drained.  Every such wait of a task, an exchange or an export goes through here and
+// is counted (b200_engine_counter "host_syncs"): the tail of a small query is bound by these round trips, not by its kernels.
+inline cudaError_t host_wait(b200_engine* e, cudaStream_t st) {
+  e->host_syncs++;
+  return cudaStreamSynchronize(st);
 }
 
 struct Exec {
@@ -219,7 +230,7 @@ struct Exec {
   // wait for everything enqueued so far, then run the deferred checks (they may throw)
   void sync() const {
     TaskCtx& t = task_ctx();
-    cudaError_t se = cudaStreamSynchronize(st());
+    cudaError_t se = host_wait(e, st());
     t.drained = true;
     std::vector<std::function<void()>> cs;
     cs.swap(t.checks);
@@ -815,23 +826,23 @@ std::vector<HostCol> download_batch(const Exec& x, const DevBatch& b, int64_t r0
         DevPtr bm = dev_alloc((size_t)(n + 7) / 8 + 16, st);
         launch_bytes_to_bitmap(c.data, (uint8_t*)bm->ptr, n, nullptr, st);
         CUDA_CHECK(cudaMemcpyAsync(h.data.data(), bm->ptr, h.data.size(), cudaMemcpyDeviceToHost, st));
-        CUDA_CHECK(cudaStreamSynchronize(st));
+        CUDA_CHECK(host_wait(x.e, st));
       }
     } else if (c.type.id == TypeId::Utf8) {
       DevColumn u = c.phys == PH_STRVIEW ? as_utf8(x, c) : c;
       h.data.resize((size_t)(n + 1) * 4);
       CUDA_CHECK(cudaMemcpyAsync(h.data.data(), u.data, h.data.size(), cudaMemcpyDeviceToHost, st));
-      CUDA_CHECK(cudaStreamSynchronize(st));
+      CUDA_CHECK(host_wait(x.e, st));
       int32_t* off = (int32_t*)h.data.data();
       int32_t first = off[0], last = off[n];
       h.extra.resize((size_t)(last - first));
       if (last > first) CUDA_CHECK(cudaMemcpyAsync(h.extra.data(), u.chars + first, h.extra.size(), cudaMemcpyDeviceToHost, st));
-      CUDA_CHECK(cudaStreamSynchronize(st));
+      CUDA_CHECK(host_wait(x.e, st));
       for (int64_t i = 0; i <= n; i++) off[i] -= first;
     } else {
       h.data.resize((size_t)n * c.width());
       if (n) CUDA_CHECK(cudaMemcpyAsync(h.data.data(), c.data, h.data.size(), cudaMemcpyDeviceToHost, st));
-      CUDA_CHECK(cudaStreamSynchronize(st));
+      CUDA_CHECK(host_wait(x.e, st));
     }
     hcs.push_back(std::move(h));
   }
@@ -2672,7 +2683,7 @@ struct Runner {
     proj.n = n;
     for (size_t c = 0; c < n_in_cols; c++) proj.cols.push_back(in->cols[c]);
     DevBatchPtr out = gather_batch(x, proj, (const int64_t*)idx->ptr, m, false);
-    if (n > SMALL_SORT_MAX_ROWS || keys.size() > (size_t)SMALL_SORT_MAX_KEYS) CUDA_CHECK(cudaStreamSynchronize(x.st()));
+    if (n > SMALL_SORT_MAX_ROWS || keys.size() > (size_t)SMALL_SORT_MAX_KEYS) CUDA_CHECK(host_wait(x.e, x.st()));
     if (met) {
       met->elapsed_ns += (uint64_t)std::chrono::duration_cast<std::chrono::nanoseconds>(std::chrono::steady_clock::now() - t0).count();
       met->input_rows += (uint64_t)n;
@@ -3002,7 +3013,7 @@ struct Runner {
       out->cols.push_back(oc);
     }
     if (error && x.get<unsigned int>(error->ptr)) throw EngineError(B200_ERR_EXECUTION, "Arithmetic overflow in a window AVG over Decimal128");
-    CUDA_CHECK(cudaStreamSynchronize(x.st()));  // the temporaries above are freed stream-ordered; the metrics take the device time
+    CUDA_CHECK(host_wait(x.e, x.st()));  // the temporaries above are freed stream-ordered; the metrics take the device time
     if (met) met->elapsed_ns += (uint64_t)std::chrono::duration_cast<std::chrono::nanoseconds>(std::chrono::steady_clock::now() - t0).count();
     return out;
   }
@@ -4909,7 +4920,7 @@ static void comm_allgather(b200_engine* e, const void* mine, void* all, size_t r
     }
     NCCL_CHECK(N.GroupEnd());
     CUDA_CHECK(cudaMemcpyAsync(all, dev, rec * (size_t)W, cudaMemcpyDeviceToHost, e->stream));
-    CUDA_CHECK(cudaStreamSynchronize(e->stream));
+    CUDA_CHECK(host_wait(e, e->stream));
   } catch (...) {
     cudaFree(dev);
     throw;
@@ -5097,6 +5108,7 @@ uint64_t b200_engine_counter(b200_engine* e, const char* name) {
   if (n == "ingest_bytes_saved") return e->narrowed_bytes_saved;
   if (n == "nlj_pairs") return e->nlj_pairs;
   if (n == "window_sorts") return e->n_window_sorts;
+  if (n == "host_syncs") return e->host_syncs;
   return 0;
 }
 
@@ -5360,27 +5372,45 @@ int b200_stage_prepare(b200_engine* e, const char* job_id, int64_t stage_id, con
   ScopeTimer tm("stage_prepare");
   return guard([&] {
     if (!e || !plan_json || !out) throw EngineError(B200_ERR_INVALID, "null argument");
-    Json j = parse_json(plan_json, plan_len ? (size_t)plan_len : strlen(plan_json));
-    PlanPtr plan = parse_plan(j);
-    if (plan->op != PlanNode::ShuffleWriter)
-      throw EngineError(B200_ERR_INVALID, "Plan passed to new_query_stage_exec is not a ShuffleWriterExec");  // execution_engine.rs:164-167
+    const size_t len = plan_len ? (size_t)plan_len : strlen(plan_json);
+    // strategy hints (which aggregate sink / table size worked) are remembered per plan SHAPE: the job id is taken out
+    // of the hashed text so that the next job that runs the same stage plan starts from what the last one learnt
+    std::string shape(plan_json, len);
+    const std::string tag = "\"job_id\":\"";
+    size_t at = shape.find(tag);
+    if (at != std::string::npos) {
+      size_t end = shape.find('"', at + tag.size());
+      if (end != std::string::npos) shape.erase(at + tag.size(), end - at - tag.size());
+    }
+    // the same shape also shares the parsed plan: parsing and typing the JSON is most of the host time of preparing a
+    // small stage, and a repeated query prepares the same few plans for every job.  Keyed by the stage id as well (the
+    // writer stores under it).  Only when the caller names the job: otherwise the job id comes from the text itself.
+    const std::string cache_key = std::to_string(stage_id) + ":" + shape;
+    std::shared_ptr<const PlanNode> plan;
+    if (job_id) {
+      std::lock_guard<std::mutex> g(e->mu);
+      auto it = e->plan_cache.find(cache_key);
+      if (it != e->plan_cache.end()) plan = it->second;
+    }
+    if (!plan) {
+      Json j = parse_json(plan_json, len);
+      PlanPtr parsed = parse_plan(j);
+      if (parsed->op != PlanNode::ShuffleWriter)
+        throw EngineError(B200_ERR_INVALID, "Plan passed to new_query_stage_exec is not a ShuffleWriterExec");  // execution_engine.rs:164-167
+      parsed->stage_id = stage_id;
+      plan = std::shared_ptr<const PlanNode>(std::move(parsed));
+      if (job_id) {
+        static const size_t PLAN_CACHE_MAX = 256;  // distinct stage plans kept; a workload with more starts over
+        std::lock_guard<std::mutex> g(e->mu);
+        if (e->plan_cache.size() >= PLAN_CACHE_MAX) e->plan_cache.clear();
+        e->plan_cache.emplace(cache_key, plan);
+      }
+    }
     auto* s = new b200_stage();
     s->eng = e;
     s->job_id = job_id ? job_id : plan->job_id;
     s->stage_id = stage_id;
-    plan->stage_id = stage_id;
-    {
-      // strategy hints (which aggregate sink / table size worked) are remembered per plan SHAPE: the job id is taken out
-      // of the hashed text so that the next job that runs the same stage plan starts from what the last one learnt
-      std::string shape(plan_json, plan_len ? (size_t)plan_len : strlen(plan_json));
-      const std::string tag = "\"job_id\":\"";
-      size_t at = shape.find(tag);
-      if (at != std::string::npos) {
-        size_t end = shape.find('"', at + tag.size());
-        if (end != std::string::npos) shape.erase(at + tag.size(), end - at - tag.size());
-      }
-      s->fingerprint = std::to_string(stage_id) + ":" + std::to_string(mix64(hash_bytes((const uint8_t*)shape.data(), (uint32_t)shape.size())));
-    }
+    s->fingerprint = std::to_string(stage_id) + ":" + std::to_string(mix64(hash_bytes((const uint8_t*)shape.data(), (uint32_t)shape.size())));
     collect_nodes(*plan, s);
     s->plan = std::move(plan);
     *out = s;
@@ -5559,7 +5589,7 @@ int b200_stage_execute(b200_stage* s, int input_partition, const volatile int32_
     try {
       res = r.execute_stage(*s->plan, input_partition);
     } catch (...) {
-      cudaStreamSynchronize(s->eng->stream);
+      host_wait(s->eng, s->eng->stream);
       Exec::abandon();
       // a cancelled or failed task leaves nothing behind (Executor::cancel_task drops the future together with
       // its partial outputs, executor.rs:217-237): remove whatever this task already stored
@@ -5610,7 +5640,7 @@ int b200_stage_execute_exchange(b200_stage* s, int input_partition, const volati
         ex.run(&sent, &recvd);
       }
     } catch (...) {
-      cudaStreamSynchronize(e->stream);
+      host_wait(e, e->stream);
       Exec::abandon();
       throw;
     }
@@ -5782,7 +5812,7 @@ int b200_exchange_stage(b200_engine* e, const char* job_id, int64_t stage_id, in
     try {
       ex.run(&sent, &recvd);
     } catch (...) {
-      cudaStreamSynchronize(e->stream);
+      host_wait(e, e->stream);
       Exec::abandon();
       throw;
     }

@@ -17,6 +17,7 @@ from __future__ import annotations
 
 import ctypes as C
 import os
+import threading
 from typing import List, Optional
 
 import pyarrow as pa
@@ -194,18 +195,37 @@ def parquet_describe(path: str) -> dict:
     return _json.loads(buf.value.decode())
 
 
+# Output arrays of b200_stage_execute / b200_stage_metrics, one of each per thread and reused by every stage executor of
+# that thread: the results are copied out before the call returns.  A fresh 8192-entry array per stage cost more host
+# time than preparing the stage itself, and every microsecond of it leaves the GPU idle between two stages.
+_out_bufs = threading.local()
+_OUT_CAP = 8192   # >= the largest shuffle fan-out the engine accepts (4096)
+_METRICS_CAP = 256
+
+
+def _partition_buffer():
+    b = getattr(_out_bufs, "partitions", None)
+    if b is None:
+        b = _out_bufs.partitions = (ShuffleWritePartition * _OUT_CAP)()
+    return b
+
+
+def _metrics_buffer():
+    b = getattr(_out_bufs, "metrics", None)
+    if b is None:
+        b = _out_bufs.metrics = (OperatorMetrics * _METRICS_CAP)()
+    return b
+
+
 class QueryStageExecutor:
     def __init__(self, engine: "GpuExecutionEngine", handle, job_id: str, stage_id: int):
         self.engine, self.h, self.job_id, self.stage_id = engine, handle, job_id, stage_id
-        self._cap = 8192   # >= the largest shuffle fan-out the engine accepts (4096)
-        self._out = (ShuffleWritePartition * self._cap)()
 
     def execute_query_stage(self, input_partition: int, cancel_flag=None) -> List[ShuffleWritePartition]:
-        cap = self._cap
-        out = self._out
+        out = _partition_buffer()
         n = C.c_int(0)
         cf = C.addressof(cancel_flag) if cancel_flag is not None else None
-        _check(load_library().b200_stage_execute(self.h, input_partition, cf, out, cap, C.byref(n)))
+        _check(load_library().b200_stage_execute(self.h, input_partition, cf, out, _OUT_CAP, C.byref(n)))
         res = [ShuffleWritePartition.from_buffer_copy(out[i]) for i in range(n.value)]
         return res
 
@@ -214,16 +234,16 @@ class QueryStageExecutor:
         Returns (ShuffleWritePartition list, {"sent_bytes", "recv_bytes"})."""
         n = C.c_int(0)
         st = ExchangeStats()
+        out = _partition_buffer()
         cf = C.addressof(cancel_flag) if cancel_flag is not None else None
-        _check(load_library().b200_stage_execute_exchange(self.h, input_partition, cf, self._out, self._cap, C.byref(n), C.byref(st)))
-        res = [ShuffleWritePartition.from_buffer_copy(self._out[i]) for i in range(n.value)]
+        _check(load_library().b200_stage_execute_exchange(self.h, input_partition, cf, out, _OUT_CAP, C.byref(n), C.byref(st)))
+        res = [ShuffleWritePartition.from_buffer_copy(out[i]) for i in range(n.value)]
         return res, {"sent_bytes": st.sent_bytes, "recv_bytes": st.recv_bytes}
 
     def collect_plan_metrics(self) -> List[dict]:
-        cap = 256
-        out = (OperatorMetrics * cap)()
+        out = _metrics_buffer()
         n = C.c_int(0)
-        _check(load_library().b200_stage_metrics(self.h, out, cap, C.byref(n)))
+        _check(load_library().b200_stage_metrics(self.h, out, _METRICS_CAP, C.byref(n)))
         return [dict(name=out[i].name.decode(), output_rows=out[i].output_rows, input_rows=out[i].input_rows,
                      elapsed_compute_ns=out[i].elapsed_compute_ns, bytes_read=out[i].bytes_read,
                      bytes_written=out[i].bytes_written, kernel_launches=out[i].kernel_launches)
