@@ -15,6 +15,8 @@
 //     filter indexes left ++ right, so the decoder emits "filter_columns" and plan.hpp remaps.
 // Scans: ParquetScanExecNode -> DataSourceExec on the table named after the files' directory (or file stem); the file
 // groups are passed through ("file_groups") for the host side to register (b200_engine_register_parquet).
+// CsvScanExecNode -> the same, plus "format": "csv", the reader options ("csv") and, when any file carries a byte range,
+// "file_ranges" shaped like "file_groups" ([start, end] or null), for b200_engine_register_csv.
 #pragma once
 #include <cstdint>
 #include <cstdio>
@@ -545,25 +547,47 @@ inline std::string plan_json(const Msg& n, const std::string& override_job) {
   const Msg m(x->b);
   auto in = [&](uint32_t f) { return plan_json(m.sub(f)); };
   switch (x->field) {
-    case 1: {  // ParquetScanExecNode { base_conf = 1 } ; FileScanExecConf { file_groups = 1, schema = 2, projection = 4 } (:1058-1086)
+    case 1:    // ParquetScanExecNode { base_conf = 1 } (:1058-1077)
+    case 2: {  // CsvScanExecNode { base_conf = 1, has_header = 2, delimiter = 3, quote = 4, escape = 5, comment = 6,
+               //                   newlines_in_values = 7, truncate_rows = 8 } (:1088-1101)
+      // FileScanExecConf { file_groups = 1, schema = 2, projection = 4 } (:1058-1086)
+      const bool csv = x->field == 2;
+      if (csv && m.has(6)) throw Unsupported("CsvScanExecNode option 'comment' is not supported by the device engine");
+      if (csv && m.u64(8)) throw Unsupported("CsvScanExecNode option 'truncate_rows' is not supported by the device engine");
       const Msg conf = m.sub(1);
-      std::string table, groups = "[";
-      bool fg = true;
+      std::string table, groups = "[", ranges = "[";
+      bool fg = true, any_range = false;
       for (auto& g : conf.subs(1)) {
-        if (!fg) groups += ",";
+        if (!fg) {
+          groups += ",";
+          ranges += ",";
+        }
         fg = false;
         groups += "[";
+        ranges += "[";
         bool ff = true;
-        for (auto& f : g.subs(1)) {  // PartitionedFile { path = 1 } (:1354)
+        for (auto& f : g.subs(1)) {  // PartitionedFile { path = 1, range = 5 } (:1354-1361)
           const std::string path = f.str(1);
           if (table.empty()) table = table_of_path(path);
           groups += std::string(ff ? "" : ",") + jstr(path);
+          ranges += ff ? "" : ",";
           ff = false;
+          if (f.has(5)) {  // FileRange { start = 1, end = 2 } (:1363-1366)
+            const Msg r = f.sub(5);
+            const int64_t a = r.i64(1), b = r.i64(2);
+            if (a < 0 || b < a) throw std::runtime_error("plan proto: file range with end before start");
+            ranges += "[" + std::to_string(a) + "," + std::to_string(b) + "]";
+            any_range = true;
+          } else {
+            ranges += "null";
+          }
         }
         groups += "]";
+        ranges += "]";
       }
       groups += "]";
-      if (table.empty()) throw std::runtime_error("plan proto: parquet scan without files");
+      ranges += "]";
+      if (table.empty()) throw std::runtime_error(csv ? "plan proto: csv scan without files" : "plan proto: parquet scan without files");
       std::string o = "{\"op\":\"DataSourceExec\",\"table\":" + jstr(table) + ",\"schema\":" + schema_json(conf.sub(2));
       std::vector<uint64_t> proj = conf.varints(4);
       if (proj.empty() && conf.has(13)) {
@@ -576,7 +600,20 @@ inline std::string plan_json(const Msg& n, const std::string& override_job) {
         }
       }
       if (!proj.empty()) o += ",\"projection\":" + u32_list_json(proj);
-      return o + ",\"file_groups\":" + groups + "}";
+      o += ",\"file_groups\":" + groups;
+      if (!csv) return o + "}";
+      // reader options as b200_engine_register_csv takes them: one ASCII byte each (escape may be absent)
+      auto opt = [&](uint32_t f, const char* name) {
+        const std::string v = m.str(f);
+        if (v.size() != 1 || (unsigned char)v[0] >= 0x80)
+          throw std::runtime_error(std::string("plan proto: CsvScanExecNode option '") + name + "' must be one ASCII byte");
+        return jstr(v);
+      };
+      o += ",\"format\":\"csv\",\"csv\":{\"has_header\":" + std::string(m.u64(2) ? "true" : "false") + ",\"delimiter\":" + opt(3, "delimiter") +
+           ",\"quote\":" + opt(4, "quote") + ",\"escape\":" + (m.has(5) ? opt(5, "escape") : std::string("null")) +
+           ",\"newlines_in_values\":" + (m.u64(7) ? "true" : "false") + "}";
+      if (any_range) o += ",\"file_ranges\":" + ranges;
+      return o + "}";
     }
     case 4: {  // ProjectionExecNode { input = 1, expr = 2, expr_name = 3 } (:1211-1215)
       const std::vector<Msg> es = m.subs(2);

@@ -410,6 +410,59 @@ void launch_pq_delta_prepare(const PqColumn& C, const PqPage* pages, int n_pages
 void launch_pq_values_delta(const PqColumn& C, const PqPage* pages, int n_pages, const unsigned long long* dense_base, const uint32_t* nonnull, void* out,
                             const PqDeltaAux& A, cudaStream_t st);
 
+// ---- CSV / TPC-H .tbl scan (csv.cu) -------------------------------------------------------------------
+static const int CSV_TILE = 1024;    // bytes per thread of the record-boundary passes
+static const int CSV_BLOCK = 256;    // tiles per block
+static const int CSV_STATES = 6;     // quote state machine: record start, field start, unquoted, quoted, quote seen, escape
+struct CsvDialect {
+  uint8_t delim, quote, escape, has_escape;
+};
+struct CsvTrans {   // what a run of bytes does to each entry state: exit state and record starts seen
+  uint8_t exit[CSV_STATES];
+  uint8_t _pad[2];
+  uint32_t cnt[CSV_STATES];
+};
+int64_t csv_tile_count(int64_t bytes);
+int64_t csv_block_count(int64_t bytes);
+// passes 1 + 2: per-tile transitions (tiles: csv_tile_count), per-block entry state and first record (csv_block_count),
+// *n_records, and *has_quote |= 1 when the span holds a quote or escape byte (both zeroed by the caller)
+void launch_csv_records_count(const uint8_t* data, int64_t bytes, const CsvDialect& d, CsvTrans* tiles, CsvTrans* blocks, uint8_t* blk_state,
+                              unsigned long long* blk_base, unsigned int* has_quote, unsigned long long* n_records, cudaStream_t st);
+// pass 3: rec_start[r] = offset of record r's first byte (empty lines are no records)
+void launch_csv_record_starts(const uint8_t* data, int64_t bytes, const CsvDialect& d, const CsvTrans* tiles, const uint8_t* blk_state,
+                              const unsigned long long* blk_base, uint64_t* rec_start, cudaStream_t st);
+// reasons in a CSV error word (bits 16-23; bits 0-15 detail, bits 24-63 the row)
+enum CsvError : int {
+  CSV_E_FIELDS = 1, CSV_E_NULL, CSV_E_INT, CSV_E_INT_RANGE, CSV_E_DEC, CSV_E_DEC_RANGE, CSV_E_DEC_SCALE, CSV_E_DEC_EXP, CSV_E_FLOAT, CSV_E_DATE,
+  CSV_E_BOOL, CSV_E_UTF8
+};
+struct CsvFieldArgs {
+  const uint8_t* data;
+  int64_t bytes;
+  const uint64_t* rec_start;
+  int64_t n_records, skip;        // records of the span; skip = 1 drops the header record
+  CsvDialect d;
+  int n_fields;                   // schema columns
+  const int32_t* slot_of_field;   // [n_fields] output slot of each schema column, -1 = not materialised
+  unsigned long long* views;      // [slots][n_total] {pointer, length}
+  int64_t n_total, row_base;      // rows of the scan; first row of this span
+  uint8_t* side;                  // unquoting buffer, offsets as in data (nullptr when the span holds no quote byte)
+  unsigned long long* err;        // field-count errors (CSV_E_FIELDS, detail = fields found)
+};
+void launch_csv_fields(const CsvFieldArgs& A, cudaStream_t st);
+enum CsvFamily : int { CSV_FAM_INT = 0, CSV_FAM_DEC, CSV_FAM_F64, CSV_FAM_F32, CSV_FAM_DATE, CSV_FAM_BOOL, CSV_FAM_UTF8 };
+struct CsvConvertArgs {
+  const unsigned long long* views;  // [n] fields
+  int64_t n;
+  void* out;                        // values (CSV_FAM_UTF8: views)
+  uint8_t* valid;
+  unsigned long long* err;          // first failing row of the column
+  unsigned long long* null_count;
+  __int128 lo, hi;                  // CSV_FAM_INT: the type's range
+  int width, is_signed, precision, scale, nullable;
+};
+void launch_csv_convert(const CsvConvertArgs& A, int family, cudaStream_t st);
+
 // ---- window functions (window.cu) ---------------------------------------------------------------
 // Kernels work on sorted positions i; perm[i] is the input row there (nullptr: the input already is in sorted order).
 static const int WIN_MAX_KEYS = 16;

@@ -4841,6 +4841,398 @@ DevBatchPtr scan_parquet(const Exec& x, const std::string& path, const std::vect
   return out;
 }
 
+// ------------------------------------------------------------------------------------------------
+// CSV scan: DataSourceExec + CsvSource (CsvScanExecNode, ballista/core/proto/datafusion.proto:1088-1101; TPC-H .tbl files,
+// benchmarks/src/bin/tpch.rs:653-683).  The host finds the byte span of each file (range rule below), streams it to HBM
+// through two bounded pinned chunks and csrc/device/csv.cu does everything else.  Rules: DESIGN.md §6 (ix).
+// ------------------------------------------------------------------------------------------------
+struct CsvFileSpec {
+  std::string path;
+  int64_t start = 0, end = -1;  // end < 0: the whole file
+};
+struct CsvScanSpec {
+  std::vector<CsvFileSpec> files;
+  Schema schema;
+  std::vector<std::string> columns;
+  bool all_columns = true;  // no "columns" key; an empty list materialises no column (the rows are still counted)
+  bool has_header = false, newlines_in_values = false;
+  CsvDialect d{',', '"', 0, 0};
+};
+
+static uint8_t csv_option_byte(const Json& j, const char* key, uint8_t dflt) {
+  const Json* v = j.find(key);
+  if (!v || v->is_null()) return dflt;
+  if (!v->is_str() || v->str().size() != 1)
+    throw EngineError(B200_ERR_INVALID, std::string("csv: option '") + key + "' must be exactly one byte");
+  return (uint8_t)v->str()[0];
+}
+
+static CsvScanSpec parse_csv_scan(const std::string& text) {
+  Json j;
+  try {
+    j = parse_json(text);
+  } catch (const std::exception& ex) {
+    throw EngineError(B200_ERR_INVALID, std::string("csv: malformed scan description: ") + ex.what());
+  }
+  if (!j.is_obj()) throw EngineError(B200_ERR_INVALID, "csv: the scan description must be a JSON object");
+  CsvScanSpec s;
+  try {
+    const Json* c = j.find("comment");
+    if (c && !c->is_null()) throw EngineError(B200_ERR_UNSUPPORTED, "csv: option 'comment' is not supported");
+    if (j.get_bool("truncate_rows", false)) throw EngineError(B200_ERR_UNSUPPORTED, "csv: option 'truncate_rows' is not supported");
+    s.has_header = j.get_bool("has_header", false);
+    s.newlines_in_values = j.get_bool("newlines_in_values", false);
+    s.d.delim = csv_option_byte(j, "delimiter", ',');
+    s.d.quote = csv_option_byte(j, "quote", '"');
+    const Json* esc = j.find("escape");
+    if (esc && !esc->is_null()) {
+      s.d.escape = csv_option_byte(j, "escape", 0);
+      s.d.has_escape = s.d.escape != s.d.quote;  // an escape equal to the quote is the doubled-quote rule
+    }
+    for (uint8_t b : {s.d.delim, s.d.quote})
+      if (b == '\n' || b == '\r') throw EngineError(B200_ERR_INVALID, "csv: delimiter and quote cannot be line terminators");
+    if (s.d.delim == s.d.quote || (s.d.has_escape && (s.d.escape == s.d.delim || s.d.escape == '\n' || s.d.escape == '\r')))
+      throw EngineError(B200_ERR_INVALID, "csv: delimiter, quote and escape must be distinct bytes");
+    s.schema = parse_schema(j.at("schema"));
+    if (s.schema.empty()) throw EngineError(B200_ERR_INVALID, "csv: empty schema");
+    const Json* cols = j.find("columns");
+    if (cols && !cols->is_null()) {
+      if (!cols->is_arr()) throw EngineError(B200_ERR_INVALID, "csv: 'columns' must be a list of names");
+      s.all_columns = false;
+      for (size_t i = 0; i < cols->size(); i++) s.columns.push_back(cols->at(i).str());
+    }
+    const Json& files = j.at("files");
+    if (!files.is_arr() || files.size() == 0) throw EngineError(B200_ERR_INVALID, "csv: 'files' must be a non-empty list");
+    for (size_t i = 0; i < files.size(); i++) {
+      const Json& f = files.at(i);
+      CsvFileSpec fs;
+      if (f.is_str()) {
+        fs.path = f.str();
+      } else {
+        fs.path = f.at("path").str();
+        const Json* r = f.find("range");
+        if (r && !r->is_null()) {
+          if (r->size() != 2) throw EngineError(B200_ERR_INVALID, "csv: a range is [start, end]");
+          fs.start = r->at(0).as_int();
+          fs.end = r->at(1).as_int();
+          if (fs.start < 0 || fs.end < fs.start) throw EngineError(B200_ERR_INVALID, "csv: bad byte range of " + fs.path);
+          if (s.newlines_in_values)
+            throw EngineError(B200_ERR_UNSUPPORTED, "csv: byte ranges together with 'newlines_in_values' are not supported");
+        }
+      }
+      s.files.push_back(fs);
+    }
+  } catch (const EngineError&) {
+    throw;
+  } catch (const std::exception& ex) {
+    throw EngineError(B200_ERR_INVALID, std::string("csv: ") + ex.what());
+  }
+  return s;
+}
+
+static int csv_family(const Field& f) {
+  const DataType& t = f.type;
+  if (t.is_integer()) return CSV_FAM_INT;
+  if (t.is_decimal()) {
+    if (t.precision < 1 || t.precision > 38 || t.scale < 0 || t.scale > t.precision)
+      throw EngineError(B200_ERR_UNSUPPORTED, "csv: column '" + f.name + "' has type " + t.str() + ", which the CSV scan does not read");
+    return CSV_FAM_DEC;
+  }
+  if (t.id == TypeId::Float64) return CSV_FAM_F64;
+  if (t.id == TypeId::Float32) return CSV_FAM_F32;
+  if (t.id == TypeId::Date32) return CSV_FAM_DATE;
+  if (t.id == TypeId::Bool) return CSV_FAM_BOOL;
+  if (t.id == TypeId::Utf8) return CSV_FAM_UTF8;
+  throw EngineError(B200_ERR_UNSUPPORTED, "csv: column '" + f.name + "' has type " + t.str() + ", which the CSV scan does not read");
+}
+
+static const char* csv_reason(int r) {
+  switch (r) {
+    case CSV_E_FIELDS: return "wrong number of fields";
+    case CSV_E_NULL: return "NULL in a non-nullable column";
+    case CSV_E_INT: return "not an integer";
+    case CSV_E_INT_RANGE: return "integer out of range";
+    case CSV_E_DEC: return "not a decimal";
+    case CSV_E_DEC_RANGE: return "decimal does not fit the precision";
+    case CSV_E_DEC_SCALE: return "decimal has more fractional digits than the scale";
+    case CSV_E_DEC_EXP: return "decimal with an exponent";
+    case CSV_E_FLOAT: return "not a floating-point number";
+    case CSV_E_DATE: return "not a valid YYYY-MM-DD date";
+    case CSV_E_BOOL: return "not a boolean";
+    case CSV_E_UTF8: return "invalid UTF-8";
+    default: return "malformed value";
+  }
+}
+
+// one file's byte span [s0, e0) on the device and where its records are
+struct CsvSpan {
+  std::string path;
+  int64_t s0 = 0, e0 = 0, skip = 0, n_records = 0, rows = 0, row_base = 0;
+  DevPtr data, tiles, blocks, blk_state, blk_base, counts, rec_start, side;
+  const unsigned long long* h_n = nullptr;
+  const unsigned int* h_quote = nullptr;
+};
+
+// first line terminator at or after `pos` (the file's size when there is none)
+static int64_t csv_find_term(FILE* f, int64_t pos, int64_t size) {
+  char buf[4096];
+  while (pos < size) {
+    if (fseeko(f, (off_t)pos, SEEK_SET) != 0) throw EngineError(B200_ERR_INVALID, "csv: seek failed");
+    const size_t n = fread(buf, 1, sizeof buf, f);
+    if (n == 0) break;
+    for (size_t i = 0; i < n; i++)
+      if (buf[i] == '\n' || buf[i] == '\r') return pos + (int64_t)i;
+    pos += (int64_t)n;
+  }
+  return size;
+}
+
+DevBatchPtr scan_csv(const Exec& x, const CsvScanSpec& spec) {
+  ScopeTimer tm("csv_scan");
+  cudaStream_t st = x.st();
+  const Schema& sch = spec.schema;
+  // materialised columns, in the requested order
+  std::vector<int> mat;
+  if (spec.all_columns) {
+    for (size_t i = 0; i < sch.size(); i++) mat.push_back((int)i);
+  } else {
+    for (auto& nm : spec.columns) {
+      int at = -1;
+      for (size_t i = 0; i < sch.size(); i++)
+        if (sch[i].name == nm) at = (int)i;
+      if (at < 0) throw EngineError(B200_ERR_INVALID, "csv: no column named " + nm);
+      // every schema column feeds at most one output slot (csv_fields_kernel writes one view per field)
+      if (std::find(mat.begin(), mat.end(), at) != mat.end()) throw EngineError(B200_ERR_INVALID, "csv: column " + nm + " is requested twice");
+      mat.push_back(at);
+    }
+  }
+  std::vector<int> fam;
+  for (int c : mat) fam.push_back(csv_family(sch[(size_t)c]));
+  std::vector<int32_t> slot_of_field(sch.size(), -1);
+  for (size_t k = 0; k < mat.size(); k++) slot_of_field[(size_t)mat[k]] = (int32_t)k;
+
+  // ---- bytes to HBM: two pinned chunks in flight, whatever the file size --------------------------------------------------
+  static const size_t kChunk = 16u << 20;
+  struct Staging {
+    uint8_t* buf[2] = {nullptr, nullptr};
+    cudaEvent_t ev[2] = {nullptr, nullptr};
+    ~Staging() {
+      for (int b = 0; b < 2; b++) {
+        if (ev[b]) {
+          cudaEventSynchronize(ev[b]);
+          cudaEventDestroy(ev[b]);
+        }
+        if (buf[b]) cudaFreeHost(buf[b]);
+      }
+    }
+  } stg;
+  for (int b = 0; b < 2; b++) {
+    if (cudaHostAlloc((void**)&stg.buf[b], kChunk, cudaHostAllocDefault) != cudaSuccess) throw EngineError(B200_ERR_OOM, "pinned staging for the CSV scan");
+    CUDA_CHECK(cudaEventCreateWithFlags(&stg.ev[b], cudaEventDisableTiming));
+  }
+  std::vector<CsvSpan> spans(spec.files.size());
+  int64_t chunk_no = 0;
+  for (size_t fi = 0; fi < spec.files.size(); fi++) {
+    const CsvFileSpec& fs = spec.files[fi];
+    CsvSpan& sp = spans[fi];
+    sp.path = fs.path;
+    FILE* f = fopen(fs.path.c_str(), "rb");
+    if (!f) throw EngineError(B200_ERR_NOT_FOUND, "csv: cannot open " + fs.path);
+    std::unique_ptr<FILE, int (*)(FILE*)> closer(f, fclose);
+    const int64_t size = fseeko(f, 0, SEEK_END) == 0 ? (int64_t)ftello(f) : -1;
+    if (size < 0) throw EngineError(B200_ERR_INVALID, "csv: cannot size " + fs.path);
+    const int64_t start = std::min<int64_t>(fs.start, size);
+    const int64_t end = fs.end < 0 ? size : std::min<int64_t>(fs.end, size);
+    // a range holds the records whose first byte lies in [start, end): from after the first terminator at or after
+    // start - 1, through the first terminator at or after end - 1
+    sp.s0 = start == 0 ? 0 : std::min(size, csv_find_term(f, start - 1, size) + 1);
+    sp.e0 = end == 0 ? 0 : end >= size ? size : std::min(size, csv_find_term(f, end - 1, size) + 1);
+    if (sp.e0 < sp.s0) sp.e0 = sp.s0;
+    sp.skip = (spec.has_header && start == 0) ? 1 : 0;
+    const int64_t bytes = sp.e0 - sp.s0;
+    sp.data = dev_alloc((size_t)bytes + 64, st);
+    for (int64_t off = 0; off < bytes; chunk_no++) {
+      const int b = (int)(chunk_no & 1);
+      const size_t n = (size_t)std::min<int64_t>((int64_t)kChunk, bytes - off);
+      CUDA_CHECK(cudaEventSynchronize(stg.ev[b]));  // the copy out of this chunk two steps ago is done
+      if (fseeko(f, (off_t)(sp.s0 + off), SEEK_SET) != 0 || fread(stg.buf[b], 1, n, f) != n) throw EngineError(B200_ERR_INVALID, "csv: short read on " + fs.path);
+      CUDA_CHECK(cudaMemcpyAsync((uint8_t*)sp.data->ptr + off, stg.buf[b], n, cudaMemcpyHostToDevice, st));
+      CUDA_CHECK(cudaEventRecord(stg.ev[b], st));
+      off += (int64_t)n;
+    }
+    if (bytes == 0) continue;
+    const int64_t nt = csv_tile_count(bytes), nb = csv_block_count(bytes);
+    sp.tiles = dev_alloc((size_t)nt * sizeof(CsvTrans), st);
+    sp.blocks = dev_alloc((size_t)nb * sizeof(CsvTrans), st);
+    sp.blk_state = dev_alloc((size_t)nb, st);
+    sp.blk_base = dev_alloc((size_t)nb * 8, st);
+    sp.counts = dev_alloc(16, st);
+    CUDA_CHECK(cudaMemsetAsync(sp.counts->ptr, 0, 16, st));
+    unsigned long long* n_rec = (unsigned long long*)sp.counts->ptr;
+    unsigned int* quote = (unsigned int*)(n_rec + 1);
+    {
+      KernelTimer kt(x, "csv_records", (uint64_t)bytes + (uint64_t)nt * sizeof(CsvTrans));
+      launch_csv_records_count((const uint8_t*)sp.data->ptr, bytes, spec.d, (CsvTrans*)sp.tiles->ptr, (CsvTrans*)sp.blocks->ptr, (uint8_t*)sp.blk_state->ptr,
+                               (unsigned long long*)sp.blk_base->ptr, quote, n_rec, st);
+    }
+    sp.h_n = x.fetch<unsigned long long>(n_rec);
+    sp.h_quote = x.fetch<unsigned int>(quote);
+  }
+  x.sync();  // one read-back for every file: record counts and whether any quote byte occurs
+  int64_t n_total = 0;
+  for (auto& sp : spans) {
+    sp.n_records = sp.h_n ? (int64_t)*sp.h_n : 0;
+    sp.rows = std::max<int64_t>(sp.n_records - sp.skip, 0);
+    sp.row_base = n_total;
+    n_total += sp.rows;
+  }
+  const size_t n_mat = mat.size();
+  DevPtr views = dev_alloc(std::max<size_t>(n_mat * (size_t)n_total, 1) * 16 + 64, st);
+  DevPtr d_slots = dev_alloc(slot_of_field.size() * 4, st);
+  CUDA_CHECK(cudaMemcpyAsync(d_slots->ptr, slot_of_field.data(), slot_of_field.size() * 4, cudaMemcpyHostToDevice, st));  // pageable: staged before returning
+  // error words: [0] field counts, [1 + k] column k; then the null count of every column
+  DevPtr words = dev_alloc((1 + 2 * n_mat) * 8, st);
+  CUDA_CHECK(cudaMemsetAsync(words->ptr, 0xFF, (1 + n_mat) * 8, st));
+  CUDA_CHECK(cudaMemsetAsync((unsigned long long*)words->ptr + 1 + n_mat, 0, n_mat * 8, st));
+  unsigned long long* w = (unsigned long long*)words->ptr;
+  for (auto& sp : spans) {
+    const int64_t bytes = sp.e0 - sp.s0;
+    if (!sp.n_records) continue;
+    sp.rec_start = dev_alloc((size_t)sp.n_records * 8, st);
+    {
+      KernelTimer kt(x, "csv_records", (uint64_t)bytes + (uint64_t)sp.n_records * 8);
+      launch_csv_record_starts((const uint8_t*)sp.data->ptr, bytes, spec.d, (const CsvTrans*)sp.tiles->ptr, (const uint8_t*)sp.blk_state->ptr,
+                               (const unsigned long long*)sp.blk_base->ptr, (uint64_t*)sp.rec_start->ptr, st);
+    }
+    sp.tiles.reset();
+    sp.blocks.reset();
+    if (*sp.h_quote) sp.side = dev_alloc((size_t)bytes + 64, st);
+    CsvFieldArgs A;
+    memset(&A, 0, sizeof A);
+    A.data = (const uint8_t*)sp.data->ptr;
+    A.bytes = bytes;
+    A.rec_start = (const uint64_t*)sp.rec_start->ptr;
+    A.n_records = sp.n_records;
+    A.skip = sp.skip;
+    A.d = spec.d;
+    A.n_fields = (int)sch.size();
+    A.slot_of_field = (const int32_t*)d_slots->ptr;
+    A.views = (unsigned long long*)views->ptr;
+    A.n_total = n_total;
+    A.row_base = sp.row_base;
+    A.side = sp.side ? (uint8_t*)sp.side->ptr : nullptr;
+    A.err = w;
+    KernelTimer kt(x, "csv_fields", (uint64_t)bytes + (uint64_t)sp.n_records * 8 + (uint64_t)sp.rows * n_mat * 16);
+    launch_csv_fields(A, st);
+  }
+  std::vector<DevPtr> outs(n_mat), valids(n_mat);
+  for (size_t k = 0; k < n_mat; k++) {
+    const Field& f = sch[(size_t)mat[k]];
+    CsvConvertArgs C;
+    memset(&C, 0, sizeof C);
+    C.views = (const unsigned long long*)views->ptr + 2 * k * (size_t)n_total;
+    C.n = n_total;
+    C.width = fam[k] == CSV_FAM_UTF8 ? 16 : f.type.is_decimal() ? 16 : f.type.id == TypeId::Bool ? 1 : f.type.width();
+    // Utf8 views are validated in place
+    outs[k] = fam[k] == CSV_FAM_UTF8 ? views : dev_alloc((size_t)std::max<int64_t>(n_total, 1) * (size_t)C.width + 64, st);
+    C.out = fam[k] == CSV_FAM_UTF8 ? (void*)C.views : outs[k]->ptr;
+    valids[k] = dev_alloc((size_t)std::max<int64_t>(n_total, 1) + 64, st);
+    C.valid = (uint8_t*)valids[k]->ptr;
+    C.err = w + 1 + k;
+    C.null_count = w + 1 + n_mat + k;
+    C.is_signed = f.type.is_signed_int();
+    if (fam[k] == CSV_FAM_INT) {
+      const int bits = 8 * f.type.width();
+      C.lo = C.is_signed ? -((__int128)1 << (bits - 1)) : 0;
+      C.hi = C.is_signed ? ((__int128)1 << (bits - 1)) - 1 : ((__int128)1 << bits) - 1;
+    }
+    C.precision = f.type.precision;
+    C.scale = f.type.scale;
+    C.nullable = f.nullable ? 1 : 0;
+    KernelTimer kt(x, "csv_convert", (uint64_t)n_total * (16 + (uint64_t)C.width + 1));
+    launch_csv_convert(C, fam[k], st);
+  }
+  const unsigned long long* hw = (const unsigned long long*)x.fetch_bytes(w, (1 + 2 * n_mat) * 8);
+  x.sync();
+  // the first failing record of the scan, a field-count error first among equals
+  int which = -1;
+  unsigned long long best = ~0ull;
+  for (size_t k = 0; k <= n_mat; k++)
+    if (hw[k] != ~0ull && (hw[k] >> 24) < (best >> 24)) {
+      best = hw[k];
+      which = (int)k - 1;
+    }
+  if (best != ~0ull) {
+    const int64_t row = (int64_t)(best >> 24);
+    const int reason = (int)((best >> 16) & 0xFF), detail = (int)(best & 0xFFFF);
+    size_t fi = 0;
+    while (fi + 1 < spans.size() && !(row >= spans[fi].row_base && row < spans[fi].row_base + spans[fi].rows)) fi++;
+    const CsvSpan& sp = spans[fi];
+    const int64_t rec = row - sp.row_base + sp.skip;
+    const uint64_t rel = x.get<uint64_t>((const uint64_t*)sp.rec_start->ptr + rec);
+    std::string value;
+    if (which >= 0) {
+      const unsigned long long* v = (const unsigned long long*)views->ptr + 2 * ((size_t)which * (size_t)n_total + (size_t)row);
+      const unsigned long long* hv = (const unsigned long long*)x.fetch_bytes(v, 16);
+      x.sync();
+      const uint64_t len = std::min<uint64_t>(hv[1], 64);
+      if (len) {
+        const char* hb = (const char*)x.fetch_bytes((const void*)hv[0], (size_t)len);
+        x.sync();
+        value.assign(hb, (size_t)len);
+      }
+      if (hv[1] > 64) value += "...";
+    } else {
+      const uint64_t len = std::min<uint64_t>(64, (uint64_t)(sp.e0 - sp.s0) - rel);
+      const char* hb = (const char*)x.fetch_bytes((const uint8_t*)sp.data->ptr + rel, (size_t)len);
+      x.sync();
+      value.assign(hb, (size_t)len);
+      const size_t nl = value.find_first_of("\r\n");
+      if (nl != std::string::npos) value.resize(nl);
+      else if (len == 64) value += "...";
+    }
+    std::string what = csv_reason(reason);
+    if (reason == CSV_E_FIELDS) what = "record has " + std::to_string(detail) + " fields, the schema " + std::to_string(sch.size());
+    const std::string col = which >= 0 ? "column '" + sch[(size_t)mat[(size_t)which]].name + "', " : "";
+    throw EngineError(B200_ERR_INVALID, "csv: " + sp.path + ": " + col + "record " + std::to_string(row - sp.row_base + 1) + " (byte offset " +
+                                            std::to_string((uint64_t)sp.s0 + rel) + "): " + what + ": '" + value + "'");
+  }
+  auto out = std::make_shared<DevBatch>();
+  out->n = n_total;
+  for (size_t k = 0; k < n_mat; k++) {
+    const Field& f = sch[(size_t)mat[k]];
+    const bool has_nulls = hw[1 + n_mat + k] != 0;
+    DevColumn col;
+    col.name = f.name;
+    col.type = f.type;
+    col.n = n_total;
+    col.nullable = has_nulls;
+    if (has_nulls) {
+      col.valid = (const uint8_t*)valids[k]->ptr;
+      col.keep.push_back(valids[k]);
+    }
+    if (fam[k] == CSV_FAM_UTF8) {
+      col.phys = PH_STRVIEW;
+      col.data = (const uint8_t*)views->ptr + 16 * k * (size_t)n_total;
+      col.keep.push_back(views);
+      for (auto& sp : spans) {
+        col.keep.push_back(sp.data);
+        if (sp.side) col.keep.push_back(sp.side);
+      }
+      KernelTimer kt(x, "csv_strings", (uint64_t)n_total * 16 * 2);
+      col = as_utf8(x, col);
+    } else {
+      col.phys = phys_of(f.type);
+      col.data = (const uint8_t*)outs[k]->ptr;
+      col.keep.push_back(outs[k]);
+    }
+    out->cols.push_back(col);
+  }
+  build_column_images(x, *out);
+  x.sync();
+  return out;
+}
+
 void collect_nodes(const PlanNode& n, b200_stage* s) {
   s->metric_index[&n] = (int)s->metrics.size();
   OpMetrics m;
@@ -5338,6 +5730,25 @@ int b200_engine_register_parquet(b200_engine* e, const char* table, int partitio
     DevBatchPtr b;
     try {
       b = scan_parquet(x, path, cols);
+    } catch (...) {
+      cudaStreamSynchronize(e->stream);
+      Exec::abandon();
+      throw;
+    }
+    std::lock_guard<std::mutex> g(e->mu);
+    e->tables[table][partition] = b;
+  });
+}
+
+int b200_engine_register_csv(b200_engine* e, const char* table, int partition, const char* scan_json) {
+  return guard(e, [&] {
+    if (!e || !table || !scan_json) throw EngineError(B200_ERR_INVALID, "null argument");
+    const CsvScanSpec spec = parse_csv_scan(scan_json);
+    CUDA_CHECK(cudaSetDevice(e->device));
+    Exec x{e, nullptr, nullptr};
+    DevBatchPtr b;
+    try {
+      b = scan_csv(x, spec);
     } catch (...) {
       cudaStreamSynchronize(e->stream);
       Exec::abandon();

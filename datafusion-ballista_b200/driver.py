@@ -42,6 +42,27 @@ def _probe_side_leaf(node: dict):
     return _probe_side_leaf(node["input"])
 
 
+def register_csv_scan(engine, node: dict, partition: int, path_map: Optional[Dict[str, str]] = None) -> None:
+    """What an executor-side shim does with a CSV leaf: register file group `partition` of a decoded CSV DataSourceExec
+    node (plan IR as the protobuf decoder emits it: "file_groups", "file_ranges", "csv" options) through
+    engine.register_csv.  The node's projection indexes the file schema, so the table is registered with the schema's
+    columns up to the last projected one, in file order, and the projection applies to it unchanged.  path_map renames
+    files (the plan's paths as seen by this host)."""
+    schema = node["schema"]
+    proj = node.get("projection", list(range(len(schema))))
+    cols = [f["name"] for f in schema[:max(proj) + 1]] if proj else []
+    ranges = node.get("file_ranges")
+    files = []
+    for i, path in enumerate(node["file_groups"][partition]):
+        path = (path_map or {}).get(path, path)
+        r = ranges[partition][i] if ranges else None
+        files.append((path, r[0], r[1]) if r else path)
+    o = node["csv"]
+    engine.register_csv(node["table"], partition, files, schema, columns=cols, has_header=o["has_header"],
+                        delimiter=o["delimiter"], quote=o["quote"], escape=o["escape"],
+                        newlines_in_values=o["newlines_in_values"])
+
+
 def run_stages(engine, stages: List[Stage], job_id: str = "job", collect: bool = True,
                metrics_out: Optional[list] = None) -> Optional[pa.Table]:
     """Execute `stages` in order on `engine`; return the last stage's output as one Table."""

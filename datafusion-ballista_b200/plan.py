@@ -128,6 +128,22 @@ def scan(table: str, schema: List[Json], projection: Optional[List[int]] = None)
     return n
 
 
+def csv_scan(table: str, schema: List[Json], projection: Optional[List[int]] = None, file_groups: Optional[List[List[str]]] = None,
+             file_ranges: Optional[List[list]] = None, has_header: bool = False, delimiter: str = ",", quote: str = '"',
+             escape: Optional[str] = None, newlines_in_values: bool = False) -> Json:
+    """DataSourceExec over CSV files (CsvScanExecNode): `schema` is the files' columns, `projection` indexes it, and the
+    reader options ride along as the protobuf decoder emits them ("format", "csv", "file_ranges")."""
+    n = scan(table, schema, projection)
+    if file_groups is not None:
+        n["file_groups"] = file_groups
+    n["format"] = "csv"
+    n["csv"] = {"has_header": has_header, "delimiter": delimiter, "quote": quote, "escape": escape,
+                "newlines_in_values": newlines_in_values}
+    if file_ranges is not None:
+        n["file_ranges"] = file_ranges
+    return n
+
+
 def shuffle_reader(stage_id: int, schema: List[Json], broadcast: bool = False) -> Json:
     return {"op": "ShuffleReaderExec", "stage_id": stage_id, "schema": schema, "broadcast": broadcast}
 

@@ -42,6 +42,21 @@ SCHEMAS: Dict[str, List[dict]] = {
 }
 
 
+def tbl_schema(table: str) -> List[dict]:
+    """The schema a dbgen .tbl file is read with (tpch.rs:1056-1060 `get_tbl_tpch_table_schema`): the table's columns and
+    a non-nullable Utf8 `__placeholder` that absorbs the empty field after each line's trailing '|'."""
+    return SCHEMAS[table] + [P.field("__placeholder", "utf8")]
+
+
+def tbl_scan(table: str, columns: List[str], path: str = None) -> dict:
+    """The CSV variant of table_scan: DataSourceExec over the table's dbgen .tbl file ('|', no header), schema tbl_schema,
+    projection into it -- what tpch.rs plans for `--format tbl`."""
+    full = tbl_schema(table)
+    names = [f["name"] for f in full]
+    return P.csv_scan(table, full, projection=[names.index(c) for c in columns],
+                      file_groups=[[path or f"/data/tpch/{table}.tbl"]], delimiter="|")
+
+
 def col_index(table: str, name: str) -> int:
     for i, f in enumerate(SCHEMAS[table]):
         if f["name"] == name:

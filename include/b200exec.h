@@ -110,6 +110,17 @@ int b200_engine_register_parquet(b200_engine* e, const char* table, int partitio
 /* Host-only: JSON description (schema, rows, page inventory per column) of a Parquet file as the scan's metadata reader
  * sees it.  No CUDA call. */
 int b200_parquet_describe(const char* path, char* out, uint64_t cap);
+/* DataSourceExec + CsvSource leaf (CsvScanExecNode, datafusion.proto:1088-1101; tpch.rs:653-683 registers TPC-H tables from
+ * dbgen's '|'-delimited .tbl files this way): the file bytes cross the bus as they are and record boundaries, fields and
+ * values are found and converted on the device.  scan_json:
+ *   {"files": [{"path": "...", "range": [start, end]}, ...],   range optional: the records whose first byte lies in it
+ *    "schema": [fields as in the plan IR], "columns": [names] (absent: all),
+ *    "has_header", "delimiter", "quote", "escape" (one-byte strings; escape may be null), "newlines_in_values"}
+ * The table partition gets exactly the requested columns in the requested order.  Malformed JSON, options or data return
+ * B200_ERR_INVALID (data errors name the file, column, record and byte offset); a missing file B200_ERR_NOT_FOUND; the
+ * options 'comment' and 'truncate_rows', Timestamp columns and ranges with newlines_in_values B200_ERR_UNSUPPORTED.  Nothing
+ * is registered after an error.  Replaces the table partition. */
+int b200_engine_register_csv(b200_engine* e, const char* table, int partition, const char* scan_json);
 int b200_engine_drop_table(b200_engine* e, const char* table);
 /* Synthetic TPC-H-shaped table generated directly in HBM (bench/test input; columns = NULL: all).
  * Rows [row_begin,row_end) of the table at milli-scale-factor `msf` become partition `partition`. */
