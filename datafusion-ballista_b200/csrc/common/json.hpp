@@ -173,6 +173,19 @@ class JsonParser {
             if (e_ - p_ < 5) fail("bad \\u escape");
             unsigned cp = (unsigned)strtoul(std::string(p_ + 1, 4).c_str(), nullptr, 16);
             p_ += 4;
+            // a surrogate pair (what JSON writers emit for a code point above U+FFFF) is one 4-byte UTF-8 sequence
+            if (cp >= 0xD800 && cp <= 0xDBFF && e_ - p_ >= 7 && p_[1] == '\\' && p_[2] == 'u') {
+              const unsigned lo = (unsigned)strtoul(std::string(p_ + 3, 4).c_str(), nullptr, 16);
+              if (lo >= 0xDC00 && lo <= 0xDFFF) {
+                cp = 0x10000 + ((cp - 0xD800) << 10) + (lo - 0xDC00);
+                p_ += 6;
+                out += (char)(0xF0 | (cp >> 18));
+                out += (char)(0x80 | ((cp >> 12) & 0x3F));
+                out += (char)(0x80 | ((cp >> 6) & 0x3F));
+                out += (char)(0x80 | (cp & 0x3F));
+                break;
+              }
+            }
             if (cp < 0x80) out += (char)cp;
             else if (cp < 0x800) {
               out += (char)(0xC0 | (cp >> 6));

@@ -21,6 +21,7 @@
 #include <vector>
 
 #include "json.hpp"
+#include "regex_dfa.hpp"
 
 namespace b200 {
 
@@ -207,7 +208,10 @@ inline DataType int_as_decimal(const DataType& t) {
   }
 }
 
-enum class BinOp : uint8_t { Add, Sub, Mul, Div, Mod, Eq, Ne, Lt, Le, Gt, Ge, And, Or, BitAnd, BitOr, BitXor, Shl, Shr };
+enum class BinOp : uint8_t {
+  Add, Sub, Mul, Div, Mod, Eq, Ne, Lt, Le, Gt, Ge, And, Or, BitAnd, BitOr, BitXor, Shl, Shr,
+  RegexMatch, RegexIMatch, RegexNotMatch, RegexNotIMatch  // ~  ~*  !~  !~*
+};
 
 inline BinOp parse_binop(const std::string& s) {
   static const std::pair<const char*, BinOp> tab[] = {
@@ -216,7 +220,8 @@ inline BinOp parse_binop(const std::string& s) {
       {"<>", BinOp::Ne},  {"<", BinOp::Lt},   {"<=", BinOp::Le},  {">", BinOp::Gt},
       {">=", BinOp::Ge},  {"and", BinOp::And}, {"or", BinOp::Or},  {"AND", BinOp::And},
       {"OR", BinOp::Or},  {"&", BinOp::BitAnd}, {"|", BinOp::BitOr}, {"^", BinOp::BitXor},
-      {"<<", BinOp::Shl}, {">>", BinOp::Shr}};
+      {"<<", BinOp::Shl}, {">>", BinOp::Shr}, {"~", BinOp::RegexMatch}, {"~*", BinOp::RegexIMatch},
+      {"!~", BinOp::RegexNotMatch}, {"!~*", BinOp::RegexNotIMatch}};
   for (auto& kv : tab)
     if (s == kv.first) return kv.second;
   throw std::runtime_error("plan IR: unknown binary operator '" + s + "'");
@@ -224,7 +229,8 @@ inline BinOp parse_binop(const std::string& s) {
 inline bool is_arith(BinOp o) { return o <= BinOp::Mod; }
 inline bool is_compare(BinOp o) { return o >= BinOp::Eq && o <= BinOp::Ge; }
 inline bool is_logic(BinOp o) { return o == BinOp::And || o == BinOp::Or; }
-inline bool is_bitwise(BinOp o) { return o >= BinOp::BitAnd; }
+inline bool is_bitwise(BinOp o) { return o >= BinOp::BitAnd && o <= BinOp::Shr; }
+inline bool is_regex(BinOp o) { return o >= BinOp::RegexMatch; }
 
 // Grouping sets (ROLLUP / CUBE / GROUPING SETS) and the bitwise operators DataFusion rewrites GROUPING() into are typed
 // here for every consumer of the plan IR, but only a consumer built with B200_PLAN_GROUPING_SETS=1 computes them (the
@@ -307,6 +313,11 @@ struct Expr {
   bool has_else = false;  // Case
   bool negated = false;   // InList / Like
   std::string pattern;    // Like
+  bool case_insensitive = false;  // Like: ILIKE
+  // ILIKE, the regex operators and regexp_like: the pattern compiled at typing (null when the pattern or the flags are a
+  // NULL literal: the result is NULL), and the key the engine caches its device copy under
+  std::shared_ptr<const rx::Dfa> regex;
+  std::string regex_key;
   std::string name;       // display only
 };
 
@@ -386,6 +397,52 @@ inline int date_part_index(const std::string& fn) {
   return -1;
 }
 
+// ILIKE, `~` / `~*` / `!~` / `!~*` and regexp_like are typed here for every consumer of the plan IR, but only a consumer
+// built with B200_PLAN_REGEX=1 computes them (the device engine: Makefile NVFLAGS).  Semantics: DESIGN.md §6 (x),
+// csrc/common/regex_dfa.hpp.  The pattern (and regexp_like's flags) must be Utf8 literals; it is compiled here, so that an
+// invalid or unsupported pattern fails when the stage is prepared.
+#ifndef B200_PLAN_REGEX
+#define B200_PLAN_REGEX 0
+#endif
+inline void type_regex(Expr& e, const std::string& what, const ExprPtr& pattern, const ExprPtr& flags, bool ci) {
+  if (!B200_PLAN_REGEX) throw PlanUnsupported(what + " is not computed by this consumer of the plan IR");
+  const DataType& t = e.args[0]->type;
+  if (!t.is_string() && t.id != TypeId::Null) throw PlanUnsupported(what + " does not support an operand of type " + t.str());
+  e.type = DataType(TypeId::Bool);
+  e.nullable = true;
+  bool null_arg = false;
+  auto literal = [&](const ExprPtr& a, const char* role) -> const std::string& {
+    if (a->kind != Expr::Lit) throw PlanUnsupported(what + ": the " + role + " must be a literal");
+    if (!a->type.is_string() && a->type.id != TypeId::Null) throw PlanUnsupported(what + ": the " + role + " must be utf8, not " + a->type.str());
+    null_arg = null_arg || a->lit.is_null;
+    return a->lit.s;
+  };
+  auto fail = [&](int rc, const std::string& msg) {
+    if (rc == rx::RX_UNSUPPORTED) throw PlanUnsupported(msg);
+    throw std::runtime_error(msg);
+  };
+  auto d = std::make_shared<rx::Dfa>();
+  std::string err;
+  int rc;
+  if (!pattern) {  // ILIKE: arrow's LIKE-to-regex translation under the flags i and s
+    rc = rx::compile_ilike(e.pattern, *d, err);
+    e.regex_key = "like:" + e.pattern;
+  } else {
+    const std::string& p = literal(pattern, "pattern");
+    bool fi = false, fs = false;
+    if (flags) {
+      const std::string& f = literal(flags, "flags argument");
+      if (!null_arg && (rc = rx::parse_regex_flags(f, fi, fs, err)) != rx::RX_OK) fail(rc, err);
+    }
+    if (null_arg) return;
+    fi = fi || ci;
+    rc = rx::compile_regex(p, fi, fs, *d, err);
+    e.regex_key = std::string(fi ? "i" : "") + (fs ? "s" : "") + ":" + p;
+  }
+  if (rc != rx::RX_OK) fail(rc, err);
+  e.regex = d;
+}
+
 // Result type and nullability of a scalar function call (DESIGN.md §3, rules [EXT] in §6).  A known function over an
 // argument type it does not take is refused with PlanUnsupported naming the type; an unknown name or a wrong argument
 // count is a malformed plan.
@@ -462,6 +519,9 @@ inline void type_scalar_fn(Expr& e) {
     need_utf8(1);
     e.type = DataType(TypeId::Bool);
     e.nullable = any_nullable();
+  } else if (f == "regexp_like") {
+    arity(2, 3);
+    type_regex(e, "regexp_like", e.args[1], n == 3 ? e.args[2] : nullptr, false);
   } else if (f == "btrim" || f == "ltrim" || f == "rtrim") {
     arity(1, 2);
     need_utf8(0);
@@ -501,6 +561,13 @@ inline ExprPtr parse_expr(const Json& j, const Schema& in) {
     e->args.push_back(parse_expr(j.at("r"), in));
     const DataType& a = e->args[0]->type;
     const DataType& b = e->args[1]->type;
+    if (is_regex(e->op)) {
+      static const char* const names[] = {"~", "~*", "!~", "!~*"};
+      const int k = (int)e->op - (int)BinOp::RegexMatch;
+      e->negated = e->op == BinOp::RegexNotMatch || e->op == BinOp::RegexNotIMatch;
+      type_regex(*e, std::string("the operator ") + names[k], e->args[1], nullptr, e->op == BinOp::RegexIMatch || e->op == BinOp::RegexNotIMatch);
+      return e;
+    }
     if (is_bitwise(e->op)) {
       // [EXT] arrow-rs bitwise kernels: integer operands of one type, the result has that type (DESIGN.md §6)
       if (!B200_PLAN_GROUPING_SETS) throw PlanUnsupported("bitwise operators are not computed by this consumer of the plan IR");
@@ -583,9 +650,11 @@ inline ExprPtr parse_expr(const Json& j, const Schema& in) {
     e->args.push_back(parse_expr(j.at("like"), in));
     e->pattern = j.at("pattern").str();
     e->negated = j.get_bool("negated", false);
+    e->case_insensitive = j.get_bool("case_insensitive", false);
     e->type = DataType(TypeId::Bool);
     e->nullable = e->args[0]->nullable;
     if (!e->args[0]->type.is_string()) throw std::runtime_error("LIKE needs a utf8 operand");
+    if (e->case_insensitive) type_regex(*e, "ILIKE", nullptr, nullptr, true);
     return e;
   }
   if (j.find("fn")) {
@@ -807,7 +876,7 @@ inline ExprPtr window_default_as(const ExprPtr& d, const DataType& to) {
 // structural equality of two typed expressions (window PARTITION BY / ORDER BY against the node's and the sort's keys)
 inline bool expr_equal(const ExprPtr& a, const ExprPtr& b) {
   if (!a || !b) return a == b;
-  if (a->kind != b->kind || a->type != b->type || a->col != b->col || a->op != b->op || a->fn != b->fn || a->negated != b->negated ||
+  if (a->kind != b->kind || a->type != b->type || a->col != b->col || a->op != b->op || a->fn != b->fn || a->negated != b->negated || a->case_insensitive != b->case_insensitive ||
       a->has_else != b->has_else || a->pattern != b->pattern || a->args.size() != b->args.size())
     return false;
   if (a->kind == Expr::Lit && (a->lit.is_null != b->lit.is_null || a->lit.i != b->lit.i || a->lit.d != b->lit.d || a->lit.s != b->lit.s ||

@@ -19,7 +19,7 @@ inline std::string dump_schema(const Schema& s) {
 }
 
 inline std::string dump_expr(const ExprPtr& e) {
-  static const char* ops[] = {"+", "-", "*", "/", "%", "=", "!=", "<", "<=", ">", ">=", "and", "or", "&", "|", "^", "<<", ">>"};
+  static const char* ops[] = {"+", "-", "*", "/", "%", "=", "!=", "<", "<=", ">", ">=", "and", "or", "&", "|", "^", "<<", ">>", "~", "~*", "!~", "!~*"};
   auto list = [&](size_t from) {
     std::string o = "[";
     for (size_t i = from; i < e->args.size(); i++) o += (i > from ? "," : "") + dump_expr(e->args[i]);
@@ -61,7 +61,8 @@ inline std::string dump_expr(const ExprPtr& e) {
       return o + "}" + ty + "}";
     }
     case Expr::InList: return "{\"in\":" + dump_expr(e->args[0]) + ",\"list\":" + list(1) + ",\"negated\":" + (e->negated ? "true" : "false") + "}";
-    case Expr::Like: return "{\"like\":" + dump_expr(e->args[0]) + ",\"pattern\":" + pbp::jstr(e->pattern) + ",\"negated\":" + (e->negated ? "true" : "false") + "}";
+    case Expr::Like: return "{\"like\":" + dump_expr(e->args[0]) + ",\"pattern\":" + pbp::jstr(e->pattern) + ",\"negated\":" + (e->negated ? "true" : "false") +
+                                  (e->case_insensitive ? ",\"case_insensitive\":true" : "") + "}";
     case Expr::Fn: return "{\"fn\":" + pbp::jstr(e->fn) + ",\"args\":" + list(0) + ty + "}";
   }
   return "null";

@@ -328,7 +328,8 @@ inline std::string binop_symbol(const std::string& op) {
   static const std::pair<const char*, const char*> tab[] = {
       {"Eq", "="},     {"NotEq", "!="},   {"Lt", "<"},       {"LtEq", "<="},  {"Gt", ">"},   {"GtEq", ">="}, {"Plus", "+"},
       {"Minus", "-"},  {"Multiply", "*"}, {"Divide", "/"},   {"Modulo", "%"}, {"And", "and"}, {"Or", "or"},
-      {"BitwiseAnd", "&"}, {"BitwiseOr", "|"}, {"BitwiseXor", "^"}, {"BitwiseShiftLeft", "<<"}, {"BitwiseShiftRight", ">>"}};
+      {"BitwiseAnd", "&"}, {"BitwiseOr", "|"}, {"BitwiseXor", "^"}, {"BitwiseShiftLeft", "<<"}, {"BitwiseShiftRight", ">>"},
+      {"RegexMatch", "~"}, {"RegexIMatch", "~*"}, {"RegexNotMatch", "!~"}, {"RegexNotIMatch", "!~*"}};
   for (auto& kv : tab)
     if (op == kv.first) return kv.second;
   throw Unsupported("binary operator " + op + " is not supported by the device engine");
@@ -410,16 +411,16 @@ inline std::string expr_json(const Msg& e) {
           {"length", "character_length"},                   {"octet_length", "octet_length"},
           {"starts_with", "starts_with"},                   {"ends_with", "ends_with"},
           {"btrim", "btrim"},     {"trim", "btrim"},        {"ltrim", "ltrim"},
-          {"rtrim", "rtrim"}};
+          {"rtrim", "rtrim"},     {"regexp_like", "regexp_like"}};
       for (auto& kv : fns)
         if (name == kv.first) return "{\"fn\":\"" + std::string(kv.second) + "\",\"args\":" + exprs_json(args) + "}";
       throw Unsupported("scalar function " + name + " is not supported by the device engine");
     }
     case 18: {  // PhysicalLikeExprNode { negated = 1, case_insensitive = 2, expr = 3, pattern = 4 } (:969-974)
-      if (m.boolean(2)) throw Unsupported("ILIKE is not supported by the device engine");
       std::string pat;
-      if (!literal_utf8(m.sub(4), pat)) throw Unsupported("LIKE with a non-literal pattern");
-      return "{\"like\":" + expr_json(m.sub(3)) + ",\"pattern\":" + jstr(pat) + ",\"negated\":" + (m.boolean(1) ? "true" : "false") + "}";
+      if (!literal_utf8(m.sub(4), pat)) throw Unsupported(std::string(m.boolean(2) ? "ILIKE" : "LIKE") + " with a non-literal pattern");
+      return "{\"like\":" + expr_json(m.sub(3)) + ",\"pattern\":" + jstr(pat) + ",\"negated\":" + (m.boolean(1) ? "true" : "false") +
+             (m.boolean(2) ? ",\"case_insensitive\":true" : "") + "}";
     }
     default: throw Unsupported("physical expression variant " + std::to_string(x->field) + " is not supported by the device engine");
   }

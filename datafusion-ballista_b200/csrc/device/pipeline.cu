@@ -24,6 +24,7 @@
 #include <stdint.h>
 
 #include "../common/hash.hpp"
+#include "../common/regex_dfa.hpp"
 #include "kernels.h"
 #include "program.h"
 
@@ -668,6 +669,28 @@ __device__ __noinline__ void scalar_bit_op(const Lane L, const uint32_t active, 
   store_valid(L, ins.dst, va & vb);
 }
 
+// ILIKE, the regex operators and regexp_like: one thread walks one row's bytes through the DFA (regex_dfa.hpp, the same
+// walk the host compiler's tests run), stopping at the matched or the dead state.  NULL in, NULL out.
+__device__ __noinline__ void scalar_regex_op(const Lane L, const uint32_t active, const int pc) {
+  const VInstr ins = PROG.code[pc];
+  const uint32_t va = fetch_valid(L, ins.a);
+  const uint32_t live = active & va;
+  const uint8_t* dfa = (const uint8_t*)PROG.imms[ins.imm].lo;
+  const uint64_t shape = PROG.imms[ins.imm].hi;
+  uint32_t bmask = 0;
+#pragma unroll 1
+  for (int r = 0; r < VM_R; r++) {
+    bool hit = false;
+    if ((live >> r) & 1) {
+      const StrRef a = ld1_str(L, ins.a, r);
+      hit = rx::dfa_is_match(dfa, shape, a.p, a.len);
+    }
+    bmask |= ((ins.aux ? !hit : hit) ? 1u : 0u) << r;
+  }
+  store_bool(L, ins.dst, bmask);
+  store_valid(L, ins.dst, va);
+}
+
 // ------------------------------------------------------------------------------------------------
 // Cold operations: one rolled loop over the thread's rows; every body exists once in the binary.
 // ------------------------------------------------------------------------------------------------
@@ -677,6 +700,7 @@ __device__ __noinline__ void cold_op(const Lane L, const uint32_t active, const 
     const uint8_t op = PROG.code[pc].op;
     if (op <= OP_CEIL) scalar_num_op(L, active, pc);
     else if (op == OP_NULLIF) scalar_nullif_op(L, active, pc);
+    else if (op == OP_REGEX) scalar_regex_op(L, active, pc);
     else if (op >= OP_BIT_AND) scalar_bit_op(L, active, pc);
     else scalar_str_op(L, active, pc);
     return;

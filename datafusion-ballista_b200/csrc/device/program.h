@@ -82,7 +82,10 @@ enum VOp : uint8_t {
   OP_TRIM,                             // a: STR -> STR view; aux = TrimSide; imm = immediate idx of the set (" " by default)
   // bitwise operators (scalar_bit_op): t = VK_I64, a and b of one integer type; aux = Phys of that type (shift counts are
   // taken modulo its bit width; >> is arithmetic for signed types, logical for unsigned ones)
-  OP_BIT_AND, OP_BIT_OR, OP_BIT_XOR, OP_SHL, OP_SHR
+  OP_BIT_AND, OP_BIT_OR, OP_BIT_XOR, OP_SHL, OP_SHR,
+  // regular expressions (scalar_regex_op): ILIKE, ~ / ~* / !~ / !~* and regexp_like.  a: STR -> BOOL; aux: 1 = negated;
+  // imm: immediate with the DFA's device pointer in lo and its shape (csrc/common/regex_dfa.hpp dfa_shape_pack) in hi
+  OP_REGEX
 };
 
 enum DatePart : uint8_t { DP_YEAR = 0, DP_QUARTER, DP_MONTH, DP_WEEK, DP_DAY, DP_DOY, DP_DOW };

@@ -123,6 +123,7 @@ struct b200_engine {
   // parsed stage plans by plan text with the job id taken out (b200_stage_prepare): the next job that runs the same stage
   // plan shares the parsed tree instead of parsing and typing the JSON again.  Plans are read-only once parsed.
   std::map<std::string, std::shared_ptr<const PlanNode>> plan_cache;
+  RegexCache regex;                          // device copies of compiled regex DFAs, by pattern and flags
 };
 
 struct b200_stage {
@@ -2496,7 +2497,7 @@ struct Runner {
     for (auto* n : chain)
       if (OpMetrics* m = x.m(n)) m->input_rows += (uint64_t)src->n;
     BuilderFactory make_pb = [&]() {
-      std::unique_ptr<PipelineBuilder> pb(new PipelineBuilder(*src, x.st()));
+      std::unique_ptr<PipelineBuilder> pb(new PipelineBuilder(*src, x.st(), &x.e->regex));
       apply_chain(*pb, chain);
       return pb;
     };
@@ -2593,7 +2594,7 @@ struct Runner {
           DevBatchPtr src = exec(*base, part);
           for (auto* c : chain)
             if (OpMetrics* m = x.m(c)) m->input_rows += (uint64_t)src->n;
-          PipelineBuilder pb(*src, x.st());
+          PipelineBuilder pb(*src, x.st(), &x.e->regex);
           apply_chain(pb, chain);
           DevBatchPtr all = run_materialize(x, pb, named_cols(pb, n.schema), src, met);
           const int64_t keep = std::min<int64_t>(all->n, n.fetch);
@@ -2658,7 +2659,7 @@ struct Runner {
     DevBatchPtr work = in;
     size_t n_in_cols = in->cols.size();
     if (need_eval && n > 0) {
-      PipelineBuilder pb(*in, x.st());
+      PipelineBuilder pb(*in, x.st(), &x.e->regex);
       std::vector<ColRef> outs = pb.cols;
       for (auto& k : keys) {
         ColRef c = pb.compile(*k.expr);
@@ -2751,7 +2752,7 @@ struct Runner {
     bool need_eval = false;
     for (auto& e : exprs) need_eval |= e->kind != Expr::Col;
     if (need_eval) {
-      PipelineBuilder pb(*in, x.st());
+      PipelineBuilder pb(*in, x.st(), &x.e->regex);
       std::vector<ColRef> outs;
       for (auto& e : exprs) {
         ColRef c = pb.compile(*e);
@@ -3290,7 +3291,7 @@ struct Runner {
       ip.name = "__pi";
       cat->cols.push_back(ib);
       cat->cols.push_back(ip);
-      PipelineBuilder pb(*cat, x.st());
+      PipelineBuilder pb(*cat, x.st(), &x.e->regex);
       pb.apply_filter(*n.join_filter);
       std::vector<ColRef> outs = {pb.cols[cat->cols.size() - 2], pb.cols[cat->cols.size() - 1]};
       DevBatchPtr kept = run_materialize(x, pb, outs, cat, met);
@@ -5466,6 +5467,7 @@ void b200_engine_destroy(b200_engine* e) {
     if (sl.done) cudaEventDestroy(sl.done);
   }
   release_window(e);
+  e->regex.clear();
   if (e->comm && NcclApi::get().ok()) NcclApi::get().CommDestroy(e->comm);
   if (e->export_arena) cudaFreeHost(e->export_arena);
   // the calling thread's arena chunk is freed on the stream it was carved for: not after that stream is gone (at exit)
@@ -5501,6 +5503,7 @@ uint64_t b200_engine_counter(b200_engine* e, const char* name) {
   if (n == "nlj_pairs") return e->nlj_pairs;
   if (n == "window_sorts") return e->n_window_sorts;
   if (n == "host_syncs") return e->host_syncs;
+  if (n == "regex_compiles") return e->regex.compiles;
   return 0;
 }
 

@@ -4,9 +4,11 @@
 // decimal result types and rescaling, checked decimal arithmetic, wrapping integer arithmetic,
 // Kleene AND/OR, safe casts, CASE / IN / LIKE.
 #pragma once
+#include <atomic>
 #include <cstdlib>
 #include <cstring>
 #include <map>
+#include <mutex>
 
 #include "device_mem.hpp"
 
@@ -28,6 +30,37 @@ inline Operand mk_operand(uint8_t kind, uint8_t vk, int idx) {
   return o;
 }
 
+// Device copies of the regex DFAs compiled at typing (Expr::regex), one per pattern and flags (Expr::regex_key), kept for
+// the engine's lifetime: a warm stage builds and uploads nothing.  `compiles` counts the uploads (b200_engine_counter
+// "regex_compiles").  An upload waits for its copy before the pointer is published: a copy from pageable memory may still
+// be in flight when cudaMemcpy returns, and another task's stream may use the table next.
+struct RegexCache {
+  std::mutex mu;
+  std::map<std::string, void*> dev;
+  std::atomic<uint64_t> compiles{0};
+  const void* get(const std::string& key, const rx::Dfa& d, cudaStream_t st) {
+    std::lock_guard<std::mutex> g(mu);
+    auto it = dev.find(key);
+    if (it != dev.end()) return it->second;
+    void* p = nullptr;
+    CUDA_CHECK(cudaMalloc(&p, d.blob.size()));
+    cudaError_t ce = cudaMemcpyAsync(p, d.blob.data(), d.blob.size(), cudaMemcpyHostToDevice, st);
+    if (ce == cudaSuccess) ce = cudaStreamSynchronize(st);
+    if (ce != cudaSuccess) {
+      cudaFree(p);
+      CUDA_CHECK(ce);
+    }
+    dev[key] = p;
+    compiles++;
+    return p;
+  }
+  void clear() {
+    std::lock_guard<std::mutex> g(mu);
+    for (auto& kv : dev) cudaFree(kv.second);
+    dev.clear();
+  }
+};
+
 class PipelineBuilder {
  public:
   Program prog;
@@ -35,7 +68,7 @@ class PipelineBuilder {
   std::vector<DevPtr> keep;  // literal pools etc.
   int block = 512;
 
-  PipelineBuilder(const DevBatch& src, cudaStream_t st) : src_(src), st_(st) {
+  PipelineBuilder(const DevBatch& src, cudaStream_t st, RegexCache* regex) : src_(src), st_(st), regex_(regex) {
     memset(&prog, 0, sizeof prog);
     src_map_.assign(src.cols.size(), -1);
     for (size_t i = 0; i < src.cols.size(); i++) {
@@ -107,7 +140,7 @@ class PipelineBuilder {
         return c;
       }
       case Expr::Lit: return literal(e.type, e.lit);
-      case Expr::Bin: return compile_bin(e);
+      case Expr::Bin: return is_regex(e.op) ? compile_regex(e) : compile_bin(e);
       case Expr::Not: {
         ColRef a = compile(*e.args[0]);
         ColRef r = new_reg(DataType(TypeId::Bool), a.nullable);
@@ -182,6 +215,7 @@ class PipelineBuilder {
         return acc;
       }
       case Expr::Like: {
+        if (e.case_insensitive) return compile_regex(e);
         ColRef a = compile(*e.args[0]);
         ColRef r = new_reg(DataType(TypeId::Bool), a.nullable);
         VInstr ins = blank(OP_LIKE, VK_STR);
@@ -195,6 +229,7 @@ class PipelineBuilder {
         return r;
       }
       case Expr::Fn: {
+        if (e.fn == "regexp_like") return compile_regex(e);
         const int part = date_part_index(e.fn);
         if (part >= 0) return unary_fn(e, OP_DATE_PART, VK_I64, (uint8_t)part, 0);
         if (e.fn == "substr") {
@@ -221,6 +256,27 @@ class PipelineBuilder {
       }
     }
     throw EngineError(B200_ERR_UNSUPPORTED, "expression kind");
+  }
+
+  // ILIKE, ~ / ~* / !~ / !~* and regexp_like: one OP_REGEX over the DFA typing compiled (NULL when the pattern is NULL)
+  ColRef compile_regex(const Expr& e) {
+    if (!e.regex || e.args[0]->type.id == TypeId::Null) return null_of(DataType(TypeId::Bool));
+    if (!regex_) throw EngineError(B200_ERR_UNSUPPORTED, "regular expressions are not evaluated in this pipeline");
+    ColRef a = compile(*e.args[0]);
+    ColRef r = new_reg(DataType(TypeId::Bool), a.nullable);
+    VInstr ins = blank(OP_REGEX, VK_STR);
+    ins.a = resolve(a);
+    ins.dst = r.op;
+    ImmDesc d;
+    memset(&d, 0, sizeof d);
+    d.lo = (uint64_t)regex_->get(e.regex_key, *e.regex, st_);
+    d.hi = e.regex->shape();
+    ins.imm = add_imm(d);
+    ins.aux = e.negated ? 1 : 0;
+    if (a.nullable) ins.flags |= IF_NULLCHK;
+    emit(ins);
+    release(a);
+    return r;
   }
 
   // one-operand function: dst = op(a); string results are views into a's bytes
@@ -505,6 +561,7 @@ class PipelineBuilder {
  private:
   const DevBatch& src_;
   cudaStream_t st_;
+  RegexCache* regex_;
   std::vector<int> src_map_;
   std::vector<int> lazy_src_;
   std::map<int, int> pins_;

@@ -112,8 +112,19 @@ def in_list(x: Json, items: Sequence[Json], negated: bool = False) -> Json:
     return {"in": x, "list": list(items), "negated": negated}
 
 
-def like(x: Json, pattern: str, negated: bool = False) -> Json:
-    return {"like": x, "pattern": pattern, "negated": negated}
+def like(x: Json, pattern: str, negated: bool = False, case_insensitive: bool = False) -> Json:
+    """[NOT] LIKE, or [NOT] ILIKE with case_insensitive (arrow's LIKE-to-regex translation under the flags i and s)."""
+    n: Json = {"like": x, "pattern": pattern, "negated": negated}
+    if case_insensitive:
+        n["case_insensitive"] = True
+    return n
+
+
+def regex_match(x: Json, pattern, negated: bool = False, case_insensitive: bool = False) -> Json:
+    """x ~ p, x ~* p, x !~ p, x !~* p: an unanchored Rust-regex match against a Utf8 literal pattern (a str, or an
+    expression such as lit_utf8(None))."""
+    p = lit_utf8(pattern) if isinstance(pattern, str) else pattern
+    return binop(("!~" if negated else "~") + ("*" if case_insensitive else ""), x, p)
 
 
 def fn(name: str, *args: Json) -> Json:
