@@ -34,30 +34,13 @@
 #include "../common/plan_dump.hpp"
 #include "parquet_meta.hpp"
 #include "arrow_ipc.hpp"
+#include "shuffle_store.hpp"
 
 using namespace b200;
 
 namespace {
 
 thread_local std::string g_err;
-
-struct Piece {
-  int64_t file_id;
-  DevBatchPtr batch;
-  int64_t r0, r1;
-  int32_t src_rank = 0;               // which executor's map task produced it (exchange)
-  std::vector<int64_t> str_bytes;     // per Utf8 column of the batch: character bytes of rows [r0, r1); empty = unknown
-};
-struct ShuffleKey {
-  std::string job;
-  int64_t stage;
-  int64_t part;
-  bool operator<(const ShuffleKey& o) const {
-    if (job != o.job) return job < o.job;
-    if (stage != o.stage) return stage < o.stage;
-    return part < o.part;
-  }
-};
 
 struct OpMetrics {
   std::string name;
@@ -74,7 +57,7 @@ struct b200_engine {
   cudaStream_t stream = nullptr;
   std::mutex mu;
   std::map<std::string, std::map<int, DevBatchPtr>> tables;
-  std::map<ShuffleKey, std::vector<Piece>> shuffle;
+  ShuffleStore shuffle;                      // its own lock: take mu first when both are held
   std::atomic<uint64_t> launches{0};
   std::atomic<uint64_t> n_fused{0}, n_fused_static{0}, n_vm{0}, n_groupby{0}, n_groupby_pf{0}, n_fastfilter{0};  // pipelines per kernel family (b200_engine_counter)
   int64_t batch_size = 8192;
@@ -520,6 +503,138 @@ DevBatchPtr gather_batch(const Exec& x, const DevBatch& in, const int64_t* idx, 
   return out;
 }
 
+// the rows of `parts`, one after the other, as one batch of `schema`: a single piece is sliced without a copy
+DevBatchPtr concat_slices(const Exec& x, const std::vector<Piece>& parts, const Schema& schema) {
+  auto out = std::make_shared<DevBatch>();
+  int64_t total = 0;
+  for (auto& p : parts) total += p.r1 - p.r0;
+  out->n = total;
+  if (parts.size() == 1) {
+    const DevBatch& b = *parts[0].batch;
+    for (auto& c : b.cols) out->cols.push_back(slice_column(c, parts[0].r0, parts[0].r1));
+    return out;
+  }
+  // few rows (the tail of a query, reduce side of a small shuffle): all copies in one kernel launch
+  const bool batched = total <= 65536;
+  PackList pl;
+  for (size_t ci = 0; ci < schema.size(); ci++) {
+    bool any_valid = false;
+    for (auto& p : parts) any_valid |= p.batch->cols[ci].valid != nullptr;
+    const DataType& t = schema[ci].type;
+    Phys ph = t.id == TypeId::Utf8 ? PH_STRVIEW : phys_of(t);
+    DevColumn oc = make_out_column(schema[ci].name, t, ph, total, any_valid, x.st());
+    oc.n = total;
+    int64_t pos = 0;
+    for (auto& p : parts) {
+      int64_t r0 = p.r0, r1 = p.r1, n = r1 - r0;
+      if (n == 0) continue;
+      DevColumn sc = slice_column(p.batch->cols[ci], r0, r1);
+      if (sc.type != t) throw EngineError(B200_ERR_INVALID, "concat: type mismatch in column " + schema[ci].name);
+      if (batched && sc.phys == PH_UTF8) {
+        // offsets + characters -> views, straight into the concatenated column (no temporary, no extra launch)
+        pl.utf8_views(sc, (uint8_t*)oc.data + pos * oc.width());
+        if (any_valid) {
+          if (sc.valid) pl.copy(sc.valid, (uint8_t*)oc.valid + pos, (uint64_t)n);
+          else CUDA_CHECK(cudaMemsetAsync((uint8_t*)oc.valid + pos, 1, (size_t)n, x.st()));
+        }
+        for (auto& k : sc.keep) oc.keep.push_back(k);
+        pos += n;
+        continue;
+      }
+      DevColumn v = as_views(x, sc);
+      if (batched) pl.copy(v.data, (uint8_t*)oc.data + pos * oc.width(), (uint64_t)n * oc.width());
+      else CUDA_CHECK(cudaMemcpyAsync((uint8_t*)oc.data + pos * oc.width(), v.data, (size_t)n * oc.width(), cudaMemcpyDeviceToDevice, x.st()));
+      if (any_valid) {
+        if (v.valid && batched) pl.copy(v.valid, (uint8_t*)oc.valid + pos, (uint64_t)n);
+        else if (v.valid) CUDA_CHECK(cudaMemcpyAsync((uint8_t*)oc.valid + pos, v.valid, (size_t)n, cudaMemcpyDeviceToDevice, x.st()));
+        else CUDA_CHECK(cudaMemsetAsync((uint8_t*)oc.valid + pos, 1, (size_t)n, x.st()));
+      }
+      if (ph == PH_STRVIEW)
+        for (auto& k : v.keep) oc.keep.push_back(k);
+      pos += n;
+    }
+    out->cols.push_back(oc);
+  }
+  pl.run(x);
+  return out;
+}
+
+DevBatchPtr concat(const Exec& x, const std::vector<DevBatchPtr>& parts, const Schema& schema) {
+  std::vector<Piece> v;
+  for (auto& p : parts) v.push_back(Piece{0, p, 0, p->n});
+  return concat_slices(x, v, schema);
+}
+
+// character bytes of every Utf8 column of `b` (rows [0, b.n)), one read-back for all of them; known values are reused
+std::vector<int64_t> string_bytes(const Exec& x, const DevBatch& b) {
+  std::vector<int64_t> out;
+  PartStrCols sc;
+  sc.n = 0;
+  std::vector<size_t> unknown;
+  for (auto& c : b.cols) {
+    if (c.type.id != TypeId::Utf8) continue;
+    if (c.phys == PH_UTF8 && c.chars_bytes >= 0) {
+      out.push_back(c.chars_bytes);
+      continue;
+    }
+    out.push_back(-1);
+    if (b.n == 0) {
+      out.back() = 0;
+      continue;
+    }
+    if (sc.n == PART_MAX_STR_COLS) throw EngineError(B200_ERR_UNSUPPORTED, "more than 16 string columns in one shuffle output");
+    sc.c[sc.n++] = PartStrCol{c.data, c.valid, c.phys == PH_STRVIEW ? 1 : 0, 0};
+    unknown.push_back(out.size() - 1);
+  }
+  if (sc.n) {
+    DevPtr acc = dev_alloc((size_t)(1 + sc.n) * 8, x.st());
+    CUDA_CHECK(cudaMemsetAsync(acc->ptr, 0, (size_t)(1 + sc.n) * 8, x.st()));
+    PidSrc none;
+    memset(&none, 0, sizeof none);
+    CUDA_CHECK(launch_partition_hist(none, b.n, 1, nullptr, (unsigned long long*)acc->ptr, sc, (unsigned long long*)acc->ptr + 1, x.st()));
+    const unsigned long long* h = (const unsigned long long*)x.fetch_bytes((const unsigned long long*)acc->ptr + 1, (size_t)sc.n * 8);
+    x.sync();
+    for (size_t k = 0; k < unknown.size(); k++) out[unknown[k]] = (int64_t)h[k];
+  }
+  return out;
+}
+
+// One column moved by the radix partition's scatter: to `out`, partition after partition, or -- part_base set -- to
+// part_base[p] + row * width for the rows of partition p
+struct ScatterCol {
+  const void* in;
+  void* out;
+  const unsigned long long* part_base;
+  int width;
+};
+
+// The radix partition after launch_partition_hist: scans the per-tile histogram into every tile's first destination
+// row, then moves the columns, GATHER_MAX_COLS per launch (each timed as `timer`)
+void partition_scatter(const Exec& x, const char* timer, const PidSrc& pid, int64_t n, uint32_t P, uint32_t n_tiles, const DevPtr& tile_hist,
+                       const std::vector<ScatterCol>& cols) {
+  const int64_t hn = (int64_t)P * n_tiles;
+  DevPtr offs = dev_alloc((size_t)(hn + 2) * 8, x.st());
+  DevPtr scratch = dev_alloc((size_t)(hn / 1024 + 4) * 8, x.st());
+  if (hn > 0) launch_scan_u32_to_u64((const uint32_t*)tile_hist->ptr, (uint64_t*)offs->ptr, hn, (uint64_t*)scratch->ptr, x.st());
+  if (n == 0) return;
+  for (size_t c0 = 0; c0 < cols.size(); c0 += GATHER_MAX_COLS) {
+    GatherCols gc;
+    memset(&gc, 0, sizeof gc);
+    uint64_t b = 0;
+    for (; gc.n < GATHER_MAX_COLS && c0 + (size_t)gc.n < cols.size(); gc.n++) {
+      const ScatterCol& c = cols[c0 + gc.n];
+      GatherCol& g = gc.c[gc.n];
+      g.in = c.in;
+      g.out = c.out;
+      g.part_base = c.part_base;
+      g.width = c.width;
+      b += (uint64_t)c.width;
+    }
+    KernelTimer kt(x, timer, (uint64_t)n * (2 * b + 4));
+    CUDA_CHECK(launch_partition_scatter(pid, n, P, (const uint64_t*)offs->ptr, gc, nullptr, x.st()));
+  }
+}
+
 // ------------------------------------------------------------------------------------------------
 // Arrow import (host -> HBM)
 // ------------------------------------------------------------------------------------------------
@@ -923,23 +1038,14 @@ bool partition_for_groupby(const Exec& x, GroupBySpec& S, std::vector<DevPtr>& k
   PartStrCols sc;
   sc.n = 0;
   CUDA_CHECK(launch_partition_hist(ps, n, K, (uint32_t*)tile_hist->ptr, (unsigned long long*)acc->ptr, sc, (unsigned long long*)acc->ptr + K, x.st()));
-  const int64_t hn = (int64_t)K * n_tiles;
-  DevPtr offs = dev_alloc((size_t)(hn + 2) * 8, x.st());
-  DevPtr scratch = dev_alloc((size_t)(hn / 1024 + 4) * 8, x.st());
-  launch_scan_u32_to_u64((const uint32_t*)tile_hist->ptr, (uint64_t*)offs->ptr, hn, (uint64_t*)scratch->ptr, x.st());
-  GatherCols gc;
-  gc.n = 0;
+  std::vector<ScatterCol> cols;
   for (int c = 0; c < S.n_cols; c++) {
     DevPtr out = dev_alloc((size_t)n * S.cols[c].width + 64, x.st());
-    GatherCol& g = gc.c[gc.n++];
-    memset(&g, 0, sizeof g);
-    g.in = S.cols[c].data;
-    g.out = out->ptr;
-    g.width = (int)S.cols[c].width;
+    cols.push_back(ScatterCol{S.cols[c].data, out->ptr, nullptr, (int)S.cols[c].width});
     S.cols[c].data = out->ptr;
     keep.push_back(out);
   }
-  CUDA_CHECK(launch_partition_scatter(ps, n, K, (const uint64_t*)offs->ptr, gc, nullptr, x.st()));
+  partition_scatter(x, "partition_scatter_agg", ps, n, K, n_tiles, tile_hist, cols);
   DevPtr row_start = dev_alloc((size_t)(K + 1) * 8 + 64, x.st()), cta_start = dev_alloc((size_t)(K + 1) * 4 + 64, x.st());
   CUDA_CHECK(launch_groupby_plan((const unsigned long long*)acc->ptr, (int)K, (unsigned long long*)row_start->ptr, (unsigned int*)cta_start->ptr, x.st()));
   S.pf_K = (int)K;
@@ -950,8 +1056,6 @@ bool partition_for_groupby(const Exec& x, GroupBySpec& S, std::vector<DevPtr>& k
   keep.push_back(cta_start);
   keep.push_back(acc);
   keep.push_back(tile_hist);
-  keep.push_back(offs);
-  keep.push_back(scratch);
   x.e->n_groupby_pf++;
   return true;
 }
@@ -2364,13 +2468,7 @@ struct Runner {
         if (it == x.e->tables.end()) throw EngineError(B200_ERR_INVALID, "table not registered: " + n.table);
         return it->second.empty() ? 0 : it->second.rbegin()->first + 1;
       }
-      case PlanNode::ShuffleReader: {
-        std::lock_guard<std::mutex> g(x.e->mu);
-        int mx = 0;
-        for (auto& kv : x.e->shuffle)
-          if (kv.first.job == job && kv.first.stage == n.reader_stage_id) mx = std::max(mx, (int)kv.first.part + 1);
-        return mx;
-      }
+      case PlanNode::ShuffleReader: return x.e->shuffle.partitions(job, n.reader_stage_id);
       case PlanNode::SortPreservingMerge: return 1;
       case PlanNode::Passthrough:
         if (n.op_name == "CoalescePartitionsExec") return 1;
@@ -2378,67 +2476,6 @@ struct Runner {
       case PlanNode::HashJoin: return n_partitions(*n.children[1]);
       default: return n_partitions(*n.children[0]);
     }
-  }
-
-  DevBatchPtr concat(const std::vector<DevBatchPtr>& parts, const Schema& schema) {
-    std::vector<std::pair<DevBatchPtr, std::pair<int64_t, int64_t>>> v;
-    for (auto& p : parts) v.push_back({p, {0, p->n}});
-    return concat_slices(v, schema);
-  }
-
-  DevBatchPtr concat_slices(const std::vector<std::pair<DevBatchPtr, std::pair<int64_t, int64_t>>>& parts, const Schema& schema) {
-    auto out = std::make_shared<DevBatch>();
-    int64_t total = 0;
-    for (auto& p : parts) total += p.second.second - p.second.first;
-    out->n = total;
-    if (parts.size() == 1) {
-      const DevBatch& b = *parts[0].first;
-      for (auto& c : b.cols) out->cols.push_back(slice_column(c, parts[0].second.first, parts[0].second.second));
-      return out;
-    }
-    // few rows (the tail of a query, reduce side of a small shuffle): all copies in one kernel launch
-    const bool batched = total <= 65536;
-    PackList pl;
-    for (size_t ci = 0; ci < schema.size(); ci++) {
-      bool any_valid = false;
-      for (auto& p : parts) any_valid |= p.first->cols[ci].valid != nullptr;
-      const DataType& t = schema[ci].type;
-      Phys ph = t.id == TypeId::Utf8 ? PH_STRVIEW : phys_of(t);
-      DevColumn oc = make_out_column(schema[ci].name, t, ph, total, any_valid, x.st());
-      oc.n = total;
-      int64_t pos = 0;
-      for (auto& p : parts) {
-        int64_t r0 = p.second.first, r1 = p.second.second, n = r1 - r0;
-        if (n == 0) continue;
-        DevColumn sc = slice_column(p.first->cols[ci], r0, r1);
-        if (sc.type != t) throw EngineError(B200_ERR_INVALID, "concat: type mismatch in column " + schema[ci].name);
-        if (batched && sc.phys == PH_UTF8) {
-          // offsets + characters -> views, straight into the concatenated column (no temporary, no extra launch)
-          pl.utf8_views(sc, (uint8_t*)oc.data + pos * oc.width());
-          if (any_valid) {
-            if (sc.valid) pl.copy(sc.valid, (uint8_t*)oc.valid + pos, (uint64_t)n);
-            else CUDA_CHECK(cudaMemsetAsync((uint8_t*)oc.valid + pos, 1, (size_t)n, x.st()));
-          }
-          for (auto& k : sc.keep) oc.keep.push_back(k);
-          pos += n;
-          continue;
-        }
-        DevColumn v = as_views(x, sc);
-        if (batched) pl.copy(v.data, (uint8_t*)oc.data + pos * oc.width(), (uint64_t)n * oc.width());
-        else CUDA_CHECK(cudaMemcpyAsync((uint8_t*)oc.data + pos * oc.width(), v.data, (size_t)n * oc.width(), cudaMemcpyDeviceToDevice, x.st()));
-        if (any_valid) {
-          if (v.valid && batched) pl.copy(v.valid, (uint8_t*)oc.valid + pos, (uint64_t)n);
-          else if (v.valid) CUDA_CHECK(cudaMemcpyAsync((uint8_t*)oc.valid + pos, v.valid, (size_t)n, cudaMemcpyDeviceToDevice, x.st()));
-          else CUDA_CHECK(cudaMemsetAsync((uint8_t*)oc.valid + pos, 1, (size_t)n, x.st()));
-        }
-        if (ph == PH_STRVIEW)
-          for (auto& k : v.keep) oc.keep.push_back(k);
-        pos += n;
-      }
-      out->cols.push_back(oc);
-    }
-    pl.run(x);
-    return out;
   }
 
   DevBatchPtr empty_batch(const Schema& s) {
@@ -2457,7 +2494,7 @@ struct Runner {
     std::vector<DevBatchPtr> parts;
     for (int p = 0; p < np; p++) parts.push_back(exec(n, p));
     if (parts.empty()) return empty_batch(n.schema);
-    return concat(parts, n.schema);
+    return concat(x, parts, n.schema);
   }
 
   // Walk down a Filter/Projection chain; returns the base node and the chain (top-down order).
@@ -2566,16 +2603,11 @@ struct Runner {
         break;
       }
       case PlanNode::ShuffleReader: {
-        std::vector<std::pair<DevBatchPtr, std::pair<int64_t, int64_t>>> pieces;
-        {
-          std::lock_guard<std::mutex> g(x.e->mu);
-          auto it = x.e->shuffle.find(ShuffleKey{job, n.reader_stage_id, n.broadcast ? 0 : part});
-          if (it != x.e->shuffle.end())
-            for (auto& p : it->second)
-              if (p.r1 > p.r0) pieces.push_back({p.batch, {p.r0, p.r1}});
-        }
+        std::vector<Piece> pieces;
+        for (Piece& p : x.e->shuffle.pieces(ShuffleKey{job, n.reader_stage_id, n.broadcast ? 0 : part}))
+          if (p.r1 > p.r0) pieces.push_back(std::move(p));
         if (pieces.empty()) out = empty_batch(n.schema);
-        else out = concat_slices(pieces, n.schema);
+        else out = concat_slices(x, pieces, n.schema);
         for (size_t c = 0; c < out->cols.size() && c < n.schema.size(); c++) {
           if (out->cols[c].type != n.schema[c].type)
             throw EngineError(B200_ERR_INVALID, "shuffle reader: column " + n.schema[c].name + " has type " + out->cols[c].type.str() + ", plan says " + n.schema[c].type.str());
@@ -3617,38 +3649,26 @@ struct Runner {
     return t;
   }
 
-  // character bytes of every Utf8 column of `b` (rows [0, b.n)), one read-back for all of them; known values are reused
-  std::vector<int64_t> string_bytes(const DevBatch& b) {
-    std::vector<int64_t> out;
-    PartStrCols sc;
-    sc.n = 0;
-    std::vector<size_t> unknown;
-    for (auto& c : b.cols) {
-      if (c.type.id != TypeId::Utf8) continue;
-      if (c.phys == PH_UTF8 && c.chars_bytes >= 0) {
-        out.push_back(c.chars_bytes);
-        continue;
-      }
-      out.push_back(-1);
-      if (b.n == 0) {
-        out.back() = 0;
-        continue;
-      }
-      if (sc.n == PART_MAX_STR_COLS) throw EngineError(B200_ERR_UNSUPPORTED, "more than 16 string columns in one shuffle output");
-      sc.c[sc.n++] = PartStrCol{c.data, c.valid, c.phys == PH_STRVIEW ? 1 : 0, 0};
-      unknown.push_back(out.size() - 1);
-    }
-    if (sc.n) {
-      DevPtr acc = dev_alloc((size_t)(1 + sc.n) * 8, x.st());
-      CUDA_CHECK(cudaMemsetAsync(acc->ptr, 0, (size_t)(1 + sc.n) * 8, x.st()));
-      PidSrc none;
-      memset(&none, 0, sizeof none);
-      CUDA_CHECK(launch_partition_hist(none, b.n, 1, nullptr, (unsigned long long*)acc->ptr, sc, (unsigned long long*)acc->ptr + 1, x.st()));
-      const unsigned long long* h = (const unsigned long long*)x.fetch_bytes((const unsigned long long*)acc->ptr + 1, (size_t)sc.n * 8);
-      x.sync();
-      for (size_t k = 0; k < unknown.size(); k++) out[unknown[k]] = (int64_t)h[k];
-    }
-    return out;
+  // what the writer reports for one output partition (ShuffleWritePartition, ballista.proto:481-492)
+  b200_shuffle_write_partition written(uint64_t part, uint64_t rows, uint64_t bytes, int64_t file_id, bool sort_shuffle) const {
+    const uint64_t bs = (uint64_t)x.e->batch_size;
+    b200_shuffle_write_partition w{};
+    w.partition_id = part;
+    w.num_rows = rows;
+    w.num_batches = (rows + bs - 1) / bs;
+    w.num_bytes = bytes;
+    w.file_id = file_id;
+    w.is_sort_shuffle = sort_shuffle ? 1 : 0;
+    return w;
+  }
+  // the writer's metrics: a repartitioning writer read the bytes it wrote (the scatter moved them); one that stores its
+  // input as it is counts that input's rows
+  static void count_written(OpMetrics* met, uint64_t rows, uint64_t bytes, bool repartitioned) {
+    if (!met) return;
+    met->output_rows += rows;
+    met->bytes_written += bytes;
+    if (repartitioned) met->bytes_read += bytes;
+    else met->input_rows += rows;
   }
 
   struct FusedExchange {
@@ -3697,13 +3717,6 @@ struct Runner {
     std::vector<unsigned long long> Mv(mrow * (size_t)W);
     CUDA_CHECK(cudaMemcpyAsync(Mv.data(), mat->ptr, Mv.size() * 8, cudaMemcpyDeviceToHost, x.st()));
     const unsigned long long* M = Mv.data();
-    // while the matrix travels: per-tile offsets of the local rows
-    const int64_t hn = (int64_t)P * n_tiles;
-    DevPtr offs = dev_alloc((size_t)(hn + 2) * 8, x.st());
-    DevPtr scratch = dev_alloc((size_t)(hn / 1024 + 4) * 8, x.st());
-    if (hn > 0) {
-      launch_scan_u32_to_u64((const uint32_t*)tile_hist->ptr, (uint64_t*)offs->ptr, hn, (uint64_t*)scratch->ptr, x.st());
-    }
     x.sync();
     auto cnt = [&](int s, uint32_t p) { return (uint64_t)M[mrow * (size_t)s + p]; };
     uint64_t any_valid = 0;
@@ -3749,41 +3762,22 @@ struct Runner {
     DevPtr bases = dev_alloc(nslots * P * 8 + 64, x.st());
     CUDA_CHECK(cudaMemcpyAsync(bases->ptr, hb, nslots * P * 8, cudaMemcpyHostToDevice, x.st()));
     std::vector<DevPtr> ones_keep;
-    {
-      GatherCols gc;
-      gc.n = 0;
-      auto flush = [&]() {
-        if (gc.n && n > 0) {
-          uint64_t b = 0;
-          for (int k = 0; k < gc.n; k++) b += (uint64_t)gc.c[k].width;
-          KernelTimer kt(x, "partition_scatter_peer", (uint64_t)n * (2 * b + 4));
-          CUDA_CHECK(launch_partition_scatter(pid, n, P, (const uint64_t*)offs->ptr, gc, nullptr, x.st()));
+    std::vector<ScatterCol> cols;
+    const unsigned long long* part_base = (const unsigned long long*)bases->ptr;
+    for (size_t c = 0; c < ncols; c++) {
+      cols.push_back(ScatterCol{pay[c].data, nullptr, part_base + c * P, pay[c].width()});
+      if (any_valid >> c & 1) {
+        const uint8_t* v = pay[c].valid;
+        if (!v && n > 0) {  // another map task has nulls in this column: this one contributes all-valid bytes
+          DevPtr ones = dev_alloc((size_t)n + 64, x.st());
+          CUDA_CHECK(cudaMemsetAsync(ones->ptr, 1, (size_t)n, x.st()));
+          ones_keep.push_back(ones);
+          v = (const uint8_t*)ones->ptr;
         }
-        gc.n = 0;
-      };
-      auto add = [&](const void* in, size_t slot, int width) {
-        GatherCol& g = gc.c[gc.n++];
-        memset(&g, 0, sizeof g);
-        g.in = in;
-        g.width = width;
-        g.part_base = (const unsigned long long*)bases->ptr + slot * P;
-        if (gc.n == GATHER_MAX_COLS) flush();
-      };
-      for (size_t c = 0; c < ncols; c++) {
-        add(pay[c].data, c, pay[c].width());
-        if (any_valid >> c & 1) {
-          const uint8_t* v = pay[c].valid;
-          if (!v && n > 0) {  // another map task has nulls in this column: this one contributes all-valid bytes
-            DevPtr ones = dev_alloc((size_t)n + 64, x.st());
-            CUDA_CHECK(cudaMemsetAsync(ones->ptr, 1, (size_t)n, x.st()));
-            ones_keep.push_back(ones);
-            v = (const uint8_t*)ones->ptr;
-          }
-          add(v, ncols + c, 1);
-        }
+        cols.push_back(ScatterCol{v, nullptr, part_base + (ncols + c) * P, 1});
       }
-      flush();
     }
+    partition_scatter(x, "partition_scatter_peer", pid, n, P, n_tiles, tile_hist, cols);
     // every executor's stores must have landed before anyone reads its window: a zero-payload all-to-all on the same
     // stream completes only after every peer's scatter kernel did
     {
@@ -3799,63 +3793,42 @@ struct Runner {
     }
     e->win_used = cursor[(size_t)me];
     // the reduce side's view: one batch per owned partition, one piece per map task
-    const int64_t bs = e->batch_size;
     uint64_t total_bytes = 0;
-    {
-      std::lock_guard<std::mutex> g(e->mu);
-      for (uint32_t p = 0; p < P; p++) {
-        const uint64_t rows = cnt(me, p);
-        if (rows) {
-          b200_shuffle_write_partition w{};
-          w.partition_id = p;
-          w.num_rows = rows;
-          w.num_batches = (rows + (uint64_t)bs - 1) / (uint64_t)bs;
-          w.num_bytes = rows * row_bytes;
-          w.file_id = input_partition;
-          w.is_sort_shuffle = root.sort_shuffle ? 1 : 0;
-          total_bytes += w.num_bytes;
-          res.push_back(w);
-          if ((int)(p % (uint32_t)W) != me) fx->sent += w.num_bytes;
+    std::map<int64_t, std::vector<Piece>> arrivals;
+    for (uint32_t p = 0; p < P; p++) {
+      const uint64_t rows = cnt(me, p);
+      if (rows) {
+        res.push_back(written(p, rows, rows * row_bytes, input_partition, root.sort_shuffle));
+        total_bytes += res.back().num_bytes;
+        if ((int)(p % (uint32_t)W) != me) fx->sent += res.back().num_bytes;
+      }
+      if ((int)(p % (uint32_t)W) != me || tot[p] == 0) continue;
+      auto b = std::make_shared<DevBatch>();
+      b->n = (int64_t)tot[p];
+      for (size_t c = 0; c < ncols; c++) {
+        DevColumn col;
+        col.name = root.schema[c].name;
+        col.type = pay[c].type;
+        col.phys = pay[c].phys;
+        col.n = b->n;
+        col.data = e->win_local + region[c * P + p];
+        col.nullable = (any_valid >> c & 1) != 0;
+        if (col.nullable) col.valid = e->win_local + region[(ncols + c) * P + p];
+        b->cols.push_back(col);
+      }
+      int64_t at = 0;
+      for (int s = 0; s < W; s++) {
+        const int64_t rs = (int64_t)cnt(s, p);
+        if (rs) {
+          arrivals[p].push_back(Piece{(int64_t)M[mrow * (size_t)s + P + 2], b, at, at + rs, s, {}});
+          if (s != me) fx->recvd += (uint64_t)rs * row_bytes;
         }
-        if ((int)(p % (uint32_t)W) != me) continue;
-        auto& v = e->shuffle[ShuffleKey{job, root.stage_id, (int64_t)p}];
-        if (tot[p] == 0) {
-          if (v.empty()) e->shuffle.erase(ShuffleKey{job, root.stage_id, (int64_t)p});
-          continue;
-        }
-        auto b = std::make_shared<DevBatch>();
-        b->n = (int64_t)tot[p];
-        for (size_t c = 0; c < ncols; c++) {
-          DevColumn col;
-          col.name = root.schema[c].name;
-          col.type = pay[c].type;
-          col.phys = pay[c].phys;
-          col.n = b->n;
-          col.data = e->win_local + region[c * P + p];
-          col.nullable = (any_valid >> c & 1) != 0;
-          if (col.nullable) col.valid = e->win_local + region[(ncols + c) * P + p];
-          b->cols.push_back(col);
-        }
-        int64_t at = 0;
-        for (int s = 0; s < W; s++) {
-          const int64_t rs = (int64_t)cnt(s, p);
-          const int64_t fid = (int64_t)M[mrow * (size_t)s + P + 2];
-          if (rs) {
-            v.erase(std::remove_if(v.begin(), v.end(), [&](const Piece& pc) { return pc.file_id == fid && pc.src_rank == s; }), v.end());
-            v.push_back(Piece{fid, b, at, at + rs, s, {}});
-            if (s != me) fx->recvd += (uint64_t)rs * row_bytes;
-          }
-          at += rs;
-        }
-        std::stable_sort(v.begin(), v.end(), [](const Piece& a, const Piece& b2) { return a.src_rank != b2.src_rank ? a.src_rank < b2.src_rank : a.file_id < b2.file_id; });
+        at += rs;
       }
     }
+    e->shuffle.install(job, root.stage_id, arrivals);
     x.sync();
-    if (met) {
-      met->output_rows += (uint64_t)n;
-      met->bytes_written += total_bytes;
-      met->bytes_read += total_bytes;
-    }
+    count_written(met, (uint64_t)n, total_bytes, true);
     e->fused_exchanges++;
     fx->done = true;
     return true;
@@ -3870,9 +3843,7 @@ struct Runner {
     if (root.op != PlanNode::ShuffleWriter) throw EngineError(B200_ERR_INVALID, "stage plan root must be a ShuffleWriterExec");
     OpMetrics* met = x.m(&root);
     const PlanNode& child = *root.children[0];
-    const int64_t bs = x.e->batch_size;
     const int32_t my_rank = x.e->rank;
-    auto nbatches = [&](uint64_t rows) { return (rows + (uint64_t)bs - 1) / (uint64_t)bs; };
     std::vector<b200_shuffle_write_partition> res;
     // no repartitioning; also hash partitioning into ONE partition (hash % 1 == 0 for every row), which
     // keeps the rows of this task together as output partition 0
@@ -3891,34 +3862,15 @@ struct Runner {
       std::vector<int64_t> cb;
       {
         ScopeTimer t2("writer: string bytes + final sync");
-        cb = string_bytes(*st);
+        cb = string_bytes(x, *st);
         x.sync();  // deferred status checks of this task's kernels
       }
-      b200_shuffle_write_partition w{};
-      w.partition_id = single ? 0u : (uint64_t)input_partition;
-      w.num_rows = (uint64_t)st->n;
-      w.num_batches = nbatches(w.num_rows);
-      w.num_bytes = slice_bytes(*st, st->n, cb);
-      w.file_id = single ? (int64_t)input_partition : -1;
-      w.is_sort_shuffle = (single && root.sort_shuffle) ? 1 : 0;
-      {
-        std::lock_guard<std::mutex> g(x.e->mu);
-        auto& v = x.e->shuffle[ShuffleKey{job, root.stage_id, single ? 0 : input_partition}];
-        if (single) {
-          const int64_t fid = (int64_t)input_partition;
-          v.erase(std::remove_if(v.begin(), v.end(), [&](const Piece& pc) { return pc.file_id == fid && pc.src_rank == my_rank; }), v.end());
-          if (st->n > 0) v.push_back(Piece{fid, st, 0, st->n, my_rank, cb});
-          else if (v.empty()) x.e->shuffle.erase(ShuffleKey{job, root.stage_id, 0});
-        } else {
-          v.clear();
-          v.push_back(Piece{-1, st, 0, st->n, my_rank, cb});
-        }
-      }
-      if (met) {
-        met->output_rows += w.num_rows;
-        met->input_rows += w.num_rows;
-        met->bytes_written += w.num_bytes;
-      }
+      const int64_t fid = single ? (int64_t)input_partition : -1;
+      const ShuffleKey key{job, root.stage_id, single ? 0 : input_partition};
+      if (single) x.e->shuffle.store(key, Piece{fid, st, 0, st->n, my_rank, cb}, false);
+      else x.e->shuffle.replace_partition(key, Piece{fid, st, 0, st->n, my_rank, cb});
+      const b200_shuffle_write_partition w = written((uint64_t)key.part, (uint64_t)st->n, slice_bytes(*st, st->n, cb), fid, single && root.sort_shuffle);
+      count_written(met, w.num_rows, w.num_bytes, false);
       if (!(single && st->n == 0)) res.push_back(w);  // only partitions with rows are reported
       return res;
     }
@@ -4013,45 +3965,19 @@ struct Runner {
     }
     const unsigned long long* hc = (const unsigned long long*)x.fetch_bytes(acc_ptr, acc_words * 8);
     // while the counts travel: scan the per-tile histogram and scatter
-    const int64_t hn = (int64_t)P * n_tiles;
-    DevPtr offs = dev_alloc((size_t)(hn + 2) * 8, x.st());
-    DevPtr scratch = dev_alloc((size_t)(hn / 1024 + 4) * 8, x.st());
-    if (hn > 0) {
-      launch_scan_u32_to_u64((const uint32_t*)tile_hist->ptr, (uint64_t*)offs->ptr, hn, (uint64_t*)scratch->ptr, x.st());
-    }
     auto st = std::make_shared<DevBatch>();
     st->n = n;
-    {
-      GatherCols gc;
-      gc.n = 0;
-      auto flush = [&]() {
-        if (gc.n && n > 0) {
-          uint64_t b = 0;
-          for (int k = 0; k < gc.n; k++) b += (uint64_t)gc.c[k].width;
-          KernelTimer kt(x, "partition_scatter", (uint64_t)n * (2 * b + 4));
-          CUDA_CHECK(launch_partition_scatter(pid, n, P, (const uint64_t*)offs->ptr, gc, nullptr, x.st()));
-        }
-        gc.n = 0;
-      };
-      auto add = [&](const void* in, void* out, int width) {
-        GatherCol& g = gc.c[gc.n++];
-        memset(&g, 0, sizeof g);
-        g.in = in;
-        g.out = out;
-        g.width = width;
-        if (gc.n == GATHER_MAX_COLS) flush();
-      };
-      for (size_t c = 0; c < n_payload; c++) {
-        const DevColumn& scn = pay[c];
-        DevColumn oc = make_out_column(root.schema[c].name, scn.type, scn.phys, n, scn.valid != nullptr, x.st());
-        oc.n = n;
-        add(scn.data, (void*)oc.data, scn.width());
-        if (scn.valid) add(scn.valid, (void*)oc.valid, 1);
-        for (auto& k : scn.keep) oc.keep.push_back(k);
-        st->cols.push_back(oc);
-      }
-      flush();
+    std::vector<ScatterCol> cols;
+    for (size_t c = 0; c < n_payload; c++) {
+      const DevColumn& scn = pay[c];
+      DevColumn oc = make_out_column(root.schema[c].name, scn.type, scn.phys, n, scn.valid != nullptr, x.st());
+      oc.n = n;
+      cols.push_back(ScatterCol{scn.data, (void*)oc.data, nullptr, scn.width()});
+      if (scn.valid) cols.push_back(ScatterCol{scn.valid, (void*)oc.valid, nullptr, 1});
+      for (auto& k : scn.keep) oc.keep.push_back(k);
+      st->cols.push_back(oc);
     }
+    partition_scatter(x, "partition_scatter", pid, n, P, n_tiles, tile_hist, cols);
     x.sync();
     std::vector<int64_t> bounds(P + 1, 0);
     for (uint32_t p = 0; p < P; p++) bounds[p + 1] = bounds[p] + (int64_t)hc[p];
@@ -4059,36 +3985,16 @@ struct Runner {
     for (int c = 0; c < sc.n; c++)
       for (uint32_t p = 0; p < P; p++) chars_per_part[(size_t)c][p] = (int64_t)hc[(size_t)P * (1 + c) + p];
     uint64_t total_bytes = 0;
-    {
-      std::lock_guard<std::mutex> g(x.e->mu);
-      for (uint32_t p = 0; p < P; p++) {
-        auto& v = x.e->shuffle[ShuffleKey{job, root.stage_id, (int64_t)p}];
-        // a re-run of the same map task replaces its previous output (task retry)
-        v.erase(std::remove_if(v.begin(), v.end(), [&](const Piece& pc) { return pc.file_id == input_partition && pc.src_rank == my_rank; }), v.end());
-        const int64_t rows = bounds[p + 1] - bounds[p];
-        if (rows == 0) {
-          if (v.empty()) x.e->shuffle.erase(ShuffleKey{job, root.stage_id, (int64_t)p});
-          continue;  // only partitions with rows are reported (sort_shuffle/writer.rs:357-369)
-        }
-        std::vector<int64_t> cb;
-        for (auto& cp : chars_per_part) cb.push_back(cp[p]);
-        v.push_back(Piece{input_partition, st, bounds[p], bounds[p + 1], my_rank, cb});
-        b200_shuffle_write_partition w{};
-        w.partition_id = p;
-        w.num_rows = (uint64_t)rows;
-        w.num_batches = nbatches(w.num_rows);
-        w.num_bytes = slice_bytes(*st, rows, cb);
-        w.file_id = input_partition;
-        w.is_sort_shuffle = root.sort_shuffle ? 1 : 0;
-        total_bytes += w.num_bytes;
-        res.push_back(w);
-      }
+    for (uint32_t p = 0; p < P; p++) {
+      const int64_t rows = bounds[p + 1] - bounds[p];
+      std::vector<int64_t> cb;
+      for (auto& cp : chars_per_part) cb.push_back(cp[p]);
+      x.e->shuffle.store(ShuffleKey{job, root.stage_id, (int64_t)p}, Piece{input_partition, st, bounds[p], bounds[p + 1], my_rank, cb}, false);
+      if (rows == 0) continue;  // only partitions with rows are reported (sort_shuffle/writer.rs:357-369)
+      res.push_back(written(p, (uint64_t)rows, slice_bytes(*st, rows, cb), input_partition, root.sort_shuffle));
+      total_bytes += res.back().num_bytes;
     }
-    if (met) {
-      met->output_rows += (uint64_t)n;
-      met->bytes_written += total_bytes;
-      met->bytes_read += total_bytes;
-    }
+    count_written(met, (uint64_t)n, total_bytes, true);
     return res;
   }
 };
@@ -4116,7 +4022,6 @@ struct ExchEntry {
 
 struct Exchange {
   Exec x;
-  Runner r;
   b200_engine* e;
   std::string job;
   int64_t stage;
@@ -4147,34 +4052,19 @@ struct Exchange {
     NcclApi& N = NcclApi::get();
     const int W = e->world, me = e->rank;
     // ---- local pieces: one (coalesced) piece per partition ------------------------------------------------
-    struct Local {
-      int p;
-      Piece piece;
-    };
-    std::vector<Local> locals;
+    std::vector<StoredPiece> locals;
     {
-      std::vector<std::pair<int, std::vector<Piece>>> snap;
-      {
-        std::lock_guard<std::mutex> g(e->mu);
-        for (int p = 0; p < P; p++) {
-          auto it = e->shuffle.find(ShuffleKey{job, stage, (int64_t)p});
-          if (it == e->shuffle.end()) continue;
-          std::vector<Piece> mine;
-          for (auto& pc : it->second)
-            if (pc.src_rank == me && pc.r1 > pc.r0) mine.push_back(pc);
-          if (!mine.empty()) snap.push_back({p, mine});
-        }
-      }
+      std::map<int64_t, std::vector<Piece>> snap;
+      for (auto& sp : e->shuffle.of_rank(job, stage, me))
+        if (sp.part >= 0 && sp.part < P && sp.piece.r1 > sp.piece.r0) snap[sp.part].push_back(sp.piece);
       for (auto& kv : snap) {
         if (kv.second.size() == 1) {
-          locals.push_back(Local{kv.first, kv.second[0]});
+          locals.push_back(StoredPiece{kv.first, kv.second[0]});
           continue;
         }
-        std::vector<std::pair<DevBatchPtr, std::pair<int64_t, int64_t>>> v;
-        for (auto& pc : kv.second) v.push_back({pc.batch, {pc.r0, pc.r1}});
         Piece c;
         c.file_id = kv.second[0].file_id;
-        c.batch = r.concat_slices(v, schema);
+        c.batch = concat_slices(x, kv.second, schema);
         c.r0 = 0;
         c.r1 = c.batch->n;
         c.src_rank = me;
@@ -4185,7 +4075,7 @@ struct Exchange {
           for (auto& pc : kv.second)
             for (size_t k = 0; k < c.str_bytes.size(); k++) c.str_bytes[k] += pc.str_bytes[k];
         }
-        locals.push_back(Local{kv.first, c});
+        locals.push_back(StoredPiece{kv.first, c});
       }
     }
     // string bytes of every outgoing slice must be known on the host (they normally are: the writer recorded them)
@@ -4197,7 +4087,7 @@ struct Exchange {
         DevBatch sl;
         sl.n = L.piece.r1 - L.piece.r0;
         for (auto& c : L.piece.batch->cols) sl.cols.push_back(slice_column(c, L.piece.r0, L.piece.r1));
-        L.piece.str_bytes = r.string_bytes(sl);
+        L.piece.str_bytes = string_bytes(x, sl);
       }
     }
     if (W <= 1) {
@@ -4210,7 +4100,7 @@ struct Exchange {
     // ---- compose headers and the payload layout per destination -----------------------------------------------
     struct Out {
       std::vector<ExchEntry> entries;
-      std::vector<const Local*> src;
+      std::vector<const StoredPiece*> src;
       uint64_t payload = 0;
       bool inl = true;
     };
@@ -4219,9 +4109,9 @@ struct Exchange {
       if (d == me) continue;
       Out& o = outs[(size_t)d];
       for (auto& L : locals) {
-        if (!goes_to(L.p, d)) continue;
+        if (!goes_to((int)L.part, d)) continue;
         ExchEntry en;
-        en.partition = L.p;
+        en.partition = L.part;
         en.file_id = L.piece.file_id;
         en.rows = L.piece.r1 - L.piece.r0;
         size_t si = 0;
@@ -4343,8 +4233,7 @@ struct Exchange {
     // ---- parse, allocate, round 2 ------------------------------------------------------------------------------
     struct RecvOp { void* ptr; uint64_t bytes; int peer; };
     std::vector<RecvOp> recvs;
-    struct Incoming { int p; Piece piece; };
-    std::vector<Incoming> incoming;
+    std::map<int64_t, std::vector<Piece>> incoming;
     uint64_t recvd = 0;
     for (int d = 0; d < W; d++) {
       if (d == me) continue;
@@ -4393,15 +4282,7 @@ struct Exchange {
           }
           b->cols.push_back(col);
         }
-        Incoming in;
-        in.p = (int)part;
-        in.piece.file_id = fid;
-        in.piece.batch = b;
-        in.piece.r0 = 0;
-        in.piece.r1 = rows;
-        in.piece.src_rank = d;
-        in.piece.str_bytes = sb;
-        incoming.push_back(in);
+        incoming[part].push_back(Piece{fid, b, 0, rows, d, sb});
       }
     }
     if (!sends.empty() || !recvs.empty()) {
@@ -4412,19 +4293,11 @@ struct Exchange {
       count_launches();
     }
     // ---- install ---------------------------------------------------------------------------------------------
-    {
-      std::lock_guard<std::mutex> g(e->mu);
-      for (int p = 0; p < P; p++) {
-        if (goes_to(p, me)) continue;
-        e->shuffle.erase(ShuffleKey{job, stage, (int64_t)p});  // handed over to its owner
-      }
-      for (auto& in : incoming) {
-        auto& v = e->shuffle[ShuffleKey{job, stage, (int64_t)in.p}];
-        v.erase(std::remove_if(v.begin(), v.end(), [&](const Piece& pc) { return pc.src_rank == in.piece.src_rank && pc.file_id == in.piece.file_id; }), v.end());
-        v.push_back(in.piece);
-        std::stable_sort(v.begin(), v.end(), [](const Piece& a, const Piece& b) { return a.src_rank != b.src_rank ? a.src_rank < b.src_rank : a.file_id < b.file_id; });
-      }
-    }
+    std::vector<int64_t> handed_over;
+    for (int p = 0; p < P; p++)
+      if (!goes_to(p, me)) handed_over.push_back(p);
+    e->shuffle.remove_parts(job, stage, handed_over);
+    e->shuffle.install(job, stage, incoming);
     *sent_out = sent;
     *recv_out = recvd;
   }
@@ -5459,7 +5332,7 @@ void b200_engine_destroy(b200_engine* e) {
   cudaSetDevice(e->device);
   cudaStreamSynchronize(e->stream);
   e->tables.clear();
-  e->shuffle.clear();
+  e->shuffle.remove_all();
   cudaStreamSynchronize(e->stream);
   for (auto& sl : e->nslot) {
     if (sl.pinned) cudaFreeHost(sl.pinned);
@@ -5543,10 +5416,9 @@ int b200_engine_register_batch(b200_engine* e, const char* table, int partition,
       if (!prev) slot = b;
     }
     if (prev) {  // append
-      Runner r{x, ""};
       Schema s;
       for (auto& c : prev->cols) s.push_back(Field{c.name, c.type, true});
-      DevBatchPtr cat = r.concat({prev, b}, s);
+      DevBatchPtr cat = concat(x, {prev, b}, s);
       // registered tables keep the canonical Arrow layout (concat leaves strings as views) and their companion images
       for (auto& c : cat->cols) c = as_utf8(x, c);
       build_column_images(x, *cat);
@@ -6007,20 +5879,7 @@ int b200_stage_execute(b200_stage* s, int input_partition, const volatile int32_
       Exec::abandon();
       // a cancelled or failed task leaves nothing behind (Executor::cancel_task drops the future together with
       // its partial outputs, executor.rs:217-237): remove whatever this task already stored
-      {
-        std::lock_guard<std::mutex> g(s->eng->mu);
-        for (auto it = s->eng->shuffle.begin(); it != s->eng->shuffle.end();) {
-          if (it->first.job == s->job_id && it->first.stage == s->stage_id) {
-            auto& v = it->second;
-            v.erase(std::remove_if(v.begin(), v.end(), [&](const Piece& pc) { return (pc.file_id == input_partition || (pc.file_id < 0 && it->first.part == input_partition)) && pc.src_rank == s->eng->rank; }), v.end());
-            if (v.empty()) {
-              it = s->eng->shuffle.erase(it);
-              continue;
-            }
-          }
-          ++it;
-        }
-      }
+      s->eng->shuffle.remove_task(s->job_id, s->stage_id, input_partition, s->eng->rank);
       throw;
     }
     if ((int)res.size() > cap) throw EngineError(B200_ERR_INVALID, "output array too small");
@@ -6050,7 +5909,7 @@ int b200_stage_execute_exchange(b200_stage* s, int input_partition, const volati
         recvd = fx.recvd;
       } else if (e->world > 1) {
         // two-step path (strings in the payload, no window, or a window too small for this exchange)
-        Exchange ex{x, Runner{x, s->job_id}, e, s->job_id, s->stage_id, (int)s->plan->n_out_partitions, EXCH_HASH, 0, s->plan->schema, s->plan->schema.size()};
+        Exchange ex{x, e, s->job_id, s->stage_id, (int)s->plan->n_out_partitions, EXCH_HASH, 0, s->plan->schema, s->plan->schema.size()};
         ex.run(&sent, &recvd);
       }
     } catch (...) {
@@ -6093,57 +5952,38 @@ int b200_partition_export(b200_engine* e, const char* job_id, int64_t stage_id, 
   ScopeTimer tm("partition_export");
   return guard(e, [&] {
     CUDA_CHECK(cudaSetDevice(e->device));
-    std::vector<std::pair<DevBatchPtr, std::pair<int64_t, int64_t>>> pieces;
-    {
-      std::lock_guard<std::mutex> g(e->mu);
-      auto it = e->shuffle.find(ShuffleKey{job_id, stage_id, out_partition});
-      if (it == e->shuffle.end()) throw EngineError(B200_ERR_NOT_FOUND, "no such shuffle partition");  // -> FetchFailed
-      for (auto& p : it->second) pieces.push_back({p.batch, {p.r0, p.r1}});
-    }
+    const std::vector<Piece> pieces = e->shuffle.pieces(ShuffleKey{job_id, stage_id, out_partition});
+    if (pieces.empty()) throw EngineError(B200_ERR_NOT_FOUND, "no such shuffle partition");  // -> FetchFailed
     Exec x{e, nullptr, nullptr};
     if (pieces.size() == 1) {
-      export_batch(x, *pieces[0].first, pieces[0].second.first, pieces[0].second.second, out, out_schema);
+      export_batch(x, *pieces[0].batch, pieces[0].r0, pieces[0].r1, out, out_schema);
       return;
     }
-    Runner r{x, job_id};
     Schema s;
-    for (auto& c : pieces[0].first->cols) s.push_back(Field{c.name, c.type, true});
-    DevBatchPtr cat = r.concat_slices(pieces, s);
+    for (auto& c : pieces[0].batch->cols) s.push_back(Field{c.name, c.type, true});
+    DevBatchPtr cat = concat_slices(x, pieces, s);
     export_batch(x, *cat, 0, cat->n, out, out_schema);
   });
 }
 
 int64_t b200_partition_rows(b200_engine* e, const char* job_id, int64_t stage_id, int out_partition) {
-  std::lock_guard<std::mutex> g(e->mu);
-  auto it = e->shuffle.find(ShuffleKey{job_id, stage_id, out_partition});
-  if (it == e->shuffle.end()) return -1;
-  int64_t n = 0;
-  for (auto& p : it->second) n += p.r1 - p.r0;
-  return n;
+  return e->shuffle.rows(ShuffleKey{job_id, stage_id, out_partition});
 }
 
 int b200_remove_job_data(b200_engine* e, const char* job_id) {
   return guard([&] {
     CUDA_CHECK(cudaSetDevice(e->device));
     std::lock_guard<std::mutex> g(e->mu);
-    for (auto it = e->shuffle.begin(); it != e->shuffle.end();) {
-      if (it->first.job == job_id) it = e->shuffle.erase(it);
-      else ++it;
-    }
     // partitions that arrived through the fused shuffle live in the exchange window: it is recycled as a whole once no
     // stored partition can refer to it any more (peers write into it only inside a collective this executor takes part in)
-    if (e->shuffle.empty()) e->win_used = 0;
+    if (e->shuffle.remove_job(job_id)) e->win_used = 0;
   });
 }
 
 int b200_remove_stage_data(b200_engine* e, const char* job_id, int64_t stage_id) {
   return guard([&] {
     CUDA_CHECK(cudaSetDevice(e->device));
-    std::lock_guard<std::mutex> g(e->mu);
-    for (auto it = e->shuffle.begin(); it != e->shuffle.end();) {
-      if (it->first.job == job_id && it->first.stage == stage_id) it = e->shuffle.erase(it);
-      else ++it;
-    }
+    e->shuffle.remove_stage(job_id, stage_id);
   });
 }
 
@@ -6220,7 +6060,7 @@ int b200_exchange_stage(b200_engine* e, const char* job_id, int64_t stage_id, in
     CUDA_CHECK(cudaSetDevice(e->device));
     Json j = parse_json(schema_json, strlen(schema_json));
     Exec x{e, nullptr, nullptr};
-    Exchange ex{x, Runner{x, job_id}, e, job_id, stage_id, n_out_partitions, mode, root, parse_schema(j), 0};
+    Exchange ex{x, e, job_id, stage_id, n_out_partitions, mode, root, parse_schema(j), 0};
     ex.ncols = ex.schema.size();
     uint64_t sent = 0, recvd = 0;
     try {
@@ -6363,15 +6203,7 @@ int b200_shuffle_write_files(b200_engine* e, const char* job_id, int64_t stage_i
     if (!e || !job_id || !work_dir) throw EngineError(B200_ERR_INVALID, "null argument");
     CUDA_CHECK(cudaSetDevice(e->device));
     Exec x{e, nullptr, nullptr};
-    struct Item { int64_t part; Piece piece; };
-    std::vector<Item> items;
-    {
-      std::lock_guard<std::mutex> g(e->mu);
-      for (auto& kv : e->shuffle)
-        if (kv.first.job == job_id && kv.first.stage == stage_id)
-          for (auto& pc : kv.second)
-            if (pc.src_rank == e->rank) items.push_back(Item{kv.first.part, pc});
-    }
+    std::vector<StoredPiece> items = e->shuffle.of_rank(job_id, stage_id, e->rank);
     const std::string base = std::string(work_dir) + "/" + job_id + "/" + std::to_string(stage_id);
     uint64_t nfiles = 0, nbytes = 0;
     const int64_t bs = e->batch_size;
@@ -6389,7 +6221,7 @@ int b200_shuffle_write_files(b200_engine* e, const char* job_id, int64_t stage_i
       }
     } else {
       // one consolidated file per map task: [schema-only stream][partition 0 streams][partition 1 streams]... + index
-      std::map<int64_t, std::vector<Item*>> by_task;
+      std::map<int64_t, std::vector<StoredPiece*>> by_task;
       for (auto& it : items) by_task[it.piece.file_id].push_back(&it);
       for (auto& kv : by_task) {
         if (kv.first < 0) throw EngineError(B200_ERR_INVALID, "sort-shuffle layout needs a file id (un-partitioned stage output)");
@@ -6398,7 +6230,7 @@ int b200_shuffle_write_files(b200_engine* e, const char* job_id, int64_t stage_i
         bool header = false;
         std::vector<std::vector<HostCol>> parts((size_t)n_out_partitions);
         std::vector<int64_t> rows((size_t)n_out_partitions, 0);
-        for (Item* it : kv.second) {
+        for (StoredPiece* it : kv.second) {
           if (it->part >= n_out_partitions) throw EngineError(B200_ERR_INVALID, "stored partition id beyond n_out_partitions");
           parts[(size_t)it->part] = download_batch(x, *it->piece.batch, it->piece.r0, it->piece.r1);
           rows[(size_t)it->part] = it->piece.r1 - it->piece.r0;
@@ -6474,17 +6306,8 @@ int b200_shuffle_read_file(b200_engine* e, const char* job_id, int64_t stage_id,
     std::vector<int64_t> sb;
     for (auto& c : b->cols)
       if (c.type.id == TypeId::Utf8) sb.push_back(c.chars_bytes);
-    std::lock_guard<std::mutex> g(e->mu);
-    auto& v = e->shuffle[ShuffleKey{job_id, stage_id, out_partition}];
-    v.erase(std::remove_if(v.begin(), v.end(), [&](const Piece& pc) { return pc.file_id == file_id && pc.src_rank == -1; }), v.end());
-    Piece pc;
-    pc.file_id = file_id;
-    pc.batch = b;
-    pc.r0 = 0;
-    pc.r1 = n;
-    pc.src_rank = -1;  // came from a file, not from one of the box's GPU executors
-    pc.str_bytes = sb;
-    v.push_back(pc);
+    // src_rank -1: came from a file, not from one of the box's GPU executors
+    e->shuffle.store(ShuffleKey{job_id, stage_id, out_partition}, Piece{file_id, b, 0, n, -1, sb}, true);
   });
 }
 
