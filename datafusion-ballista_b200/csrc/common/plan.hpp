@@ -210,7 +210,8 @@ inline DataType int_as_decimal(const DataType& t) {
 
 enum class BinOp : uint8_t {
   Add, Sub, Mul, Div, Mod, Eq, Ne, Lt, Le, Gt, Ge, And, Or, BitAnd, BitOr, BitXor, Shl, Shr,
-  RegexMatch, RegexIMatch, RegexNotMatch, RegexNotIMatch  // ~  ~*  !~  !~*
+  RegexMatch, RegexIMatch, RegexNotMatch, RegexNotIMatch,  // ~  ~*  !~  !~*
+  StringConcat                                             // ||
 };
 
 inline BinOp parse_binop(const std::string& s) {
@@ -221,7 +222,7 @@ inline BinOp parse_binop(const std::string& s) {
       {">=", BinOp::Ge},  {"and", BinOp::And}, {"or", BinOp::Or},  {"AND", BinOp::And},
       {"OR", BinOp::Or},  {"&", BinOp::BitAnd}, {"|", BinOp::BitOr}, {"^", BinOp::BitXor},
       {"<<", BinOp::Shl}, {">>", BinOp::Shr}, {"~", BinOp::RegexMatch}, {"~*", BinOp::RegexIMatch},
-      {"!~", BinOp::RegexNotMatch}, {"!~*", BinOp::RegexNotIMatch}};
+      {"!~", BinOp::RegexNotMatch}, {"!~*", BinOp::RegexNotIMatch}, {"||", BinOp::StringConcat}};
   for (auto& kv : tab)
     if (s == kv.first) return kv.second;
   throw std::runtime_error("plan IR: unknown binary operator '" + s + "'");
@@ -230,7 +231,7 @@ inline bool is_arith(BinOp o) { return o <= BinOp::Mod; }
 inline bool is_compare(BinOp o) { return o >= BinOp::Eq && o <= BinOp::Ge; }
 inline bool is_logic(BinOp o) { return o == BinOp::And || o == BinOp::Or; }
 inline bool is_bitwise(BinOp o) { return o >= BinOp::BitAnd && o <= BinOp::Shr; }
-inline bool is_regex(BinOp o) { return o >= BinOp::RegexMatch; }
+inline bool is_regex(BinOp o) { return o >= BinOp::RegexMatch && o <= BinOp::RegexNotIMatch; }
 
 // Grouping sets (ROLLUP / CUBE / GROUPING SETS) and the bitwise operators DataFusion rewrites GROUPING() into are typed
 // here for every consumer of the plan IR, but only a consumer built with B200_PLAN_GROUPING_SETS=1 computes them (the
@@ -443,6 +444,21 @@ inline void type_regex(Expr& e, const std::string& what, const ExprPtr& pattern,
   e.regex = d;
 }
 
+// concat, `||`, concat_ws, repeat and reverse are typed here for every consumer of the plan IR, but only a consumer built
+// with B200_PLAN_STRINGS=1 computes them (the device engine: Makefile NVFLAGS).  Semantics: DESIGN.md §6 (xi).  Their
+// arguments are the ones DataFusion's planner leaves after its casts (Utf8; repeat's count Int64).
+#ifndef B200_PLAN_STRINGS
+#define B200_PLAN_STRINGS 0
+#endif
+inline bool is_string_builder(const std::string& f) { return f == "concat" || f == "concat_ws" || f == "repeat" || f == "reverse"; }
+// string functions whose reference semantics this engine does not restate: refused by name
+inline bool is_refused_string_fn(const std::string& f) {
+  static const char* const names[] = {"lpad", "rpad", "to_hex", "to_char", "left", "right", "split_part", "translate", "initcap"};
+  for (const char* n : names)
+    if (f == n) return true;
+  return false;
+}
+
 // Result type and nullability of a scalar function call (DESIGN.md §3, rules [EXT] in §6).  A known function over an
 // argument type it does not take is refused with PlanUnsupported naming the type; an unknown name or a wrong argument
 // count is a malformed plan.
@@ -528,6 +544,27 @@ inline void type_scalar_fn(Expr& e) {
     if (n == 2) need_utf8(1);
     e.type = DataType(TypeId::Utf8);
     e.nullable = any_nullable();
+  } else if (is_string_builder(f)) {
+    if (!B200_PLAN_STRINGS) throw PlanUnsupported(f + " is not computed by this consumer of the plan IR");
+    if (f == "concat") {
+      if (n == 0) throw std::runtime_error("plan IR: concat takes at least one argument");
+    } else if (f == "concat_ws") {
+      if (n < 2) throw std::runtime_error("plan IR: concat_ws takes at least two arguments");
+    } else {
+      arity(f == "repeat" ? 2 : 1, f == "repeat" ? 2 : 1);
+    }
+    for (size_t i = 0; i < n; i++) {
+      if (f == "repeat" && i == 1) {
+        if (arg_t(1).id != TypeId::Int64 && arg_t(1).id != TypeId::Null) refuse(1);
+      } else {
+        need_utf8(i);
+      }
+    }
+    e.type = DataType(TypeId::Utf8);
+    // concat skips NULL arguments (never NULL); concat_ws is NULL iff its separator is
+    e.nullable = f == "concat" ? false : f == "concat_ws" ? e.args[0]->nullable : any_nullable();
+  } else if (is_refused_string_fn(f)) {
+    throw PlanUnsupported("scalar function " + f + " is not supported by the device engine");
   } else {
     throw std::runtime_error("plan IR: unknown scalar function '" + f + "'");
   }
@@ -566,6 +603,14 @@ inline ExprPtr parse_expr(const Json& j, const Schema& in) {
       const int k = (int)e->op - (int)BinOp::RegexMatch;
       e->negated = e->op == BinOp::RegexNotMatch || e->op == BinOp::RegexNotIMatch;
       type_regex(*e, std::string("the operator ") + names[k], e->args[1], nullptr, e->op == BinOp::RegexIMatch || e->op == BinOp::RegexNotIMatch);
+      return e;
+    }
+    if (e->op == BinOp::StringConcat) {
+      if (!B200_PLAN_STRINGS) throw PlanUnsupported("the operator || is not computed by this consumer of the plan IR");
+      for (const DataType* t : {&a, &b})
+        if (!t->is_string() && t->id != TypeId::Null) throw PlanUnsupported("the operator || does not support an operand of type " + t->str());
+      e->type = DataType(TypeId::Utf8);
+      e->nullable = e->args[0]->nullable || e->args[1]->nullable;
       return e;
     }
     if (is_bitwise(e->op)) {

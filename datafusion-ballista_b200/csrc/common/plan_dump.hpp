@@ -19,7 +19,7 @@ inline std::string dump_schema(const Schema& s) {
 }
 
 inline std::string dump_expr(const ExprPtr& e) {
-  static const char* ops[] = {"+", "-", "*", "/", "%", "=", "!=", "<", "<=", ">", ">=", "and", "or", "&", "|", "^", "<<", ">>", "~", "~*", "!~", "!~*"};
+  static const char* ops[] = {"+", "-", "*", "/", "%", "=", "!=", "<", "<=", ">", ">=", "and", "or", "&", "|", "^", "<<", ">>", "~", "~*", "!~", "!~*", "||"};
   auto list = [&](size_t from) {
     std::string o = "[";
     for (size_t i = from; i < e->args.size(); i++) o += (i > from ? "," : "") + dump_expr(e->args[i]);

@@ -329,7 +329,8 @@ inline std::string binop_symbol(const std::string& op) {
       {"Eq", "="},     {"NotEq", "!="},   {"Lt", "<"},       {"LtEq", "<="},  {"Gt", ">"},   {"GtEq", ">="}, {"Plus", "+"},
       {"Minus", "-"},  {"Multiply", "*"}, {"Divide", "/"},   {"Modulo", "%"}, {"And", "and"}, {"Or", "or"},
       {"BitwiseAnd", "&"}, {"BitwiseOr", "|"}, {"BitwiseXor", "^"}, {"BitwiseShiftLeft", "<<"}, {"BitwiseShiftRight", ">>"},
-      {"RegexMatch", "~"}, {"RegexIMatch", "~*"}, {"RegexNotMatch", "!~"}, {"RegexNotIMatch", "!~*"}};
+      {"RegexMatch", "~"}, {"RegexIMatch", "~*"}, {"RegexNotMatch", "!~"}, {"RegexNotIMatch", "!~*"},
+      {"StringConcat", "||"}};
   for (auto& kv : tab)
     if (op == kv.first) return kv.second;
   throw Unsupported("binary operator " + op + " is not supported by the device engine");
@@ -403,7 +404,7 @@ inline std::string expr_json(const Msg& e) {
         return "{\"fn\":\"date_part_" + part + "\",\"args\":[" + expr_json(args[1]) + "]}";
       }
       if (name == "substr" || name == "substring") return "{\"fn\":\"substr\",\"args\":" + exprs_json(args) + "}";
-      // the scalar functions of DESIGN §3 that make no new string bytes, under the names the function registry resolves
+      // the scalar functions of DESIGN §3, under the names the function registry resolves
       static const std::pair<const char*, const char*> fns[] = {
           {"abs", "abs"},         {"round", "round"},       {"floor", "floor"},
           {"ceil", "ceil"},       {"nullif", "nullif"},     {"coalesce", "coalesce"},
@@ -411,7 +412,9 @@ inline std::string expr_json(const Msg& e) {
           {"length", "character_length"},                   {"octet_length", "octet_length"},
           {"starts_with", "starts_with"},                   {"ends_with", "ends_with"},
           {"btrim", "btrim"},     {"trim", "btrim"},        {"ltrim", "ltrim"},
-          {"rtrim", "rtrim"},     {"regexp_like", "regexp_like"}};
+          {"rtrim", "rtrim"},     {"regexp_like", "regexp_like"},
+          {"concat", "concat"},   {"concat_ws", "concat_ws"}, {"repeat", "repeat"},
+          {"reverse", "reverse"}};
       for (auto& kv : fns)
         if (name == kv.first) return "{\"fn\":\"" + std::string(kv.second) + "\",\"args\":" + exprs_json(args) + "}";
       throw Unsupported("scalar function " + name + " is not supported by the device engine");

@@ -692,6 +692,264 @@ __device__ __noinline__ void scalar_regex_op(const Lane L, const uint32_t active
 }
 
 // ------------------------------------------------------------------------------------------------
+// String builders (OP_CONCAT and up): every result is written into the launch's character arena.
+// Reservation: one 64-bit bump counter (RunStatus::arena_need), one atomic per warp per op and row slot.  A row whose
+// bytes do not fit writes nothing but still counts, so the counter ends at the exact need and the host re-runs the launch
+// with that capacity.  Such a row's view is "unwritten": {arena, need << 32}.  Every other reader takes the low 32 bits
+// (length 0, nothing to read); the builders read the need, so a result built over it counts its true size too.
+// ------------------------------------------------------------------------------------------------
+struct BuildSrc {
+  const uint8_t* p;
+  uint32_t len;
+  bool unwritten;
+};
+__device__ __noinline__ BuildSrc ld_build_src(const Lane L, const Operand o, int r) {
+  BuildSrc b;
+  if (o.kind == OPD_REG) {
+    const ulonglong2 x = ((const ulonglong2*)(L.regs + PROG.regs[o.idx].smem_off))[r * L.B + L.tid];
+    b.unwritten = (x.y >> 32) != 0;
+    b.p = (const uint8_t*)x.x;
+    b.len = b.unwritten ? (uint32_t)(x.y >> 32) : (uint32_t)x.y;
+    return b;
+  }
+  const StrRef s = ld1_str(L, o, r);
+  b.p = s.p;
+  b.len = s.len;
+  b.unwritten = false;
+  return b;
+}
+// warp-aggregated reservation of len bytes (0 for rows that build nothing); every lane of the warp calls it
+__device__ __forceinline__ unsigned long long arena_reserve(unsigned long long len) {
+  const unsigned mask = __activemask();
+  if (mask != 0xFFFFFFFFu) return atomicAdd(&PROG.status->arena_need, len);
+  const int lane = threadIdx.x & 31;
+  unsigned long long incl = len;
+#pragma unroll
+  for (int d = 1; d < 32; d <<= 1) {
+    const unsigned long long t = __shfl_up_sync(mask, incl, d);
+    if (lane >= d) incl += t;
+  }
+  unsigned long long base = 0;
+  if (lane == 31 && incl) base = atomicAdd(&PROG.status->arena_need, incl);
+  base = __shfl_sync(mask, base, 31);
+  return base + incl - len;
+}
+// destination of a row's bytes, or nullptr when they do not fit (or an input was unwritten): store_built then records
+// the need instead of a view
+__device__ __forceinline__ uint8_t* arena_at(unsigned long long base, unsigned long long len, bool unwritten) {
+  if (unwritten || base + len > PROG.arena_cap) return nullptr;
+  return PROG.arena + base;
+}
+__device__ __forceinline__ void store_built(const Lane L, const Operand dst, int r, const uint8_t* out, unsigned long long len) {
+  const ulonglong2 v = out ? make_ulonglong2((unsigned long long)out, len) : make_ulonglong2((unsigned long long)PROG.arena, len << 32);
+  ((ulonglong2*)(L.regs + PROG.regs[dst.idx].smem_off))[r * L.B + L.tid] = v;
+}
+__device__ __forceinline__ void copy_bytes(uint8_t* d, const uint8_t* s, uint32_t n) {
+  for (uint32_t i = 0; i < n; i++) d[i] = s[i];
+}
+__device__ __forceinline__ uint32_t u128_digits(u128 v) {
+  uint32_t n = 1;
+  while (v >= 10) {
+    v /= 10;
+    n++;
+  }
+  return n;
+}
+// the digits of v, right-aligned ending at `end`
+__device__ __forceinline__ void put_digits(uint8_t* end, u128 v, uint32_t n) {
+  for (uint32_t i = 0; i < n; i++) {
+    *--end = (uint8_t)('0' + (uint32_t)(v % 10));
+    v /= 10;
+  }
+}
+
+// CAST(x AS Utf8): arrow's display of integers, Decimal128 (exactly `scale` fractional digits) and Bool, and chrono's
+// %Y-%m-%d of a Date32 (4 digits within years 0..9999, else an explicit sign)
+struct ToStr {
+  uint32_t len;
+  bool neg;
+  u128 mag;     // integer / decimal magnitude; date: |year|
+  uint32_t nd;  // digits of mag
+  int64_t month, day;
+};
+__device__ __noinline__ ToStr to_str_shape(const Lane L, const VInstr& ins, int r) {
+  ToStr t;
+  t.neg = false;
+  t.month = t.day = 0;
+  if (ins.aux == TS_BOOL) {
+    t.mag = ld1_i64(L, ins.a, r) != 0;
+    t.len = t.mag ? 4 : 5;
+    t.nd = 0;
+    return t;
+  }
+  if (ins.aux == TS_DATE32) {
+    const int64_t y = civil_from_days_dev(ld1_i64(L, ins.a, r), &t.month, &t.day);
+    t.neg = y < 0;
+    t.mag = (u128)(y < 0 ? -y : y);
+    t.nd = u128_digits(t.mag);
+    if (t.nd < 4) t.nd = 4;
+    t.len = t.nd + 6 + ((y < 0 || y > 9999) ? 1 : 0);
+    return t;
+  }
+  i128 v;
+  if (ins.aux == TS_DEC128) v = ld1_i128(L, ins.a, r);
+  else if (ins.aux == TS_UINT64) v = (i128)(uint64_t)ld1_i64(L, ins.a, r);
+  else v = (i128)ld1_i64(L, ins.a, r);
+  t.neg = v < 0;
+  t.mag = t.neg ? (u128)0 - (u128)v : (u128)v;
+  t.nd = u128_digits(t.mag);
+  const uint32_t s = ins.aux == TS_DEC128 ? (uint32_t)ins.imm : 0;
+  if (s > 0 && t.nd <= s) t.nd = s + 1;  // 0.0ddd
+  t.len = t.nd + (t.neg ? 1 : 0) + (s > 0 ? 1 : 0);
+  return t;
+}
+__device__ __noinline__ void to_str_write(uint8_t* out, const ToStr& t, const VInstr& ins) {
+  if (ins.aux == TS_BOOL) {
+    const char* w = t.mag ? "true" : "false";
+    for (uint32_t i = 0; i < t.len; i++) out[i] = (uint8_t)w[i];
+    return;
+  }
+  uint8_t* end = out + t.len;
+  if (ins.aux == TS_DATE32) {
+    put_digits(end, (u128)t.day, 2);
+    end[-3] = '-';
+    put_digits(end - 3, (u128)t.month, 2);
+    end[-6] = '-';
+    put_digits(end - 6, t.mag, t.nd);
+    if (t.len > t.nd + 6) out[0] = t.neg ? '-' : '+';
+    return;
+  }
+  const uint32_t s = ins.aux == TS_DEC128 ? (uint32_t)ins.imm : 0;
+  if (s == 0) {
+    put_digits(end, t.mag, t.nd);
+  } else {
+    u128 p = 1;
+    for (uint32_t i = 0; i < s; i++) p *= 10;
+    put_digits(end, t.mag % p, s);
+    end[-(int)s - 1] = '.';
+    put_digits(end - s - 1, t.mag / p, t.nd - s);
+  }
+  if (t.neg) out[0] = '-';
+}
+
+// OP_CONCAT's i-th argument: eight per immediate, from the instruction's first one on
+__device__ __forceinline__ Operand build_arg(const int first, int i) {
+  const ImmDesc& d = PROG.imms[first + (i >> 3)];
+  const uint32_t w = (uint32_t)(((i & 7) < 4 ? d.lo : d.hi) >> (16 * (i & 3))) & 0xFFFFu;
+  Operand o;
+  o.kind = (uint8_t)(w >> 12);
+  o.vk = VK_STR;
+  o.idx = (uint16_t)(w & 0xFFFu);
+  return o;
+}
+
+// concat / || / concat_ws, repeat, reverse and the casts to Utf8: for each row slot, the live rows' lengths, one warp
+// reservation, then the bytes.  A thread that wrote bytes fences them before it goes on: a later instruction of the same
+// program may publish a view of them to other threads (a group key of the global table, a string MIN / MAX cell).
+__device__ __noinline__ void scalar_build_op(const Lane L, const uint32_t active, const int pc) {
+  const VInstr ins = PROG.code[pc];
+  uint32_t vout = 0xFFFFFFFFu;
+  int n = 0;
+  const int args = ins.imm;
+  if (ins.op == OP_CONCAT) {
+    n = (int)PROG.imms[args]._pad;
+    for (int i = 0; i < n; i++) {
+      if (ins.aux & BUILD_NULLS) vout &= fetch_valid(L, build_arg(args, i));
+    }
+    if (ins.aux & BUILD_WS) vout = fetch_valid(L, ins.a);
+  } else {
+    vout = fetch_valid(L, ins.a);
+    if (ins.b.kind != OPD_NONE) vout &= fetch_valid(L, ins.b);
+  }
+  const uint32_t live = active & vout;
+  bool wrote = false;
+#pragma unroll 1
+  for (int r = 0; r < VM_R; r++) {
+    const bool lv = (live >> r) & 1;
+    unsigned long long len = 0;
+    bool unwritten = false;
+    BuildSrc a;
+    a.len = 0;
+    a.unwritten = false;
+    int64_t times = 0;
+    ToStr ts;
+    if (lv) {
+      if (ins.op == OP_CONCAT) {
+        BuildSrc sep;
+        sep.len = 0;
+        sep.unwritten = false;
+        if (ins.aux & BUILD_WS) sep = ld_build_src(L, ins.a, r);
+        int present = 0;
+        for (int i = 0; i < n; i++) {
+          const Operand o = build_arg(args, i);
+          if (!((fetch_valid(L, o) >> r) & 1)) continue;
+          const BuildSrc x = ld_build_src(L, o, r);
+          len += x.len + (present ? sep.len : 0);
+          unwritten |= x.unwritten;
+          present++;
+        }
+        if (present > 1) unwritten |= sep.unwritten;
+        if (len > 0x7FFFFFFFull) raise(4);
+      } else if (ins.op == OP_REPEAT) {
+        a = ld_build_src(L, ins.a, r);
+        times = ld1_i64(L, ins.b, r);
+        if (times < 0) times = 0;
+        if (a.len && (uint64_t)times > 0x7FFFFFFFull / a.len) raise(5);
+        else len = (unsigned long long)a.len * (unsigned long long)times;
+        unwritten = a.unwritten;
+      } else if (ins.op == OP_REVERSE) {
+        a = ld_build_src(L, ins.a, r);
+        len = a.len;
+        unwritten = a.unwritten;
+      } else {
+        ts = to_str_shape(L, ins, r);
+        len = ts.len;
+        if (ins.aux == TS_DATE32 && (ts.mag > (ts.neg ? 262144u : 262143u))) raise(6);
+      }
+      if (len > 0x7FFFFFFFull) len = 0;  // the launch fails (raised above)
+    }
+    const unsigned long long base = arena_reserve(len);
+    uint8_t* out = lv ? arena_at(base, len, unwritten) : nullptr;
+    if (out && len) {
+      wrote = true;
+      if (ins.op == OP_CONCAT) {
+        BuildSrc sep;
+        sep.len = 0;
+        if (ins.aux & BUILD_WS) sep = ld_build_src(L, ins.a, r);
+        uint8_t* w = out;
+        bool first = true;
+        for (int i = 0; i < n; i++) {
+          const Operand o = build_arg(args, i);
+          if (!((fetch_valid(L, o) >> r) & 1)) continue;
+          if (!first) {
+            copy_bytes(w, sep.p, sep.len);
+            w += sep.len;
+          }
+          first = false;
+          const BuildSrc x = ld_build_src(L, o, r);
+          copy_bytes(w, x.p, x.len);
+          w += x.len;
+        }
+      } else if (ins.op == OP_REPEAT) {
+        for (int64_t k = 0; k < times; k++) copy_bytes(out + (uint64_t)k * a.len, a.p, a.len);
+      } else if (ins.op == OP_REVERSE) {
+        for (uint32_t i = 0; i < a.len;) {
+          // a sequence cut short (invalid UTF-8: nothing upstream of every source checks it) keeps its bytes as they are
+          const uint32_t k = min(utf8_seq_len(a.p[i]), a.len - i);
+          copy_bytes(out + a.len - i - k, a.p + i, k);
+          i += k;
+        }
+      } else {
+        to_str_write(out, ts, ins);
+      }
+    }
+    store_built(L, ins.dst, r, lv ? out : PROG.arena, lv ? len : 0);
+  }
+  if (wrote) __threadfence();
+  store_valid(L, ins.dst, vout);
+}
+
+// ------------------------------------------------------------------------------------------------
 // Cold operations: one rolled loop over the thread's rows; every body exists once in the binary.
 // ------------------------------------------------------------------------------------------------
 template <bool SFN>
@@ -701,6 +959,7 @@ __device__ __noinline__ void cold_op(const Lane L, const uint32_t active, const 
     if (op <= OP_CEIL) scalar_num_op(L, active, pc);
     else if (op == OP_NULLIF) scalar_nullif_op(L, active, pc);
     else if (op == OP_REGEX) scalar_regex_op(L, active, pc);
+    else if (op > OP_REGEX) scalar_build_op(L, active, pc);
     else if (op >= OP_BIT_AND) scalar_bit_op(L, active, pc);
     else scalar_str_op(L, active, pc);
     return;
@@ -1897,18 +2156,24 @@ __device__ __forceinline__ ulonglong2 atom_cas_b128(unsigned long long* p, ulong
 
 // string MIN / MAX of a table cell: compare-and-swap of the whole 16-byte view, no lock.  The cell only ever moves
 // towards the final answer, so a row that does not beat the value it last read can stop -- most rows issue no atomic.
-// (The characters a view points at never change, so relaxed ordering suffices.)  Kept apart from table_merge, which the
-// fused kernel's and the add-only register sink's flushes call: they never see a string accumulator.
+// Input characters never change during a launch, so relaxed ordering suffices for them; a string builder's bytes
+// (Program::arena) are written in the same launch by another thread, which fences them before it installs the view, so
+// a program that builds strings reads the cell with acquire (a fence after the load or the failed CAS) before it
+// compares bytes.  Kept apart from table_merge, which the fused kernel's and the add-only register sink's flushes call:
+// they never see a string accumulator.
 __device__ __noinline__ void table_merge_str(int kind, unsigned long long slot, int a, Acc128 x) {
   const AggTable& T = PROG.table;
   unsigned long long* cell = T.acc + ((unsigned long long)a * T.cap + slot) * 2;
   const bool is_min = kind == ACC_MIN_STR;
+  const bool acquire = PROG.arena != nullptr;
   ulonglong2 cur = ld_relaxed_b128(cell);
+  if (acquire) __threadfence();
   const ulonglong2 val = make_ulonglong2(x.lo, x.hi);
   while (str_beats(is_min, x.lo, x.hi, cur.x, cur.y)) {
     const ulonglong2 seen = atom_cas_b128(cell, cur, val);
     if (seen.x == cur.x && seen.y == cur.y) return;
     cur = seen;
+    if (acquire) __threadfence();
   }
 }
 

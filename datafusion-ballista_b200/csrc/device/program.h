@@ -85,8 +85,21 @@ enum VOp : uint8_t {
   OP_BIT_AND, OP_BIT_OR, OP_BIT_XOR, OP_SHL, OP_SHR,
   // regular expressions (scalar_regex_op): ILIKE, ~ / ~* / !~ / !~* and regexp_like.  a: STR -> BOOL; aux: 1 = negated;
   // imm: immediate with the DFA's device pointer in lo and its shape (csrc/common/regex_dfa.hpp dfa_shape_pack) in hi
-  OP_REGEX
+  OP_REGEX,
+  // string builders (scalar_build_op): each writes its result's bytes into the launch's character arena (Program::arena)
+  // and yields an ordinary {ptr, len} view.  Semantics: DESIGN.md §6 (xi).
+  OP_CONCAT,    // imm: first immediate of the argument operands (below); aux: BUILD_* flags; a: separator (BUILD_WS)
+  OP_REPEAT,    // a: STR, b: I64 count
+  OP_REVERSE,   // a: STR -> its code points in reverse order
+  OP_TO_STR     // CAST(a AS Utf8); aux = ToStrKind; imm = scale (TS_DEC128)
 };
+enum BuildFlags : uint8_t {
+  BUILD_NULLS = 1,  // `||`: NULL if any argument is NULL (else NULL arguments are skipped: concat, concat_ws)
+  BUILD_WS = 2      // concat_ws: operand a is the separator, written between the present arguments; NULL iff it is
+};
+enum ToStrKind : uint8_t { TS_INT = 0, TS_UINT64, TS_DEC128, TS_DATE32, TS_BOOL };
+// OP_CONCAT's arguments travel in consecutive immediates, eight per immediate: 16 bits each (kind << 12 | idx, all
+// VK_STR), four in lo and four in hi; the first immediate's _pad holds their count
 
 enum DatePart : uint8_t { DP_YEAR = 0, DP_QUARTER, DP_MONTH, DP_WEEK, DP_DAY, DP_DOY, DP_DOW };
 enum TrimSide : uint8_t { TRIM_BOTH = 0, TRIM_LEADING, TRIM_TRAILING };
@@ -197,6 +210,7 @@ struct RunStatus {
   unsigned long long in_active;  // rows that passed all filters
   unsigned int pack_overflow;    // OP_STR_PACK8 met a string longer than 7 bytes: re-lower without packing
   unsigned int _pad;             // (keeps the struct 8-byte aligned; the group-by kernel reports "outside my pattern" through pack_overflow too)
+  unsigned long long arena_need; // string builders: bytes reserved in the character arena, counted past its capacity
 };
 
 struct Program {
@@ -245,6 +259,9 @@ struct Program {
   uint8_t set_mask[32];
   uint64_t set_id[32];
   Operand key_hashes[VM_MAX_KEYS];
+  // string builders (OP_CONCAT and up): the launch's character arena; a reservation beyond arena_cap writes nothing
+  uint8_t* arena;
+  unsigned long long arena_cap;
 };
 
 // ---- fused fast path (scan -> filter -> decimal products -> <=4-group SUM/COUNT aggregate) -----------

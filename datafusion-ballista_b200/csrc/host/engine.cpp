@@ -102,6 +102,7 @@ struct b200_engine {
   std::atomic<uint64_t> narrowed_bytes_saved{0};         // PCIe bytes not sent thanks to narrowing (b200_engine_counter)
   std::atomic<uint64_t> n_window_sorts{0};               // sorts the window operator ran itself (b200_engine_counter)
   std::atomic<uint64_t> nlj_pairs{0};                    // (build row, probe row) pairs the nested-loop join evaluated (b200_engine_counter)
+  std::atomic<uint64_t> string_arena_retries{0};         // launches re-run because their character arena was too small
   std::atomic<uint64_t> host_syncs{0};                   // host waits on the stream inside tasks, exchanges and exports (host_wait)
   // parsed stage plans by plan text with the job id taken out (b200_stage_prepare): the next job that runs the same stage
   // plan shares the parsed tree instead of parsing and typing the JSON again.  Plans are read-only once parsed.
@@ -989,6 +990,9 @@ struct FusedPlan {
 static void throw_run_error(unsigned int error) {
   if (error == 1) throw EngineError(B200_ERR_EXECUTION, "Arithmetic overflow");
   if (error == 2) throw EngineError(B200_ERR_EXECUTION, "Divide by zero");
+  if (error == 4) throw EngineError(B200_ERR_EXECUTION, "concat: a result row is longer than 2147483647 bytes");
+  if (error == 5) throw EngineError(B200_ERR_EXECUTION, "repeat: a result row is longer than 2147483647 bytes");
+  if (error == 6) throw EngineError(B200_ERR_EXECUTION, "CAST(Date32 AS Utf8): a date outside chrono's range (years -262144..262143)");
   if (error) throw EngineError(B200_ERR_EXECUTION, "execution error in expression");
 }
 
@@ -1067,6 +1071,19 @@ RunOutcome launch_program(const Exec& x, PipelineBuilder& pb, int reg_groups, co
   DevPtr dstat = dev_alloc(sizeof(RunStatus), x.st());
   CUDA_CHECK(cudaMemsetAsync(dstat->ptr, 0, sizeof(RunStatus), x.st()));
   P.status = (RunStatus*)dstat->ptr;
+  // string builders: a character arena of its own for every launch (a second pass must not overwrite the bytes the
+  // first one published).  Its views join the outputs' lifetimes through pb.keep.  Without a sound bound the caller
+  // must learn the need, so the launch waits.
+  P.arena = nullptr;
+  P.arena_cap = 0;
+  if (pb.arena_ops) {
+    const uint64_t cap = pb.arena_capacity();
+    DevPtr arena = dev_alloc(cap + 16, x.st());
+    P.arena = (uint8_t*)arena->ptr;
+    P.arena_cap = cap;
+    pb.keep.push_back(arena);
+    if (!pb.arena_sound()) wait = true;
+  }
   DevPtr tstate;
   if (P.sink == SINK_MATERIALIZE) {
     const int64_t tile_rows = ff ? 1024 : (int64_t)pb.block * VM_R;
@@ -1157,13 +1174,15 @@ RunOutcome launch_program(const Exec& x, PipelineBuilder& pb, int reg_groups, co
   const RunStatus* hs = x.fetch<RunStatus>(dstat->ptr);
   const unsigned int* he = extra_fetch ? x.fetch<unsigned int>(extra_fetch) : nullptr;
   if (!wait) {
-    x.defer([hs, e0, e1, met, dstat, tstate]() {
+    const unsigned long long arena_cap = P.arena ? P.arena_cap : ~0ull;
+    x.defer([hs, e0, e1, met, dstat, tstate, arena_cap]() {
       float ms = 0;
       cudaEventElapsedTime(&ms, e0, e1);
       cudaEventDestroy(e0);
       cudaEventDestroy(e1);
       if (met) met->elapsed_ns += (uint64_t)(ms * 1e6);
       throw_run_error(hs->error);
+      if (hs->arena_need > arena_cap) throw EngineError(B200_ERR_EXECUTION, "string arena: the bytes built exceed their bound");
     });
     memset(&o.status, 0, sizeof o.status);
     return o;
@@ -1218,6 +1237,13 @@ DevBatchPtr run_materialize(const Exec& x, PipelineBuilder& pb, const std::vecto
   FastFilterSpec ffs;
   const bool use_ff = filters && match_fast_filter(P, ffs);
   RunOutcome r = launch_program(x, pb, 1, nullptr, filters, met, nullptr, nullptr, nullptr, use_ff ? &ffs : nullptr);
+  // the character arena was too small: run again with what it needed (the launch rewrites every output row).  The need
+  // is exact unless a CASE / COALESCE moved an unwritten intermediate, so the loop ends after one re-run in practice.
+  while (P.arena && r.status.arena_need > P.arena_cap) {
+    pb.arena_floor = r.status.arena_need;
+    x.e->string_arena_retries++;
+    r = launch_program(x, pb, 1, nullptr, filters, met, nullptr, nullptr, nullptr, use_ff ? &ffs : nullptr);
+  }
   out->n = filters ? (int64_t)r.status.out_rows : src->n;
   uint64_t wbytes = 0;
   for (auto& c : out->cols) {
@@ -2237,6 +2263,7 @@ DevBatchPtr run_aggregate(const Exec& x, const BuilderFactory& make_pb, const Pl
   unsigned int n_groups = 0;
   int reg_groups = 0;
   bool gb_bailed = false, pf_off = false, gs_grown = false;
+  uint64_t arena_floor = 0;  // string builders: the character arena an earlier attempt needed
   for (;;) {
     x.check_cancel();
     ScopeTimer t_iter("  agg: lower+alloc+launch+sync");
@@ -2244,6 +2271,7 @@ DevBatchPtr run_aggregate(const Exec& x, const BuilderFactory& make_pb, const Pl
     PipelineBuilder& pb = *pbp;
     L = AggLowered();
     lower_aggregate(pb, node, L, pack_mode);
+    pb.arena_floor = arena_floor;
     Program& P = pb.prog;
     P.n_keys = (uint8_t)n_keys;
     P.n_acc = (uint8_t)L.accs.size();
@@ -2341,6 +2369,11 @@ DevBatchPtr run_aggregate(const Exec& x, const BuilderFactory& make_pb, const Pl
       ScopeTimer t_l("    agg: launch_program (incl. sync)");
       ro = launch_program(x, pb, reg_groups, use_fused ? &fspec : nullptr, true, met, tm.T.n_groups, &n_groups, use_gb ? &gspec : nullptr);
     }
+    if (P.arena && ro.status.arena_need > P.arena_cap) {
+      arena_floor = ro.status.arena_need;  // the same table size again (re-allocated, so re-initialised) with that arena
+      x.e->string_arena_retries++;
+      continue;
+    }
     if (ro.status.pack_overflow && use_gb) {
       gb_bailed = true;  // operands outside the dedicated kernel's ranges: same table size on the general sink
       continue;
@@ -2371,6 +2404,7 @@ DevBatchPtr run_aggregate(const Exec& x, const BuilderFactory& make_pb, const Pl
     P.mom_pass = 1;
     RunOutcome r2 = launch_program(x, *pbp, reg_groups, nullptr, true, met);
     P.mom_pass = 0;
+    if (P.arena && r2.status.arena_need > P.arena_cap) throw EngineError(B200_ERR_EXECUTION, "aggregate: the second pass built more string bytes than the first");
     if (r2.status.overflow) throw EngineError(B200_ERR_EXECUTION, "aggregate: a group of the first pass was not found by the second");
   }
   {
@@ -5377,6 +5411,7 @@ uint64_t b200_engine_counter(b200_engine* e, const char* name) {
   if (n == "window_sorts") return e->n_window_sorts;
   if (n == "host_syncs") return e->host_syncs;
   if (n == "regex_compiles") return e->regex.compiles;
+  if (n == "string_arena_retries") return e->string_arena_retries;
   return 0;
 }
 

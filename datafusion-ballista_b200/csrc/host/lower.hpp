@@ -20,6 +20,7 @@ struct ColRef {
   bool nullable = false;
   std::string name;
   std::vector<DevPtr> keep;  // allocations a string value may point into
+  uint64_t str_bound = ~0ull;  // strings: bound on the bytes of all its rows in one launch (~0: unknown)
 };
 
 inline Operand mk_operand(uint8_t kind, uint8_t vk, int idx) {
@@ -67,6 +68,11 @@ class PipelineBuilder {
   std::vector<ColRef> cols;  // current (virtual) schema
   std::vector<DevPtr> keep;  // literal pools etc.
   int block = 512;
+  // string builders (OP_CONCAT and up): how many the program holds and the sum of their outputs' bounds (~0: some
+  // output has none); arena_floor: the need a previous launch of this program reported (launch_program sizes the arena)
+  int arena_ops = 0;
+  uint64_t arena_bound = 0;
+  uint64_t arena_floor = 0;
 
   PipelineBuilder(const DevBatch& src, cudaStream_t st, RegexCache* regex) : src_(src), st_(st), regex_(regex) {
     memset(&prog, 0, sizeof prog);
@@ -78,6 +84,7 @@ class PipelineBuilder {
       c.nullable = src.cols[i].valid != nullptr;
       c.name = src.cols[i].name;
       c.keep = src.cols[i].keep;
+      if (src.cols[i].phys == PH_UTF8 && src.cols[i].chars_bytes >= 0) c.str_bound = (uint64_t)src.cols[i].chars_bytes;
       lazy_src_.push_back((int)i);
       cols.push_back(c);
     }
@@ -140,7 +147,9 @@ class PipelineBuilder {
         return c;
       }
       case Expr::Lit: return literal(e.type, e.lit);
-      case Expr::Bin: return is_regex(e.op) ? compile_regex(e) : compile_bin(e);
+      case Expr::Bin:
+        if (e.op == BinOp::StringConcat) return compile_concat(e, 0, BUILD_NULLS);
+        return is_regex(e.op) ? compile_regex(e) : compile_bin(e);
       case Expr::Not: {
         ColRef a = compile(*e.args[0]);
         ColRef r = new_reg(DataType(TypeId::Bool), a.nullable);
@@ -230,6 +239,7 @@ class PipelineBuilder {
       }
       case Expr::Fn: {
         if (e.fn == "regexp_like") return compile_regex(e);
+        if (is_string_builder(e.fn)) return compile_build_fn(e);
         const int part = date_part_index(e.fn);
         if (part >= 0) return unary_fn(e, OP_DATE_PART, VK_I64, (uint8_t)part, 0);
         if (e.fn == "substr") {
@@ -237,6 +247,7 @@ class PipelineBuilder {
           ColRef s = compile(*e.args[1]);
           ColRef r = new_reg(e.type, a.nullable || s.nullable);
           r.keep = a.keep;
+          r.str_bound = a.str_bound;
           VInstr ins = blank(OP_SUBSTR, VK_STR);
           ins.a = resolve(a);
           ins.b = resolve(s);
@@ -279,11 +290,159 @@ class PipelineBuilder {
     return r;
   }
 
+  // ---- string builders: results written into the launch's character arena (DESIGN.md §4.1) ------------------------
+  static uint64_t sat_add(uint64_t a, uint64_t b) { return a > ~0ull - b ? ~0ull : a + b; }
+  static uint64_t sat_mul(uint64_t a, uint64_t b) { return b && a > ~0ull / b ? ~0ull : a * b; }
+  // a builder's result register; `bound`: at most that many bytes over the launch's rows (~0: unknown)
+  ColRef built_reg(bool nullable, uint64_t bound) {
+    ColRef r = new_reg(DataType(TypeId::Utf8), nullable);
+    r.str_bound = bound;
+    arena_ops++;
+    arena_bound = sat_add(arena_bound, bound);
+    return r;
+  }
+  // the arena a launch starts with: the sum of the builders' bounds when every one has a bound, else a guess the retry
+  // corrects (launch_program); never below what an earlier launch of this program needed
+  uint64_t arena_capacity() const {
+    const uint64_t first = arena_sound() ? arena_bound : std::min(sat_mul(rows(), 32 * (uint64_t)arena_ops), arena_first_cap());
+    return std::max<uint64_t>(std::max(first, arena_floor), 256);
+  }
+  // the first arena holds the builders' bound only up to max(64 bytes per row, 64 MiB): a bound over all input rows can be
+  // far above the need (a long literal behind a selective filter, repeat(s, 1000)); above it the launch starts from that
+  // size and learns the need (launch_program waits for it)
+  uint64_t arena_first_cap() const { return std::max<uint64_t>(sat_mul(rows(), 64), 64ull << 20); }
+  bool arena_sound() const { return arena_bound != ~0ull && arena_bound <= arena_first_cap(); }
+  uint64_t rows() const { return (uint64_t)std::max<int64_t>(prog.n_rows, 0); }
+  // concat(args[from..]) (NULL arguments skipped), concat_ws(args[0], args[1..]) (BUILD_WS) or a || b (BUILD_NULLS)
+  ColRef compile_concat(const Expr& e, size_t from, uint8_t flags) {
+    const bool ws = flags & BUILD_WS;
+    ColRef sep;
+    if (ws) {
+      sep = compile(*e.args[0]);
+      pin(sep);
+    }
+    std::vector<ColRef> parts;
+    auto drop_parts = [&]() {
+      for (auto& c : parts) {
+        unpin(c);
+        release(c);
+      }
+    };
+    uint64_t bound = 0;
+    bool nullable = false;
+    for (size_t i = from; i < e.args.size(); i++) {
+      ColRef a = compile(*e.args[i]);
+      if (a.type.id == TypeId::Null) {
+        if (!(flags & BUILD_NULLS)) continue;  // concat / concat_ws skip it
+        drop_parts();
+        return null_of(e.type);
+      }
+      pin(a);
+      parts.push_back(a);
+      bound = sat_add(bound, a.str_bound);
+      nullable = nullable || a.nullable;
+    }
+    if (ws) bound = sat_add(bound, sat_mul(sep.str_bound, parts.size() > 1 ? parts.size() - 1 : 0));
+    ColRef r = emit_concat(parts, ws ? &sep : nullptr, flags, bound, (flags & BUILD_NULLS) ? nullable : (ws && sep.nullable));
+    drop_parts();
+    if (ws) {
+      unpin(sep);
+      release(sep);
+    }
+    return r;
+  }
+  ColRef emit_concat(const std::vector<ColRef>& parts, const ColRef* sep, uint8_t flags, uint64_t bound, bool nullable) {
+    // the arguments in consecutive immediates, eight per immediate (program.h); the first holds their count
+    std::vector<ImmDesc> ds(std::max<size_t>((parts.size() + 7) / 8, 1));
+    memset(ds.data(), 0, ds.size() * sizeof(ImmDesc));
+    for (size_t i = 0; i < parts.size(); i++) {
+      const Operand o = resolve(parts[i]);
+      const uint64_t w = ((uint64_t)o.kind << 12) | o.idx;
+      ImmDesc& d = ds[i / 8];
+      ((i & 7) < 4 ? d.lo : d.hi) |= w << (16 * (i & 3));
+    }
+    ds[0]._pad = (uint32_t)parts.size();
+    if (prog.n_imms + (int)ds.size() > VM_MAX_IMMS) throw EngineError(B200_ERR_UNSUPPORTED, "too many literals in one pipeline");
+    const int imm = prog.n_imms;
+    for (auto& d : ds) prog.imms[prog.n_imms++] = d;
+    ColRef r = built_reg(nullable, bound);
+    VInstr ins = blank(OP_CONCAT, VK_STR);
+    ins.imm = imm;
+    ins.aux = flags;
+    if (sep) ins.a = resolve(*sep);
+    ins.dst = r.op;
+    ins.flags = IF_NULLCHK;
+    emit(ins);
+    return r;
+  }
+  ColRef compile_build_fn(const Expr& e) {
+    const std::string& f = e.fn;
+    if (f == "concat") return compile_concat(e, 0, 0);
+    if (f == "concat_ws") {
+      if (e.args[0]->type.id == TypeId::Null) return null_of(e.type);
+      return compile_concat(e, 1, BUILD_WS);
+    }
+    for (auto& a : e.args)
+      if (a->type.id == TypeId::Null) return null_of(e.type);
+    ColRef a = compile(*e.args[0]);
+    pin(a);
+    ColRef b;
+    uint64_t bound = a.str_bound;
+    if (f == "repeat") {
+      b = compile(*e.args[1]);
+      if (b.op.kind != OPD_IMM) bound = ~0ull;  // a column count: no bound, the launch's need decides
+      else bound = sat_mul(bound, (uint64_t)std::max<int64_t>((int64_t)prog.imms[b.op.idx].lo, 0));
+    }
+    unpin(a);
+    ColRef r = built_reg(a.nullable || b.nullable, bound);
+    VInstr ins = blank(f == "repeat" ? OP_REPEAT : OP_REVERSE, VK_STR);
+    ins.a = resolve(a);
+    if (f == "repeat") ins.b = resolve(b);
+    ins.dst = r.op;
+    ins.flags = IF_NULLCHK;
+    emit(ins);
+    release(a);
+    release(b);
+    return r;
+  }
+  // CAST(a AS Utf8) of the source types DESIGN.md §6 (xi) lists; each has a longest text, which bounds the arena
+  ColRef cast_to_utf8(const ColRef& a) {
+    const DataType& t = a.type;
+    uint8_t kind;
+    uint64_t widest;
+    if (t.is_signed_int() || t.is_unsigned_int()) {
+      kind = t.id == TypeId::UInt64 ? TS_UINT64 : TS_INT;
+      widest = 20;
+    } else if (t.is_decimal() && t.scale >= 0) {
+      kind = TS_DEC128;
+      widest = 41;
+    } else if (t.id == TypeId::Date32) {
+      kind = TS_DATE32;
+      widest = 13;
+    } else if (t.id == TypeId::Bool) {
+      kind = TS_BOOL;
+      widest = 5;
+    } else {
+      throw EngineError(B200_ERR_UNSUPPORTED, "cast " + t.str() + " -> Utf8");
+    }
+    ColRef r = built_reg(a.nullable, sat_mul(widest, (uint64_t)std::max<int64_t>(prog.n_rows, 0)));
+    VInstr ins = blank(OP_TO_STR, vk_of(t));
+    ins.a = resolve(a);
+    ins.dst = r.op;
+    ins.aux = kind;
+    ins.imm = kind == TS_DEC128 ? t.scale : 0;
+    ins.flags = IF_NULLCHK;
+    emit(ins);
+    release(a);
+    return r;
+  }
+
   // one-operand function: dst = op(a); string results are views into a's bytes
   ColRef unary_fn(const Expr& e, uint8_t op, uint8_t t, uint8_t aux, int32_t imm) {
     ColRef a = compile(*e.args[0]);
     ColRef r = new_reg(e.type, a.nullable);
     r.keep = a.keep;
+    r.str_bound = a.str_bound;
     VInstr ins = blank(op, t);
     ins.a = resolve(a);
     ins.dst = r.op;
@@ -672,6 +831,7 @@ class PipelineBuilder {
         idx = add_imm(d);
     }
     c.op = mk_operand(OPD_IMM, vk_of(t), idx);
+    if (t.pk() == PK::Str) c.str_bound = l.is_null ? 0 : sat_mul(l.s.size(), (uint64_t)std::max<int64_t>(prog.n_rows, 0));
     return c;
   }
   ColRef literal_bool(bool v) {
@@ -1104,6 +1264,7 @@ class PipelineBuilder {
       o.type = to;
       return o;
     }
+    if (to.id == TypeId::Utf8) return cast_to_utf8(a);
     throw EngineError(B200_ERR_UNSUPPORTED, "cast " + a.type.str() + " -> " + to.str());
   }
 };

@@ -131,6 +131,14 @@ def fn(name: str, *args: Json) -> Json:
     return {"fn": name, "args": list(args)}
 
 
+def str_concat(*xs: Json) -> Json:
+    """x0 || x1 || ...: Utf8 operands, NULL if any is NULL (left-associated, as DataFusion parses it)."""
+    out = xs[0]
+    for x in xs[1:]:
+        out = binop("||", out, x)
+    return out
+
+
 # ---- operators -----------------------------------------------------------------------------------
 def scan(table: str, schema: List[Json], projection: Optional[List[int]] = None) -> Json:
     n: Json = {"op": "DataSourceExec", "table": table, "schema": schema}
