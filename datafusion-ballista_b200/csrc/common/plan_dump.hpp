@@ -129,6 +129,7 @@ inline std::string dump_plan(const PlanNode& n) {
         o += ",\"mode\":" + pbp::jstr(n.partition_mode) + ",\"on\":[";
         for (size_t i = 0; i < n.on.size(); i++) o += std::string(i ? "," : "") + "[" + dump_expr(n.on[i].first) + "," + dump_expr(n.on[i].second) + "]";
         o += "]";
+        if (n.null_equals_null) o += ",\"null_equals_null\":true";
       }
       if (n.join_filter) o += ",\"filter\":" + dump_expr(n.join_filter);
       if (n.has_projection) o += ",\"projection\":" + dump_ints(n.projection);

@@ -544,6 +544,14 @@ inline std::string join_common_json(const Msg& m, uint32_t f_on, uint32_t f_type
   return o;
 }
 
+// NullEquality { NULL_EQUALS_NOTHING = 0, NULL_EQUALS_NULL = 1 } (datafusion_common.proto:98-101): with NULL_EQUALS_NULL a
+// NULL join key matches a NULL key (INTERSECT / EXCEPT, IS NOT DISTINCT FROM keys)
+inline std::string null_equality_json(const Msg& m, uint32_t f) {
+  const uint64_t v = m.u64(f);
+  if (v > 1) throw Unsupported("join null equality " + std::to_string(v));
+  return v == 1 ? ",\"null_equals_null\":true" : "";
+}
+
 inline std::string plan_json(const Msg& n, const std::string& override_job) {
   DepthGuard dg;
   const Entry* x = n.oneof({1, 2, 3, 4, 6, 7, 8, 9, 10, 11, 12, 13, 14, 15, 16, 17, 18, 19, 20, 21, 22, 23, 24, 25, 26, 27, 28, 29, 30, 31, 32, 33, 34, 35, 36, 37, 38});
@@ -688,11 +696,15 @@ inline std::string plan_json(const Msg& n, const std::string& override_job) {
       if (m.has(7)) o += ",\"input_schema\":" + schema_json(m.sub(7));
       return o + ",\"input\":" + in(4) + "}";
     }
-    case 9: {  // HashJoinExecNode { left = 1, right = 2, on = 3, join_type = 4, partition_mode = 6, filter = 8, projection = 9 } (:1134-1145)
+    case 9: {  // HashJoinExecNode { left = 1, right = 2, on = 3, join_type = 4, partition_mode = 6, null_equality = 7, filter = 8, projection = 9,
+               // null_aware = 10 } (:1134-1145)
       const uint64_t pm = m.u64(6);
       if (pm > 1) throw Unsupported("hash join partition mode Auto must be resolved by the planner");
-      std::string o = "{\"op\":\"HashJoinExec\",\"left\":" + in(1) + ",\"right\":" + in(2) + join_common_json(m, 3, 4, 8) + ",\"mode\":\"" +
-                      (pm == 0 ? "CollectLeft" : "Partitioned") + "\"";
+      // a null-aware anti join (NOT IN) returns nothing once the subquery side holds a NULL key anywhere; tasks here are
+      // independent, so no task can know that of a side spread over partitions
+      if (m.boolean(10)) throw Unsupported("null-aware hash join (NOT IN)");
+      std::string o = "{\"op\":\"HashJoinExec\",\"left\":" + in(1) + ",\"right\":" + in(2) + join_common_json(m, 3, 4, 8) + null_equality_json(m, 7) +
+                      ",\"mode\":\"" + (pm == 0 ? "CollectLeft" : "Partitioned") + "\"";
       const std::vector<uint64_t> proj = m.varints(9);
       if (!proj.empty()) o += ",\"projection\":" + u32_list_json(proj);
       return o + "}";
@@ -780,8 +792,10 @@ inline std::string plan_json(const Msg& n, const std::string& override_job) {
       if (m.i64(3, -1) >= 0) o += ",\"fetch\":" + std::to_string(m.i64(3));
       return o + "}";
     }
-    case 34: {  // SortMergeJoinExecNode { left = 1, right = 2, on = 3, join_type = 4, filter = 5, sort_options = 6 { asc = 2, nulls_first = 3 } } (:1433-1441)
-      std::string o = "{\"op\":\"SortMergeJoinExec\",\"left\":" + in(1) + ",\"right\":" + in(2) + join_common_json(m, 3, 4, 5) + ",\"sort_options\":[";
+    case 34: {  // SortMergeJoinExecNode { left = 1, right = 2, on = 3, join_type = 4, filter = 5, sort_options = 6 { asc = 2, nulls_first = 3 },
+                // null_equality = 7 } (:1433-1441)
+      std::string o = "{\"op\":\"SortMergeJoinExec\",\"left\":" + in(1) + ",\"right\":" + in(2) + join_common_json(m, 3, 4, 5) + null_equality_json(m, 7) +
+                      ",\"sort_options\":[";
       bool first = true;
       for (auto& so : m.subs(6)) {
         o += std::string(first ? "" : ",") + "{\"asc\":" + (so.boolean(2) ? "true" : "false") + ",\"nulls_first\":" + (so.boolean(3) ? "true" : "false") + "}";

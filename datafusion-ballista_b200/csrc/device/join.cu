@@ -171,7 +171,9 @@ void launch_join_probe2(const JoinKeys& K, bool exact, int mode, const JoinNode*
   else launch_probe_mode<false>(mode, g, K, nodes, heads, n_buckets - 1, probe_hash, n_probe, counter, cap, out_b, out_p, probe_mark, build_mark, st);
 }
 
-// exact comparison of every key column of build row bi and probe row pi (hash-tagged tables)
+// exact comparison of every key column of build row bi and probe row pi (hash-tagged tables).  Fixed-width keys compare
+// their bytes: Float32 / Float64 keys are equal when their bit patterns are, as the engine's `=` has it (NaN = NaN with
+// the same payload, -0.0 <> 0.0).  hash_f64 puts +-0.0 and every NaN in one bucket, which only costs a failed check.
 __device__ bool join_keys_equal(const JoinKeys& K, int64_t bi, int64_t pi) {
   for (int k = 0; k < K.n_keys; k++) {
     const KeyCol& b = K.build[k];
@@ -188,9 +190,6 @@ __device__ bool join_keys_equal(const JoinKeys& K, int64_t bi, int64_t pi) {
       const uint8_t *s = (const uint8_t*)x[0], *t = (const uint8_t*)y[0];
       for (uint32_t i = 0; i < (uint32_t)x[1]; i++)
         if (s[i] != t[i]) return false;
-    } else if (b.phys == PH_F64) {
-      const double x = ((const double*)b.data)[bi], y = ((const double*)p.data)[pi];
-      if (!(x == y || (x != x && y != y))) return false;
     } else {
       const uint8_t* x = (const uint8_t*)b.data + bi * b.width;
       const uint8_t* y = (const uint8_t*)p.data + pi * p.width;

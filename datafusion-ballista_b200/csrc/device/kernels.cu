@@ -518,103 +518,8 @@ void launch_bytes_to_bitmap(const uint8_t* bytes, uint8_t* bitmap, int64_t n, un
 }
 
 // ------------------------------------------------------------------------------------------------
-// Hash join (bucket-chained table on the build side; two-pass probe: count -> scan -> write)
+// Join output helpers (join_output in engine.cpp): row flags -> row indices, pair indices -> row marks
 // ------------------------------------------------------------------------------------------------
-__global__ void join_build_kernel(const uint64_t* build_hash, const uint8_t* build_ok, int64_t n, int32_t* heads, uint64_t mask, int32_t* next) {
-  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
-    if (build_ok && !build_ok[i]) {
-      next[i] = -1;
-      continue;
-    }
-    uint64_t b = mix64(build_hash[i]) & mask;
-    next[i] = atomicExch(&heads[b], (int32_t)i);
-  }
-}
-void launch_join_build(const uint64_t* build_hash, const uint8_t* build_ok, int64_t n_build, int32_t* heads, uint64_t n_buckets, int32_t* next,
-                       cudaStream_t st) {
-  launch_kernel(join_build_kernel, grid_for(n_build, 256, 4), 256, 0, st, build_hash, build_ok, n_build, heads, n_buckets - 1, next);
-}
-
-__device__ __forceinline__ bool key_cols_equal(const JoinKeys& K, int64_t bi, int64_t pi) {
-  for (int k = 0; k < K.n_keys; k++) {
-    const KeyCol& b = K.build[k];
-    const KeyCol& p = K.probe[k];
-    bool bv = !b.valid || b.valid[bi], pv = !p.valid || p.valid[pi];
-    if (!bv || !pv) {
-      if (K.null_equals_null && !bv && !pv) continue;
-      return false;
-    }
-    if (b.phys == PH_STRVIEW) {
-      const unsigned long long* x = (const unsigned long long*)b.data + 2 * bi;
-      const unsigned long long* y = (const unsigned long long*)p.data + 2 * pi;
-      if (x[1] != y[1]) return false;
-      const uint8_t *s = (const uint8_t*)x[0], *t = (const uint8_t*)y[0];
-      for (uint32_t i = 0; i < (uint32_t)x[1]; i++)
-        if (s[i] != t[i]) return false;
-    } else if (b.phys == PH_F64) {
-      double x = ((const double*)b.data)[bi], y = ((const double*)p.data)[pi];
-      if (!(x == y || (x != x && y != y))) return false;
-    } else {
-      const uint8_t* x = (const uint8_t*)b.data + bi * b.width;
-      const uint8_t* y = (const uint8_t*)p.data + pi * p.width;
-      switch (b.width) {
-        case 16:
-          if (((const uint64_t*)x)[0] != ((const uint64_t*)y)[0] || ((const uint64_t*)x)[1] != ((const uint64_t*)y)[1]) return false;
-          break;
-        case 8:
-          if (*(const uint64_t*)x != *(const uint64_t*)y) return false;
-          break;
-        case 4:
-          if (*(const uint32_t*)x != *(const uint32_t*)y) return false;
-          break;
-        case 2:
-          if (*(const uint16_t*)x != *(const uint16_t*)y) return false;
-          break;
-        default:
-          if (*x != *y) return false;
-      }
-    }
-  }
-  return true;
-}
-
-template <bool WRITE>
-__global__ void join_probe_kernel(JoinKeys K, const uint64_t* build_hash, const int32_t* heads, uint64_t mask, const int32_t* next,
-                                  const uint64_t* probe_hash, const uint8_t* probe_ok, int64_t n_probe, uint32_t* counts, uint8_t* build_mark,
-                                  const uint64_t* offsets, int64_t* out_b, int64_t* out_p) {
-  for (int64_t j = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; j < n_probe; j += (int64_t)gridDim.x * blockDim.x) {
-    uint32_t c = 0;
-    if (!probe_ok || probe_ok[j]) {
-      const uint64_t h = probe_hash[j];
-      uint64_t w = WRITE ? offsets[j] : 0;
-      for (int32_t i = heads[mix64(h) & mask]; i >= 0; i = next[i]) {
-        if (build_hash[i] != h) continue;
-        if (!key_cols_equal(K, i, j)) continue;
-        if (WRITE) {
-          out_b[w] = i;
-          out_p[w] = j;
-          w++;
-        } else {
-          c++;
-          if (build_mark) build_mark[i] = 1;
-        }
-      }
-    }
-    if (!WRITE) counts[j] = c;
-  }
-}
-void launch_join_probe_count(const JoinKeys& K, const uint64_t* build_hash, const int32_t* heads, uint64_t n_buckets, const int32_t* next,
-                             const uint64_t* probe_hash, const uint8_t* probe_ok, int64_t n_probe, uint32_t* counts, uint8_t* build_mark,
-                             cudaStream_t st) {
-  launch_kernel(join_probe_kernel<false>, grid_for(n_probe, 256, 2), 256, 0, st, K, build_hash, heads, n_buckets - 1, next, probe_hash, probe_ok, n_probe, counts,
-                                                                       build_mark, nullptr, nullptr, nullptr);
-}
-void launch_join_probe_write(const JoinKeys& K, const uint64_t* build_hash, const int32_t* heads, uint64_t n_buckets, const int32_t* next,
-                             const uint64_t* probe_hash, const uint8_t* probe_ok, int64_t n_probe, const uint64_t* offsets, int64_t* out_build_idx,
-                             int64_t* out_probe_idx, cudaStream_t st) {
-  launch_kernel(join_probe_kernel<true>, grid_for(n_probe, 256, 2), 256, 0, st, K, build_hash, heads, n_buckets - 1, next, probe_hash, probe_ok, n_probe, nullptr,
-                                                                      nullptr, offsets, out_build_idx, out_probe_idx);
-}
 __global__ void flag_to_u32_kernel(const uint8_t* flags, uint8_t want, uint32_t* out, int64_t n) {
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) out[i] = (flags[i] != 0) == (want != 0);
 }
@@ -627,12 +532,6 @@ __global__ void select_indices_kernel(const uint32_t* flag01, const uint64_t* of
 }
 void launch_select_indices(const uint32_t* flag01, const uint64_t* offs, int64_t* out_idx, int64_t n, cudaStream_t st) {
   launch_kernel(select_indices_kernel, grid_for(n, 256, 4), 256, 0, st, flag01, offs, out_idx, n);
-}
-__global__ void counts_to_flag_kernel(const uint32_t* counts, uint8_t* flags, int64_t n) {
-  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) flags[i] = counts[i] ? 1 : 0;
-}
-void launch_counts_to_flag(const uint32_t* counts, uint8_t* flags, int64_t n, cudaStream_t st) {
-  launch_kernel(counts_to_flag_kernel, grid_for(n, 256, 4), 256, 0, st, counts, flags, n);
 }
 __global__ void mark_from_idx_kernel(const int64_t* idx, int64_t n, uint8_t* marks) {
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)

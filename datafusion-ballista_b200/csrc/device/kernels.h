@@ -187,13 +187,6 @@ struct PackJob {
 };
 void launch_pack_jobs(const PackJob* jobs_dev, int n_jobs, cudaStream_t st);
 
-void launch_join_build(const uint64_t* build_hash, const uint8_t* build_ok, int64_t n_build, int32_t* heads, uint64_t n_buckets, int32_t* next, cudaStream_t st);
-// pass 1: counts per probe row (+ marks); pass 2: write pairs at offsets
-void launch_join_probe_count(const JoinKeys& K, const uint64_t* build_hash, const int32_t* heads, uint64_t n_buckets, const int32_t* next,
-                             const uint64_t* probe_hash, const uint8_t* probe_ok, int64_t n_probe, uint32_t* counts, uint8_t* build_mark, cudaStream_t st);
-void launch_join_probe_write(const JoinKeys& K, const uint64_t* build_hash, const int32_t* heads, uint64_t n_buckets, const int32_t* next,
-                             const uint64_t* probe_hash, const uint8_t* probe_ok, int64_t n_probe, const uint64_t* offsets,
-                             int64_t* out_build_idx, int64_t* out_probe_idx, cudaStream_t st);
 // ---- FilterExec + column projection without the tile VM (filter.cu) ------------------------------------------
 static const int FF_MAX_COLS = 16, FF_MAX_OPS = 48, FF_MAX_IMMS = 40, FF_MAX_OUT = 24;
 enum FfOpKind : uint8_t { FF_CMP = 0, FF_AND = 1, FF_OR = 2, FF_NOT = 3, FF_FILTER_REG = 4 };
@@ -278,7 +271,6 @@ void launch_join_probe2(const JoinKeys& K, bool exact, int mode, const JoinNode*
 // compaction helpers: indices of rows whose flag byte == want
 void launch_flag_to_u32(const uint8_t* flags, uint8_t want, uint32_t* out, int64_t n, cudaStream_t st);
 void launch_select_indices(const uint32_t* flag01, const uint64_t* offs, int64_t* out_idx, int64_t n, cudaStream_t st);
-void launch_counts_to_flag(const uint32_t* counts, uint8_t* flags, int64_t n, cudaStream_t st);
 void launch_mark_from_idx(const int64_t* idx, int64_t n, uint8_t* marks, cudaStream_t st);
 
 // ---- nested-loop join (nlj.cu) ------------------------------------------------------------------

@@ -3255,8 +3255,10 @@ struct Runner {
     // single probe partition.
     if (collect_left && emits_build_rows(n.join_type) && n_partitions(*n.children[1]) > 1)
       throw EngineError(B200_ERR_UNSUPPORTED, "CollectLeft hash join that emits build-side rows over more than one probe partition: plan it as Partitioned");
-    // one integer-like key: the table is keyed by the key itself (no hash column, no second look at the keys)
-    const bool exact = nk == 1 && exact_key(lk[0]->type) && lk[0]->type.id == rk[0]->type.id;
+    // one integer-like key: the table is keyed by the key itself (no hash column, no second look at the keys).  That
+    // table keeps NULL keys out, so a join where NULL matches NULL takes the hash-tagged table, whose key check
+    // (join_keys_equal) pairs two NULLs.
+    const bool exact = nk == 1 && exact_key(lk[0]->type) && lk[0]->type.id == rk[0]->type.id && !n.null_equals_null;
     JoinSide L = prepare_side(*n.children[0], part, collect_left, lk, !exact, met);
     JoinSide R = prepare_side(*n.children[1], part, false, rk, !exact, met);
     const int64_t nb = L.n, np = R.n;
@@ -3270,14 +3272,15 @@ struct Runner {
     for (size_t k = 0; k < nk; k++) {
       const DevColumn& b = L.keys[k];
       const DevColumn& p = R.keys[k];
-      if (b.phys != p.phys) throw EngineError(B200_ERR_UNSUPPORTED, "join key physical types differ (" + b.type.str() + " vs " + p.type.str() + "): add casts");
+      // the exact-key table compares 64-bit images of the values (jkey_image widens each side by its own width), so a key
+      // whose cast to the other side's type left its source column as it was (CAST(i32 AS i64)) still matches; the
+      // hash-tagged table compares key bytes and needs one physical type
+      if (!exact && b.phys != p.phys) throw EngineError(B200_ERR_UNSUPPORTED, "join key physical types differ (" + b.type.str() + " vs " + p.type.str() + "): add casts");
       K.build[k] = KeyCol{b.data, b.valid, (uint8_t)b.phys, (uint8_t)b.width()};
       K.probe[k] = KeyCol{p.data, p.valid, (uint8_t)p.phys, (uint8_t)p.width()};
       key_bytes_b += (uint64_t)b.width();
       key_bytes_p += (uint64_t)p.width();
     }
-    const bool exact_ok = exact && !(n.null_equals_null && (L.keys[0].valid || R.keys[0].valid));
-    if (exact && !exact_ok) throw EngineError(B200_ERR_UNSUPPORTED, "null_equals_null join on a nullable integer key");
     x.check_cancel();
     const uint64_t n_buckets = next_pow2((uint64_t)std::max<int64_t>(nb, 1) * 2);
     DevPtr heads = dev_alloc((size_t)n_buckets * 4, x.st());

@@ -219,13 +219,17 @@ def grouping_id(mask: Sequence[bool]) -> int:
 
 def hash_join(left: Json, right: Json, on: Sequence[Sequence[Json]], join_type: str = "Inner",
               mode: str = "CollectLeft", filter: Optional[Json] = None,
-              projection: Optional[List[int]] = None) -> Json:
+              projection: Optional[List[int]] = None, null_equals_null: bool = False) -> Json:
+    """HashJoinExecNode (datafusion.proto:1134-1144).  `null_equals_null`: a NULL key matches a NULL key
+    (NullEquality::NullEqualsNull, as DataFusion plans INTERSECT / EXCEPT and IS NOT DISTINCT FROM keys)."""
     n: Json = {"op": "HashJoinExec", "left": left, "right": right, "on": [list(p) for p in on],
                "join_type": join_type, "mode": mode}
     if filter is not None:
         n["filter"] = filter
     if projection is not None:
         n["projection"] = projection
+    if null_equals_null:
+        n["null_equals_null"] = True
     return n
 
 
@@ -242,7 +246,8 @@ def nested_loop_join(left: Json, right: Json, join_type: str = "Inner", filter: 
 
 
 def sort_merge_join(left: Json, right: Json, on: Sequence[Sequence[Json]], join_type: str = "Inner",
-                    filter: Optional[Json] = None, sort_options: Optional[Sequence[Json]] = None) -> Json:
+                    filter: Optional[Json] = None, sort_options: Optional[Sequence[Json]] = None,
+                    null_equals_null: bool = False) -> Json:
     """SortMergeJoinExecNode (datafusion.proto:1433): Ballista's default join strategy (extension.rs:683).
     Inputs are co-partitioned on the keys; the output is ordered by them."""
     n: Json = {"op": "SortMergeJoinExec", "left": left, "right": right, "on": [list(p) for p in on], "join_type": join_type}
@@ -250,6 +255,8 @@ def sort_merge_join(left: Json, right: Json, on: Sequence[Sequence[Json]], join_
         n["filter"] = filter
     if sort_options is not None:
         n["sort_options"] = list(sort_options)
+    if null_equals_null:
+        n["null_equals_null"] = True
     return n
 
 

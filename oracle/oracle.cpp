@@ -701,7 +701,9 @@ OCol eval(const Expr& e, const OBatch& b) {
 // ------------------------------------------------------------------------------------------------
 // Row key encoding (group-by / join keys)
 // ------------------------------------------------------------------------------------------------
-static inline bool encode_key_col(const OCol& c, size_t r, std::string& out) {
+// float_bits: floats are encoded by their bit pattern (join keys: equal when `=` says so, -0.0 <> 0.0, NaN = NaN only
+// with the same payload); otherwise +-0.0 and every NaN are one group key
+static inline bool encode_key_col(const OCol& c, size_t r, std::string& out, bool float_bits = false) {
   if (!c.is_valid(r)) {
     out.push_back('\0');
     return false;
@@ -712,8 +714,10 @@ static inline bool encode_key_col(const OCol& c, size_t r, std::string& out) {
     case PK::I64: out.append((const char*)&c.i[r], 8); break;
     case PK::F64: {
       double v = c.f[r];
-      if (v == 0.0) v = 0.0;
-      if (v != v) v = std::nan("");
+      if (!float_bits) {
+        if (v == 0.0) v = 0.0;
+        if (v != v) v = std::nan("");
+      }
       out.append((const char*)&v, 8);
       break;
     }
@@ -737,6 +741,12 @@ bool encode_key(const std::vector<const OCol*>& keys, size_t r, std::string& out
   out.clear();
   bool all_valid = true;
   for (auto* c : keys) all_valid &= encode_key_col(*c, r, out);
+  return all_valid;
+}
+static bool encode_join_key(const std::vector<OCol>& keys, size_t r, std::string& out) {  // same, floats by their bits
+  out.clear();
+  bool all_valid = true;
+  for (auto& c : keys) all_valid &= encode_key_col(c, r, out, true);
   return all_valid;
 }
 
@@ -1030,13 +1040,13 @@ OBatch do_hash_join(const PlanNode& node, const OBatch& L, const OBatch& R) {
   std::unordered_map<std::string, std::vector<int64_t>> table;
   std::string k;
   for (size_t r = 0; r < L.n; r++) {
-    bool allv = encode_key(lk, r, k);
+    bool allv = encode_join_key(lk, r, k);
     if (!allv && !node.null_equals_null) continue;
     table[k].push_back((int64_t)r);
   }
   std::vector<int64_t> li, ri;
   for (size_t r = 0; r < R.n; r++) {
-    bool allv = encode_key(rk, r, k);
+    bool allv = encode_join_key(rk, r, k);
     if (!allv && !node.null_equals_null) continue;
     auto it = table.find(k);
     if (it == table.end()) continue;

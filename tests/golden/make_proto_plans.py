@@ -172,6 +172,8 @@ def set_join_common(j, t, left_schema, right_schema):
         set_expr(on.left, l)
         set_expr(on.right, r)
     j.join_type = _JOIN[t["join_type"]]
+    if t.get("null_equals_null"):
+        j.null_equality = 1     # NullEquality::NULL_EQUALS_NULL (datafusion_common.proto:98-101)
     if "filter" in t:
         used = cols_of(t["filter"], [])
         nl = len(left_schema)
