@@ -166,6 +166,15 @@ inline i128 pow10_i128(int n) {
   return r;
 }
 
+// 10^n as the double nearest to it (exact for 0 <= n <= 22): the scale factor of the decimal <-> float casts, the same
+// table the device uses (pipeline.cu pow10_f64_dev)
+inline double pow10_f64(int n) {
+  static const double t[39] = {1e0,  1e1,  1e2,  1e3,  1e4,  1e5,  1e6,  1e7,  1e8,  1e9,  1e10, 1e11, 1e12, 1e13,
+                               1e14, 1e15, 1e16, 1e17, 1e18, 1e19, 1e20, 1e21, 1e22, 1e23, 1e24, 1e25, 1e26, 1e27,
+                               1e28, 1e29, 1e30, 1e31, 1e32, 1e33, 1e34, 1e35, 1e36, 1e37, 1e38};
+  return t[n < 0 ? 0 : n > 38 ? 38 : n];
+}
+
 inline i128 parse_i128(const std::string& s) {
   size_t k = 0;
   bool neg = false;

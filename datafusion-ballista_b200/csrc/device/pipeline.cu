@@ -123,6 +123,13 @@ __device__ __noinline__ i128 pow10_dev(int n) {
   for (int i = 0; i < n; i++) r *= 10;
   return r;
 }
+// 10^n as the double nearest to it (exact for n <= 22): the scale factor of the decimal <-> float casts
+__device__ __noinline__ double pow10_f64_dev(int n) {
+  const double t[39] = {1e0,  1e1,  1e2,  1e3,  1e4,  1e5,  1e6,  1e7,  1e8,  1e9,  1e10, 1e11, 1e12, 1e13,
+                        1e14, 1e15, 1e16, 1e17, 1e18, 1e19, 1e20, 1e21, 1e22, 1e23, 1e24, 1e25, 1e26, 1e27,
+                        1e28, 1e29, 1e30, 1e31, 1e32, 1e33, 1e34, 1e35, 1e36, 1e37, 1e38};
+  return t[n < 0 ? 0 : n > 38 ? 38 : n];
+}
 __device__ __noinline__ i128 div_i128_dev(i128 a, i128 b) { return a / b; }
 __device__ __noinline__ i128 mod_i128_dev(i128 a, i128 b) { return a % b; }
 __device__ __forceinline__ long long f64_order_key(double a) {
@@ -980,12 +987,18 @@ __device__ __noinline__ void cold_op(const Lane L, const uint32_t active, const 
     switch (ins.op) {
       case OP_DIV:
       case OP_MOD: {
-        if (ins.t == VK_I64) {
+        if (ins.t == VK_I64) {  // aux = Phys of the result type
           int64_t a = ld1_i64(L, ins.a, r), b = ld1_i64(L, ins.b, r), o = 0;
           if (b == 0) {
             if (lv) raise(2);
-          } else if (a == INT64_MIN && b == -1) {
-            if (ins.op == OP_DIV && lv) raise(1);
+          } else if (ins.aux == PH_U64) {
+            o = (int64_t)(ins.op == OP_DIV ? (uint64_t)a / (uint64_t)b : (uint64_t)a % (uint64_t)b);
+          } else if (b == -1) {  // the type's minimum / -1 overflows it; MIN % -1 is 0 [EXT]
+            const int64_t mn = ins.aux == PH_I8 ? INT8_MIN : ins.aux == PH_I16 ? INT16_MIN : ins.aux == PH_I32 ? INT32_MIN : INT64_MIN;
+            if (ins.op == OP_DIV) {
+              if (a == mn && lv) raise(1);
+              o = (int64_t)(0 - (uint64_t)a);
+            }
           } else {
             o = ins.op == OP_DIV ? a / b : a % b;
           }
@@ -1013,7 +1026,8 @@ __device__ __noinline__ void cold_op(const Lane L, const uint32_t active, const 
         break;
       }
       case OP_NEG: {
-        if (ins.t == VK_F64) st1_f64(L, ins.dst, r, -ld1_f64(L, ins.a, r));
+        // floats: the sign bit flipped, a NaN's too (Rust's -x); nvcc's FP negation of a NaN does not flip it
+        if (ins.t == VK_F64) st1_f64(L, ins.dst, r, __longlong_as_double(__double_as_longlong(ld1_f64(L, ins.a, r)) ^ (long long)0x8000000000000000ull));
         else if (ins.t == VK_I128) st1_i128(L, ins.dst, r, (i128)((u128)0 - (u128)ld1_i128(L, ins.a, r)));
         else st1_i64(L, ins.dst, r, (int64_t)(0 - (uint64_t)ld1_i64(L, ins.a, r)));
         break;
@@ -1033,17 +1047,19 @@ __device__ __noinline__ void cold_op(const Lane L, const uint32_t active, const 
         bmask |= (cmp_result(ins.op, cm) ? 1u : 0u) << r;
         break;
       }
-      case OP_CAST_I64_F64: {
+      case OP_CAST_I64_F64: {  // imm = 1: to Float32, rounded once from the integer
         int64_t a = ld1_i64(L, ins.a, r);
-        double o = ins.aux == PH_U64 ? (double)(uint64_t)a : (double)a;
-        if (ins.imm == 1) o = (double)(float)o;
+        double o;
+        if (ins.imm == 1) o = ins.aux == PH_U64 ? (double)(float)(uint64_t)a : (double)(float)a;
+        else o = ins.aux == PH_U64 ? (double)(uint64_t)a : (double)a;
         st1_f64(L, ins.dst, r, o);
         break;
       }
-      case OP_CAST_I64_I128:
+      case OP_CAST_I64_I128:  // aux = PH_U64: the operand's 64 bits are zero-extended
       case OP_CAST_I128_I128_UP: {
         i128 o;
-        bool ovf = mul_i128_fast(ld1_i128(L, ins.a, r), pow10_dev(ins.imm), &o);
+        const i128 a = ins.aux == PH_U64 ? (i128)(uint64_t)ld1_i64(L, ins.a, r) : ld1_i128(L, ins.a, r);
+        bool ovf = mul_i128_fast(a, pow10_dev(ins.imm), &o);
         if (ovf && lv) raise(1);
         st1_i128(L, ins.dst, r, o);
         break;
@@ -1072,25 +1088,31 @@ __device__ __noinline__ void cold_op(const Lane L, const uint32_t active, const 
       }
       case OP_CAST_I128_F64: {
         i128 a = ld1_i128(L, ins.a, r);
-        st1_f64(L, ins.dst, r, (double)a / pow(10.0, (double)ins.imm));
+        st1_f64(L, ins.dst, r, (double)a / pow10_f64_dev(ins.imm));
         break;
       }
-      case OP_CAST_F64_I64: {
+      case OP_CAST_F64_I64: {  // aux = PH_U64: the target is UInt64, [0, 2^64)
         double t = trunc(ld1_f64(L, ins.a, r));
         int64_t o = 0;
-        if (!(t >= -9.2233720368547758e18 && t < 9.2233720368547758e18)) vout &= ~(1u << r);
-        else o = (int64_t)t;
+        if (ins.aux == PH_U64) {
+          if (!(t >= 0.0 && t < 1.8446744073709552e19)) vout &= ~(1u << r);
+          else o = (int64_t)(uint64_t)t;
+        } else if (!(t >= -9.2233720368547758e18 && t < 9.2233720368547758e18)) {
+          vout &= ~(1u << r);
+        } else {
+          o = (int64_t)t;
+        }
         st1_i64(L, ins.dst, r, o);
         break;
       }
-      case OP_CAST_I128_I64: {
+      case OP_CAST_I128_I64: {  // aux = PH_U64: the target is UInt64
         i128 q = div_i128_dev(ld1_i128(L, ins.a, r), pow10_dev(ins.imm));
-        if (!fits_i64(q)) vout &= ~(1u << r);
+        if (ins.aux == PH_U64 ? (q < 0 || hi64(q) != 0) : !fits_i64(q)) vout &= ~(1u << r);
         st1_i64(L, ins.dst, r, (int64_t)q);
         break;
       }
       case OP_CAST_F64_I128: {
-        double t = round(ld1_f64(L, ins.a, r) * pow(10.0, (double)ins.imm));
+        double t = round(ld1_f64(L, ins.a, r) * pow10_f64_dev(ins.imm));
         i128 o = 0;
         if (!(fabs(t) < 1.7e38)) vout &= ~(1u << r);
         else o = (i128)t;
@@ -1098,7 +1120,7 @@ __device__ __noinline__ void cold_op(const Lane L, const uint32_t active, const 
         break;
       }
       case OP_WRAP_I64:
-      case OP_NARROW_I64: {
+      case OP_NARROW_I64: {  // OP_NARROW_I64 imm = 1: a negative 64-bit image is out of range too (UInt64 in or out)
         int64_t a = ld1_i64(L, ins.a, r), w;
         switch (ins.aux) {
           case PH_I8: w = (int8_t)a; break;
@@ -1109,7 +1131,7 @@ __device__ __noinline__ void cold_op(const Lane L, const uint32_t active, const 
           case PH_U32: w = (uint32_t)a; break;
           default: w = a;
         }
-        if (ins.op == OP_NARROW_I64 && w != a) vout &= ~(1u << r);
+        if (ins.op == OP_NARROW_I64 && (w != a || (ins.imm == 1 && a < 0))) vout &= ~(1u << r);
         st1_i64(L, ins.dst, r, w);
         break;
       }
@@ -1822,6 +1844,17 @@ __device__ __noinline__ uint32_t run_generic(const Lane L, uint32_t active, cons
       break;
     case OP_SELECT:
     case OP_MOV: cold_move(L, pc); break;
+    case OP_ACTIVE: {  // CASE: the rows the next instructions run for
+      const VInstr& ins = PROG.code[pc];
+      uint32_t m = ins.a.kind == OPD_NONE ? active : fetch_bool(L, ins.a);
+      if (ins.b.kind != OPD_NONE) {
+        const uint32_t c = fetch_bool(L, ins.b) & fetch_valid(L, ins.b);
+        m &= ins.aux ? ~c : c;
+      }
+      if (ins.dst.kind == OPD_REG) store_bool(L, ins.dst, m);
+      if (ins.a.kind != OPD_NONE) active = m;
+      break;
+    }
     case OP_NOP: break;
     default: cold_op<SFN>(L, active, pc); break;
   }

@@ -72,6 +72,9 @@ enum VOp : uint8_t {
   OP_DEC_MUL_LIT_PLUS,                 // fused: dst = a * (imm + b)
   OP_MADD_I64,                         // dst = a + b * imm64 (imm = immediate index); wrapping
   OP_STR_PACK8,                        // dst(I64) = len<<imm | bytes of a string of <= aux bytes (imm = 56/aux = 7 or imm = 24/aux = 3); longer -> pack_overflow
+  // CASE (lower.hpp compile_case): m = a (a bool register) or, without a, the rows active now; with b, m &= b (TRUE rows;
+  // aux = 1: m &= ~b); dst (a never-NULL bool register), if given, = m; with a, the rows active from here on = m
+  OP_ACTIVE,
   // scalar functions (cold: scalar_num_op / scalar_nullif_op / scalar_str_op in pipeline.cu); every op from OP_ABS on is one
   OP_ABS,                              // t = VK_I64 | VK_F64 | VK_I128; aux = Phys of a signed integer (its minimum raises overflow)
   OP_ROUND,                            // t = VK_F64; imm = immediate idx of the factor f; aux = PH_F32 for f32 arithmetic

@@ -889,11 +889,31 @@ class PipelineBuilder {
   static int scale_of(const DataType& t) { return t.is_decimal() ? t.scale : 0; }
   static int precision_of(const DataType& t) { return t.is_decimal() ? t.precision : int_as_decimal(t).precision; }
 
+  // a UInt64 operand meeting a decimal: its value as Decimal128(20, 0), zero-extended (a 64-bit operand of a 128-bit
+  // instruction is sign-extended); any other operand as it is
+  ColRef widen_u64(const ColRef& a) {
+    if (a.type.id != TypeId::UInt64) return a;
+    const DataType t = DataType::decimal(20, 0);
+    if (is_literal(a)) {
+      if (prog.imms[a.op.idx].is_null) return null_of(t);
+      return dec_literal((i128)prog.imms[a.op.idx].lo, t);
+    }
+    ColRef r = new_reg(t, a.nullable);
+    VInstr ins = blank(OP_CAST_I64_I128, VK_I128);
+    ins.a = resolve(a);
+    ins.dst = r.op;
+    ins.aux = PH_U64;
+    if (a.nullable) ins.flags |= IF_NULLCHK;
+    emit(ins);
+    return r;
+  }
+
   ColRef to_f64(const ColRef& a) {
     if (a.type.pk() == PK::F64) return a;
     if (is_literal(a) && !prog.imms[a.op.idx].is_null) {
       LitValue l;
-      if (a.type.is_decimal()) l.f = (double)imm_i128(a) / std::pow(10.0, a.type.scale);
+      if (a.type.is_decimal()) l.f = (double)imm_i128(a) / pow10_f64(a.type.scale);
+      else if (a.type.id == TypeId::UInt64) l.f = (double)prog.imms[a.op.idx].lo;
       else l.f = (double)(int64_t)prog.imms[a.op.idx].lo;
       return literal(DataType(TypeId::Float64), l);
     }
@@ -936,6 +956,11 @@ class PipelineBuilder {
       b = y;
       t = VK_F64;
     } else if (a.type.is_decimal() || b.type.is_decimal()) {
+      for (ColRef* x : {&a, &b}) {
+        ColRef w = widen_u64(*x);
+        if (w.op.kind == OPD_REG && !(x->op.kind == OPD_REG && x->op.idx == w.op.idx)) temps.push_back(w);
+        *x = w;
+      }
       int sa = scale_of(a.type), sb = scale_of(b.type), s = std::max(sa, sb);
       int pa = precision_of(a.type) + (s - sa), pb = precision_of(b.type) + (s - sb);
       DataType ta = DataType::decimal(std::min(38, pa), s), tb = DataType::decimal(std::min(38, pb), s);
@@ -1075,6 +1100,11 @@ class PipelineBuilder {
       if (x.op.kind == OPD_REG && !(a.op.kind == OPD_REG && a.op.idx == x.op.idx)) release(x);
       if (y.op.kind == OPD_REG && !(b.op.kind == OPD_REG && b.op.idx == y.op.idx)) release(y);
     } else if (rt.is_decimal()) {
+      for (ColRef* x : {&a, &b}) {
+        ColRef w = widen_u64(*x);
+        if (w.op.kind == OPD_REG && !(x->op.kind == OPD_REG && x->op.idx == w.op.idx)) release(*x);
+        *x = w;
+      }
       int s1 = scale_of(a.type), s2 = scale_of(b.type);
       ColRef x = a, y = b;
       int imm = 0;
@@ -1104,6 +1134,7 @@ class PipelineBuilder {
       ins.a = resolve(a);
       ins.b = resolve(b);
       ins.dst = r.op;
+      if (vop == OP_DIV || vop == OP_MOD) ins.aux = phys_of(rt);  // unsigned division, the minimum / -1 overflow
       ins.flags = IF_CHECKED | (nullable ? IF_NULLCHK : 0);
       emit(ins);
       r = wrap_int(r, rt);
@@ -1113,43 +1144,65 @@ class PipelineBuilder {
     return r;
   }
 
+  // CASE WHEN c1 THEN v1 ... [ELSE e] END, as lazily as DataFusion's CaseExpr evaluates it (evaluate_selection): each WHEN
+  // runs for the rows no earlier WHEN took, each THEN for the rows its WHEN took, the ELSE for the rest.  OP_ACTIVE
+  // narrows the active rows around each part and restores them after the last, so an operation that can fail (a division,
+  // a checked decimal operation, a cast to a decimal) fails only for a row its part is evaluated for.
   ColRef compile_case(const Expr& e) {
     const size_t npairs = (e.args.size() - (e.has_else ? 1 : 0)) / 2;
+    const uint8_t vk = vk_of(e.type);
     ColRef dst = new_reg(e.type, true);
     pin(dst);
     {
-      ColRef init;
-      if (e.has_else) {
-        ColRef v = compile(*e.args.back());
-        init = cast_to(v, e.type);
-      } else {
-        LitValue l;
-        l.is_null = true;
-        init = literal(e.type, l);
-      }
-      VInstr ins = blank(OP_MOV, vk_of(e.type));
-      ins.a = resolve(init);
+      LitValue l;
+      l.is_null = true;
+      VInstr ins = blank(OP_MOV, vk);
+      ins.a = resolve(literal(e.type, l));
       ins.dst = dst.op;
       ins.flags = IF_NULLCHK;
       emit(ins);
-      dst.keep.insert(dst.keep.end(), init.keep.begin(), init.keep.end());
-      release(init);
     }
-    for (size_t w = npairs; w-- > 0;) {
-      ColRef c = compile(*e.args[2 * w]);
-      pin(c);
-      ColRef v0 = compile(*e.args[2 * w + 1]);
-      ColRef v = cast_to(v0, e.type);
-      unpin(c);
-      VInstr ins = blank(OP_SELECT, vk_of(e.type));
-      ins.a = resolve(c);
+    auto mask = [&](const ColRef* a, const ColRef* b, uint8_t negate, const ColRef* out) {
+      VInstr ins = blank(OP_ACTIVE, VK_BOOL);
+      if (a) ins.a = resolve(*a);
+      if (b) ins.b = resolve(*b);
+      if (out) ins.dst = out->op;
+      ins.aux = negate;
+      emit(ins);
+    };
+    ColRef entry = new_reg(DataType(TypeId::Bool), false);
+    pin(entry);
+    ColRef rem = new_reg(DataType(TypeId::Bool), false);
+    pin(rem);
+    ColRef sel = new_reg(DataType(TypeId::Bool), false);
+    pin(sel);
+    mask(nullptr, nullptr, 0, &entry);
+    mask(nullptr, nullptr, 0, &rem);
+    auto select = [&](const ColRef& cond, const Expr& value) {
+      ColRef v = cast_to(compile(value), e.type);
+      VInstr ins = blank(OP_SELECT, vk);
+      ins.a = resolve(cond);
       ins.b = resolve(v);
       ins.dst = dst.op;
       ins.flags = IF_NULLCHK;
       emit(ins);
       dst.keep.insert(dst.keep.end(), v.keep.begin(), v.keep.end());
-      release(c);
       release(v);
+    };
+    for (size_t w = 0; w < npairs; w++) {
+      ColRef c = compile(*e.args[2 * w]);  // for the remaining rows
+      pin(c);
+      mask(&rem, &c, 0, &sel);             // its THEN: for the remaining rows where it is TRUE
+      select(sel, *e.args[2 * w + 1]);
+      mask(&rem, &c, 1, &rem);             // the rows left for the next WHEN / the ELSE
+      unpin(c);
+      release(c);
+    }
+    if (e.has_else) select(rem, *e.args.back());
+    mask(&entry, nullptr, 0, nullptr);
+    for (ColRef* r : {&entry, &rem, &sel}) {
+      unpin(*r);
+      release(*r);
     }
     unpin(dst);
     return dst;
@@ -1178,18 +1231,16 @@ class PipelineBuilder {
       return literal(to, l);
     }
     if (dst == PK::I64 && (from == PK::I64 || from == PK::Bool)) {
-      if (to.width() >= 8 || from == PK::Bool) {
+      if (from == PK::Bool) return simple(OP_MOV, VK_I64, 0, 0, false);
+      // a value of a signed type going to UInt64, or a UInt64 going to any other type: a negative 64-bit image is out
+      // of range (a negative value, or one at or above 2^63)
+      const bool sign_check = (to.id == TypeId::UInt64 && a.type.is_signed_int()) || (a.type.id == TypeId::UInt64 && to.is_integer() && to.id != TypeId::UInt64);
+      if (!sign_check && (to.width() >= 8 || (a.type.width() <= to.width() && a.type.is_signed_int() == to.is_signed_int()))) {
         ColRef o = a;
         o.type = to;
-        if (from == PK::Bool) return simple(OP_MOV, VK_I64, 0, 0, false);
         return o;
       }
-      if (a.type.width() <= to.width() && a.type.is_signed_int() == to.is_signed_int()) {
-        ColRef o = a;
-        o.type = to;
-        return o;
-      }
-      return simple(OP_NARROW_I64, VK_I64, 0, phys_of(to), true);
+      return simple(OP_NARROW_I64, VK_I64, sign_check ? 1 : 0, phys_of(to), true);
     }
     if (dst == PK::Bool && from == PK::I64) {
       ColRef zero = literal(a.type, LitValue());
@@ -1205,7 +1256,7 @@ class PipelineBuilder {
       return o;
     }
     if (dst == PK::I64 && from == PK::F64) {
-      ColRef r = simple(OP_CAST_F64_I64, VK_I64, 0, 0, true);
+      ColRef r = simple(OP_CAST_F64_I64, VK_I64, 0, to.id == TypeId::UInt64 ? PH_U64 : 0, true);
       if (to.width() < 8) {
         ColRef n = new_reg(to, true);
         VInstr ins = blank(OP_NARROW_I64, VK_I64);
@@ -1220,7 +1271,7 @@ class PipelineBuilder {
       return r;
     }
     if (dst == PK::I128 && from == PK::I64) {
-      ColRef r = simple(OP_CAST_I64_I128, VK_I128, to.scale, 0, false);
+      ColRef r = simple(OP_CAST_I64_I128, VK_I128, to.scale, a.type.id == TypeId::UInt64 ? PH_U64 : 0, false);
       prog.code[prog.n_instr - 1].flags |= IF_CHECKED;
       // value must fit the target precision (error, like arrow's cast of ints to decimal) [EXT]
       VInstr chk = blank(OP_CHECK_PRECISION, VK_I128);
@@ -1243,9 +1294,18 @@ class PipelineBuilder {
       emit(chk);
       return r;
     }
-    if (dst == PK::I128 && from == PK::F64) return simple(OP_CAST_F64_I128, VK_I128, to.scale, 0, true);
+    if (dst == PK::I128 && from == PK::F64) {
+      ColRef r = simple(OP_CAST_F64_I128, VK_I128, to.scale, 0, true);
+      VInstr chk = blank(OP_CHECK_PRECISION, VK_I128);  // beyond the precision: NULL (safe cast)
+      chk.a = r.op;
+      chk.dst = r.op;
+      chk.aux = to.precision;
+      chk.flags = IF_NULLCHK;
+      emit(chk);
+      return r;
+    }
     if (dst == PK::I64 && from == PK::I128) {
-      ColRef r = simple(OP_CAST_I128_I64, VK_I64, a.type.scale, 0, true);
+      ColRef r = simple(OP_CAST_I128_I64, VK_I64, a.type.scale, to.id == TypeId::UInt64 ? PH_U64 : 0, true);
       if (to.width() < 8) {
         ColRef n = new_reg(to, true);
         VInstr ins = blank(OP_NARROW_I64, VK_I64);

@@ -22,6 +22,7 @@
 #include <cmath>
 #include <cstdio>
 #include <deque>
+#include <functional>
 #include <map>
 #include <mutex>
 #include <string>
@@ -309,7 +310,7 @@ int total_cmp(double a, double b) {
   y ^= (int64_t)((uint64_t)(y >> 63) >> 1);
   return x < y ? -1 : x > y ? 1 : 0;
 }
-double dec_to_f64(i128 v, int scale) { return (double)v / std::pow(10.0, scale); }
+double dec_to_f64(i128 v, int scale) { return (double)v / pow10_f64(scale); }  // arrow: x as f64 / 10_f64.powi(scale)
 
 bool like_match(const char* s, size_t sn, const char* p, size_t pn) {
   // SQL LIKE with % and _ (no escape), bytewise
@@ -357,7 +358,10 @@ int32_t year_of_days(int64_t z) {  // civil-from-days (proleptic Gregorian)
 OCol eval(const Expr& e, const OBatch& b);
 
 // numeric view of a column as decimal(scale) / double
-i128 as_dec(const OCol& c, size_t r) { return c.type.is_decimal() ? c.d[r] : (i128)c.i[r]; }
+i128 as_dec(const OCol& c, size_t r) {
+  if (c.type.is_decimal()) return c.d[r];
+  return c.type.id == TypeId::UInt64 ? (i128)(uint64_t)c.i[r] : (i128)c.i[r];
+}
 int dec_scale(const OCol& c) { return c.type.is_decimal() ? c.type.scale : 0; }
 double as_f64(const OCol& c, size_t r) {
   switch (c.type.pk()) {
@@ -436,14 +440,20 @@ OCol eval_arith(const Expr& e, const OCol& l, const OCol& r) {
         case BinOp::Add: z = (int64_t)((uint64_t)x + (uint64_t)y); break;
         case BinOp::Sub: z = (int64_t)((uint64_t)x - (uint64_t)y); break;
         case BinOp::Mul: z = (int64_t)((uint64_t)x * (uint64_t)y); break;
-        case BinOp::Div:
+        case BinOp::Div:  // arrow's div_checked: a quotient outside the type (its minimum / -1) is an error
           if (y == 0) exec_fail("Divide by zero");
+          if (rt.id == TypeId::UInt64) {
+            z = (int64_t)((uint64_t)x / (uint64_t)y);
+            break;
+          }
           if (x == INT64_MIN && y == -1) exec_fail("Arithmetic overflow: integer divide");
           z = x / y;
+          if (wrap_int(z, rt.id) != z) exec_fail("Arithmetic overflow: integer divide");
           break;
-        case BinOp::Mod:
+        case BinOp::Mod:  // the dividend's sign; MIN % -1 is 0 [EXT]
           if (y == 0) exec_fail("Divide by zero");
-          z = (y == -1) ? 0 : x % y;
+          if (rt.id == TypeId::UInt64) z = (int64_t)((uint64_t)x % (uint64_t)y);
+          else z = (y == -1) ? 0 : x % y;
           break;
         default: break;
       }
@@ -465,21 +475,32 @@ OCol eval_cast(const OCol& c, const DataType& to) {
     }
     if (dst == PK::I64 && from == PK::I64) {
       int64_t v = c.i[k];
-      if (wrap_int(v, to.id) != v) o.set_null(k);  // arrow "safe" cast: overflow -> NULL [EXT]
+      // arrow "safe" cast: overflow -> NULL [EXT]; a negative 64-bit image is a negative value going to UInt64 or a
+      // UInt64 at or above 2^63 going to another type
+      const bool sign_bad = v < 0 && c.type.is_integer() && to.is_integer() && ((c.type.id == TypeId::UInt64) != (to.id == TypeId::UInt64));
+      if (sign_bad || wrap_int(v, to.id) != v) o.set_null(k);
       else o.i[k] = v;
     } else if (dst == PK::I64 && from == PK::Bool) {
       o.i[k] = c.i[k];
     } else if (dst == PK::Bool && from == PK::I64) {
       o.i[k] = c.i[k] != 0;
+    } else if (dst == PK::F64 && from == PK::I64 && to.id == TypeId::Float32) {  // rounded once, as Rust's `as f32`
+      o.f[k] = c.type.id == TypeId::UInt64 ? (double)(float)(uint64_t)c.i[k] : (double)(float)c.i[k];
     } else if (dst == PK::F64 && (from == PK::I64 || from == PK::F64 || from == PK::I128)) {
       double v = as_f64(c, k);
       o.f[k] = to.id == TypeId::Float32 ? (double)(float)v : v;
     } else if (dst == PK::I64 && from == PK::F64) {
       double v = std::trunc(c.f[k]);
-      if (!(v >= -9.2233720368547758e18 && v < 9.2233720368547758e18) || wrap_int((int64_t)v, to.id) != (int64_t)v) o.set_null(k);
-      else o.i[k] = (int64_t)v;
+      if (to.id == TypeId::UInt64) {
+        if (!(v >= 0.0 && v < 1.8446744073709552e19)) o.set_null(k);
+        else o.i[k] = (int64_t)(uint64_t)v;
+      } else if (!(v >= -9.2233720368547758e18 && v < 9.2233720368547758e18) || wrap_int((int64_t)v, to.id) != (int64_t)v) {
+        o.set_null(k);
+      } else {
+        o.i[k] = (int64_t)v;
+      }
     } else if (dst == PK::I128 && from == PK::I64) {
-      i128 v = rescale_up((i128)c.i[k], to.scale);
+      i128 v = rescale_up(as_dec(c, k), to.scale);
       if (v >= pow10_i128(to.precision) || v <= -pow10_i128(to.precision)) exec_fail("cast: value does not fit " + to.str());
       o.d[k] = v;
     } else if (dst == PK::I128 && from == PK::I128) {
@@ -497,13 +518,19 @@ OCol eval_cast(const OCol& c, const DataType& to) {
       if (v >= pow10_i128(to.precision) || v <= -pow10_i128(to.precision)) o.set_null(k);
       else o.d[k] = v;
     } else if (dst == PK::I128 && from == PK::F64) {
-      double v = std::round(c.f[k] * std::pow(10.0, to.scale));
-      if (!(std::fabs(v) < 1.7e38)) o.set_null(k);
+      double v = std::round(c.f[k] * pow10_f64(to.scale));  // half away from zero; beyond the precision: NULL
+      if (!(std::fabs(v) < 1.7e38) || (i128)v >= pow10_i128(to.precision) || (i128)v <= -pow10_i128(to.precision)) o.set_null(k);
       else o.d[k] = (i128)v;
     } else if (dst == PK::I64 && from == PK::I128) {
       i128 v = c.d[k] / pow10_i128(c.type.scale);  // truncation toward zero [EXT]
-      if (v > INT64_MAX || v < INT64_MIN || wrap_int((int64_t)v, to.id) != (int64_t)v) o.set_null(k);
-      else o.i[k] = (int64_t)v;
+      if (to.id == TypeId::UInt64) {
+        if (v < 0 || v > (i128)UINT64_MAX) o.set_null(k);
+        else o.i[k] = (int64_t)(uint64_t)v;
+      } else if (v > INT64_MAX || v < INT64_MIN || wrap_int((int64_t)v, to.id) != (int64_t)v) {
+        o.set_null(k);
+      } else {
+        o.i[k] = (int64_t)v;
+      }
     } else if (dst == PK::Str && from == PK::Str) {
       o.s[k] = c.s[k];
     } else if (dst == PK::Str && from == PK::I64) {
@@ -605,26 +632,41 @@ OCol eval(const Expr& e, const OBatch& b) {
       return o;
     }
     case Expr::Cast: return eval_cast(eval(*e.args[0], b), e.type);
-    case Expr::Case: {
+    case Expr::Case: {  // DataFusion's CaseExpr: each WHEN on the rows left, each THEN / the ELSE on the rows it takes
       OCol o = make_col(e.type, n);
-      std::vector<uint8_t> done(n, 0);
+      for (size_t k = 0; k < n; k++) o.set_null(k);
+      std::vector<int64_t> rem(n);
+      for (size_t k = 0; k < n; k++) rem[k] = (int64_t)k;
+      auto on_rows = [&](const Expr& x, const std::vector<int64_t>& rows) {  // x over those rows (its columns only)
+        std::vector<uint8_t> used(b.cols.size(), 0);
+        std::function<void(const Expr&)> mark = [&](const Expr& y) {
+          if (y.kind == Expr::Col && (size_t)y.col < used.size()) used[(size_t)y.col] = 1;
+          for (auto& a : y.args) mark(*a);
+        };
+        mark(x);
+        OBatch sub;
+        sub.n = rows.size();
+        for (size_t i = 0; i < b.cols.size(); i++) sub.cols.push_back(used[i] ? take(b.cols[i], rows) : make_col(b.cols[i].type, 0));
+        return eval(x, sub);
+      };
+      auto put = [&](const OCol& v, size_t j, size_t k) {
+        o.copy_row_from(v, j, k);
+        if (v.is_valid(j)) o.valid[k] = 1;
+      };
       size_t npairs = (e.args.size() - (e.has_else ? 1 : 0)) / 2;
-      for (size_t w = 0; w < npairs; w++) {
-        OCol c = eval(*e.args[2 * w], b);
-        OCol v = eval_cast(eval(*e.args[2 * w + 1], b), e.type);
-        for (size_t k = 0; k < n; k++) {
-          if (done[k] || !c.is_valid(k) || !c.i[k]) continue;
-          done[k] = 1;
-          o.copy_row_from(v, k, k);
+      for (size_t w = 0; w < npairs && !rem.empty(); w++) {
+        OCol c = on_rows(*e.args[2 * w], rem);
+        std::vector<int64_t> hit, left;
+        for (size_t j = 0; j < rem.size(); j++) (c.is_valid(j) && c.i[j] ? hit : left).push_back(rem[j]);
+        if (!hit.empty()) {
+          OCol v = eval_cast(on_rows(*e.args[2 * w + 1], hit), e.type);
+          for (size_t j = 0; j < hit.size(); j++) put(v, j, (size_t)hit[j]);
         }
+        rem.swap(left);
       }
-      if (e.has_else) {
-        OCol v = eval_cast(eval(*e.args.back(), b), e.type);
-        for (size_t k = 0; k < n; k++)
-          if (!done[k]) o.copy_row_from(v, k, k);
-      } else {
-        for (size_t k = 0; k < n; k++)
-          if (!done[k]) o.set_null(k);
+      if (e.has_else && !rem.empty()) {
+        OCol v = eval_cast(on_rows(*e.args.back(), rem), e.type);
+        for (size_t j = 0; j < rem.size(); j++) put(v, j, (size_t)rem[j]);
       }
       return o;
     }
