@@ -328,6 +328,11 @@ struct Expr {
   // NULL literal: the result is NULL), and the key the engine caches its device copy under
   std::shared_ptr<const rx::Dfa> regex;
   std::string regex_key;
+  // regexp_count / regexp_replace: `regex` is the forward span DFA and regex_rev the reverse one (regex_dfa.hpp); the
+  // count's start (1-based code points) and the replacement's g flag
+  std::shared_ptr<const rx::Dfa> regex_rev;
+  int64_t regex_start = 1;
+  bool regex_global = false;
   std::string name;       // display only
 };
 
@@ -453,6 +458,70 @@ inline void type_regex(Expr& e, const std::string& what, const ExprPtr& pattern,
   e.regex = d;
 }
 
+// regexp_count(str, pattern [, start [, flags]]) -> Int64 and regexp_replace(str, pattern, replacement [, flags]) -> Utf8,
+// gated like type_regex.  Rules [EXT, DESIGN.md §6 (xiii)], restated from DataFusion 53 and unpinned:
+//   regexp_count: a NULL or empty str counts 0, and a NULL or empty pattern 0 for every row (no row is NULL, though the
+//     result is typed nullable as a scalar UDF's is); start is a non-NULL Int64 literal >= 1 counted in code points (the
+//     haystack loses its first start - 1 of them); the flags must be a non-NULL literal without g.
+//   regexp_replace: NULL when any argument is; a NULL literal makes every row NULL; the flag g replaces every match, else
+//     only the first; the replacement is a literal inserted verbatim, refused when it holds '\' or '$' (DataFusion rewrites
+//     \N into ${N} and Rust expands $name / ${N} / $$: group references a DFA cannot give).
+// Both DFAs are compiled here, so that a bad pattern fails when the stage is prepared; their cache keys ("fwd:" / "rev:"
+// + regex_key) never equal an is_match key.
+inline void type_regex_fn(Expr& e) {
+  const std::string& f = e.fn;
+  const bool count = f == "regexp_count";
+  const size_t n = e.args.size();
+  if (!B200_PLAN_REGEX) throw PlanUnsupported(f + " is not computed by this consumer of the plan IR");
+  const DataType& t = e.args[0]->type;
+  if (!t.is_string() && t.id != TypeId::Null) throw PlanUnsupported(f + " does not support an operand of type " + t.str());
+  e.type = DataType(count ? TypeId::Int64 : TypeId::Utf8);
+  e.nullable = true;
+  bool null_arg = false;
+  auto literal = [&](const ExprPtr& a, const char* role) -> const std::string& {
+    if (a->kind != Expr::Lit) throw PlanUnsupported(f + ": the " + role + " must be a literal");
+    if (!a->type.is_string() && a->type.id != TypeId::Null) throw PlanUnsupported(f + ": the " + role + " must be utf8, not " + a->type.str());
+    null_arg = null_arg || a->lit.is_null;
+    return a->lit.s;
+  };
+  auto fail = [&](int rc, const std::string& msg) {
+    if (rc == rx::RX_UNSUPPORTED) throw PlanUnsupported(msg);
+    throw std::runtime_error(msg);
+  };
+  const std::string& p = literal(e.args[1], "pattern");
+  const bool null_pattern = null_arg;
+  if (count && n >= 3) {
+    const Expr& s = *e.args[2];
+    if (s.kind != Expr::Lit || s.type.id != TypeId::Int64 || s.lit.is_null)
+      throw PlanUnsupported("regexp_count: the start must be a non-NULL Int64 literal");
+    if (s.lit.i < 1) throw std::runtime_error("regexp_count: the start must be at least 1, not " + std::to_string(s.lit.i));
+    e.regex_start = s.lit.i;
+  }
+  if (!count) {
+    const std::string& r = literal(e.args[2], "replacement");
+    if (r.find_first_of("\\$") != std::string::npos)
+      throw PlanUnsupported("regexp_replace: the replacement '" + r + "' holds '\\' or '$' (a group reference), which is not supported by the device engine");
+  }
+  bool fi = false, fs = false;
+  std::string err;
+  if (n == 4) {
+    // the flags literal is checked on its own, whatever the other arguments are (a NULL pattern included)
+    const std::string& fl = literal(e.args[3], "flags argument");
+    const bool null_flags = e.args[3]->lit.is_null;
+    if (count && null_flags) throw PlanUnsupported("regexp_count: the flags argument must not be NULL");
+    int rc;
+    if (!null_flags && (rc = rx::parse_regex_flags(fl, fi, fs, err, f.c_str(), count ? nullptr : &e.regex_global)) != rx::RX_OK) fail(rc, err);
+  }
+  if (null_arg || (count && (null_pattern || p.empty()))) return;  // every row NULL (replace) or 0 (count)
+  auto fwd = std::make_shared<rx::Dfa>();
+  auto rev = std::make_shared<rx::Dfa>();
+  const int rc = rx::compile_regex_spans(p, fi, fs, *fwd, *rev, err);
+  if (rc != rx::RX_OK) fail(rc, err);
+  e.regex = fwd;
+  e.regex_rev = rev;
+  e.regex_key = std::string(fi ? "i" : "") + (fs ? "s" : "") + ":" + p;
+}
+
 // concat, `||`, concat_ws, repeat and reverse are typed here for every consumer of the plan IR, but only a consumer built
 // with B200_PLAN_STRINGS=1 computes them (the device engine: Makefile NVFLAGS).  Semantics: DESIGN.md §6 (xi).  Their
 // arguments are the ones DataFusion's planner leaves after its casts (Utf8; repeat's count Int64).
@@ -547,6 +616,9 @@ inline void type_scalar_fn(Expr& e) {
   } else if (f == "regexp_like") {
     arity(2, 3);
     type_regex(e, "regexp_like", e.args[1], n == 3 ? e.args[2] : nullptr, false);
+  } else if (f == "regexp_count" || f == "regexp_replace") {
+    arity(f == "regexp_count" ? 2 : 3, 4);
+    type_regex_fn(e);
   } else if (f == "btrim" || f == "ltrim" || f == "rtrim") {
     arity(1, 2);
     need_utf8(0);

@@ -413,6 +413,7 @@ inline std::string expr_json(const Msg& e) {
           {"starts_with", "starts_with"},                   {"ends_with", "ends_with"},
           {"btrim", "btrim"},     {"trim", "btrim"},        {"ltrim", "ltrim"},
           {"rtrim", "rtrim"},     {"regexp_like", "regexp_like"},
+          {"regexp_count", "regexp_count"},                 {"regexp_replace", "regexp_replace"},
           {"concat", "concat"},   {"concat_ws", "concat_ws"}, {"repeat", "repeat"},
           {"reverse", "reverse"}};
       for (auto& kv : fns)

@@ -18,6 +18,9 @@
 // unanchored search (start of text resolved in the start state) -> one blob the walk reads:
 //   [256] byte -> class   [n_states, padded to 8] accepts-at-end flag   [n_states][n_cls] uint16 next state
 // State 0 is dead (the walk stops: no match), state 1 has matched (the walk stops: match).
+// regexp_count and regexp_replace need match spans, so the same parser and NFA also give two span DFAs (SpanDfaBuilder,
+// DESIGN.md §6 (xiii)): a forward leftmost-first one and a reverse anchored one, in the same blob layout with per-state
+// flags instead of an absorbing matched state.
 #pragma once
 #include <stdint.h>
 
@@ -63,6 +66,126 @@ B200_RX_HD inline bool dfa_is_match(const uint8_t* blob, uint64_t shape, const u
   uint32_t st = (uint32_t)shape & 0xFFFFu;
   for (uint32_t i = 0; i < n && st > kMatched; i++) st = rx_ld16(tr + st * n_cls + rx_ld8(blob + s[i]));
   return rx_ld8(blob + 256 + st) != 0;
+}
+
+// ---- match spans: regexp_count and regexp_replace [EXT, DESIGN.md §6 (xiii)] ------------------------------------------------
+// Two more DFAs per pattern (SpanDfaBuilder below): a forward one that finds where the leftmost-first match beginning at or
+// after a search start ends (Regex::find), and a reverse one that runs back from that end to find where it begins.  A
+// state's flags byte says whether a match ends (forward) or begins (reverse) at the current offset.
+static const uint32_t kSpanHere = 1, kSpanAtEdge = 2;                // flags: here; only at the text's end / offset 0
+static const uint32_t kSpanStartEdge = 1, kSpanStartInside = 2;      // start states: at the text's edge or not
+
+// bytes of the UTF-8 sequence led by c (1 for a stray continuation byte), at most `left`
+B200_RX_HD inline uint32_t rx_cp_len(uint32_t c, uint32_t left) {
+  const uint32_t k = c >= 0xF0 ? 4 : c >= 0xE0 ? 3 : c >= 0xC0 ? 2 : 1;
+  return k < left ? k : left;
+}
+// byte offset of s[0..n) after its first k code points (n when it has fewer)
+B200_RX_HD inline uint32_t rx_skip_cps(const uint8_t* s, uint32_t n, int64_t k) {
+  uint32_t i = 0;
+  for (; k > 0 && i < n; k--) i += rx_cp_len(s[i], n - i);
+  return i;
+}
+
+// End of the leftmost-first match of s[0..n) that begins at or after pos, or -1: the forward walk runs until the dead
+// state or the end of the text and keeps the last offset where a match ended.
+B200_RX_HD inline int64_t dfa_find_end(const uint8_t* blob, uint64_t shape, const uint8_t* s, uint32_t n, uint32_t pos) {
+  const uint32_t n_states = (uint32_t)(shape >> 32), n_cls = (uint32_t)(shape >> 16) & 0xFFFFu;
+  const uint16_t* tr = (const uint16_t*)(blob + dfa_trans_offset(n_states));
+  uint32_t st = pos == 0 ? kSpanStartEdge : kSpanStartInside;
+  int64_t end = -1;
+  for (uint32_t i = pos;; i++) {
+    if (rx_ld8(blob + 256 + st) & (i == n ? kSpanAtEdge : kSpanHere)) end = i;
+    if (i == n) break;
+    st = rx_ld16(tr + st * n_cls + rx_ld8(blob + s[i]));
+    if (st == kDead) break;
+  }
+  return end;
+}
+// Start of the match that ends at `end`: the reverse walk runs from end back to pos (never further) and keeps the smallest
+// offset where the reversed pattern accepts.  end is an offset where a match found from pos ends, so one exists.
+B200_RX_HD inline uint32_t dfa_find_start(const uint8_t* blob, uint64_t shape, const uint8_t* s, uint32_t n, uint32_t pos, uint32_t end) {
+  const uint32_t n_states = (uint32_t)(shape >> 32), n_cls = (uint32_t)(shape >> 16) & 0xFFFFu;
+  const uint16_t* tr = (const uint16_t*)(blob + dfa_trans_offset(n_states));
+  uint32_t st = end == n ? kSpanStartEdge : kSpanStartInside;
+  uint32_t start = end;
+  for (uint32_t j = end;; j--) {
+    if (rx_ld8(blob + 256 + st) & (j == 0 ? kSpanAtEdge : kSpanHere)) start = j;
+    if (j == pos) break;
+    st = rx_ld16(tr + st * n_cls + rx_ld8(blob + s[j - 1]));
+    if (st == kDead) break;
+  }
+  return start;
+}
+
+// The span DFAs of one pattern and the state of one find_iter over s[0..n) (the Rust regex crate's iteration):
+//   1. search from pos;
+//   2. an empty match ending where the last reported match ended is not reported: the search restarts one code point on;
+//   3. after any other empty match the next search starts one code point past it;
+//   4. after a non-empty match it starts at the match's end.
+struct RxSpans {
+  const uint8_t* fwd;
+  uint64_t fwd_shape;
+  const uint8_t* rev;
+  uint64_t rev_shape;
+};
+struct RxIter {
+  uint32_t pos;
+  int64_t last;  // end of the last reported match, -1 before the first
+};
+// The next reported match of the iteration: its span in [*ms, *me), false when there is none
+B200_RX_HD inline bool dfa_next_match(const RxSpans& d, const uint8_t* s, uint32_t n, RxIter& it, uint32_t* ms, uint32_t* me) {
+  while (it.pos <= n) {
+    const int64_t e = dfa_find_end(d.fwd, d.fwd_shape, s, n, it.pos);
+    if (e < 0) return false;
+    const uint32_t b = dfa_find_start(d.rev, d.rev_shape, s, n, it.pos, (uint32_t)e);
+    const uint32_t step = (uint32_t)e < n ? rx_cp_len(s[e], n - (uint32_t)e) : 1;
+    if (b == (uint32_t)e && e == it.last) {  // rule 2
+      it.pos = (uint32_t)e + step;
+      continue;
+    }
+    *ms = b;
+    *me = (uint32_t)e;
+    it.last = e;
+    it.pos = b == (uint32_t)e ? (uint32_t)e + step : (uint32_t)e;  // rules 3 and 4
+    return true;
+  }
+  return false;
+}
+// regexp_count: the number of reported matches in s[0..n)
+B200_RX_HD inline uint32_t dfa_count(const RxSpans& d, const uint8_t* s, uint32_t n) {
+  RxIter it = {0, -1};
+  uint32_t ms, me, c = 0;
+  while (dfa_next_match(d, s, n, it, &ms, &me)) c++;
+  return c;
+}
+// regexp_count of one non-NULL row: an empty str counts 0 before `start` applies (DataFusion returns 0 for it at once);
+// otherwise the haystack loses its first `skip` (start - 1) code points -- past the end it is '', where a pattern that
+// matches empty still counts 1 -- and its matches are counted
+B200_RX_HD inline uint32_t regexp_count_row(const RxSpans& d, const uint8_t* s, uint32_t n, int64_t skip) {
+  if (n == 0) return 0;
+  const uint32_t off = rx_skip_cps(s, n, skip);
+  return dfa_count(d, s + off, n - off);
+}
+// regexp_replace: s[0..n) with the first match (every match when `global`) replaced by rep[0..rep_len).  Returns the
+// result's length; writes the result to out unless it is null (the length pass).
+B200_RX_HD inline uint64_t dfa_replace(const RxSpans& d, const uint8_t* s, uint32_t n, const uint8_t* rep, uint32_t rep_len, bool global,
+                                       uint8_t* out) {
+  RxIter it = {0, -1};
+  uint32_t ms, me, done = 0;
+  uint64_t len = 0;
+  while (dfa_next_match(d, s, n, it, &ms, &me)) {
+    if (out) {
+      for (uint32_t i = done; i < ms; i++) out[len + i - done] = s[i];
+      for (uint32_t i = 0; i < rep_len; i++) out[len + ms - done + i] = rep[i];
+    }
+    len += (ms - done) + rep_len;
+    done = me;
+    if (!global) break;
+  }
+  if (out)
+    for (uint32_t i = done; i < n; i++) out[len + i - done] = s[i];
+  return len + (n - done);
 }
 
 }  // namespace rx
@@ -197,6 +320,7 @@ struct Node {
   CpSet set;
   std::vector<Node> kids;
   int mn = 0, mx = -1;  // Rep: mx = -1 is unbounded
+  bool greedy = true;   // Rep: false after a trailing '?' (only the leftmost-first span DFA tells the two apart)
 };
 
 class Parser {
@@ -354,7 +478,10 @@ class Parser {
       r.mn = (int)lo;
       r.mx = unbounded ? -1 : (int)hi;
     }
-    if (peek() == '?') pos_++;  // lazy: the same is_match
+    if (peek() == '?') {  // lazy: the same is_match, another leftmost-first span
+      pos_++;
+      r.greedy = false;
+    }
   }
 
   Node parse_atom(Flags& f, int depth, bool& is_flags) {
@@ -632,10 +759,15 @@ struct NState {
   int a = -1, b = -1;
 };
 
+// kMatch: the is_match NFA (split order is irrelevant there).  kForward: the same language with every split in priority
+// order, lazy repetitions preferring to stop, and the Rust `regex` crate's shapes for repetitions (below).  kReverse: the
+// reversed language (concatenations and UTF-8 sequences backwards, ^ and $ swapped), read from a match end backwards.
+enum NfaMode { kNfaMatch, kNfaForward, kNfaReverse };
+
 class NfaBuilder {
  public:
   std::vector<NState> st;
-  explicit NfaBuilder(const Parser& p) : p_(p) {}
+  explicit NfaBuilder(const Parser& p, NfaMode mode = kNfaMatch) : p_(p), mode_(mode) {}
 
   int add(NState::Kind k, int a = -1, int b = -1, uint8_t lo = 0, uint8_t hi = 0) {
     if (st.size() >= kMaxNfa) p_.unsupported("a pattern this large (its automaton exceeds " + std::to_string(kMaxNfa) + " NFA states)");
@@ -658,13 +790,64 @@ class NfaBuilder {
     if (n.k == Node::Rep) return n.mx == 0 || compiles_to_nothing(n.kids[0]);
     return false;
   }
+  // Rust's minimum_len() == 0: a repetition of such a body is compiled as (x+)? in priority order
+  static bool possibly_empty(const Node& n) {
+    switch (n.k) {
+      case Node::Set: return false;
+      case Node::Cat:
+        for (auto& k : n.kids)
+          if (!possibly_empty(k)) return false;
+        return true;
+      case Node::Alt:
+        for (auto& k : n.kids)
+          if (possibly_empty(k)) return true;
+        return false;
+      case Node::Rep: return n.mn == 0 || possibly_empty(n.kids[0]);
+      default: return true;
+    }
+  }
+  // a split preferring `first` (greedy) or `second` (lazy)
+  int prio_split(bool greedy, int first, int second) { return greedy ? add(NState::Split, first, second) : add(NState::Split, second, first); }
+  // x+ in priority order: x, then a split between x again (its start) and `next`
+  int compile_plus(const Node& r, int next) {
+    const int loop = prio_split(r.greedy, -1, next);
+    const int body = compile(r.kids[0], loop);
+    (r.greedy ? st[(size_t)loop].a : st[(size_t)loop].b) = body;
+    return body;
+  }
+  // repetitions in priority order, shaped like the Rust regex crate's Thompson compiler: x{n,m} is n copies of x, then m - n
+  // nested optional copies; x{n,} with n >= 1 is n - 1 copies, then x+; x* is a loop, or (x+)? when x can match empty
+  int compile_rep_ordered(const Node& n, int next) {
+    const Node& x = n.kids[0];
+    int cont = next;
+    if (n.mx < 0) {
+      if (n.mn == 0) {
+        if (possibly_empty(x)) return prio_split(n.greedy, compile_plus(n, next), next);
+        const int loop = prio_split(n.greedy, -1, next);
+        const int body = compile(x, loop);
+        (n.greedy ? st[(size_t)loop].a : st[(size_t)loop].b) = body;
+        return loop;
+      }
+      cont = compile_plus(n, next);
+      for (int k = 1; k < n.mn; k++) cont = compile(x, cont);
+      return cont;
+    }
+    for (int k = 0; k < n.mx - n.mn; k++) cont = prio_split(n.greedy, compile(x, cont), next);
+    for (int k = 0; k < n.mn; k++) cont = compile(x, cont);
+    return cont;
+  }
   int compile(const Node& n, int next) {
+    const bool rev = mode_ == kNfaReverse;
     switch (n.k) {
       case Node::Empty: return next;
-      case Node::Start: return add(NState::Start, next);
-      case Node::End: return add(NState::End, next);
+      case Node::Start: return add(rev ? NState::End : NState::Start, next);
+      case Node::End: return add(rev ? NState::Start : NState::End, next);
       case Node::Cat:
-        for (size_t i = n.kids.size(); i-- > 0;) next = compile(n.kids[i], next);
+        if (rev) {
+          for (size_t i = 0; i < n.kids.size(); i++) next = compile(n.kids[i], next);
+        } else {
+          for (size_t i = n.kids.size(); i-- > 0;) next = compile(n.kids[i], next);
+        }
         return next;
       case Node::Alt: {
         int entry = compile(n.kids.back(), next);
@@ -676,6 +859,7 @@ class NfaBuilder {
         // a body that compiles to no state repeats to nothing: without this, nested counts ((?:){1000}){1000}... would
         // loop without adding a state, so the state cap would never stop them
         if (n.mx == 0 || compiles_to_nothing(x)) return next;
+        if (mode_ == kNfaForward) return compile_rep_ordered(n, next);
         int cont = next;
         if (n.mx < 0) {
           const int loop = add(NState::Split, -1, next);
@@ -695,7 +879,11 @@ class NfaBuilder {
         int entry = -1;
         for (size_t i = seqs.size(); i-- > 0;) {
           int s = next;
-          for (size_t j = seqs[i].size(); j-- > 0;) s = add(NState::Byte, s, -1, seqs[i][j].first, seqs[i][j].second);
+          const size_t len = seqs[i].size();
+          for (size_t k = 0; k < len; k++) {
+            const size_t j = rev ? k : len - 1 - k;
+            s = add(NState::Byte, s, -1, seqs[i][j].first, seqs[i][j].second);
+          }
           entry = entry < 0 ? s : add(NState::Split, s, entry);
         }
         return entry;
@@ -707,28 +895,34 @@ class NfaBuilder {
  private:
   static const size_t kMaxNfa = 1 << 18;
   const Parser& p_;
+  NfaMode mode_;
 };
 
 // ---- subset construction ---------------------------------------------------------------------------------------------------
+// byte equivalence classes: bytes no Byte state tells apart.  Writes the 256-entry byte -> class map as the blob's head and
+// one representative byte per class; returns the number of classes.
+inline uint32_t byte_classes(const std::vector<NState>& nfa, std::vector<uint8_t>& blob, std::vector<uint8_t>& rep) {
+  bool brk[257] = {false};
+  for (auto& s : nfa)
+    if (s.k == NState::Byte) brk[s.lo] = brk[(int)s.hi + 1] = true;
+  blob.assign(256, 0);
+  uint32_t cls = 0;
+  for (int b = 0; b < 256; b++) {
+    if (b > 0 && brk[b]) cls++;
+    blob[(size_t)b] = (uint8_t)cls;
+    if (rep.size() == cls) rep.push_back((uint8_t)b);
+  }
+  return cls + 1;
+}
+
 class DfaBuilder {
  public:
   DfaBuilder(const std::vector<NState>& nfa, int start, const Parser& p) : nfa_(nfa), start_(start), p_(p), mark_(nfa.size(), 0) {}
 
   Dfa build() {
-    // byte equivalence classes: bytes no Byte state tells apart
-    bool brk[257] = {false};
-    for (auto& s : nfa_)
-      if (s.k == NState::Byte) brk[s.lo] = brk[(int)s.hi + 1] = true;
     Dfa d;
-    d.blob.assign(256, 0);
-    uint32_t cls = 0;
     std::vector<uint8_t> rep;
-    for (int b = 0; b < 256; b++) {
-      if (b > 0 && brk[b]) cls++;
-      d.blob[(size_t)b] = (uint8_t)cls;
-      if (rep.size() == cls) rep.push_back((uint8_t)b);
-    }
-    d.n_cls = cls + 1;
+    d.n_cls = byte_classes(nfa_, d.blob, rep);
     n_cls_ = d.n_cls;
     keys_.clear();
     states_.clear();
@@ -830,6 +1024,148 @@ class DfaBuilder {
   }
 };
 
+// ---- span DFAs (regexp_count, regexp_replace) ---------------------------------------------------------------------------
+// The same blob layout as the is_match DFA, but no state is absorbing: a flags byte per state (kSpanHere, kSpanAtEdge),
+// state 0 dead, states 1 and 2 the two start states (kSpanStartEdge, kSpanStartInside).
+//   forward (kNfaForward NFA, unanchored): the state after reading s[pos..i) is the ordered thread list of a Pike VM
+//     running leftmost-first.  The closure follows splits in priority order and stops at the first Match: every thread of
+//     lower priority, the restart of the unanchored search included, is dropped.  The restart (a new match beginning at
+//     the next byte) is a flag of the state, the last item of the list; once any match was seen it is gone for good.
+//     kSpanHere: a match ends at i; kSpanAtEdge: a match ends at i if i is the end of the text.  Start states: at
+//     offset 0 (^ holds) or not.
+//   reverse (kNfaReverse NFA, anchored at the match end, every thread kept): the state after reading s[j..end) backwards.
+//     kSpanHere: s[j..end) matches; kSpanAtEdge: it matches if j is offset 0 (the original ^ holds).  Start states: the
+//     walk begins at the end of the text (the original $ holds) or not.
+class SpanDfaBuilder {
+ public:
+  SpanDfaBuilder(const std::vector<NState>& nfa, int start, const Parser& p, bool forward)
+      : nfa_(nfa), start_(start), p_(p), forward_(forward), mark_(nfa.size(), 0) {}
+
+  Dfa build() {
+    Dfa d;
+    std::vector<uint8_t> rep;
+    d.n_cls = byte_classes(nfa_, d.blob, rep);
+    n_cls_ = d.n_cls;
+    states_.push_back(SState());  // dead
+    std::vector<int> fr;
+    // a restart that reaches nothing (every match needs ^) is left out, so such a search stops at its first dead end
+    const bool restart_useful = forward_ && (closure({start_}, false, false, fr) || !fr.empty());
+    for (int k = 0; k < 2; k++) {  // kSpanStartEdge, kSpanStartInside: always their own slots
+      const bool edge = k == 0;
+      const bool m = closure({start_}, edge, false, fr);
+      add_state(fr, edge, m, restart_useful && !m);
+    }
+    std::vector<uint16_t> trans;
+    for (size_t i = 0; i < states_.size(); i++) {
+      for (uint32_t c = 0; c < d.n_cls; c++) {
+        if (i == kDead) {
+          trans.push_back((uint16_t)kDead);
+          continue;
+        }
+        std::vector<int> seed;
+        for (int s : states_[i].fr)
+          if (nfa_[(size_t)s].k == NState::Byte && rep[c] >= nfa_[(size_t)s].lo && rep[c] <= nfa_[(size_t)s].hi) seed.push_back(nfa_[(size_t)s].a);
+        const bool restart = states_[i].restart;
+        if (restart) seed.push_back(start_);  // lowest priority: a match beginning at the next byte
+        std::vector<int> nf;
+        const bool m = closure(seed, false, false, nf);
+        trans.push_back((uint16_t)intern(nf, false, m, restart && !m));
+      }
+    }
+    d.n_states = (uint32_t)states_.size();
+    d.start = kSpanStartEdge;
+    d.blob.resize(dfa_trans_offset(d.n_states), 0);
+    for (size_t i = 1; i < states_.size(); i++) d.blob[256 + i] = states_[i].flags;
+    const size_t off = d.blob.size();
+    d.blob.resize(off + trans.size() * 2);
+    memcpy(d.blob.data() + off, trans.data(), trans.size() * 2);
+    return d;
+  }
+
+ private:
+  struct SState {
+    std::vector<int> fr;  // Byte and (unpassed) End states: in priority order (forward) or sorted (reverse)
+    bool at_start = false, matched = false, restart = false;
+    uint8_t flags = 0;
+  };
+  typedef std::pair<std::vector<int>, int> Key;
+  const std::vector<NState>& nfa_;
+  int start_;
+  const Parser& p_;
+  bool forward_;
+  std::vector<uint32_t> mark_;
+  uint32_t gen_ = 0;
+  uint32_t n_cls_ = 1;
+  uint64_t work_ = 0;
+  static const uint64_t kMaxWork = (uint64_t)1 << 25;
+  std::map<Key, uint32_t> keys_;
+  std::vector<SState> states_;
+
+  uint32_t add_state(const std::vector<int>& fr, bool at_start, bool matched, bool restart) {
+    const uint32_t id = (uint32_t)states_.size();
+    if (id >= kMaxStates) p_.unsupported("a pattern whose DFA exceeds " + std::to_string(kMaxStates) + " states");
+    if ((uint64_t)(id + 1) * n_cls_ * 2 > kMaxTransBytes)
+      p_.unsupported("a pattern whose DFA table exceeds 1 MiB (over " + std::to_string(id) + " states x " + std::to_string(n_cls_) + " byte classes)");
+    SState s;
+    s.fr = fr;
+    s.at_start = at_start;
+    s.matched = matched;
+    s.restart = restart;
+    std::vector<int> ignored;
+    s.flags = (uint8_t)((matched ? kSpanHere : 0) | ((matched || closure(fr, at_start, true, ignored)) ? kSpanAtEdge : 0));
+    states_.push_back(s);
+    keys_.emplace(Key(fr, (at_start ? 1 : 0) | (matched ? 2 : 0) | (restart ? 4 : 0)), id);
+    return id;
+  }
+  uint32_t intern(const std::vector<int>& fr, bool at_start, bool matched, bool restart) {
+    if (fr.empty() && !matched && !restart) return kDead;
+    auto it = keys_.find(Key(fr, (at_start ? 1 : 0) | (matched ? 2 : 0) | (restart ? 4 : 0)));
+    if (it != keys_.end()) return it->second;
+    return add_state(fr, at_start, matched, restart);
+  }
+  // epsilon closure of `seed`, each seed in turn and depth first along the splits' priority.  Forward: stops at the first
+  // Match (the threads after it lose to it).  Reverse: explores everything and sorts the frontier.  Says whether Match
+  // was reached.
+  bool closure(const std::vector<int>& seed, bool at_start, bool at_end, std::vector<int>& fr) {
+    gen_++;
+    fr.clear();
+    bool matched = false;
+    std::vector<int> stack;
+    for (int sd : seed) {
+      stack.assign(1, sd);
+      while (!stack.empty()) {
+        const int s = stack.back();
+        stack.pop_back();
+        if (++work_ > kMaxWork) p_.unsupported("a pattern this expensive to compile (its DFA construction exceeds " + std::to_string(kMaxWork) + " steps)");
+        if (s < 0 || mark_[(size_t)s] == gen_) continue;
+        mark_[(size_t)s] = gen_;
+        const NState& n = nfa_[(size_t)s];
+        switch (n.k) {
+          case NState::Byte: fr.push_back(s); break;
+          case NState::Match:
+            matched = true;
+            if (forward_) return true;
+            break;
+          case NState::Eps: stack.push_back(n.a); break;
+          case NState::Split:
+            stack.push_back(n.b);
+            stack.push_back(n.a);
+            break;
+          case NState::Start:
+            if (at_start) stack.push_back(n.a);
+            break;
+          case NState::End:
+            if (at_end) stack.push_back(n.a);
+            else fr.push_back(s);
+            break;
+        }
+      }
+    }
+    if (!forward_) std::sort(fr.begin(), fr.end());
+    return matched;
+  }
+};
+
 inline Dfa compile_node(const Parser& p, const Node& root) {
   NfaBuilder nb(p);
   const int match = nb.add(NState::Match);
@@ -852,20 +1188,44 @@ inline int compile_regex(const std::string& pattern, bool ci, bool dotall, Dfa& 
   }
 }
 
-// regexp_like's flags argument: only i and s [EXT]
-inline int parse_regex_flags(const std::string& flags, bool& ci, bool& dotall, std::string& err) {
+// The forward (leftmost-first, unanchored) and reverse (anchored at a match end) span DFAs of `pattern` under the flags i
+// and s: what regexp_count and regexp_replace walk (dfa_next_match).  Same return codes and messages as compile_regex.
+inline int compile_regex_spans(const std::string& pattern, bool ci, bool dotall, Dfa& fwd, Dfa& rev, std::string& err) {
+  try {
+    Parser p(pattern, pattern);
+    Node root = p.parse(ci, dotall);
+    for (int k = 0; k < 2; k++) {
+      NfaBuilder nb(p, k == 0 ? kNfaForward : kNfaReverse);
+      const int match = nb.add(NState::Match);
+      const int start = nb.compile(root, match);
+      SpanDfaBuilder db(nb.st, start, p, k == 0);
+      (k == 0 ? fwd : rev) = db.build();
+    }
+    return RX_OK;
+  } catch (const Error& e) {
+    err = e.msg;
+    return e.code;
+  }
+}
+
+// The flags argument of regexp_like, regexp_count and regexp_replace (`fn` names the function): only i and s [EXT], and g
+// where `global` is given (regexp_replace); the other functions refuse g as DataFusion does.
+inline int parse_regex_flags(const std::string& flags, bool& ci, bool& dotall, std::string& err, const char* fn = "regexp_like",
+                             bool* global = nullptr) {
   ci = dotall = false;
+  if (global) *global = false;
   for (char c : flags) {
     if (c == 'i') ci = true;
     else if (c == 's') dotall = true;
+    else if (c == 'g' && global) *global = true;
     else if (c == 'g') {
-      err = "regexp_like does not support the \"global\" option (flag 'g')";
+      err = std::string(fn) + " does not support the \"global\" option (flag 'g')";
       return RX_INVALID;
     } else if (c == 'm' || c == 'x' || c == 'U' || c == 'u' || c == 'R') {
-      err = std::string("regexp_like: the flag '") + c + "' is not supported by the device engine";
+      err = std::string(fn) + ": the flag '" + c + "' is not supported by the device engine";
       return RX_UNSUPPORTED;
     } else {
-      err = std::string("regexp_like: unrecognized flag '") + c + "' in '" + flags + "'";
+      err = std::string(fn) + ": unrecognized flag '" + c + "' in '" + flags + "'";
       return RX_INVALID;
     }
   }

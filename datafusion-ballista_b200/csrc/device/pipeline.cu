@@ -956,6 +956,81 @@ __device__ __noinline__ void scalar_build_op(const Lane L, const uint32_t active
   store_valid(L, ins.dst, vout);
 }
 
+// the span DFAs of OP_REGEX_COUNT / OP_REGEX_REPLACE: two consecutive immediates from ins.imm on
+__device__ __forceinline__ rx::RxSpans regex_spans(const VInstr& ins) {
+  const ImmDesc& f = PROG.imms[ins.imm];
+  const ImmDesc& b = PROG.imms[ins.imm + 1];
+  rx::RxSpans d;
+  d.fwd = (const uint8_t*)f.lo;
+  d.fwd_shape = f.hi;
+  d.rev = (const uint8_t*)b.lo;
+  d.rev_shape = b.hi;
+  return d;
+}
+
+// regexp_count: one thread per row slot counts 0 for an empty row, else skips start - 1 code points, then loops forward
+// walk -> reverse walk -> iteration rule (regex_dfa.hpp regexp_count_row, the walk the host compiler's tests run).  A NULL
+// row counts 0: the result is never NULL.
+__device__ __noinline__ void scalar_regex_count_op(const Lane L, const uint32_t active, const int pc) {
+  const VInstr ins = PROG.code[pc];
+  const uint32_t live = active & fetch_valid(L, ins.a);
+  const rx::RxSpans d = regex_spans(ins);
+  const uint32_t skip = PROG.imms[ins.imm]._pad;
+#pragma unroll 1
+  for (int r = 0; r < VM_R; r++) {
+    int64_t c = 0;
+    if ((live >> r) & 1) {
+      const StrRef a = ld1_str(L, ins.a, r);
+      c = rx::regexp_count_row(d, a.p, a.len, skip);
+    }
+    st1_i64(L, ins.dst, r, c);
+  }
+  store_valid(L, ins.dst, 0xFFFFFFFFu);
+}
+
+// regexp_replace: the string builders' protocol (scalar_build_op) -- a length pass over the row's matches, one warp
+// reservation, then a write pass.  An input that is itself unwritten (an earlier builder's row that did not fit) counts
+// the bound len + (len + 1) * |replacement| (g) or len + |replacement|, so the re-run's arena holds the row.
+__device__ __noinline__ void scalar_regex_replace_op(const Lane L, const uint32_t active, const int pc) {
+  const VInstr ins = PROG.code[pc];
+  const uint32_t vout = fetch_valid(L, ins.a);
+  const uint32_t live = active & vout;
+  const rx::RxSpans d = regex_spans(ins);
+  const bool global = ins.aux != 0;
+  bool wrote = false;
+#pragma unroll 1
+  for (int r = 0; r < VM_R; r++) {
+    const bool lv = (live >> r) & 1;
+    unsigned long long len = 0;
+    BuildSrc a;
+    a.p = nullptr;
+    a.len = 0;
+    a.unwritten = false;
+    StrRef rep;
+    rep.p = nullptr;
+    rep.len = 0;
+    if (lv) {
+      a = ld_build_src(L, ins.a, r);
+      rep = ld1_str(L, ins.b, r);
+      if (a.unwritten) len = a.len + (global ? ((unsigned long long)a.len + 1) : 1ull) * rep.len;
+      else len = rx::dfa_replace(d, a.p, a.len, rep.p, rep.len, global, nullptr);
+      if (len > 0x7FFFFFFFull) {
+        raise(7);
+        len = 0;
+      }
+    }
+    const unsigned long long base = arena_reserve(len);
+    uint8_t* out = lv ? arena_at(base, len, a.unwritten) : nullptr;
+    if (out && len) {
+      wrote = true;
+      rx::dfa_replace(d, a.p, a.len, rep.p, rep.len, global, out);
+    }
+    store_built(L, ins.dst, r, lv ? out : PROG.arena, lv ? len : 0);
+  }
+  if (wrote) __threadfence();
+  store_valid(L, ins.dst, vout);
+}
+
 // ------------------------------------------------------------------------------------------------
 // Cold operations: one rolled loop over the thread's rows; every body exists once in the binary.
 // ------------------------------------------------------------------------------------------------
@@ -966,6 +1041,8 @@ __device__ __noinline__ void cold_op(const Lane L, const uint32_t active, const 
     if (op <= OP_CEIL) scalar_num_op(L, active, pc);
     else if (op == OP_NULLIF) scalar_nullif_op(L, active, pc);
     else if (op == OP_REGEX) scalar_regex_op(L, active, pc);
+    else if (op == OP_REGEX_COUNT) scalar_regex_count_op(L, active, pc);
+    else if (op == OP_REGEX_REPLACE) scalar_regex_replace_op(L, active, pc);
     else if (op > OP_REGEX) scalar_build_op(L, active, pc);
     else if (op >= OP_BIT_AND) scalar_bit_op(L, active, pc);
     else scalar_str_op(L, active, pc);

@@ -94,7 +94,12 @@ enum VOp : uint8_t {
   OP_CONCAT,    // imm: first immediate of the argument operands (below); aux: BUILD_* flags; a: separator (BUILD_WS)
   OP_REPEAT,    // a: STR, b: I64 count
   OP_REVERSE,   // a: STR -> its code points in reverse order
-  OP_TO_STR     // CAST(a AS Utf8); aux = ToStrKind; imm = scale (TS_DEC128)
+  OP_TO_STR,    // CAST(a AS Utf8); aux = ToStrKind; imm = scale (TS_DEC128)
+  // regexp_count and regexp_replace over the span DFAs (regex_dfa.hpp; DESIGN.md §6 (xiii)).  imm: two consecutive
+  // immediates, the forward DFA and the reverse one (device pointer in lo, shape in hi); the first one's _pad holds the
+  // code points the count skips (start - 1, saturated)
+  OP_REGEX_COUNT,   // a: STR -> I64, never NULL (scalar_regex_count_op)
+  OP_REGEX_REPLACE  // a: STR, b: the replacement (STR literal) -> STR in the arena; aux: 1 = every match (g) (scalar_regex_replace_op)
 };
 enum BuildFlags : uint8_t {
   BUILD_NULLS = 1,  // `||`: NULL if any argument is NULL (else NULL arguments are skipped: concat, concat_ws)

@@ -993,6 +993,7 @@ static void throw_run_error(unsigned int error) {
   if (error == 4) throw EngineError(B200_ERR_EXECUTION, "concat: a result row is longer than 2147483647 bytes");
   if (error == 5) throw EngineError(B200_ERR_EXECUTION, "repeat: a result row is longer than 2147483647 bytes");
   if (error == 6) throw EngineError(B200_ERR_EXECUTION, "CAST(Date32 AS Utf8): a date outside chrono's range (years -262144..262143)");
+  if (error == 7) throw EngineError(B200_ERR_EXECUTION, "regexp_replace: a result row is longer than 2147483647 bytes");
   if (error) throw EngineError(B200_ERR_EXECUTION, "execution error in expression");
 }
 

@@ -239,6 +239,7 @@ class PipelineBuilder {
       }
       case Expr::Fn: {
         if (e.fn == "regexp_like") return compile_regex(e);
+        if (e.fn == "regexp_count" || e.fn == "regexp_replace") return compile_regex_fn(e);
         if (is_string_builder(e.fn)) return compile_build_fn(e);
         const int part = date_part_index(e.fn);
         if (part >= 0) return unary_fn(e, OP_DATE_PART, VK_I64, (uint8_t)part, 0);
@@ -431,6 +432,54 @@ class PipelineBuilder {
     ins.dst = r.op;
     ins.aux = kind;
     ins.imm = kind == TS_DEC128 ? t.scale : 0;
+    ins.flags = IF_NULLCHK;
+    emit(ins);
+    release(a);
+    return r;
+  }
+
+  // regexp_count (OP_REGEX_COUNT, I64) and regexp_replace (OP_REGEX_REPLACE, a string builder) over the span DFAs typing
+  // compiled; typing left them null where every row is 0 (count) or NULL (replace)
+  ColRef compile_regex_fn(const Expr& e) {
+    const bool count = e.fn == "regexp_count";
+    if (!e.regex || e.args[0]->type.id == TypeId::Null) {
+      if (!count) return null_of(e.type);
+      LitValue zero;
+      return literal(DataType(TypeId::Int64), zero);
+    }
+    if (!regex_) throw EngineError(B200_ERR_UNSUPPORTED, "regular expressions are not evaluated in this pipeline");
+    ImmDesc d[2];
+    memset(d, 0, sizeof d);
+    d[0].lo = (uint64_t)regex_->get("fwd:" + e.regex_key, *e.regex, st_);
+    d[0].hi = e.regex->shape();
+    d[0]._pad = (uint32_t)std::min<int64_t>(e.regex_start - 1, 0xFFFFFFFFll);
+    d[1].lo = (uint64_t)regex_->get("rev:" + e.regex_key, *e.regex_rev, st_);
+    d[1].hi = e.regex_rev->shape();
+    if (prog.n_imms + 2 > VM_MAX_IMMS) throw EngineError(B200_ERR_UNSUPPORTED, "too many literals in one pipeline");
+    const int imm = prog.n_imms;
+    prog.imms[prog.n_imms++] = d[0];
+    prog.imms[prog.n_imms++] = d[1];
+    ColRef a = compile(*e.args[0]);
+    ColRef r;
+    VInstr ins = blank(count ? OP_REGEX_COUNT : OP_REGEX_REPLACE, VK_STR);
+    ins.imm = imm;
+    if (count) {
+      r = new_reg(DataType(TypeId::Int64), true);
+    } else {
+      const uint64_t rep = e.args[2]->lit.s.size();
+      // per row len + (len + 1) * |replacement| with g, len + |replacement| without
+      const uint64_t bound = e.regex_global ? sat_add(a.str_bound, sat_mul(sat_add(a.str_bound, rows()), rep))
+                                            : sat_add(a.str_bound, sat_mul(rows(), rep));
+      pin(a);
+      ColRef b = compile(*e.args[2]);
+      unpin(a);
+      ins.b = resolve(b);
+      ins.aux = e.regex_global ? 1 : 0;
+      r = built_reg(a.nullable, bound);
+      release(b);
+    }
+    ins.a = resolve(a);
+    ins.dst = r.op;
     ins.flags = IF_NULLCHK;
     emit(ins);
     release(a);

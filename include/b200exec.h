@@ -77,8 +77,8 @@ uint64_t b200_engine_kernel_launches(b200_engine* e);
 /* Introspection for tests and bench.py: how many pipelines ran on which kernel family so far.
  * name: "fused" (fused.cuh kernel, any variant), "fused_static" (an ahead-of-time shape),
  * "vm" (tile VM pipeline_kernel); "ingest_bytes_saved": host->device bytes NOT sent because
- * Decimal128 values were narrowed on the host and widened on the device; "regex_compiles": regex DFAs (ILIKE, ~, regexp_like)
- * uploaded to the device, once per pattern and flags for the engine's lifetime; "string_arena_retries": pipeline launches
+ * Decimal128 values were narrowed on the host and widened on the device; "regex_compiles": regex DFAs (ILIKE, ~, regexp_like;
+ * two per pattern for regexp_count / regexp_replace) uploaded to the device, once per pattern and flags for the engine's lifetime; "string_arena_retries": pipeline launches
  * run again because the character arena of their string builders (concat, ||, concat_ws, repeat, reverse, casts to Utf8)
  * was too small.  Unknown names return 0. */
 uint64_t b200_engine_counter(b200_engine* e, const char* name);
