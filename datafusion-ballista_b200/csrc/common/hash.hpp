@@ -50,6 +50,34 @@ B200_HD uint64_t hash_f64(double d) {
   return mix64(bits + kHashSeed);
 }
 
+// Float32 <-> Float64 that keep every bit of a Float32, for group keys and MIN / MAX, which must give back the input's
+// bits.  The hardware widening sets a signalling NaN's quiet bit (0x7F800001 and 0x7FC00001 would both become
+// 0x7FF8000020000000), so a NaN is widened from its bits: sign, all-ones exponent, the 23 payload bits on top of the 52.
+// The narrowing is its inverse; a NaN whose top 23 payload bits are zero (made by Float64 arithmetic, not by a widened
+// Float32) narrows as the hardware does.  The widening keeps the IEEE total order of the Float32 bit patterns.
+B200_HD uint64_t f32_bits_to_f64_bits(uint32_t b) {
+  const uint32_t a = b & 0x7FFFFFFFu;
+  if (a > 0x7F800000u) return ((uint64_t)(b >> 31) << 63) | 0x7FF0000000000000ull | ((uint64_t)(a & 0x7FFFFFu) << 29);
+  float f;
+  double d;
+  uint64_t r;
+  memcpy(&f, &b, 4);
+  d = (double)f;
+  memcpy(&r, &d, 8);
+  return r;
+}
+B200_HD uint32_t f64_bits_to_f32_bits(uint64_t b) {
+  const uint32_t pay = (uint32_t)(b >> 29) & 0x7FFFFFu;
+  if ((b & 0x7FFFFFFFFFFFFFFFull) > 0x7FF0000000000000ull && pay) return ((uint32_t)(b >> 63) << 31) | 0x7F800000u | pay;
+  double d;
+  float f;
+  uint32_t r;
+  memcpy(&d, &b, 8);
+  f = (float)d;
+  memcpy(&r, &f, 4);
+  return r;
+}
+
 B200_HD uint64_t hash_i128(uint64_t lo, uint64_t hi) {
   // values that fit in 64 bits (sign-extended) hash like the same i64
   if ((int64_t)hi == ((int64_t)lo >> 63)) return hash_i64((int64_t)lo);

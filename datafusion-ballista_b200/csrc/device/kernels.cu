@@ -133,7 +133,7 @@ __global__ void agg_extract_kernel(AggTable T, AggExtractArgs A) {
           unsigned char v = T.key_valid[(unsigned long long)o.a * T.cap + s];
           if (o.phys == PH_DEC128 || o.phys == PH_STRVIEW) ((ulonglong2*)o.data)[pos] = make_ulonglong2(w0, w1);
           else if (o.phys == PH_F64) ((unsigned long long*)o.data)[pos] = w0;
-          else if (o.phys == PH_F32) ((float*)o.data)[pos] = (float)__longlong_as_double((long long)w0);
+          else if (o.phys == PH_F32) ((uint32_t*)o.data)[pos] = f64_bits_to_f32_bits(w0);
           else store_typed_i64(o.data, o.phys, pos, (long long)w0);
           if (o.valid) o.valid[pos] = v;
           break;
@@ -168,22 +168,19 @@ __global__ void agg_extract_kernel(AggTable T, AggExtractArgs A) {
               store_typed_i64(o.data, o.phys, pos, (long long)lo);
               ok = true;
               break;
-            case AO_MINMAX_F64: ((double*)o.data)[pos] = f64_from_key((long long)lo); break;
+            case AO_MINMAX_F64: {
+              const double v = f64_from_key((long long)lo);
+              if (o.phys == PH_F32) ((uint32_t*)o.data)[pos] = f64_bits_to_f32_bits((uint64_t)__double_as_longlong(v));
+              else ((double*)o.data)[pos] = v;
+              break;
+            }
             case AO_MINMAX_STR:
               ok = ok && hi != ACC_STR_NONE;
               ((ulonglong2*)o.data)[pos] = ok ? make_ulonglong2(lo, hi) : make_ulonglong2(0ull, 0ull);
               break;
             case AO_AVG_DEC: {
-              i128 sum = mk128(lo, hi);
               i128 res = 0;
-              if (ok) {
-                // DecimalAverager::avg [EXT]: sum * 10^imm / count, truncating; overflow is an error
-                i128 mul = 1;
-                for (int k = 0; k < o.imm; k++) mul *= 10;
-                i128 lim = ((i128)1 << 126) / (mul > 0 ? mul : 1);
-                if (sum > lim || sum < -lim) atomicMax(A.error, 1u);
-                res = (sum * mul) / (i128)cnt;
-              }
+              if (ok && !avg_decimal(mk128(lo, hi), cnt, o.imm, o.prec, &res)) atomicMax(A.error, 1u);
               ((ulonglong2*)o.data)[pos] = make_ulonglong2((unsigned long long)res, (unsigned long long)((u128)res >> 64));
               break;
             }

@@ -66,8 +66,22 @@ struct AggOut {
   uint8_t phys;   // output encoding
   int32_t imm;
   uint8_t st[6];  // AO_STAT: count acc, sum-x acc, sum-y acc, xx / yy / xy co-moment columns
-  uint8_t _pad[2];
+  uint8_t prec;   // AO_AVG_DEC: result precision
+  uint8_t _pad;
 };
+#ifdef __CUDACC__
+// DecimalAverager::avg [EXT]: sum * 10^k / count, truncating toward zero, for the grouped and the window AVG.  Returns
+// false (an overflow error) when sum * 10^k leaves the i128 range or the quotient has more than `prec` digits.
+__device__ __forceinline__ bool avg_decimal(__int128 sum, unsigned long long count, int k, int prec, __int128* out) {
+  __int128 mul = 1, lim = 1;
+  for (int i = 0; i < k; i++) mul *= 10;
+  for (int i = 0; i < prec; i++) lim *= 10;
+  const __int128 max = (__int128)(~(unsigned __int128)0 >> 1), min = -max - 1;
+  if (sum > max / mul || sum < min / mul) return false;
+  *out = sum * mul / (__int128)count;
+  return *out < lim && *out > -lim;
+}
+#endif
 struct AggExtractArgs {
   AggOut out[VM_MAX_OUT];
   int n_out;
@@ -517,6 +531,7 @@ struct WinEval {
   uint8_t fn, units, s_kind, e_kind;
   uint8_t acc, op, read, fin;
   uint8_t out_phys;
+  uint8_t prec;         // WFIN_AVG over Decimal128: result precision
   int32_t imm;          // WFIN_AVG over Decimal128: result scale - input scale
   int64_t s_off, e_off;
   int64_t arg;          // WF_NTILE: n; WF_NTH: n; WF_OFFSET: signed distance (LEAD +k, LAG -k)

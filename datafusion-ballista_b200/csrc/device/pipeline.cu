@@ -312,7 +312,8 @@ __device__ __noinline__ double ld1_f64(const Lane L, const Operand o, int r) {
   if (o.kind == OPD_COL) {
     const ColDesc& cd = PROG.cols[o.idx];
     const uint8_t* base = L.stage + cd.smem_off;
-    return cd.phys == PH_F32 ? (double)((const float*)base)[e] : ((const double*)base)[e];
+    if (cd.phys == PH_F32) return __longlong_as_double((long long)f32_bits_to_f64_bits(((const uint32_t*)base)[e]));
+    return ((const double*)base)[e];
   }
   if (o.kind == OPD_REG) return ((const double*)(L.regs + PROG.regs[o.idx].smem_off))[e];
   return __longlong_as_double((long long)PROG.imms[o.idx].lo);
@@ -2113,7 +2114,7 @@ __device__ __forceinline__ void sink_materialize(const Lane L, const uint32_t ac
       fetch_f64(L, oc.src, a);
       if (oc.phys == PH_F32) {
 #pragma unroll
-        FOR_R if ((active >> r) & 1) ((float*)oc.data)[pos[r]] = (float)a[r];
+        FOR_R if ((active >> r) & 1) ((uint32_t*)oc.data)[pos[r]] = f64_bits_to_f32_bits((uint64_t)__double_as_longlong(a[r]));
       } else {
 #pragma unroll
         FOR_R if ((active >> r) & 1) ((double*)oc.data)[pos[r]] = a[r];
@@ -2171,10 +2172,7 @@ __device__ __forceinline__ bool key_equal(const KeyVal& a, unsigned long long w0
     return str_eq(x, y);
   }
   if (a.vk == VK_I128) return a.w0 == w0 && a.w1 == w1;
-  if (a.vk == VK_F64) {
-    double p = __longlong_as_double((long long)a.w0), q = __longlong_as_double((long long)w0);
-    return (p == q) || (p != p && q != q);
-  }
+  // every other key, floats included, by its 64-bit image: -0.0 and 0.0 are two groups, NaNs one per payload (DESIGN §6)
   return a.w0 == w0;
 }
 
@@ -2328,7 +2326,7 @@ __device__ __noinline__ void load_key(const Lane L, const Operand ko, int r, Key
     out->w1 = hi64(a);
   } else if (ko.vk == VK_F64) {
     double a = ld1_f64(L, ko, r);
-    out->w0 = (unsigned long long)__double_as_longlong(a == 0.0 ? 0.0 : a);
+    out->w0 = (unsigned long long)__double_as_longlong(a);
   } else {
     out->w0 = (unsigned long long)ld1_i64(L, ko, r);
   }

@@ -372,14 +372,7 @@ template <>
 __device__ void win_finish<i128>(const WinEval& E, const WElem<i128>& r, int64_t o) {
   const bool ok = r.c > 0;
   i128 v = ok ? r.v : 0;
-  if (ok && E.fin == WFIN_AVG) {
-    // DecimalAverager::avg [EXT]: sum * 10^imm / count, truncating; overflow is an error (as the grouped AVG)
-    i128 mul = 1;
-    for (int k = 0; k < E.imm; k++) mul *= 10;
-    const i128 lim = ((i128)1 << 126) / mul;
-    if (v > lim || v < -lim) atomicMax(E.error, 1u);
-    v = (v * mul) / (i128)r.c;
-  }
+  if (ok && E.fin == WFIN_AVG && !avg_decimal(r.v, (unsigned long long)r.c, E.imm, E.prec, &v)) atomicMax(E.error, 1u);
   ((ulonglong2*)E.out)[o] = make_ulonglong2((unsigned long long)v, (unsigned long long)((u128)v >> 64));
   E.out_valid[o] = ok ? 1 : 0;
 }

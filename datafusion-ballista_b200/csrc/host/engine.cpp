@@ -2462,6 +2462,7 @@ DevBatchPtr run_aggregate(const Exec& x, const BuilderFactory& make_pb, const Pl
     o.b = r.b;
     o.phys = r.phys;
     o.imm = r.imm;
+    o.prec = r.type.precision;
     memcpy(o.st, r.st, sizeof o.st);
     wbytes += (uint64_t)oc.width() * n_groups;
     out->cols.push_back(oc);
@@ -2985,6 +2986,7 @@ struct Runner {
           if (we.fn == WinFn::Avg) {
             E.fin = WFIN_AVG;
             E.imm = we.result_type.scale - at.scale;
+            E.prec = we.result_type.precision;
           }
           break;
         default:  // Min, Max

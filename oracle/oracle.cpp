@@ -178,7 +178,11 @@ OBatch import_batch(ArrowArray* arr, ArrowSchema* sch) {
         case TypeId::Int64:
         case TypeId::Timestamp: c.i[r] = ((const int64_t*)ic.data)[p]; break;
         case TypeId::UInt64: c.i[r] = (int64_t)((const uint64_t*)ic.data)[p]; break;
-        case TypeId::Float32: c.f[r] = ((const float*)ic.data)[p]; break;
+        case TypeId::Float32: {
+          const uint64_t w = f32_bits_to_f64_bits(((const uint32_t*)ic.data)[p]);
+          memcpy(&c.f[r], &w, 8);
+          break;
+        }
         case TypeId::Float64: c.f[r] = ((const double*)ic.data)[p]; break;
         case TypeId::Decimal128: memcpy(&c.d[r], ic.data + 16 * p, 16); break;
         case TypeId::Utf8: {
@@ -245,7 +249,9 @@ void export_batch(const OBatch& b, const Schema* names, ArrowArray* out, ArrowSc
       case TypeId::Float32:
         h.data.resize(n * 4);
         for (size_t r = 0; r < n; r++) {
-          float v = (float)c.f[r];
+          uint64_t w;
+          memcpy(&w, &c.f[r], 8);
+          const uint32_t v = f64_bits_to_f32_bits(w);
           memcpy(&h.data[r * 4], &v, 4);
         }
         break;
@@ -743,9 +749,9 @@ OCol eval(const Expr& e, const OBatch& b) {
 // ------------------------------------------------------------------------------------------------
 // Row key encoding (group-by / join keys)
 // ------------------------------------------------------------------------------------------------
-// float_bits: floats are encoded by their bit pattern (join keys: equal when `=` says so, -0.0 <> 0.0, NaN = NaN only
-// with the same payload); otherwise +-0.0 and every NaN are one group key
-static inline bool encode_key_col(const OCol& c, size_t r, std::string& out, bool float_bits = false) {
+// floats are encoded by their bit pattern, for group and join keys alike: equal when `=` says so, -0.0 <> 0.0, NaN = NaN
+// only with the same payload
+static inline bool encode_key_col(const OCol& c, size_t r, std::string& out) {
   if (!c.is_valid(r)) {
     out.push_back('\0');
     return false;
@@ -754,15 +760,7 @@ static inline bool encode_key_col(const OCol& c, size_t r, std::string& out, boo
   switch (c.type.pk()) {
     case PK::Bool:
     case PK::I64: out.append((const char*)&c.i[r], 8); break;
-    case PK::F64: {
-      double v = c.f[r];
-      if (!float_bits) {
-        if (v == 0.0) v = 0.0;
-        if (v != v) v = std::nan("");
-      }
-      out.append((const char*)&v, 8);
-      break;
-    }
+    case PK::F64: out.append((const char*)&c.f[r], 8); break;
     case PK::I128: out.append((const char*)&c.d[r], 16); break;
     case PK::Str: {
       uint32_t len = (uint32_t)c.s[r].size();
@@ -783,12 +781,6 @@ bool encode_key(const std::vector<const OCol*>& keys, size_t r, std::string& out
   out.clear();
   bool all_valid = true;
   for (auto* c : keys) all_valid &= encode_key_col(*c, r, out);
-  return all_valid;
-}
-static bool encode_join_key(const std::vector<OCol>& keys, size_t r, std::string& out) {  // same, floats by their bits
-  out.clear();
-  bool all_valid = true;
-  for (auto& c : keys) all_valid &= encode_key_col(c, r, out, true);
   return all_valid;
 }
 
@@ -1053,9 +1045,12 @@ OBatch do_aggregate(const PlanNode& node, const OBatch& in) {
               continue;
             }
             if (ae.result_type.is_decimal()) {
-              // DecimalAverager::avg [EXT]: sum * 10^(target_scale - sum_scale) / count, truncating
-              i128 v = checked_mul(ac.sd, pow10_i128(ae.result_type.scale - ae.sum_type.scale));
-              c.d[g] = v / (i128)ac.cnt;
+              // DecimalAverager::avg [EXT]: sum * 10^(target_scale - sum_scale) / count, truncating; an overflow of the
+              // product or a quotient beyond the result precision is an error
+              i128 v = checked_mul(ac.sd, pow10_i128(ae.result_type.scale - ae.sum_type.scale)) / (i128)ac.cnt;
+              if (v >= pow10_i128(ae.result_type.precision) || v <= -pow10_i128(ae.result_type.precision))
+                exec_fail("Arithmetic overflow: decimal average");
+              c.d[g] = v;
             } else {
               c.f[g] = ac.f64_sum() / (double)ac.cnt;
             }
@@ -1082,13 +1077,13 @@ OBatch do_hash_join(const PlanNode& node, const OBatch& L, const OBatch& R) {
   std::unordered_map<std::string, std::vector<int64_t>> table;
   std::string k;
   for (size_t r = 0; r < L.n; r++) {
-    bool allv = encode_join_key(lk, r, k);
+    bool allv = encode_key(lk, r, k);
     if (!allv && !node.null_equals_null) continue;
     table[k].push_back((int64_t)r);
   }
   std::vector<int64_t> li, ri;
   for (size_t r = 0; r < R.n; r++) {
-    bool allv = encode_join_key(rk, r, k);
+    bool allv = encode_key(rk, r, k);
     if (!allv && !node.null_equals_null) continue;
     auto it = table.find(k);
     if (it == table.end()) continue;
