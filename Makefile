@@ -10,7 +10,7 @@ OUT       := $(PKG)/lib
 # B200_PLAN_REGEX: ... and ILIKE, the regex operators and regexp_like (plan.hpp)
 # B200_PLAN_STRINGS: ... and concat, ||, concat_ws, repeat and reverse (plan.hpp)
 NVFLAGS   := $(ARCH) -lineinfo -O3 -std=c++17 -Xcompiler -fPIC -Xcompiler -Wno-unused-function -DB200_PLAN_STAT_AGGREGATES=1 -DB200_PLAN_GROUPING_SETS=1 -DB200_PLAN_WINDOW=1 -DB200_PLAN_REGEX=1 -DB200_PLAN_STRINGS=1
-OBJS      := $(OUT)/pipeline.o $(OUT)/kernels.o $(OUT)/shuffle.o $(OUT)/join.o $(OUT)/nlj.o $(OUT)/groupby.o $(OUT)/parquet.o $(OUT)/csv.o $(OUT)/filter.o $(OUT)/window.o $(OUT)/engine.o $(OUT)/host_narrow.o
+OBJS      := $(OUT)/pipeline.o $(OUT)/kernels.o $(OUT)/shuffle.o $(OUT)/join.o $(OUT)/nlj.o $(OUT)/groupby.o $(OUT)/parquet.o $(OUT)/csv.o $(OUT)/json.o $(OUT)/filter.o $(OUT)/window.o $(OUT)/engine.o $(OUT)/host_narrow.o
 CXX       ?= g++
 COMMON    := $(wildcard $(SRC)/common/*.hpp) $(wildcard $(SRC)/device/*.h) $(wildcard $(SRC)/device/*.cuh) $(wildcard $(SRC)/host/*.hpp) include/b200exec.h include/b200_arrow_abi.h
 
@@ -29,6 +29,9 @@ $(OUT)/parquet.o: $(SRC)/device/parquet.cu $(COMMON)
 	@mkdir -p $(OUT)
 	$(NVCC) $(NVFLAGS) -c $< -o $@
 $(OUT)/csv.o: $(SRC)/device/csv.cu $(COMMON)
+	@mkdir -p $(OUT)
+	$(NVCC) $(NVFLAGS) -c $< -o $@
+$(OUT)/json.o: $(SRC)/device/json.cu $(COMMON)
 	@mkdir -p $(OUT)
 	$(NVCC) $(NVFLAGS) -c $< -o $@
 $(OUT)/groupby.o: $(SRC)/device/groupby.cu $(COMMON)

@@ -17,6 +17,8 @@
 // groups are passed through ("file_groups") for the host side to register (b200_engine_register_parquet).
 // CsvScanExecNode -> the same, plus "format": "csv", the reader options ("csv") and, when any file carries a byte range,
 // "file_ranges" shaped like "file_groups" ([start, end] or null), for b200_engine_register_csv.
+// JsonScanExecNode -> the same with "format": "json" and "file_ranges", for b200_engine_register_json: the node carries no
+// reader options (no compression, no JSON-array flag), so it is an uncompressed newline-delimited scan.
 #pragma once
 #include <cstdint>
 #include <cstdio>
@@ -561,10 +563,11 @@ inline std::string plan_json(const Msg& n, const std::string& override_job) {
   auto in = [&](uint32_t f) { return plan_json(m.sub(f)); };
   switch (x->field) {
     case 1:    // ParquetScanExecNode { base_conf = 1 } (:1058-1077)
-    case 2: {  // CsvScanExecNode { base_conf = 1, has_header = 2, delimiter = 3, quote = 4, escape = 5, comment = 6,
+    case 2:    // CsvScanExecNode { base_conf = 1, has_header = 2, delimiter = 3, quote = 4, escape = 5, comment = 6,
                //                   newlines_in_values = 7, truncate_rows = 8 } (:1088-1101)
+    case 31: {  // JsonScanExecNode { base_conf = 1 } (:1103-1105)
       // FileScanExecConf { file_groups = 1, schema = 2, projection = 4 } (:1058-1086)
-      const bool csv = x->field == 2;
+      const bool csv = x->field == 2, json = x->field == 31;
       if (csv && m.has(6)) throw Unsupported("CsvScanExecNode option 'comment' is not supported by the device engine");
       if (csv && m.u64(8)) throw Unsupported("CsvScanExecNode option 'truncate_rows' is not supported by the device engine");
       const Msg conf = m.sub(1);
@@ -600,7 +603,8 @@ inline std::string plan_json(const Msg& n, const std::string& override_job) {
       }
       groups += "]";
       ranges += "]";
-      if (table.empty()) throw std::runtime_error(csv ? "plan proto: csv scan without files" : "plan proto: parquet scan without files");
+      if (table.empty())
+        throw std::runtime_error(csv ? "plan proto: csv scan without files" : json ? "plan proto: json scan without files" : "plan proto: parquet scan without files");
       std::string o = "{\"op\":\"DataSourceExec\",\"table\":" + jstr(table) + ",\"schema\":" + schema_json(conf.sub(2));
       std::vector<uint64_t> proj = conf.varints(4);
       if (proj.empty() && conf.has(13)) {
@@ -614,6 +618,7 @@ inline std::string plan_json(const Msg& n, const std::string& override_job) {
       }
       if (!proj.empty()) o += ",\"projection\":" + u32_list_json(proj);
       o += ",\"file_groups\":" + groups;
+      if (json) return o + ",\"format\":\"json\"" + (any_range ? ",\"file_ranges\":" + ranges : std::string()) + "}";
       if (!csv) return o + "}";
       // reader options as b200_engine_register_csv takes them: one ASCII byte each (escape may be absent)
       auto opt = [&](uint32_t f, const char* name) {

@@ -469,6 +469,65 @@ struct CsvConvertArgs {
 };
 void launch_csv_convert(const CsvConvertArgs& A, int family, cudaStream_t st);
 
+// ---- newline-delimited JSON scan (json.cu) ------------------------------------------------------------
+static const int JSON_TILE = 1024;   // bytes per thread of the record-boundary passes
+static const int JSON_BLOCK = 256;   // tiles per block
+int64_t json_tile_count(int64_t bytes);
+int64_t json_block_count(int64_t bytes);
+// passes 1 + 2: records (lines holding more than whitespace) per tile (tile_cnt: json_tile_count) and the first record of
+// every block (blk_base: json_block_count), *n_records, and *has_backslash |= 1 when the span holds a '\' (both zeroed by
+// the caller)
+void launch_json_records_count(const uint8_t* data, int64_t bytes, uint32_t* tile_cnt, unsigned long long* blk_base, unsigned int* has_backslash,
+                               unsigned long long* n_records, cudaStream_t st);
+// pass 3: rec_start[r] = offset of record r's first byte
+void launch_json_record_starts(const uint8_t* data, int64_t bytes, const uint32_t* tile_cnt, const unsigned long long* blk_base, uint64_t* rec_start,
+                               cudaStream_t st);
+// reasons in a JSON error word, after the converters' CSV_E_* (bits 16-23; bits 0-15 detail, bits 24-63 the row)
+enum JsonError : int {
+  JSON_E_NOT_OBJECT = 32,   // the line is not one object
+  JSON_E_SYNTAX,            // a byte where the grammar allows none
+  JSON_E_UNTERMINATED,      // the line ends inside the object
+  JSON_E_TRAILING,          // bytes after the object
+  JSON_E_CONTROL,           // raw byte below 0x20 in a string
+  JSON_E_UTF8,              // invalid UTF-8 in a string
+  JSON_E_ESCAPE,            // unknown escape or bad \uXXXX
+  JSON_E_SURROGATE,         // lone surrogate
+  JSON_E_NUMBER,            // not an RFC 8259 number
+  JSON_E_LITERAL,           // not true / false / null
+  JSON_E_DUPLICATE,         // a materialised key twice in one object (detail: the slot)
+  JSON_E_DEPTH,             // a skipped value nested deeper than JSON_MAX_DEPTH
+  JSON_E_KIND,              // a value of another JSON kind than the column reads (detail: the kind)
+};
+static const int JSON_MAX_DEPTH = 64;
+// kinds of a JSON view (bits 32-39 of its length word; json_fields_kernel writes them, text_convert<FAM, true> checks them)
+enum JsonKind : int { JK_NUMBER = 1, JK_STRING, JK_TRUE, JK_FALSE, JK_NULL, JK_NESTED };
+// materialised names as the field pass looks them up: an open-addressing table of n_slots entries (power of two), each
+// {FNV-1a hash, offset into names, length, output slot or -1}, staged in shared memory
+struct JsonKey {
+  uint32_t hash;
+  uint16_t off, len;
+  int32_t slot;
+};
+struct JsonFieldArgs {
+  const uint8_t* data;
+  int64_t bytes;
+  const uint64_t* rec_start;
+  int64_t n_records;
+  const JsonKey* keys;            // [n_keys] (n_keys a power of two)
+  int n_keys;
+  const uint8_t* names;           // [names_bytes]
+  int names_bytes;
+  unsigned long long* views;      // [slots][n_total] {pointer, length | kind << 32}, zeroed by the caller (missing = NULL)
+  int64_t n_total, row_base;      // rows of the scan; first row of this span
+  uint8_t* side;                  // unescaping buffer, offsets as in data (nullptr when the span holds no '\')
+  unsigned long long* err;        // structural errors (JSON_E_*)
+};
+void launch_json_fields(const JsonFieldArgs& A, cudaStream_t st);
+// as launch_csv_convert, with JSON's NULL (null pointer) and kinds (text_convert.cuh)
+void launch_json_convert(const CsvConvertArgs& A, int family, cudaStream_t st);
+static inline __host__ __device__ uint32_t json_hash_step(uint32_t h, uint8_t b) { return (h ^ b) * 16777619u; }
+static const uint32_t JSON_HASH_SEED = 2166136261u;  // FNV-1a
+
 // ---- window functions (window.cu) ---------------------------------------------------------------
 // Kernels work on sorted positions i; perm[i] is the input row there (nullptr: the input already is in sorted order).
 static const int WIN_MAX_KEYS = 16;

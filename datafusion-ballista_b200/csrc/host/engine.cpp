@@ -4760,12 +4760,12 @@ DevBatchPtr scan_parquet(const Exec& x, const std::string& path, const std::vect
 // benchmarks/src/bin/tpch.rs:653-683).  The host finds the byte span of each file (range rule below), streams it to HBM
 // through two bounded pinned chunks and csrc/device/csv.cu does everything else.  Rules: DESIGN.md §6 (ix).
 // ------------------------------------------------------------------------------------------------
-struct CsvFileSpec {
+struct ScanFileSpec {
   std::string path;
   int64_t start = 0, end = -1;  // end < 0: the whole file
 };
 struct CsvScanSpec {
-  std::vector<CsvFileSpec> files;
+  std::vector<ScanFileSpec> files;
   Schema schema;
   std::vector<std::string> columns;
   bool all_columns = true;  // no "columns" key; an empty list materialises no column (the rows are still counted)
@@ -4819,7 +4819,7 @@ static CsvScanSpec parse_csv_scan(const std::string& text) {
     if (!files.is_arr() || files.size() == 0) throw EngineError(B200_ERR_INVALID, "csv: 'files' must be a non-empty list");
     for (size_t i = 0; i < files.size(); i++) {
       const Json& f = files.at(i);
-      CsvFileSpec fs;
+      ScanFileSpec fs;
       if (f.is_str()) {
         fs.path = f.str();
       } else {
@@ -4844,12 +4844,15 @@ static CsvScanSpec parse_csv_scan(const std::string& text) {
   return s;
 }
 
-static int csv_family(const Field& f) {
+// the converter family of a column of a text scan (fmt / name: "csv" / "CSV", "json" / "JSON")
+static int text_family(const Field& f, const char* fmt, const char* name) {
   const DataType& t = f.type;
+  auto refuse = [&]() {
+    return EngineError(B200_ERR_UNSUPPORTED, std::string(fmt) + ": column '" + f.name + "' has type " + t.str() + ", which the " + name + " scan does not read");
+  };
   if (t.is_integer()) return CSV_FAM_INT;
   if (t.is_decimal()) {
-    if (t.precision < 1 || t.precision > 38 || t.scale < 0 || t.scale > t.precision)
-      throw EngineError(B200_ERR_UNSUPPORTED, "csv: column '" + f.name + "' has type " + t.str() + ", which the CSV scan does not read");
+    if (t.precision < 1 || t.precision > 38 || t.scale < 0 || t.scale > t.precision) throw refuse();
     return CSV_FAM_DEC;
   }
   if (t.id == TypeId::Float64) return CSV_FAM_F64;
@@ -4857,7 +4860,7 @@ static int csv_family(const Field& f) {
   if (t.id == TypeId::Date32) return CSV_FAM_DATE;
   if (t.id == TypeId::Bool) return CSV_FAM_BOOL;
   if (t.id == TypeId::Utf8) return CSV_FAM_UTF8;
-  throw EngineError(B200_ERR_UNSUPPORTED, "csv: column '" + f.name + "' has type " + t.str() + ", which the CSV scan does not read");
+  throw refuse();
 }
 
 static const char* csv_reason(int r) {
@@ -4878,27 +4881,172 @@ static const char* csv_reason(int r) {
   }
 }
 
-// one file's byte span [s0, e0) on the device and where its records are
-struct CsvSpan {
+// one file's byte span [s0, e0) on the device
+struct TextSpan {
   std::string path;
-  int64_t s0 = 0, e0 = 0, skip = 0, n_records = 0, rows = 0, row_base = 0;
-  DevPtr data, tiles, blocks, blk_state, blk_base, counts, rec_start, side;
+  int64_t s0 = 0, e0 = 0;
+  DevPtr data;
+};
+// ... and where its CSV records are
+struct CsvSpan : TextSpan {
+  int64_t skip = 0, n_records = 0, rows = 0, row_base = 0;
+  DevPtr tiles, blocks, blk_state, blk_base, counts, rec_start, side;
   const unsigned long long* h_n = nullptr;
   const unsigned int* h_quote = nullptr;
 };
 
-// first line terminator at or after `pos` (the file's size when there is none)
-static int64_t csv_find_term(FILE* f, int64_t pos, int64_t size) {
+// first line terminator ('\n', and '\r' when cr_terminates) at or after `pos` (the file's size when there is none)
+static int64_t text_find_term(FILE* f, int64_t pos, int64_t size, bool cr_terminates, const char* fmt) {
   char buf[4096];
   while (pos < size) {
-    if (fseeko(f, (off_t)pos, SEEK_SET) != 0) throw EngineError(B200_ERR_INVALID, "csv: seek failed");
+    if (fseeko(f, (off_t)pos, SEEK_SET) != 0) throw EngineError(B200_ERR_INVALID, std::string(fmt) + ": seek failed");
     const size_t n = fread(buf, 1, sizeof buf, f);
     if (n == 0) break;
     for (size_t i = 0; i < n; i++)
-      if (buf[i] == '\n' || buf[i] == '\r') return pos + (int64_t)i;
+      if (buf[i] == '\n' || (cr_terminates && buf[i] == '\r')) return pos + (int64_t)i;
     pos += (int64_t)n;
   }
   return size;
+}
+
+// Text scans (CSV, newline-delimited JSON): finds each file's byte span and streams it to HBM through two pinned chunks in
+// flight, whatever the file size.  A range holds the records whose first byte lies in [start, end): from after the first
+// terminator at or after start - 1, through the first terminator at or after end - 1.  on_file(span, start) runs once a
+// file's bytes are enqueued, so its first device pass overlaps the reading of the next file.  fmt prefixes the messages
+// ("csv"), name the staging one ("CSV").
+template <class Span, class OnFile>
+static void stream_text_spans(const Exec& x, const std::vector<ScanFileSpec>& files, bool cr_terminates, const char* fmt, const char* name,
+                              std::vector<Span>& spans, OnFile&& on_file) {
+  cudaStream_t st = x.st();
+  static const size_t kChunk = 16u << 20;
+  struct Staging {
+    uint8_t* buf[2] = {nullptr, nullptr};
+    cudaEvent_t ev[2] = {nullptr, nullptr};
+    ~Staging() {
+      for (int b = 0; b < 2; b++) {
+        if (ev[b]) {
+          cudaEventSynchronize(ev[b]);
+          cudaEventDestroy(ev[b]);
+        }
+        if (buf[b]) cudaFreeHost(buf[b]);
+      }
+    }
+  } stg;
+  for (int b = 0; b < 2; b++) {
+    if (cudaHostAlloc((void**)&stg.buf[b], kChunk, cudaHostAllocDefault) != cudaSuccess)
+      throw EngineError(B200_ERR_OOM, std::string("pinned staging for the ") + name + " scan");
+    CUDA_CHECK(cudaEventCreateWithFlags(&stg.ev[b], cudaEventDisableTiming));
+  }
+  const std::string pre = std::string(fmt) + ": ";
+  spans.assign(files.size(), Span());
+  int64_t chunk_no = 0;
+  for (size_t fi = 0; fi < files.size(); fi++) {
+    const ScanFileSpec& fs = files[fi];
+    Span& sp = spans[fi];
+    sp.path = fs.path;
+    FILE* f = fopen(fs.path.c_str(), "rb");
+    if (!f) throw EngineError(B200_ERR_NOT_FOUND, pre + "cannot open " + fs.path);
+    std::unique_ptr<FILE, int (*)(FILE*)> closer(f, fclose);
+    const int64_t size = fseeko(f, 0, SEEK_END) == 0 ? (int64_t)ftello(f) : -1;
+    if (size < 0) throw EngineError(B200_ERR_INVALID, pre + "cannot size " + fs.path);
+    const int64_t start = std::min<int64_t>(fs.start, size);
+    const int64_t end = fs.end < 0 ? size : std::min<int64_t>(fs.end, size);
+    sp.s0 = start == 0 ? 0 : std::min(size, text_find_term(f, start - 1, size, cr_terminates, fmt) + 1);
+    sp.e0 = end == 0 ? 0 : end >= size ? size : std::min(size, text_find_term(f, end - 1, size, cr_terminates, fmt) + 1);
+    if (sp.e0 < sp.s0) sp.e0 = sp.s0;
+    const int64_t bytes = sp.e0 - sp.s0;
+    sp.data = dev_alloc((size_t)bytes + 64, st);
+    for (int64_t off = 0; off < bytes; chunk_no++) {
+      const int b = (int)(chunk_no & 1);
+      const size_t n = (size_t)std::min<int64_t>((int64_t)kChunk, bytes - off);
+      CUDA_CHECK(cudaEventSynchronize(stg.ev[b]));  // the copy out of this chunk two steps ago is done
+      if (fseeko(f, (off_t)(sp.s0 + off), SEEK_SET) != 0 || fread(stg.buf[b], 1, n, f) != n) throw EngineError(B200_ERR_INVALID, pre + "short read on " + fs.path);
+      CUDA_CHECK(cudaMemcpyAsync((uint8_t*)sp.data->ptr + off, stg.buf[b], n, cudaMemcpyHostToDevice, st));
+      CUDA_CHECK(cudaEventRecord(stg.ev[b], st));
+      off += (int64_t)n;
+    }
+    on_file(sp, start);
+  }
+}
+
+// the converter pass of a text scan (CSV, JSON): one launch per materialised column k over views [k][n_total]; the error word
+// of column k is w[1 + k], its null count w[1 + n_mat + k]
+static void convert_text_columns(const Exec& x, const Schema& sch, const std::vector<int>& mat, const std::vector<int>& fam, const DevPtr& views,
+                                 int64_t n_total, unsigned long long* w, std::vector<DevPtr>& outs, std::vector<DevPtr>& valids, const char* timer,
+                                 void (*launch)(const CsvConvertArgs&, int, cudaStream_t)) {
+  cudaStream_t st = x.st();
+  const size_t n_mat = mat.size();
+  outs.assign(n_mat, DevPtr());
+  valids.assign(n_mat, DevPtr());
+  for (size_t k = 0; k < n_mat; k++) {
+    const Field& f = sch[(size_t)mat[k]];
+    CsvConvertArgs C;
+    memset(&C, 0, sizeof C);
+    C.views = (const unsigned long long*)views->ptr + 2 * k * (size_t)n_total;
+    C.n = n_total;
+    C.width = fam[k] == CSV_FAM_UTF8 ? 16 : f.type.is_decimal() ? 16 : f.type.id == TypeId::Bool ? 1 : f.type.width();
+    // Utf8 views are converted in place
+    outs[k] = fam[k] == CSV_FAM_UTF8 ? views : dev_alloc((size_t)std::max<int64_t>(n_total, 1) * (size_t)C.width + 64, st);
+    C.out = fam[k] == CSV_FAM_UTF8 ? (void*)C.views : outs[k]->ptr;
+    valids[k] = dev_alloc((size_t)std::max<int64_t>(n_total, 1) + 64, st);
+    C.valid = (uint8_t*)valids[k]->ptr;
+    C.err = w + 1 + k;
+    C.null_count = w + 1 + n_mat + k;
+    C.is_signed = f.type.is_signed_int();
+    if (fam[k] == CSV_FAM_INT) {
+      const int bits = 8 * f.type.width();
+      C.lo = C.is_signed ? -((__int128)1 << (bits - 1)) : 0;
+      C.hi = C.is_signed ? ((__int128)1 << (bits - 1)) - 1 : ((__int128)1 << bits) - 1;
+    }
+    C.precision = f.type.precision;
+    C.scale = f.type.scale;
+    C.nullable = f.nullable ? 1 : 0;
+    KernelTimer kt(x, timer, (uint64_t)n_total * (16 + (uint64_t)C.width + 1));
+    launch(C, fam[k], st);
+  }
+}
+
+// the table partition a text scan registers: the converted columns (Utf8 views compacted into Arrow Utf8, keeping the spans'
+// bytes alive until then) and their column images; hw = the read-back error words and null counts
+template <class Span>
+static DevBatchPtr text_scan_batch(const Exec& x, const Schema& sch, const std::vector<int>& mat, const std::vector<int>& fam, const DevPtr& views,
+                                   int64_t n_total, const std::vector<DevPtr>& outs, const std::vector<DevPtr>& valids, const unsigned long long* hw,
+                                   const std::vector<Span>& spans, const char* timer) {
+  const size_t n_mat = mat.size();
+  auto out = std::make_shared<DevBatch>();
+  out->n = n_total;
+  for (size_t k = 0; k < n_mat; k++) {
+    const Field& f = sch[(size_t)mat[k]];
+    const bool has_nulls = hw[1 + n_mat + k] != 0;
+    DevColumn col;
+    col.name = f.name;
+    col.type = f.type;
+    col.n = n_total;
+    col.nullable = has_nulls;
+    if (has_nulls) {
+      col.valid = (const uint8_t*)valids[k]->ptr;
+      col.keep.push_back(valids[k]);
+    }
+    if (fam[k] == CSV_FAM_UTF8) {
+      col.phys = PH_STRVIEW;
+      col.data = (const uint8_t*)views->ptr + 16 * k * (size_t)n_total;
+      col.keep.push_back(views);
+      for (auto& sp : spans) {
+        col.keep.push_back(sp.data);
+        if (sp.side) col.keep.push_back(sp.side);
+      }
+      KernelTimer kt(x, timer, (uint64_t)n_total * 16 * 2);
+      col = as_utf8(x, col);
+    } else {
+      col.phys = phys_of(f.type);
+      col.data = (const uint8_t*)outs[k]->ptr;
+      col.keep.push_back(outs[k]);
+    }
+    out->cols.push_back(col);
+  }
+  build_column_images(x, *out);
+  x.sync();
+  return out;
 }
 
 DevBatchPtr scan_csv(const Exec& x, const CsvScanSpec& spec) {
@@ -4921,60 +5069,15 @@ DevBatchPtr scan_csv(const Exec& x, const CsvScanSpec& spec) {
     }
   }
   std::vector<int> fam;
-  for (int c : mat) fam.push_back(csv_family(sch[(size_t)c]));
+  for (int c : mat) fam.push_back(text_family(sch[(size_t)c], "csv", "CSV"));
   std::vector<int32_t> slot_of_field(sch.size(), -1);
   for (size_t k = 0; k < mat.size(); k++) slot_of_field[(size_t)mat[k]] = (int32_t)k;
 
-  // ---- bytes to HBM: two pinned chunks in flight, whatever the file size --------------------------------------------------
-  static const size_t kChunk = 16u << 20;
-  struct Staging {
-    uint8_t* buf[2] = {nullptr, nullptr};
-    cudaEvent_t ev[2] = {nullptr, nullptr};
-    ~Staging() {
-      for (int b = 0; b < 2; b++) {
-        if (ev[b]) {
-          cudaEventSynchronize(ev[b]);
-          cudaEventDestroy(ev[b]);
-        }
-        if (buf[b]) cudaFreeHost(buf[b]);
-      }
-    }
-  } stg;
-  for (int b = 0; b < 2; b++) {
-    if (cudaHostAlloc((void**)&stg.buf[b], kChunk, cudaHostAllocDefault) != cudaSuccess) throw EngineError(B200_ERR_OOM, "pinned staging for the CSV scan");
-    CUDA_CHECK(cudaEventCreateWithFlags(&stg.ev[b], cudaEventDisableTiming));
-  }
-  std::vector<CsvSpan> spans(spec.files.size());
-  int64_t chunk_no = 0;
-  for (size_t fi = 0; fi < spec.files.size(); fi++) {
-    const CsvFileSpec& fs = spec.files[fi];
-    CsvSpan& sp = spans[fi];
-    sp.path = fs.path;
-    FILE* f = fopen(fs.path.c_str(), "rb");
-    if (!f) throw EngineError(B200_ERR_NOT_FOUND, "csv: cannot open " + fs.path);
-    std::unique_ptr<FILE, int (*)(FILE*)> closer(f, fclose);
-    const int64_t size = fseeko(f, 0, SEEK_END) == 0 ? (int64_t)ftello(f) : -1;
-    if (size < 0) throw EngineError(B200_ERR_INVALID, "csv: cannot size " + fs.path);
-    const int64_t start = std::min<int64_t>(fs.start, size);
-    const int64_t end = fs.end < 0 ? size : std::min<int64_t>(fs.end, size);
-    // a range holds the records whose first byte lies in [start, end): from after the first terminator at or after
-    // start - 1, through the first terminator at or after end - 1
-    sp.s0 = start == 0 ? 0 : std::min(size, csv_find_term(f, start - 1, size) + 1);
-    sp.e0 = end == 0 ? 0 : end >= size ? size : std::min(size, csv_find_term(f, end - 1, size) + 1);
-    if (sp.e0 < sp.s0) sp.e0 = sp.s0;
+  std::vector<CsvSpan> spans;
+  stream_text_spans(x, spec.files, true, "csv", "CSV", spans, [&](CsvSpan& sp, int64_t start) {
     sp.skip = (spec.has_header && start == 0) ? 1 : 0;
     const int64_t bytes = sp.e0 - sp.s0;
-    sp.data = dev_alloc((size_t)bytes + 64, st);
-    for (int64_t off = 0; off < bytes; chunk_no++) {
-      const int b = (int)(chunk_no & 1);
-      const size_t n = (size_t)std::min<int64_t>((int64_t)kChunk, bytes - off);
-      CUDA_CHECK(cudaEventSynchronize(stg.ev[b]));  // the copy out of this chunk two steps ago is done
-      if (fseeko(f, (off_t)(sp.s0 + off), SEEK_SET) != 0 || fread(stg.buf[b], 1, n, f) != n) throw EngineError(B200_ERR_INVALID, "csv: short read on " + fs.path);
-      CUDA_CHECK(cudaMemcpyAsync((uint8_t*)sp.data->ptr + off, stg.buf[b], n, cudaMemcpyHostToDevice, st));
-      CUDA_CHECK(cudaEventRecord(stg.ev[b], st));
-      off += (int64_t)n;
-    }
-    if (bytes == 0) continue;
+    if (bytes == 0) return;
     const int64_t nt = csv_tile_count(bytes), nb = csv_block_count(bytes);
     sp.tiles = dev_alloc((size_t)nt * sizeof(CsvTrans), st);
     sp.blocks = dev_alloc((size_t)nb * sizeof(CsvTrans), st);
@@ -4991,7 +5094,7 @@ DevBatchPtr scan_csv(const Exec& x, const CsvScanSpec& spec) {
     }
     sp.h_n = x.fetch<unsigned long long>(n_rec);
     sp.h_quote = x.fetch<unsigned int>(quote);
-  }
+  });
   x.sync();  // one read-back for every file: record counts and whether any quote byte occurs
   int64_t n_total = 0;
   for (auto& sp : spans) {
@@ -5039,33 +5142,8 @@ DevBatchPtr scan_csv(const Exec& x, const CsvScanSpec& spec) {
     KernelTimer kt(x, "csv_fields", (uint64_t)bytes + (uint64_t)sp.n_records * 8 + (uint64_t)sp.rows * n_mat * 16);
     launch_csv_fields(A, st);
   }
-  std::vector<DevPtr> outs(n_mat), valids(n_mat);
-  for (size_t k = 0; k < n_mat; k++) {
-    const Field& f = sch[(size_t)mat[k]];
-    CsvConvertArgs C;
-    memset(&C, 0, sizeof C);
-    C.views = (const unsigned long long*)views->ptr + 2 * k * (size_t)n_total;
-    C.n = n_total;
-    C.width = fam[k] == CSV_FAM_UTF8 ? 16 : f.type.is_decimal() ? 16 : f.type.id == TypeId::Bool ? 1 : f.type.width();
-    // Utf8 views are validated in place
-    outs[k] = fam[k] == CSV_FAM_UTF8 ? views : dev_alloc((size_t)std::max<int64_t>(n_total, 1) * (size_t)C.width + 64, st);
-    C.out = fam[k] == CSV_FAM_UTF8 ? (void*)C.views : outs[k]->ptr;
-    valids[k] = dev_alloc((size_t)std::max<int64_t>(n_total, 1) + 64, st);
-    C.valid = (uint8_t*)valids[k]->ptr;
-    C.err = w + 1 + k;
-    C.null_count = w + 1 + n_mat + k;
-    C.is_signed = f.type.is_signed_int();
-    if (fam[k] == CSV_FAM_INT) {
-      const int bits = 8 * f.type.width();
-      C.lo = C.is_signed ? -((__int128)1 << (bits - 1)) : 0;
-      C.hi = C.is_signed ? ((__int128)1 << (bits - 1)) - 1 : ((__int128)1 << bits) - 1;
-    }
-    C.precision = f.type.precision;
-    C.scale = f.type.scale;
-    C.nullable = f.nullable ? 1 : 0;
-    KernelTimer kt(x, "csv_convert", (uint64_t)n_total * (16 + (uint64_t)C.width + 1));
-    launch_csv_convert(C, fam[k], st);
-  }
+  std::vector<DevPtr> outs, valids;
+  convert_text_columns(x, sch, mat, fam, views, n_total, w, outs, valids, "csv_convert", launch_csv_convert);
   const unsigned long long* hw = (const unsigned long long*)x.fetch_bytes(w, (1 + 2 * n_mat) * 8);
   x.sync();
   // the first failing record of the scan, a field-count error first among equals
@@ -5111,40 +5189,269 @@ DevBatchPtr scan_csv(const Exec& x, const CsvScanSpec& spec) {
     throw EngineError(B200_ERR_INVALID, "csv: " + sp.path + ": " + col + "record " + std::to_string(row - sp.row_base + 1) + " (byte offset " +
                                             std::to_string((uint64_t)sp.s0 + rel) + "): " + what + ": '" + value + "'");
   }
-  auto out = std::make_shared<DevBatch>();
-  out->n = n_total;
-  for (size_t k = 0; k < n_mat; k++) {
-    const Field& f = sch[(size_t)mat[k]];
-    const bool has_nulls = hw[1 + n_mat + k] != 0;
-    DevColumn col;
-    col.name = f.name;
-    col.type = f.type;
-    col.n = n_total;
-    col.nullable = has_nulls;
-    if (has_nulls) {
-      col.valid = (const uint8_t*)valids[k]->ptr;
-      col.keep.push_back(valids[k]);
-    }
-    if (fam[k] == CSV_FAM_UTF8) {
-      col.phys = PH_STRVIEW;
-      col.data = (const uint8_t*)views->ptr + 16 * k * (size_t)n_total;
-      col.keep.push_back(views);
-      for (auto& sp : spans) {
-        col.keep.push_back(sp.data);
-        if (sp.side) col.keep.push_back(sp.side);
-      }
-      KernelTimer kt(x, "csv_strings", (uint64_t)n_total * 16 * 2);
-      col = as_utf8(x, col);
-    } else {
-      col.phys = phys_of(f.type);
-      col.data = (const uint8_t*)outs[k]->ptr;
-      col.keep.push_back(outs[k]);
-    }
-    out->cols.push_back(col);
+  return text_scan_batch(x, sch, mat, fam, views, n_total, outs, valids, hw, spans, "csv_strings");
+}
+
+// ------------------------------------------------------------------------------------------------
+// Newline-delimited JSON scan: DataSourceExec + JsonSource (JsonScanExecNode, ballista/core/proto/datafusion.proto:1103-1105).
+// The host finds the byte span of each file (the CSV scan's range rule with '\n' the only terminator; '\r' is whitespace),
+// streams it to HBM and csrc/device/json.cu does everything else.  Rules: DESIGN.md §6 (xv).
+// ------------------------------------------------------------------------------------------------
+struct JsonScanSpec {
+  std::vector<ScanFileSpec> files;
+  Schema schema;
+  std::vector<std::string> columns;
+  bool all_columns = true;  // no "columns" key; an empty list materialises no column (the records are still counted and checked)
+};
+
+static JsonScanSpec parse_json_scan(const std::string& text) {
+  Json j;
+  try {
+    j = parse_json(text);
+  } catch (const std::exception& ex) {
+    throw EngineError(B200_ERR_INVALID, std::string("json: malformed scan description: ") + ex.what());
   }
-  build_column_images(x, *out);
+  if (!j.is_obj()) throw EngineError(B200_ERR_INVALID, "json: the scan description must be a JSON object");
+  JsonScanSpec s;
+  try {
+    if (!j.get_bool("newline_delimited", true))
+      throw EngineError(B200_ERR_UNSUPPORTED, "json: 'newline_delimited': false (a JSON array of objects) is not supported");
+    const Json* c = j.find("compression");
+    if (c && !c->is_null()) {
+      std::string v = c->str();
+      for (auto& ch : v) ch = (char)tolower((unsigned char)ch);
+      if (v != "uncompressed" && !v.empty()) throw EngineError(B200_ERR_UNSUPPORTED, "json: compression '" + c->str() + "' is not supported");
+    }
+    s.schema = parse_schema(j.at("schema"));
+    if (s.schema.empty()) throw EngineError(B200_ERR_INVALID, "json: empty schema");
+    const Json* cols = j.find("columns");
+    if (cols && !cols->is_null()) {
+      if (!cols->is_arr()) throw EngineError(B200_ERR_INVALID, "json: 'columns' must be a list of names");
+      s.all_columns = false;
+      for (size_t i = 0; i < cols->size(); i++) s.columns.push_back(cols->at(i).str());
+    }
+    const Json& files = j.at("files");
+    if (!files.is_arr() || files.size() == 0) throw EngineError(B200_ERR_INVALID, "json: 'files' must be a non-empty list");
+    for (size_t i = 0; i < files.size(); i++) {
+      const Json& f = files.at(i);
+      ScanFileSpec fs;
+      if (f.is_str()) {
+        fs.path = f.str();
+      } else {
+        fs.path = f.at("path").str();
+        const Json* r = f.find("range");
+        if (r && !r->is_null()) {
+          if (r->size() != 2) throw EngineError(B200_ERR_INVALID, "json: a range is [start, end]");
+          fs.start = r->at(0).as_int();
+          fs.end = r->at(1).as_int();
+          if (fs.start < 0 || fs.end < fs.start) throw EngineError(B200_ERR_INVALID, "json: bad byte range of " + fs.path);
+        }
+      }
+      s.files.push_back(fs);
+    }
+  } catch (const EngineError&) {
+    throw;
+  } catch (const std::exception& ex) {
+    throw EngineError(B200_ERR_INVALID, std::string("json: ") + ex.what());
+  }
+  return s;
+}
+
+static const char* json_kind_name(int k) {
+  switch (k) {
+    case JK_NUMBER: return "a number";
+    case JK_STRING: return "a string";
+    case JK_TRUE:
+    case JK_FALSE: return "a boolean";
+    case JK_NULL: return "null";
+    default: return "an object or array";
+  }
+}
+
+static std::string json_reason(int r, int detail, int family) {
+  switch (r) {
+    case JSON_E_NOT_OBJECT: return "the line is not one JSON object";
+    case JSON_E_SYNTAX: return "invalid JSON";
+    case JSON_E_UNTERMINATED: return "the line ends inside the object (an object must fit on one line)";
+    case JSON_E_TRAILING: return "bytes after the object";
+    case JSON_E_CONTROL: return "raw control character in a string";
+    case JSON_E_UTF8: return "invalid UTF-8 in a string";
+    case JSON_E_ESCAPE: return "invalid escape in a string";
+    case JSON_E_SURROGATE: return "lone surrogate in a \\u escape";
+    case JSON_E_NUMBER: return "invalid number";
+    case JSON_E_LITERAL: return "invalid literal (only true, false and null)";
+    case JSON_E_DUPLICATE: return "key appears twice in the object";
+    case JSON_E_DEPTH: return "value nested deeper than " + std::to_string(JSON_MAX_DEPTH) + " levels";
+    case JSON_E_KIND:
+      return std::string("expected ") + (family == CSV_FAM_BOOL ? "a boolean" : family == CSV_FAM_DATE || family == CSV_FAM_UTF8 ? "a string" : "a number") +
+             ", found " + json_kind_name(detail);
+    default: return csv_reason(r);
+  }
+}
+
+// one file's byte span and where its JSON records are
+struct JsonSpan : TextSpan {
+  int64_t n_records = 0, row_base = 0;
+  DevPtr tiles, blk, counts, rec_start, side;
+  const unsigned long long* h_n = nullptr;
+  const unsigned int* h_backslash = nullptr;
+};
+
+DevBatchPtr scan_json(const Exec& x, const JsonScanSpec& spec) {
+  ScopeTimer tm("json_scan");
+  cudaStream_t st = x.st();
+  const Schema& sch = spec.schema;
+  // materialised columns, in the requested order
+  std::vector<int> mat;
+  if (spec.all_columns) {
+    for (size_t i = 0; i < sch.size(); i++) mat.push_back((int)i);
+  } else {
+    for (auto& nm : spec.columns) {
+      int at = -1;
+      for (size_t i = 0; i < sch.size(); i++)
+        if (sch[i].name == nm) at = (int)i;
+      if (at < 0) throw EngineError(B200_ERR_INVALID, "json: no column named " + nm);
+      // every key feeds at most one output slot (json_fields_kernel writes one view per key)
+      if (std::find(mat.begin(), mat.end(), at) != mat.end()) throw EngineError(B200_ERR_INVALID, "json: column " + nm + " is requested twice");
+      mat.push_back(at);
+    }
+  }
+  std::vector<int> fam;
+  for (int c : mat) fam.push_back(text_family(sch[(size_t)c], "json", "JSON"));
+  const size_t n_mat = mat.size();
+  // the key table of the field pass: open addressing, at most half full
+  int n_keys = 1;
+  while (n_keys < 2 * (int)n_mat) n_keys <<= 1;
+  std::vector<JsonKey> keys((size_t)n_keys, JsonKey{0, 0, 0, -1});
+  std::string names;
+  for (size_t k = 0; k < n_mat; k++) {
+    const std::string& nm = sch[(size_t)mat[k]].name;
+    uint32_t h = JSON_HASH_SEED;
+    for (unsigned char b : nm) h = json_hash_step(h, b);
+    uint32_t at = h & (uint32_t)(n_keys - 1);
+    while (keys[at].slot >= 0) at = (at + 1) & (uint32_t)(n_keys - 1);
+    if (names.size() + nm.size() > 0xFFFF) throw EngineError(B200_ERR_UNSUPPORTED, "json: the materialised column names are too long for the key table");
+    keys[at] = JsonKey{h, (uint16_t)names.size(), (uint16_t)nm.size(), (int32_t)k};
+    names += nm;
+  }
+  if (keys.size() * sizeof(JsonKey) + names.size() > 48 * 1024)
+    throw EngineError(B200_ERR_UNSUPPORTED, "json: too many materialised columns for the key table");
+
+  std::vector<JsonSpan> spans;
+  stream_text_spans(x, spec.files, false, "json", "JSON", spans, [&](JsonSpan& sp, int64_t) {
+    const int64_t bytes = sp.e0 - sp.s0;
+    if (bytes == 0) return;
+    const int64_t nt = json_tile_count(bytes), nb = json_block_count(bytes);
+    sp.tiles = dev_alloc((size_t)nt * 4, st);
+    sp.blk = dev_alloc((size_t)nb * 8, st);
+    sp.counts = dev_alloc(16, st);
+    CUDA_CHECK(cudaMemsetAsync(sp.counts->ptr, 0, 16, st));
+    unsigned long long* n_rec = (unsigned long long*)sp.counts->ptr;
+    unsigned int* bs = (unsigned int*)(n_rec + 1);
+    {
+      KernelTimer kt(x, "json_records", (uint64_t)bytes + (uint64_t)nt * 4);
+      launch_json_records_count((const uint8_t*)sp.data->ptr, bytes, (uint32_t*)sp.tiles->ptr, (unsigned long long*)sp.blk->ptr, bs, n_rec, st);
+    }
+    sp.h_n = x.fetch<unsigned long long>(n_rec);
+    sp.h_backslash = x.fetch<unsigned int>(bs);
+  });
+  x.sync();  // one read-back for every file: record counts and whether any '\' occurs
+  int64_t n_total = 0;
+  for (auto& sp : spans) {
+    sp.n_records = sp.h_n ? (int64_t)*sp.h_n : 0;
+    sp.row_base = n_total;
+    n_total += sp.n_records;
+  }
+  // views start zeroed: a key that never appears is NULL
+  DevPtr views = dev_alloc(std::max<size_t>(n_mat * (size_t)n_total, 1) * 16 + 64, st);
+  if (n_mat && n_total) CUDA_CHECK(cudaMemsetAsync(views->ptr, 0, n_mat * (size_t)n_total * 16, st));
+  DevPtr d_keys = dev_alloc(keys.size() * sizeof(JsonKey) + names.size() + 16, st);
+  CUDA_CHECK(cudaMemcpyAsync(d_keys->ptr, keys.data(), keys.size() * sizeof(JsonKey), cudaMemcpyHostToDevice, st));  // pageable: staged before returning
+  if (!names.empty())
+    CUDA_CHECK(cudaMemcpyAsync((uint8_t*)d_keys->ptr + keys.size() * sizeof(JsonKey), names.data(), names.size(), cudaMemcpyHostToDevice, st));
+  // error words: [0] structure, [1 + k] column k; then the null count of every column
+  DevPtr words = dev_alloc((1 + 2 * n_mat) * 8, st);
+  CUDA_CHECK(cudaMemsetAsync(words->ptr, 0xFF, (1 + n_mat) * 8, st));
+  CUDA_CHECK(cudaMemsetAsync((unsigned long long*)words->ptr + 1 + n_mat, 0, n_mat * 8, st));
+  unsigned long long* w = (unsigned long long*)words->ptr;
+  for (auto& sp : spans) {
+    const int64_t bytes = sp.e0 - sp.s0;
+    if (!sp.n_records) continue;
+    sp.rec_start = dev_alloc((size_t)sp.n_records * 8, st);
+    {
+      KernelTimer kt(x, "json_records", (uint64_t)bytes + (uint64_t)sp.n_records * 8);
+      launch_json_record_starts((const uint8_t*)sp.data->ptr, bytes, (const uint32_t*)sp.tiles->ptr, (const unsigned long long*)sp.blk->ptr,
+                                (uint64_t*)sp.rec_start->ptr, st);
+    }
+    sp.tiles.reset();
+    sp.blk.reset();
+    if (*sp.h_backslash) sp.side = dev_alloc((size_t)bytes + 64, st);
+    JsonFieldArgs A;
+    memset(&A, 0, sizeof A);
+    A.data = (const uint8_t*)sp.data->ptr;
+    A.bytes = bytes;
+    A.rec_start = (const uint64_t*)sp.rec_start->ptr;
+    A.n_records = sp.n_records;
+    A.keys = (const JsonKey*)d_keys->ptr;
+    A.n_keys = n_mat ? n_keys : 0;
+    A.names = (const uint8_t*)d_keys->ptr + keys.size() * sizeof(JsonKey);
+    A.names_bytes = n_mat ? (int)names.size() : 0;
+    A.views = (unsigned long long*)views->ptr;
+    A.n_total = n_total;
+    A.row_base = sp.row_base;
+    A.side = sp.side ? (uint8_t*)sp.side->ptr : nullptr;
+    A.err = w;
+    KernelTimer kt(x, "json_fields", (uint64_t)bytes + (uint64_t)sp.n_records * 8 + (uint64_t)sp.n_records * n_mat * 16);
+    launch_json_fields(A, st);
+  }
+  std::vector<DevPtr> outs, valids;
+  convert_text_columns(x, sch, mat, fam, views, n_total, w, outs, valids, "json_convert", launch_json_convert);
+  const unsigned long long* hw = (const unsigned long long*)x.fetch_bytes(w, (1 + 2 * n_mat) * 8);
   x.sync();
-  return out;
+  // the first failing record of the scan, a structural error first among equals
+  int which = -1;
+  unsigned long long best = ~0ull;
+  for (size_t k = 0; k <= n_mat; k++)
+    if (hw[k] != ~0ull && (hw[k] >> 24) < (best >> 24)) {
+      best = hw[k];
+      which = (int)k - 1;
+    }
+  if (best != ~0ull) {
+    const int64_t row = (int64_t)(best >> 24);
+    const int reason = (int)((best >> 16) & 0xFF), detail = (int)(best & 0xFFFF);
+    size_t fi = 0;
+    while (fi + 1 < spans.size() && !(row >= spans[fi].row_base && row < spans[fi].row_base + spans[fi].n_records)) fi++;
+    const JsonSpan& sp = spans[fi];
+    const uint64_t rel = x.get<uint64_t>((const uint64_t*)sp.rec_start->ptr + (row - sp.row_base));
+    std::string value;
+    if (which >= 0) {
+      const unsigned long long* v = (const unsigned long long*)views->ptr + 2 * ((size_t)which * (size_t)n_total + (size_t)row);
+      const unsigned long long* hv = (const unsigned long long*)x.fetch_bytes(v, 16);
+      x.sync();
+      const uint64_t full = hv[1] & 0xFFFFFFFFull, len = std::min<uint64_t>(full, 64);
+      if (len && hv[0]) {
+        const char* hb = (const char*)x.fetch_bytes((const void*)hv[0], (size_t)len);
+        x.sync();
+        value.assign(hb, (size_t)len);
+      }
+      if (full > 64) value += "...";
+    } else {
+      const uint64_t len = std::min<uint64_t>(64, (uint64_t)(sp.e0 - sp.s0) - rel);
+      const char* hb = (const char*)x.fetch_bytes((const uint8_t*)sp.data->ptr + rel, (size_t)len);
+      x.sync();
+      value.assign(hb, (size_t)len);
+      const size_t nl = value.find('\n');
+      if (nl != std::string::npos) value.resize(nl);
+      else if (len == 64) value += "...";
+    }
+    const int col_at = which >= 0 ? which : reason == JSON_E_DUPLICATE ? detail : -1;
+    const std::string what = json_reason(reason, detail, which >= 0 ? fam[(size_t)which] : -1);
+    const std::string col = col_at >= 0 ? "column '" + sch[(size_t)mat[(size_t)col_at]].name + "', " : "";
+    throw EngineError(reason == JSON_E_DEPTH ? B200_ERR_UNSUPPORTED : B200_ERR_INVALID,
+                      "json: " + sp.path + ": " + col + "record " + std::to_string(row - sp.row_base + 1) + " (byte offset " +
+                          std::to_string((uint64_t)sp.s0 + rel) + "): " + what + ": '" + value + "'");
+  }
+  return text_scan_batch(x, sch, mat, fam, views, n_total, outs, valids, hw, spans, "json_strings");
 }
 
 void collect_nodes(const PlanNode& n, b200_stage* s) {
@@ -5665,6 +5972,25 @@ int b200_engine_register_csv(b200_engine* e, const char* table, int partition, c
     DevBatchPtr b;
     try {
       b = scan_csv(x, spec);
+    } catch (...) {
+      cudaStreamSynchronize(e->stream);
+      Exec::abandon();
+      throw;
+    }
+    std::lock_guard<std::mutex> g(e->mu);
+    e->tables[table][partition] = b;
+  });
+}
+
+int b200_engine_register_json(b200_engine* e, const char* table, int partition, const char* scan_json) {
+  return guard(e, [&] {
+    if (!e || !table || !scan_json) throw EngineError(B200_ERR_INVALID, "null argument");
+    const JsonScanSpec spec = parse_json_scan(scan_json);
+    CUDA_CHECK(cudaSetDevice(e->device));
+    Exec x{e, nullptr, nullptr};
+    DevBatchPtr b;
+    try {
+      b = ::scan_json(x, spec);
     } catch (...) {
       cudaStreamSynchronize(e->stream);
       Exec::abandon();

@@ -63,6 +63,23 @@ def register_csv_scan(engine, node: dict, partition: int, path_map: Optional[Dic
                         newlines_in_values=o["newlines_in_values"])
 
 
+def register_json_scan(engine, node: dict, partition: int, path_map: Optional[Dict[str, str]] = None) -> None:
+    """What an executor-side shim does with a newline-delimited JSON leaf: register file group `partition` of a decoded
+    JSON DataSourceExec node ("format": "json", "file_groups", "file_ranges") through engine.register_json, the table laid
+    out as register_csv_scan lays it out (the schema's columns up to the last projected one, in file order).  path_map
+    renames files (the plan's paths as seen by this host)."""
+    schema = node["schema"]
+    proj = node.get("projection", list(range(len(schema))))
+    cols = [f["name"] for f in schema[:max(proj) + 1]] if proj else []
+    ranges = node.get("file_ranges")
+    files = []
+    for i, path in enumerate(node["file_groups"][partition]):
+        path = (path_map or {}).get(path, path)
+        r = ranges[partition][i] if ranges else None
+        files.append((path, r[0], r[1]) if r else path)
+    engine.register_json(node["table"], partition, files, schema, columns=cols)
+
+
 def run_stages(engine, stages: List[Stage], job_id: str = "job", collect: bool = True,
                metrics_out: Optional[list] = None) -> Optional[pa.Table]:
     """Execute `stages` in order on `engine`; return the last stage's output as one Table."""

@@ -69,7 +69,7 @@ class ArrowArray(C.Structure):
 EXPORTED_SYMBOLS = [
     "b200_engine_create", "b200_engine_destroy", "b200_last_error", "b200_engine_set_stream",
     "b200_engine_synchronize", "b200_engine_kernel_launches", "b200_engine_counter", "b200_engine_set_config",
-    "b200_engine_register_batch", "b200_engine_register_parquet", "b200_engine_register_csv", "b200_parquet_describe", "b200_engine_drop_table", "b200_engine_tpch_generate",
+    "b200_engine_register_batch", "b200_engine_register_parquet", "b200_engine_register_csv", "b200_engine_register_json", "b200_parquet_describe", "b200_engine_drop_table", "b200_engine_tpch_generate",
     "b200_engine_export_table", "b200_tpch_table_rows", "b200_stage_prepare", "b200_stage_execute", "b200_stage_metrics",
     "b200_stage_release", "b200_partition_export", "b200_partition_rows",
     "b200_remove_job_data", "b200_remove_stage_data", "b200_host_alloc_pinned", "b200_host_free_pinned",
@@ -106,6 +106,7 @@ def load_library():
     L.b200_engine_register_batch.argtypes = [vp, cp, ci, vp, vp]
     L.b200_engine_register_parquet.argtypes = [vp, cp, ci, cp, cp]
     L.b200_engine_register_csv.argtypes = [vp, cp, ci, cp]
+    L.b200_engine_register_json.argtypes = [vp, cp, ci, cp]
     L.b200_parquet_describe.argtypes = [cp, vp, u64]
     L.b200_engine_drop_table.argtypes = [vp, cp]
     L.b200_engine_tpch_generate.argtypes = [vp, cp, i64, ci, i64, i64, cp]
@@ -396,6 +397,24 @@ class GpuExecutionEngine:
     def register_csv_json(self, table: str, partition: int, scan_json: str) -> None:
         """b200_engine_register_csv with the scan description as it crosses the C ABI."""
         _check(load_library().b200_engine_register_csv(self.h, table.encode(), partition, scan_json.encode()))
+        self._parts.setdefault(table, set()).add(partition)
+
+    def register_json(self, table: str, partition: int, files, schema: List[dict], columns: Optional[List[str]] = None) -> None:
+        """Scan newline-delimited JSON files into a table partition with records, tokens and values found on the device
+        (b200_engine_register_json).  files: paths or (path, start, end) byte ranges; schema: the files' columns as plan-IR
+        fields; columns: the ones to materialise, in this order (None: all)."""
+        import json as _json
+        fl = []
+        for f in ([files] if isinstance(files, (str, tuple)) else files):
+            fl.append({"path": f[0], "range": [int(f[1]), int(f[2])]} if isinstance(f, tuple) else {"path": f})
+        spec = {"files": fl, "schema": schema}
+        if columns is not None:
+            spec["columns"] = list(columns)
+        self.register_json_json(table, partition, _json.dumps(spec))
+
+    def register_json_json(self, table: str, partition: int, scan_json: str) -> None:
+        """b200_engine_register_json with the scan description as it crosses the C ABI."""
+        _check(load_library().b200_engine_register_json(self.h, table.encode(), partition, scan_json.encode()))
         self._parts.setdefault(table, set()).add(partition)
 
     def drop_table(self, table: str) -> None:

@@ -163,6 +163,19 @@ def csv_scan(table: str, schema: List[Json], projection: Optional[List[int]] = N
     return n
 
 
+def json_scan(table: str, schema: List[Json], projection: Optional[List[int]] = None, file_groups: Optional[List[List[str]]] = None,
+              file_ranges: Optional[List[list]] = None) -> Json:
+    """DataSourceExec over newline-delimited JSON files (JsonScanExecNode): `schema` is the files' columns, `projection`
+    indexes it, and "format" / "file_ranges" ride along as the protobuf decoder emits them."""
+    n = scan(table, schema, projection)
+    if file_groups is not None:
+        n["file_groups"] = file_groups
+    n["format"] = "json"
+    if file_ranges is not None:
+        n["file_ranges"] = file_ranges
+    return n
+
+
 def shuffle_reader(stage_id: int, schema: List[Json], broadcast: bool = False) -> Json:
     return {"op": "ShuffleReaderExec", "stage_id": stage_id, "schema": schema, "broadcast": broadcast}
 

@@ -124,6 +124,17 @@ int b200_parquet_describe(const char* path, char* out, uint64_t cap);
  * options 'comment' and 'truncate_rows', Timestamp columns and ranges with newlines_in_values B200_ERR_UNSUPPORTED.  Nothing
  * is registered after an error.  Replaces the table partition. */
 int b200_engine_register_csv(b200_engine* e, const char* table, int partition, const char* scan_json);
+/* DataSourceExec + JsonSource leaf over newline-delimited JSON (JsonScanExecNode, datafusion.proto:1103-1105): the file
+ * bytes cross the bus as they are and records, tokens and values are found and converted on the device.  scan_json:
+ *   {"files": [{"path": "...", "range": [start, end]} | "path", ...],   range optional: the records whose first byte lies in it
+ *    "schema": [fields as in the plan IR], "columns": [names] (absent: all)}
+ * Each non-blank line is one JSON object (RFC 8259, strict); a missing key and null are NULL; numbers feed integer,
+ * Decimal128 and float columns, strings Utf8 and Date32 columns, true / false Bool columns (DESIGN.md §6 (xv)).  The table
+ * partition gets exactly the requested columns in the requested order.  Malformed JSON, options or data return
+ * B200_ERR_INVALID (data errors name the file, column, record and byte offset); a missing file B200_ERR_NOT_FOUND;
+ * "newline_delimited": false (a JSON array), compression, Timestamp columns and values nested deeper than 64 levels
+ * B200_ERR_UNSUPPORTED.  Nothing is registered after an error.  Replaces the table partition. */
+int b200_engine_register_json(b200_engine* e, const char* table, int partition, const char* scan_json);
 int b200_engine_drop_table(b200_engine* e, const char* table);
 /* Synthetic TPC-H-shaped table generated directly in HBM (bench/test input; columns = NULL: all).
  * Rows [row_begin,row_end) of the table at milli-scale-factor `msf` become partition `partition`. */
