@@ -4,7 +4,7 @@ ARCH      := -gencode arch=compute_90a,code=sm_90a
 PKG       := datafusion-ballista_b200
 SRC       := $(PKG)/csrc
 OUT       := $(PKG)/lib
-# B200_PLAN_STAT_AGGREGATES: this library computes VAR / STDDEV / COVAR / CORR (plan.hpp); set for every unit alike
+# B200_PLAN_STAT_AGGREGATES: this library computes VAR / STDDEV / COVAR / CORR, regr_*, bool_* and bit_* (plan.hpp); set for every unit alike
 # B200_PLAN_GROUPING_SETS: ... and grouping sets and the bitwise operators (plan.hpp)
 # B200_PLAN_WINDOW: ... and window functions (plan.hpp)
 # B200_PLAN_REGEX: ... and ILIKE, the regex operators and regexp_like (plan.hpp)

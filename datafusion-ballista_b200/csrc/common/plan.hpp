@@ -797,20 +797,28 @@ inline ExprPtr parse_expr(const Json& j, const Schema& in) {
 // ----------------------------------------------------------------------------------------------
 // Aggregates
 // ----------------------------------------------------------------------------------------------
-enum class AggFn : uint8_t { Sum, Min, Max, Count, Avg, VarSamp, VarPop, StddevSamp, StddevPop, CovarSamp, CovarPop, Corr };
+enum class AggFn : uint8_t { Sum, Min, Max, Count, Avg, VarSamp, VarPop, StddevSamp, StddevPop, CovarSamp, CovarPop, Corr,
+                              RegrSlope, RegrIntercept, RegrCount, RegrR2, RegrAvgx, RegrAvgy, RegrSxx, RegrSyy, RegrSxy,
+                              BoolAnd, BoolOr, BitAnd, BitOr, BitXor };
 enum class AggMode : uint8_t { Partial, Final, FinalPartitioned, Single, SinglePartitioned };
 
 inline bool agg_mode_consumes_states(AggMode m) { return m == AggMode::Final || m == AggMode::FinalPartitioned; }
 inline bool agg_mode_emits_states(AggMode m) { return m == AggMode::Partial; }
 
-// The statistical aggregates: variance / standard deviation (one argument), covariance / correlation (two arguments)
-inline bool agg_is_stat(AggFn f) { return f >= AggFn::VarSamp; }
-inline bool agg_is_bivariate(AggFn f) { return f == AggFn::CovarSamp || f == AggFn::CovarPop || f == AggFn::Corr; }
+// The statistical aggregates: variance / standard deviation (one argument), covariance / correlation and the linear
+// regression aggregates (two arguments).  All of them need the two-pass co-moment machinery.
+inline bool agg_is_regr(AggFn f) { return f >= AggFn::RegrSlope && f <= AggFn::RegrSxy; }
+inline bool agg_is_stat(AggFn f) { return f >= AggFn::VarSamp && f <= AggFn::RegrSxy; }
+inline bool agg_is_bivariate(AggFn f) { return f == AggFn::CovarSamp || f == AggFn::CovarPop || f == AggFn::Corr || agg_is_regr(f); }
+// bool_and / bool_or / bit_and / bit_or / bit_xor: one-pass folds of a 64-bit word, one state column of the argument's type
+inline bool agg_is_bitwise(AggFn f) { return f >= AggFn::BoolAnd && f <= AggFn::BitXor; }
 // [EXT] partial state columns, read by position and checked by suffix in Final modes:
 //  var / stddev:  [count] UInt64, [mean] Float64, [m2] Float64  (datafusion-functions-aggregate variance.rs)
 //  covar:         [count], [mean1], [mean2], [algo_const]        (covariance.rs)
 //  corr:          [count], [mean1], [m2_1], [mean2], [m2_2], [algo_const]  -- unpinned: no reference test fixes it
+//  regr_*:        [count], [mean_x], [mean_y], [m2_x], [m2_y], [algo_const]  -- unpinned (regr.rs; DESIGN.md §6 (xvi))
 inline std::vector<std::string> stat_state_suffixes(AggFn f) {
+  if (agg_is_regr(f)) return {"count", "mean_x", "mean_y", "m2_x", "m2_y", "algo_const"};
   if (f == AggFn::Corr) return {"count", "mean1", "m2_1", "mean2", "m2_2", "algo_const"};
   if (agg_is_bivariate(f)) return {"count", "mean1", "mean2", "algo_const"};
   return {"count", "mean", "m2"};
@@ -820,6 +828,9 @@ struct AggExpr {
   AggFn fn = AggFn::Sum;
   ExprPtr arg;           // null for COUNT(*) and in Final modes
   ExprPtr arg2;          // COVAR / CORR: the second argument (raw modes only)
+  // Final regr_* whose node carries the original arguments and "input_schema" (the protobuf form): y and x typed against
+  // that schema.  Every regr_* over one pair has the same partial state, so the engine merges it once per pair.
+  ExprPtr state_y, state_x;
   DataType input_type;   // type of arg (after AVG's integer->f64 coercion); for Final: taken from IR
   DataType sum_type;     // accumulator type for Sum/Avg
   DataType result_type;  // final value type
@@ -850,13 +861,30 @@ inline DataType avg_result_type(const DataType& t) {
 inline void check_stat_arg(const std::string& fn, const DataType& t) {
   if (!(t.is_integer() || t.is_float() || t.is_decimal())) throw PlanUnsupported(fn + " does not support an argument of type " + t.str());
 }
+// [EXT] bool_and / bool_or take Bool; bit_and / bit_or / bit_xor take Int8-Int64 and UInt8-UInt64.  The result (and the
+// partial state) has the argument's type.
+inline void check_bitwise_arg(AggFn f, const std::string& fn, const DataType& t) {
+  const bool ok = (f == AggFn::BoolAnd || f == AggFn::BoolOr) ? t.id == TypeId::Bool : t.is_integer();
+  if (!ok) throw PlanUnsupported(fn + " does not support an argument of type " + t.str());
+}
+inline const char* bitwise_state_suffix(AggFn f) {
+  switch (f) {
+    case AggFn::BoolAnd: return "bool_and";
+    case AggFn::BoolOr: return "bool_or";
+    case AggFn::BitAnd: return "bit_and";
+    case AggFn::BitOr: return "bit_or";
+    default: return "bit_xor";
+  }
+}
 
-// The statistical aggregates are typed here for every consumer of the plan IR, but only a consumer built with
-// B200_PLAN_STAT_AGGREGATES=1 computes them (the device engine: Makefile NVFLAGS, for every translation unit of the
-// library alike).  Any other consumer -- the CPU oracle -- refuses such a plan instead of mis-evaluating it.
+// The statistical, regression, bool and bit aggregates are typed here for every consumer of the plan IR, but only a
+// consumer built with B200_PLAN_STAT_AGGREGATES=1 computes them (the device engine: Makefile NVFLAGS, for every
+// translation unit of the library alike).  Any other consumer -- the CPU oracle -- refuses such a plan instead of
+// mis-evaluating it.
 #ifndef B200_PLAN_STAT_AGGREGATES
 #define B200_PLAN_STAT_AGGREGATES 0
 #endif
+// the gated names; AggFn::Sum: not one of them
 inline AggFn parse_stat_aggfn(const std::string& s) {
   // the lower-cased names and aliases the function registry resolves (datafusion-functions-aggregate)
   if (s == "var" || s == "var_samp" || s == "var_sample") return AggFn::VarSamp;
@@ -866,11 +894,25 @@ inline AggFn parse_stat_aggfn(const std::string& s) {
   if (s == "covar" || s == "covar_samp") return AggFn::CovarSamp;
   if (s == "covar_pop") return AggFn::CovarPop;
   if (s == "corr") return AggFn::Corr;
+  if (s == "regr_slope") return AggFn::RegrSlope;
+  if (s == "regr_intercept") return AggFn::RegrIntercept;
+  if (s == "regr_count") return AggFn::RegrCount;
+  if (s == "regr_r2") return AggFn::RegrR2;
+  if (s == "regr_avgx") return AggFn::RegrAvgx;
+  if (s == "regr_avgy") return AggFn::RegrAvgy;
+  if (s == "regr_sxx") return AggFn::RegrSxx;
+  if (s == "regr_syy") return AggFn::RegrSyy;
+  if (s == "regr_sxy") return AggFn::RegrSxy;
+  if (s == "bool_and") return AggFn::BoolAnd;
+  if (s == "bool_or") return AggFn::BoolOr;
+  if (s == "bit_and") return AggFn::BitAnd;
+  if (s == "bit_or") return AggFn::BitOr;
+  if (s == "bit_xor") return AggFn::BitXor;
   return AggFn::Sum;
 }
 inline AggFn parse_aggfn(const std::string& s) {
   const AggFn st = parse_stat_aggfn(s);
-  if (agg_is_stat(st)) {
+  if (st != AggFn::Sum) {
     if (!B200_PLAN_STAT_AGGREGATES) throw PlanUnsupported("aggregate '" + s + "' is not computed by this consumer of the plan IR");
     return st;
   }
@@ -1219,7 +1261,22 @@ inline PlanPtr parse_plan(const Json& j) {
           if (!name_ok || !type_ok)
             throw PlanUnsupported("Final " + a.at("fn").str() + ": state column '" + f.name + "' (" + f.type.str() + ") is not the expected '" + want + "'");
         }
+        if (agg_is_regr(ae.fn) && j.has("input_schema") && a.has("args") && a.at("args").size() == 2) {
+          const auto is = parse_schema(j.at("input_schema"));
+          ae.state_y = parse_expr(a.at("args").at(0), is);
+          ae.state_x = parse_expr(a.at("args").at(1), is);
+          check_stat_arg(a.at("fn").str(), ae.state_y->type);
+          check_stat_arg(a.at("fn").str(), ae.state_x->type);
+        }
         ae.input_type = DataType(TypeId::Float64);
+        ae.sum_type = ae.input_type;
+        ae.result_type = ae.fn == AggFn::RegrCount ? DataType(TypeId::UInt64) : ae.input_type;
+        state_col += ae.n_state_cols();
+      } else if (from_states && agg_is_bitwise(ae.fn)) {
+        // one state column of the argument's type, merged with the same operation
+        if (state_col >= c->schema.size()) throw std::runtime_error("Final aggregate: missing state column of " + ae.name);
+        check_bitwise_arg(ae.fn, "Final " + a.at("fn").str() + " state column '" + c->schema[state_col].name + "':", c->schema[state_col].type);
+        ae.input_type = c->schema[state_col].type;
         ae.sum_type = ae.input_type;
         ae.result_type = ae.input_type;
         state_col += ae.n_state_cols();
@@ -1261,6 +1318,9 @@ inline PlanPtr parse_plan(const Json& j) {
             check_stat_arg(a.at("fn").str(), ae.arg2->type);
           }
           it = DataType(TypeId::Float64);
+        } else if (agg_is_bitwise(ae.fn)) {
+          if (a.at("args").size() != 1) throw std::runtime_error(a.at("fn").str() + " takes 1 argument(s)");
+          check_bitwise_arg(ae.fn, a.at("fn").str(), it);
         }
         switch (ae.fn) {
           case AggFn::Sum:
@@ -1278,6 +1338,11 @@ inline PlanPtr parse_plan(const Json& j) {
             ae.input_type = it;
             ae.sum_type = DataType(TypeId::Int64);
             ae.result_type = DataType(TypeId::Int64);
+            break;
+          case AggFn::RegrCount:
+            ae.input_type = it;
+            ae.sum_type = it;
+            ae.result_type = DataType(TypeId::UInt64);
             break;
           default:
             ae.input_type = it;
@@ -1298,11 +1363,14 @@ inline PlanPtr parse_plan(const Json& j) {
           n->schema.push_back(Field{ae.name + "[count]", DataType(TypeId::Int64), false});
         } else if (ae.fn == AggFn::Sum) {
           n->schema.push_back(Field{ae.name + "[sum]", ae.sum_type, true});
+        } else if (agg_is_bitwise(ae.fn)) {
+          n->schema.push_back(Field{ae.name + "[" + bitwise_state_suffix(ae.fn) + "]", ae.sum_type, true});
         } else {
           n->schema.push_back(Field{ae.name + (ae.fn == AggFn::Min ? "[min]" : "[max]"), ae.sum_type, true});
         }
       } else {
-        n->schema.push_back(Field{ae.name, ae.result_type, ae.fn != AggFn::Count});
+        // [EXT] COUNT and regr_count are never NULL (0 for an empty group)
+        n->schema.push_back(Field{ae.name, ae.result_type, ae.fn != AggFn::Count && ae.fn != AggFn::RegrCount});
       }
       if (!n->grouping_sets.empty() && agg_is_stat(ae.fn))
         throw PlanUnsupported(a.at("fn").str() + " (" + ae.name + ") alongside grouping sets is not supported");

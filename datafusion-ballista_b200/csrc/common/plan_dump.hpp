@@ -84,7 +84,9 @@ inline std::string dump_sort_keys(const std::vector<SortKey>& ks) {
 inline std::string dump_plan(const PlanNode& n) {
   static const char* join_types[] = {"Inner", "Left", "Right", "Full", "LeftSemi", "RightSemi", "LeftAnti", "RightAnti"};
   static const char* agg_modes[] = {"Partial", "Final", "FinalPartitioned", "Single", "SinglePartitioned"};
-  static const char* agg_fns[] = {"sum", "min", "max", "count", "avg", "var_samp", "var_pop", "stddev_samp", "stddev_pop", "covar_samp", "covar_pop", "corr"};
+  static const char* agg_fns[] = {"sum", "min", "max", "count", "avg", "var_samp", "var_pop", "stddev_samp", "stddev_pop", "covar_samp", "covar_pop", "corr",
+                                  "regr_slope", "regr_intercept", "regr_count", "regr_r2", "regr_avgx", "regr_avgy", "regr_sxx", "regr_syy", "regr_sxy",
+                                  "bool_and", "bool_or", "bit_and", "bit_or", "bit_xor"};
   std::string o = "{\"op\":" + pbp::jstr(n.op_name);
   auto child = [&](size_t i) { return dump_plan(*n.children[i]); };
   switch (n.op) {

@@ -46,6 +46,8 @@ __global__ void agg_table_init_kernel(AggTable T, AccKinds kinds) {
         case ACC_MAX_F64: lo = 0x8000000000000000ull; break;
         case ACC_MIN_STR:
         case ACC_MAX_STR: hi = ACC_STR_NONE; break;
+        case ACC_AND: lo = ~0ull; break;
+        case ACC_RANGE_F64: lo = 0x7FFFFFFFFFFFFFFFull; hi = 0x8000000000000000ull; break;
         default: break;
       }
       T.acc[((unsigned long long)a * T.cap + i) * 2 + 0] = lo;
@@ -84,20 +86,53 @@ struct StatVal {
   bool ok;
 };
 __device__ __noinline__ StatVal stat_value(const unsigned long long* acc, unsigned long long cap, unsigned long long s, int code, int c_n, int c_sx,
-                                           int c_sy, int c_xx, int c_yy, int c_xy) {
+                                           int c_sy, int c_xx, int c_yy, int c_xy, int r_x, int r_y, int r_m2x, int r_m2y) {
   auto f64 = [&](int a) { return __longlong_as_double((long long)acc[((unsigned long long)a * cap + s) * 2]); };
   const unsigned long long n = acc[((unsigned long long)c_n * cap + s) * 2];
   const double dn = (double)n;
+  // an argument is constant in the group when the RANGE_F64 accumulator r (over its values, or over the states' means)
+  // holds one value and the largest state m2 (r_m2, Final modes) is 0: then that value is its mean, and its m2 and its
+  // co-moments are exactly 0, as DataFusion's Welford update keeps them for a constant argument (a rounded centre or a
+  // weighted mean of the state means would leave a residue that turns a NULL slope into noise)
+  auto constant = [&](int r, int r_m2, double* v) {
+    if (r == 255 || !n) return false;
+    const unsigned long long lo = acc[((unsigned long long)r * cap + s) * 2], hi = acc[((unsigned long long)r * cap + s) * 2 + 1];
+    if (lo != hi) return false;
+    if (r_m2 != 255 && f64_from_key((long long)acc[((unsigned long long)r_m2 * cap + s) * 2 + 1]) != 0.0) return false;
+    *v = f64_from_key((long long)lo);
+    return true;
+  };
+  double cx = 0.0, cy = 0.0;
+  const bool kx = constant(r_x, r_m2x, &cx), ky = constant(r_y, r_m2y, &cy);
   // a co-moment column c, corrected by its first-order sums (program.h, MomDesc)
   auto mom = [&](int c) { return n ? f64(c) - f64(c + 1) * f64(c + 2) / dn : f64(c); };
+  const double sxx = kx ? 0.0 : mom(c_xx), syy = ky ? 0.0 : mom(c_yy), sxy = (kx || ky) ? 0.0 : mom(c_xy);
+  // the partial state's means: the pass-1 centre plus the pass-2 mean deviation from it (c_xy + 1 / + 2 hold
+  // Σw(x - mx) / Σw(y - my) around exactly these centres), which removes the rounding of the f64 sum to first order
+  const double mx = kx ? cx : n ? f64(c_sx) / dn + f64(c_xy + 1) / dn : 0.0;
+  const double my = ky ? cy : n ? f64(c_sy) / dn + f64(c_xy + 2) / dn : 0.0;
   switch (code) {
-    // the partial state's means: the pass-1 centre plus the pass-2 mean deviation from it (c_xy + 1 / + 2 hold
-    // Σw(x - mx) / Σw(y - my) around exactly these centres), which removes the rounding of the f64 sum to first order
-    case SO_MEAN_X: return StatVal{n ? f64(c_sx) / dn + f64(c_xy + 1) / dn : 0.0, true};
-    case SO_MEAN_Y: return StatVal{n ? f64(c_sy) / dn + f64(c_xy + 2) / dn : 0.0, true};
-    case SO_M2_X: return StatVal{mom(c_xx), true};
-    case SO_M2_Y: return StatVal{mom(c_yy), true};
-    case SO_CO: return StatVal{mom(c_xy), true};
+    case SO_MEAN_X: return StatVal{mx, true};
+    case SO_MEAN_Y: return StatVal{my, true};
+    case SO_M2_X: return StatVal{sxx, true};
+    case SO_M2_Y: return StatVal{syy, true};
+    case SO_CO: return StatVal{sxy, true};
+    case SO_REGR_AVGX: return StatVal{mx, n > 0};
+    case SO_REGR_AVGY: return StatVal{my, n > 0};
+    case SO_REGR_SXX: return StatVal{sxx, n > 0};
+    case SO_REGR_SYY: return StatVal{syy, n > 0};
+    case SO_REGR_SXY: return StatVal{sxy, n > 0};
+    case SO_REGR_SLOPE:
+    case SO_REGR_INTERCEPT: {
+      if (n <= 1 || sxx == 0.0) return StatVal{0.0, false};
+      const double slope = (sxy / dn) / (sxx / dn);
+      return StatVal{code == SO_REGR_SLOPE ? slope : my - slope * mx, true};
+    }
+    case SO_REGR_R2: {
+      if (n <= 1 || sxx == 0.0 || syy == 0.0) return StatVal{0.0, false};
+      const double cov = sxy / dn;
+      return StatVal{cov * cov / ((sxx / dn) * (syy / dn)), true};
+    }
     case SO_VAR_SAMP:
     case SO_STDDEV_SAMP:
     case SO_COVAR_SAMP: {
@@ -150,7 +185,7 @@ __global__ void agg_extract_kernel(AggTable T, AggExtractArgs A) {
           break;
         }
         case AO_STAT: {
-          const StatVal r = stat_value(T.acc, T.cap, s, o.imm, o.st[0], o.st[1], o.st[2], o.st[3], o.st[4], o.st[5]);
+          const StatVal r = stat_value(T.acc, T.cap, s, o.imm, o.st[0], o.st[1], o.st[2], o.st[3], o.st[4], o.st[5], o.st[6], o.st[7], o.st[8], o.st[9]);
           ((double*)o.data)[pos] = r.v;
           if (o.valid) o.valid[pos] = r.ok ? 1 : 0;
           break;

@@ -53,9 +53,13 @@ enum AggOutKind : uint8_t {
 // what an AO_STAT column holds.  n = count, mean = sum / n, m2 / co = the pass-2 co-moments.  [EXT] NULL rules: sample
 // variants n <= 1, population variants n = 0, CORR n < 2 or either m2 = 0; partial states are never NULL (an empty
 // group's mean and moments are 0, as DataFusion's accumulators start)
+// The regression aggregates (regr_*; [EXT], unpinned: DESIGN.md §6 (xvi)) with sxx, syy, sxy the co-moments: avgx / avgy /
+// sxx / syy / sxy NULL when n = 0; slope = (sxy/n) / (sxx/n) and intercept = my - slope * mx NULL when n <= 1 or sxx = 0;
+// r2 = (sxy/n)^2 / ((sxx/n)(syy/n)) NULL when n <= 1, sxx = 0 or syy = 0.
 enum StatOut : uint8_t {
   SO_MEAN_X = 0, SO_MEAN_Y, SO_M2_X, SO_M2_Y, SO_CO,
-  SO_VAR_SAMP, SO_VAR_POP, SO_STDDEV_SAMP, SO_STDDEV_POP, SO_COVAR_SAMP, SO_COVAR_POP, SO_CORR
+  SO_VAR_SAMP, SO_VAR_POP, SO_STDDEV_SAMP, SO_STDDEV_POP, SO_COVAR_SAMP, SO_COVAR_POP, SO_CORR,
+  SO_REGR_SLOPE, SO_REGR_INTERCEPT, SO_REGR_R2, SO_REGR_AVGX, SO_REGR_AVGY, SO_REGR_SXX, SO_REGR_SYY, SO_REGR_SXY
 };
 struct AggOut {
   void* data;
@@ -65,7 +69,10 @@ struct AggOut {
   uint8_t a, b;
   uint8_t phys;   // output encoding
   int32_t imm;
-  uint8_t st[6];  // AO_STAT: count acc, sum-x acc, sum-y acc, xx / yy / xy co-moment columns
+  // AO_STAT: count acc, sum-x acc, sum-y acc, xx / yy / xy co-moment columns; then (255: none) the RANGE_F64 accs of x, y
+  // (raw rows) or of the states' means, and those of the states' m2_x, m2_y (Final): an argument is constant in the group
+  // when its range is one value (and every state's m2 is 0), and then its m2 and co-moments are exactly 0 (DESIGN.md §4.1)
+  uint8_t st[10];
   uint8_t prec;   // AO_AVG_DEC: result precision
   uint8_t _pad;
 };

@@ -2332,6 +2332,34 @@ __device__ __noinline__ void load_key(const Lane L, const Operand ko, int r, Key
   }
 }
 
+// merge into an AND / OR / XOR or RANGE_F64 cell: one 64-bit atomic per word.  Kept apart from table_merge, which the
+// fused kernel's flush calls: a larger table_merge costs that kernel spill stores around the call.
+__device__ __noinline__ void table_merge_word(int kind, unsigned long long slot, int a, Acc128 x) {
+  const AggTable& T = PROG.table;
+  unsigned long long* cell = T.acc + ((unsigned long long)a * T.cap + slot) * 2;
+  switch (kind) {
+    case ACC_AND: atomicAnd(&cell[0], (unsigned long long)x.lo); break;
+    case ACC_OR: atomicOr(&cell[0], (unsigned long long)x.lo); break;
+    case ACC_XOR: atomicXor(&cell[0], (unsigned long long)x.lo); break;
+    default:
+      atomicMin((long long*)&cell[0], (long long)x.lo);
+      atomicMax((long long*)&cell[1], (long long)x.hi);
+  }
+}
+
+// row r's contribution to an AND / OR / XOR accumulator (the operand sign-extended to 64 bits, a bool as 0 / 1) or to a
+// RANGE_F64 one (the double's total-order key as both the smallest and the largest value)
+__device__ __noinline__ Acc128 acc_word(const Lane L, const AccDesc ad, int r) {
+  Acc128 x;
+  if (ad.kind == ACC_RANGE_F64) {
+    x.lo = x.hi = (uint64_t)f64_order_key(ld1_f64(L, ad.src, r));
+  } else {
+    x.lo = (uint64_t)ld1_i64(L, ad.src, r);
+    x.hi = 0;
+  }
+  return x;
+}
+
 // per-row path (high cardinality): every live row upserts its group and updates with atomics
 __device__ __noinline__ uint32_t sink_agg_global(const Lane L, uint32_t active) {
   if (*(volatile unsigned int*)&PROG.status->overflow) return active;
@@ -2366,8 +2394,11 @@ __device__ __noinline__ uint32_t sink_agg_global(const Lane L, uint32_t active) 
         x.lo = (uint64_t)__double_as_longlong(ld1_f64(L, ad.src, r));
       } else if (ad.kind == ACC_MIN_F64 || ad.kind == ACC_MAX_F64) {
         x.lo = (uint64_t)f64_order_key(ld1_f64(L, ad.src, r));
+      } else if (ad.kind >= ACC_AND) {
+        x = acc_word(L, ad, r);
       }
       if (ad.kind == ACC_MIN_STR || ad.kind == ACC_MAX_STR) table_merge_str(ad.kind, slot, a, x);
+      else if (ad.kind >= ACC_AND) table_merge_word(ad.kind, slot, a, x);
       else table_merge(ad.kind, slot, a, x);
     }
   }
@@ -2430,6 +2461,8 @@ __device__ __noinline__ uint32_t sink_agg_global_gsets(const Lane L, uint32_t ac
         x[a].lo = (uint64_t)__double_as_longlong(ld1_f64(L, ad.src, r));
       } else if (ad.kind == ACC_MIN_F64 || ad.kind == ACC_MAX_F64) {
         x[a].lo = (uint64_t)f64_order_key(ld1_f64(L, ad.src, r));
+      } else if (ad.kind >= ACC_AND) {
+        x[a] = acc_word(L, ad, r);
       }
     }
     for (int s = 0; s < n_sets; s++) {
@@ -2461,6 +2494,7 @@ __device__ __noinline__ uint32_t sink_agg_global_gsets(const Lane L, uint32_t ac
         const uint8_t kind = PROG.acc[a].kind;
         if (kind == ACC_MIN_I128 || kind == ACC_MAX_I128) table_minmax_i128_cas(kind, slot, a, x[a]);
         else if (kind == ACC_MIN_STR || kind == ACC_MAX_STR) table_merge_str(kind, slot, a, x[a]);
+        else if (kind >= ACC_AND) table_merge_word(kind, slot, a, x[a]);
         else table_merge(kind, slot, a, x[a]);
       }
     }
@@ -2597,13 +2631,13 @@ __device__ __noinline__ void reg_merge_big(RegGroupTable* gt, int G, int g, int 
   table_merge(ACC_SUM_I128, slot, a, x);
 }
 
-// ---- side accumulators of the general register sink: string MIN / MAX and UInt64 MIN / MAX ----------------------------
-// Their per-thread state lives in memory, not in the register matrix: the 64-bit value (string: the view's pointer) in
-// the acc_side scratch, a string's length in the acc_hi scratch (ACC_STR_NONE: no value yet).  They are folded in by one
-// rolled call per tile and merged by their own flush, all of it only in the pipeline_kernel variants instantiated with
-// SIDE = true (launched when the program has such an accumulator): every other variant, the fused kernel included,
-// compiles exactly as it does without them.
-__device__ __forceinline__ bool acc_is_side(const AccDesc& ad) { return ad.kind == ACC_MIN_STR || ad.kind == ACC_MAX_STR || ad.zext; }
+// ---- side accumulators of the general register sink: string MIN / MAX, UInt64 MIN / MAX, AND / OR / XOR, RANGE_F64 ------
+// Their per-thread state lives in memory, not in the register matrix: the 64-bit value (string: the view's pointer;
+// RANGE_F64: the smallest key) in the acc_side scratch, a string's length (RANGE_F64: the largest key) in the acc_hi
+// scratch (ACC_STR_NONE: no string yet).  They are folded in by one rolled call per tile and merged by their own flush,
+// all of it only in the pipeline_kernel variants instantiated with SIDE = true (launched when the program has such an
+// accumulator): every other variant, the fused kernel included, compiles exactly as it does without them.
+__device__ __forceinline__ bool acc_is_side(const AccDesc& ad) { return ad.kind == ACC_MIN_STR || ad.kind == ACC_MAX_STR || ad.zext || ad.kind >= ACC_AND; }
 
 __device__ __noinline__ void reg_side_init(unsigned long long* hi, unsigned long long* side) {
   for (int a = 0; a < PROG.n_acc && a < VM_REG_ACC; a++) {
@@ -2613,6 +2647,11 @@ __device__ __noinline__ void reg_side_init(unsigned long long* hi, unsigned long
       const int w = g * VM_REG_ACC + a;
       if (ad.zext) {
         side[w] = ad.kind == ACC_MIN_I128 ? ~0ull : 0ull;  // UInt64 identities: no value orders below / above them
+      } else if (ad.kind == ACC_RANGE_F64) {
+        side[w] = 0x7FFFFFFFFFFFFFFFull;
+        hi[w] = 0x8000000000000000ull;
+      } else if (ad.kind >= ACC_AND) {
+        side[w] = ad.kind == ACC_AND ? ~0ull : 0ull;
       } else {
         side[w] = 0;
         hi[w] = ACC_STR_NONE;
@@ -2633,6 +2672,15 @@ __device__ __noinline__ void reg_side_rows(const Lane L, uint32_t active, uint32
       if (ad.zext) {
         const uint64_t u = (uint64_t)ld1_i64(L, ad.src, r);
         if (ad.kind == ACC_MIN_I128 ? u < side[w] : u > side[w]) side[w] = u;
+      } else if (ad.kind >= ACC_AND) {
+        const Acc128 x = acc_word(L, ad, r);
+        if (ad.kind == ACC_AND) side[w] &= x.lo;
+        else if (ad.kind == ACC_OR) side[w] |= x.lo;
+        else if (ad.kind == ACC_XOR) side[w] ^= x.lo;
+        else {
+          if ((long long)x.lo < (long long)side[w]) side[w] = x.lo;
+          if ((long long)x.hi > (long long)hi[w]) hi[w] = x.hi;
+        }
       } else {
         const StrRef s = ld1_str(L, ad.src, r);
         if (str_beats(ad.kind == ACC_MIN_STR, (uint64_t)s.p, s.len, side[w], hi[w])) {
@@ -2834,10 +2882,20 @@ __device__ __noinline__ Acc128 acc_combine(int kind, Acc128 x, Acc128 y) {
   }
 }
 
-// acc_combine plus the side accumulators (a zero-extended UInt64 compares correctly as a 128-bit integer)
+// acc_combine plus the side accumulators (a zero-extended UInt64 compares correctly as a 128-bit integer); AND / OR /
+// XOR combine the whole 64-bit words, RANGE_F64 the smallest (lo) and the largest (hi) keys
 __device__ __noinline__ Acc128 acc_combine_side(int kind, Acc128 x, Acc128 y) {
   if (kind == ACC_MIN_STR || kind == ACC_MAX_STR) return str_beats(kind == ACC_MIN_STR, y.lo, y.hi, x.lo, x.hi) ? y : x;
-  return acc_combine(kind, x, y);
+  switch (kind) {
+    case ACC_AND: x.lo &= y.lo; return x;
+    case ACC_OR: x.lo |= y.lo; return x;
+    case ACC_XOR: x.lo ^= y.lo; return x;
+    case ACC_RANGE_F64:
+      if ((long long)y.lo < (long long)x.lo) x.lo = y.lo;
+      if ((long long)y.hi > (long long)x.hi) x.hi = y.hi;
+      return x;
+    default: return acc_combine(kind, x, y);
+  }
 }
 
 // rolled CTA reduction of scratch[a][thread] -> scratch[a][0], then merge into the global table.  SIDE (general register
@@ -2850,7 +2908,9 @@ __device__ __noinline__ void reg_flush_group(RegGroupTable* gt, Acc128* scratch,
     for (int a = 0; a < n_acc; a++)
       if (acc_is_side(PROG.acc[a])) {
         scratch[a * B + tid].lo = PROG.acc_side[t + a];
-        scratch[a * B + tid].hi = PROG.acc[a].zext ? 0ull : PROG.acc_hi[t + a];
+        const uint8_t kind = PROG.acc[a].kind;
+        const bool two_words = kind == ACC_MIN_STR || kind == ACC_MAX_STR || kind == ACC_RANGE_F64;
+        scratch[a * B + tid].hi = two_words ? PROG.acc_hi[t + a] : 0ull;
       }
   }
   __syncthreads();
@@ -2882,6 +2942,7 @@ __device__ __noinline__ void reg_flush_group(RegGroupTable* gt, Acc128* scratch,
       for (int a = 0; a < n_acc; a++) {
         const int kind = PROG.acc[a].kind;
         if (SIDE && (kind == ACC_MIN_STR || kind == ACC_MAX_STR)) table_merge_str(kind, slot, a, scratch[a * B]);
+        else if (SIDE && kind >= ACC_AND) table_merge_word(kind, slot, a, scratch[a * B]);
         else table_merge(kind, slot, a, scratch[a * B]);
       }
     }

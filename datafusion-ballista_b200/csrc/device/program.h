@@ -170,9 +170,14 @@ struct OutCol {
 //  MIN_STR / MAX_STR: the string view {ptr, len} of the best value so far (unsigned bytewise order, a proper prefix
 //  first), len = ACC_STR_NONE while no value has been seen -- the identity of both (an empty string is a value).
 //  The characters stay where the rows had them; the host copies the extracted results into buffers of their own.
-//  String MIN / MAX and the zero-extended UInt64 MIN / MAX are the register sink's "side" accumulators (pipeline.cu).
+//  AND / OR / XOR (bool_and / bool_or, bit_and / bit_or / bit_xor): a 64-bit word in lo (the operand sign-extended to
+//  64 bits; the extraction truncates it to the output's width); identities all-ones, 0 and 0.
+//  RANGE_F64: the total-order keys of the smallest (lo) and the largest (hi) double seen (the regression aggregates'
+//  test for a constant argument, DESIGN.md §4.1); identity (MIN_F64's, MAX_F64's).
+//  String MIN / MAX, the zero-extended UInt64 MIN / MAX, AND / OR / XOR and RANGE_F64 are the register sink's "side"
+//  accumulators (pipeline.cu).
 enum AccKind : uint8_t { ACC_SUM_I128 = 0, ACC_SUM_F64, ACC_COUNT, ACC_MIN_I128, ACC_MAX_I128, ACC_MIN_F64, ACC_MAX_F64, ACC_COUNT_STAR,
-                         ACC_MIN_STR, ACC_MAX_STR };
+                         ACC_MIN_STR, ACC_MAX_STR, ACC_AND, ACC_OR, ACC_XOR, ACC_RANGE_F64 };
 static const unsigned long long ACC_STR_NONE = ~0ull;
 
 struct AccDesc {
@@ -245,7 +250,7 @@ struct Program {
   Operand keys[VM_MAX_KEYS];    // aggregate sinks: group keys
   Operand key_hash;             // aggregate sinks: I64 register holding the row hash (OPD_NONE if no keys)
   uint8_t keys_all_i64;         // every key is an integer-like 64-bit value (ints, dates, bools, packed strings)
-  uint8_t has_side_acc;         // some accumulator is a string MIN / MAX or a UInt64 MIN / MAX (zext)
+  uint8_t has_side_acc;         // some accumulator is a side accumulator (AccKind above)
   uint8_t _pad1[2];
   AccDesc acc[VM_MAX_ACC];
   AggTable table;

@@ -1285,7 +1285,9 @@ struct AggLowered {
     std::string name;
     bool with_valid;
     int key_idx;
-    uint8_t st[6];  // AO_STAT: count, sum x, sum y accumulators; xx, yy, xy co-moments (indices into `moms` until lowered)
+    // AO_STAT: count, sum x, sum y accumulators; xx, yy, xy co-moments (indices into `moms` until lowered); the RANGE_F64
+    // accumulators of the regression aggregates' constant test, or 255 (AggOut::st)
+    uint8_t st[10];
   };
   std::vector<OutRecipe> outs;
 };
@@ -1455,6 +1457,14 @@ void lower_aggregate(PipelineBuilder& pb, const PlanNode& node, AggLowered& L, i
     push(s ? AO_MINMAX_STR : f ? AO_MINMAX_F64 : sum_out_kind(t), a, c, t, name, v.nullable || scalar);
     if (s) L.outs.back().phys = PH_STRVIEW;  // copied into a buffer of its own after the extraction
   };
+  // bool_and / bool_or / bit_and / bit_or / bit_xor of a value (raw rows or a partial state column): a 64-bit AND / OR /
+  // XOR word, NULL without a non-NULL value, written in the output's width
+  auto push_bitwise = [&](AggFn fn, const ColRef& v, const DataType& t, const std::string& name) {
+    const uint8_t kind = (fn == AggFn::BoolAnd || fn == AggFn::BitAnd) ? ACC_AND : (fn == AggFn::BoolOr || fn == AggFn::BitOr) ? ACC_OR : ACC_XOR;
+    int a = add_acc(pb, L, kind, &v);
+    int c = v.nullable ? add_acc(pb, L, ACC_COUNT, &v) : star;
+    push(AO_ACC_I64, a, c, t, name, v.nullable || scalar);
+  };
   // VAR / STDDEV / COVAR / CORR: the group's count and f64 sums (pass 1) and its centred co-moments (pass 2), then the
   // result or the partial state columns computed from them at extraction
   auto f64_expr = [](const ExprPtr& e) -> ExprPtr {
@@ -1474,16 +1484,24 @@ void lower_aggregate(PipelineBuilder& pb, const PlanNode& node, AggLowered& L, i
     c->nullable = pb.cols.at(i).nullable;
     return c;
   };
-  auto push_stat = [&](const AggExpr& ae, int cnt, int sx, int sy, int mxx, int myy, int mxy) {
+  // ranges: the regression aggregates' RANGE_F64 accumulators (x, y, and in Final modes the states' m2_x, m2_y), else 255
+  auto push_stat = [&](const AggExpr& ae, int cnt, int sx, int sy, int mxx, int myy, int mxy, std::array<int, 4> ranges = {255, 255, 255, 255}) {
     const std::string& nm = ae.name;
-    const uint8_t st[6] = {(uint8_t)cnt, (uint8_t)sx, (uint8_t)sy, (uint8_t)mxx, (uint8_t)myy, (uint8_t)mxy};
+    const uint8_t st[10] = {(uint8_t)cnt, (uint8_t)sx, (uint8_t)sy, (uint8_t)mxx, (uint8_t)myy, (uint8_t)mxy,
+                            (uint8_t)ranges[0], (uint8_t)ranges[1], (uint8_t)ranges[2], (uint8_t)ranges[3]};
     auto out = [&](int code, const std::string& name) {
       push(AO_STAT, 0, 0, DataType(TypeId::Float64), name, true, code);
       memcpy(L.outs.back().st, st, sizeof st);
     };
     if (emit_states) {
       push(AO_COUNT, cnt, 255, DataType(TypeId::UInt64), nm + "[count]", false);
-      if (ae.fn == AggFn::Corr) {
+      if (agg_is_regr(ae.fn)) {
+        out(SO_MEAN_X, nm + "[mean_x]");
+        out(SO_MEAN_Y, nm + "[mean_y]");
+        out(SO_M2_X, nm + "[m2_x]");
+        out(SO_M2_Y, nm + "[m2_y]");
+        out(SO_CO, nm + "[algo_const]");
+      } else if (ae.fn == AggFn::Corr) {
         out(SO_MEAN_X, nm + "[mean1]");
         out(SO_M2_X, nm + "[m2_1]");
         out(SO_MEAN_Y, nm + "[mean2]");
@@ -1506,12 +1524,35 @@ void lower_aggregate(PipelineBuilder& pb, const PlanNode& node, AggLowered& L, i
       case AggFn::StddevPop: out(SO_STDDEV_POP, nm); break;
       case AggFn::CovarSamp: out(SO_COVAR_SAMP, nm); break;
       case AggFn::CovarPop: out(SO_COVAR_POP, nm); break;
+      case AggFn::RegrCount: push(AO_COUNT, cnt, 255, DataType(TypeId::UInt64), nm, false); break;
+      case AggFn::RegrSlope: out(SO_REGR_SLOPE, nm); break;
+      case AggFn::RegrIntercept: out(SO_REGR_INTERCEPT, nm); break;
+      case AggFn::RegrR2: out(SO_REGR_R2, nm); break;
+      case AggFn::RegrAvgx: out(SO_REGR_AVGX, nm); break;
+      case AggFn::RegrAvgy: out(SO_REGR_AVGY, nm); break;
+      case AggFn::RegrSxx: out(SO_REGR_SXX, nm); break;
+      case AggFn::RegrSyy: out(SO_REGR_SYY, nm); break;
+      case AggFn::RegrSxy: out(SO_REGR_SXY, nm); break;
       default: out(SO_CORR, nm); break;
     }
   };
+  // Final regr_*: the pairs merged so far (RegrMerged::st as AggOut::st, co-moments as indices into L.moms)
+  struct RegrMerged {
+    ExprPtr y, x;
+    int st[10];
+  };
+  std::vector<RegrMerged> regr_merged;
   auto lower_stat_states = [&](const AggExpr& ae) {
     // Chan's merge: n = sum n_i, mean = sum n_i * mean_i / n, m2 = sum (m2_i + n_i * (mean_i - mean)^2), and the same for the
     // co-moment with both means.  Pass 1 sums n_i and n_i * mean_i, pass 2 the rest around the merged means.
+    // every regr_* over one (y, x) pair has the same partial state: merged once, by the first of them
+    if (ae.state_y)
+      for (const RegrMerged& p : regr_merged)
+        if (expr_equal(p.y, ae.state_y) && expr_equal(p.x, ae.state_x)) {
+          if (ae.fn == AggFn::RegrCount) push(AO_COUNT, p.st[0], 255, DataType(TypeId::UInt64), ae.name, false);
+          else push_stat(ae, p.st[0], p.st[1], p.st[2], p.st[3], p.st[4], p.st[5], {p.st[6], p.st[7], p.st[8], p.st[9]});
+          return;
+        }
     const size_t c0 = state_col;
     ColRef n_i = pb.cols.at(c0);
     const int cnt = add_acc(pb, L, ACC_SUM_I128, &n_i);
@@ -1532,6 +1573,42 @@ void lower_aggregate(PipelineBuilder& pb, const PlanNode& node, AggLowered& L, i
       const int sx = weighted(c0 + 1);
       const int mxx = add_mom(pb, L, mean, mean, &w, &m2, cnt, sx, sx);
       push_stat(ae, cnt, sx, sx, mxx, mxx, mxx);
+      return;
+    }
+    if (agg_is_regr(ae.fn)) {  // [count] [mean_x] [mean_y] [m2_x] [m2_y] [algo_const]
+      if (ae.fn == AggFn::RegrCount && !emit_states) {  // the merged count alone
+        push(AO_COUNT, cnt, 255, DataType(TypeId::UInt64), ae.name, false);
+        return;
+      }
+      ColRef mean_x = pb.cols.at(c0 + 1), mean_y = pb.cols.at(c0 + 2), m2_x = pb.cols.at(c0 + 3), m2_y = pb.cols.at(c0 + 4), co = pb.cols.at(c0 + 5);
+      const int sx = weighted(c0 + 1), sy = weighted(c0 + 2);
+      const int mxy = add_mom(pb, L, mean_x, mean_y, &w, &co, cnt, sx, sy);
+      const int mxx = add_mom(pb, L, mean_x, mean_x, &w, &m2_x, cnt, sx, sx);
+      const int myy = add_mom(pb, L, mean_y, mean_y, &w, &m2_y, cnt, sy, sy);
+      // the constant test over the states: the range of the non-empty states' means and the largest state m2
+      auto mean_range = [&](size_t mean_col) {
+        auto zero = std::make_shared<Expr>();
+        zero->kind = Expr::Lit;
+        zero->type = pb.cols.at(c0).type;
+        zero->nullable = false;
+        auto nonempty = std::make_shared<Expr>();
+        nonempty->kind = Expr::Bin;
+        nonempty->op = BinOp::Gt;
+        nonempty->type = DataType(TypeId::Bool);
+        nonempty->args = {col_expr(c0), zero};
+        nonempty->nullable = pb.cols.at(c0).nullable;
+        auto e = std::make_shared<Expr>();
+        e->kind = Expr::Case;
+        e->type = DataType(TypeId::Float64);
+        e->nullable = true;
+        e->args = {nonempty, col_expr(mean_col)};
+        ColRef v = pb.compile(*e);
+        return add_acc(pb, L, ACC_RANGE_F64, &v);
+      };
+      const int rx = mean_range(c0 + 1), ry = mean_range(c0 + 2);
+      const int rm2x = add_acc(pb, L, ACC_RANGE_F64, &m2_x), rm2y = add_acc(pb, L, ACC_RANGE_F64, &m2_y);
+      push_stat(ae, cnt, sx, sy, mxx, myy, mxy, {rx, ry, rm2x, rm2y});
+      if (ae.state_y) regr_merged.push_back(RegrMerged{ae.state_y, ae.state_x, {cnt, sx, sy, mxx, myy, mxy, rx, ry, rm2x, rm2y}});
       return;
     }
     const bool corr = ae.fn == AggFn::Corr;  // corr: [count] [mean1] [m2_1] [mean2] [m2_2] [algo_const]; covar: [count] [mean1] [mean2] [algo_const]
@@ -1576,6 +1653,23 @@ void lower_aggregate(PipelineBuilder& pb, const PlanNode& node, AggLowered& L, i
       stat_args.emplace(key, r);
       return r;
     };
+    if (agg_is_regr(ae.fn)) {
+      // regr_*(y, x): the second argument is the independent variable.  The same pair, the same cache keys and the same
+      // co-moments as corr(x, y), so the nine functions and CORR over one pair share one set of pass-1 sums and three
+      // co-moments; the RANGE_F64 accumulators make the m2 of a constant argument exactly 0 (stat_value)
+      const ColRef x = arg(ae.arg2, ae.arg), y = arg(ae.arg, ae.arg2);
+      const int cnt = x.nullable ? add_acc(pb, L, ACC_COUNT, &x) : star;
+      if (ae.fn == AggFn::RegrCount && !emit_states) {  // the count alone: no sums, no second pass
+        push(AO_COUNT, cnt, 255, DataType(TypeId::UInt64), ae.name, false);
+        return;
+      }
+      const int sx = add_acc(pb, L, ACC_SUM_F64, &x), sy = add_acc(pb, L, ACC_SUM_F64, &y);
+      const int mxy = add_mom(pb, L, x, y, nullptr, nullptr, cnt, sx, sy);
+      const int mxx = add_mom(pb, L, x, x, nullptr, nullptr, cnt, sx, sx);
+      const int myy = add_mom(pb, L, y, y, nullptr, nullptr, cnt, sy, sy);
+      push_stat(ae, cnt, sx, sy, mxx, myy, mxy, {add_acc(pb, L, ACC_RANGE_F64, &x), add_acc(pb, L, ACC_RANGE_F64, &y), 255, 255});
+      return;
+    }
     const ColRef x = arg(ae.arg, ae.arg2);
     const int cnt = x.nullable ? add_acc(pb, L, ACC_COUNT, &x) : star;
     const int sx = add_acc(pb, L, ACC_SUM_F64, &x);
@@ -1603,6 +1697,15 @@ void lower_aggregate(PipelineBuilder& pb, const PlanNode& node, AggLowered& L, i
         state_col += (size_t)ae.n_state_cols();
       } else {
         lower_stat_rows(ae);
+      }
+      continue;
+    }
+    if (agg_is_bitwise(ae.fn)) {
+      if (from_states) {
+        push_bitwise(ae.fn, pb.cols.at(state_col), ae.result_type, nm);
+        state_col += (size_t)ae.n_state_cols();
+      } else {
+        push_bitwise(ae.fn, pb.compile(*ae.arg), ae.result_type, emit_states ? nm + "[" + bitwise_state_suffix(ae.fn) + "]" : nm);
       }
       continue;
     }
@@ -2333,7 +2436,7 @@ DevBatchPtr run_aggregate(const Exec& x, const BuilderFactory& make_pb, const Pl
       P.acc_hi = (unsigned long long*)hi->ptr;
       // string / UInt64 MIN / MAX keep their per-thread values in a scratch of their own (initialised by the kernel)
       for (size_t a = 0; a < L.accs.size(); a++)
-        P.has_side_acc |= (L.accs[a].kind == ACC_MIN_STR || L.accs[a].kind == ACC_MAX_STR || L.accs[a].zext) ? 1 : 0;
+        P.has_side_acc |= (L.accs[a].kind == ACC_MIN_STR || L.accs[a].kind == ACC_MAX_STR || L.accs[a].zext || L.accs[a].kind >= ACC_AND) ? 1 : 0;
       if (P.has_side_acc) {
         DevPtr side = dev_alloc(hi_bytes, x.st());
         tm.keep.push_back(side);
@@ -2428,16 +2531,34 @@ DevBatchPtr run_aggregate(const Exec& x, const BuilderFactory& make_pb, const Pl
   out->n = n_groups;
   AggExtractArgs A;
   memset(&A, 0, sizeof A);
-  if (L.outs.size() > (size_t)VM_MAX_OUT) throw EngineError(B200_ERR_UNSUPPORTED, "too many aggregate output columns");
-  A.n_out = (int)L.outs.size();
+  // identical recipes -- the partial states of several regr_* over one pair, say -- are extracted once and the column
+  // is shared by every output that names it
+  std::vector<int> same_as(L.outs.size(), -1);
+  size_t n_unique = 0;
+  for (size_t j = 0; j < L.outs.size(); j++) {
+    const auto& r = L.outs[j];
+    for (size_t i = 0; i < j && same_as[j] < 0; i++) {
+      const auto& q = L.outs[i];
+      if (same_as[i] < 0 && (r.kind == AO_STAT || (r.kind == AO_COUNT && r.type.id == TypeId::UInt64)) && q.kind == r.kind && q.a == r.a && q.b == r.b && q.imm == r.imm &&
+          q.phys == r.phys && q.type.id == r.type.id && q.with_valid == r.with_valid && memcmp(q.st, r.st, sizeof r.st) == 0)
+        same_as[j] = (int)i;
+    }
+    if (same_as[j] < 0) n_unique++;
+  }
+  if (n_unique > (size_t)VM_MAX_OUT) throw EngineError(B200_ERR_UNSUPPORTED, "too many aggregate output columns");
+  A.n_out = (int)n_unique;
   A.n_keys = table_keys;
   DevPtr counter = dev_alloc(16, x.st());
   CUDA_CHECK(cudaMemsetAsync(counter->ptr, 0, 16, x.st()));
   A.counter = (unsigned long long*)counter->ptr;
   A.error = (unsigned int*)((uint8_t*)counter->ptr + 8);
   uint64_t wbytes = 0;
-  for (size_t j = 0; j < L.outs.size(); j++) {
+  for (size_t j = 0, k = 0; j < L.outs.size(); j++) {
     const auto& r = L.outs[j];
+    if (same_as[j] >= 0) {
+      out->cols.push_back(out->cols[(size_t)same_as[j]]);
+      continue;
+    }
     DevColumn oc = make_out_column(r.name, r.type, r.phys, n_groups, r.with_valid, x.st());
     oc.n = n_groups;
     if (r.key_idx >= 0) {
@@ -2448,7 +2569,7 @@ DevBatchPtr run_aggregate(const Exec& x, const BuilderFactory& make_pb, const Pl
         for (auto& k : pb.keep) oc.keep.push_back(k);
       }
     }
-    AggOut& o = A.out[j];
+    AggOut& o = A.out[k++];
     o.data = (void*)oc.data;
     o.valid = (uint8_t*)oc.valid;
     o.aux = nullptr;
