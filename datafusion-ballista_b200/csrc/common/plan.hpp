@@ -799,7 +799,7 @@ inline ExprPtr parse_expr(const Json& j, const Schema& in) {
 // ----------------------------------------------------------------------------------------------
 enum class AggFn : uint8_t { Sum, Min, Max, Count, Avg, VarSamp, VarPop, StddevSamp, StddevPop, CovarSamp, CovarPop, Corr,
                               RegrSlope, RegrIntercept, RegrCount, RegrR2, RegrAvgx, RegrAvgy, RegrSxx, RegrSyy, RegrSxy,
-                              BoolAnd, BoolOr, BitAnd, BitOr, BitXor };
+                              BoolAnd, BoolOr, BitAnd, BitOr, BitXor, FirstValue, LastValue };
 enum class AggMode : uint8_t { Partial, Final, FinalPartitioned, Single, SinglePartitioned };
 
 inline bool agg_mode_consumes_states(AggMode m) { return m == AggMode::Final || m == AggMode::FinalPartitioned; }
@@ -812,6 +812,10 @@ inline bool agg_is_stat(AggFn f) { return f >= AggFn::VarSamp && f <= AggFn::Reg
 inline bool agg_is_bivariate(AggFn f) { return f == AggFn::CovarSamp || f == AggFn::CovarPop || f == AggFn::Corr || agg_is_regr(f); }
 // bool_and / bool_or / bit_and / bit_or / bit_xor: one-pass folds of a 64-bit word, one state column of the argument's type
 inline bool agg_is_bitwise(AggFn f) { return f >= AggFn::BoolAnd && f <= AggFn::BitXor; }
+// first_value / last_value: the value of the first / last candidate row under an ordering (DESIGN.md §6 (xvii))
+inline bool agg_is_first_last(AggFn f) { return f == AggFn::FirstValue || f == AggFn::LastValue; }
+// ordering keys of one first_value / last_value (a stated limit: more are refused, never run partly)
+static const size_t kMaxFirstLastKeys = 4;
 // [EXT] partial state columns, read by position and checked by suffix in Final modes:
 //  var / stddev:  [count] UInt64, [mean] Float64, [m2] Float64  (datafusion-functions-aggregate variance.rs)
 //  covar:         [count], [mean1], [mean2], [algo_const]        (covariance.rs)
@@ -823,6 +827,12 @@ inline std::vector<std::string> stat_state_suffixes(AggFn f) {
   if (agg_is_bivariate(f)) return {"count", "mean1", "mean2", "algo_const"};
   return {"count", "mean", "m2"};
 }
+
+struct SortKey {
+  ExprPtr expr;
+  bool asc = true;
+  bool nulls_first = false;
+};
 
 struct AggExpr {
   AggFn fn = AggFn::Sum;
@@ -836,7 +846,14 @@ struct AggExpr {
   DataType result_type;  // final value type
   bool distinct = false;
   std::string name;
-  int n_state_cols() const { return agg_is_stat(fn) ? (int)stat_state_suffixes(fn).size() : fn == AggFn::Avg ? 2 : 1; }
+  // first_value / last_value: the ordering (raw modes: expressions over the input; Final modes: the state's ordering
+  // columns, under the directions the node carries) and IGNORE NULLS
+  std::vector<SortKey> order_by;
+  bool ignore_nulls = false;
+  int n_state_cols() const {
+    if (agg_is_first_last(fn)) return 2 + (int)order_by.size();
+    return agg_is_stat(fn) ? (int)stat_state_suffixes(fn).size() : fn == AggFn::Avg ? 2 : 1;
+  }
 };
 
 // [EXT] datafusion-functions-aggregate 53: SUM(Decimal128(p,s)) -> Decimal128(min(38,p+10), s);
@@ -867,6 +884,13 @@ inline void check_bitwise_arg(AggFn f, const std::string& fn, const DataType& t)
   const bool ok = (f == AggFn::BoolAnd || f == AggFn::BoolOr) ? t.id == TypeId::Bool : t.is_integer();
   if (!ok) throw PlanUnsupported(fn + " does not support an argument of type " + t.str());
 }
+// [EXT] first_value / last_value take and return any type the engine holds; their ordering keys likewise
+inline void check_first_last_type(const std::string& what, const DataType& t) {
+  const bool ok = t.id == TypeId::Bool || t.is_integer() || t.is_float() || t.is_decimal() || t.id == TypeId::Date32 || t.id == TypeId::Timestamp ||
+                  t.id == TypeId::Utf8;
+  if (!ok) throw PlanUnsupported(what + " of type " + t.str() + " is not supported");
+}
+inline const char* first_last_state_suffix(AggFn f) { return f == AggFn::FirstValue ? "first_value" : "last_value"; }
 inline const char* bitwise_state_suffix(AggFn f) {
   switch (f) {
     case AggFn::BoolAnd: return "bool_and";
@@ -908,6 +932,8 @@ inline AggFn parse_stat_aggfn(const std::string& s) {
   if (s == "bit_and") return AggFn::BitAnd;
   if (s == "bit_or") return AggFn::BitOr;
   if (s == "bit_xor") return AggFn::BitXor;
+  if (s == "first_value") return AggFn::FirstValue;
+  if (s == "last_value") return AggFn::LastValue;
   return AggFn::Sum;
 }
 inline AggFn parse_aggfn(const std::string& s) {
@@ -945,12 +971,6 @@ inline JoinType parse_join_type(const std::string& s) {
     if (s == kv.first) return kv.second;
   throw std::runtime_error("plan IR: unknown join type '" + s + "'");
 }
-
-struct SortKey {
-  ExprPtr expr;
-  bool asc = true;
-  bool nulls_first = false;
-};
 
 struct NamedExpr {
   ExprPtr expr;
@@ -1248,7 +1268,49 @@ inline PlanPtr parse_plan(const Json& j) {
       ae.distinct = a.get_bool("distinct", false);
       if (ae.distinct) throw std::runtime_error("DISTINCT aggregates must be lowered to two-level aggregation by the planner");
       ae.name = a.get_str("name", a.at("fn").str() + "_" + std::to_string(i));
-      if (from_states && agg_is_stat(ae.fn)) {
+      if (agg_is_first_last(ae.fn)) {
+        const std::string fnn = a.at("fn").str();
+        ae.ignore_nulls = a.get_bool("ignore_nulls", false);
+        Json no_keys;
+        const Json& ob = a.has("order_by") ? a.at("order_by") : no_keys;
+        if (ob.size() > kMaxFirstLastKeys)
+          throw PlanUnsupported(fnn + " (" + ae.name + ") with " + std::to_string(ob.size()) + " ordering keys is not supported (at most " +
+                                std::to_string(kMaxFirstLastKeys) + ")");
+        if (from_states) {
+          // [<name>[first_value|last_value]] (x), one column per ordering key, [is_set] Bool: read positionally and refused
+          // when the layout differs.  The ordering comes from those columns, under the directions this node carries.
+          const size_t nk = ob.size();
+          if (state_col + 1 + nk >= c->schema.size()) throw std::runtime_error("Final aggregate: missing state columns of " + ae.name);
+          auto ends_with = [](const std::string& a, const std::string& b) { return a.size() >= b.size() && a.compare(a.size() - b.size(), b.size(), b) == 0; };
+          const Field& fv = c->schema[state_col];
+          const std::string want = std::string("[") + first_last_state_suffix(ae.fn) + "]";
+          if (!ends_with(fv.name, want)) throw PlanUnsupported("Final " + fnn + ": state column '" + fv.name + "' is not the expected '" + want + "'");
+          const Field& fs = c->schema[state_col + 1 + nk];
+          if (!ends_with(fs.name, "is_set") || fs.type.id != TypeId::Bool)
+            throw PlanUnsupported("Final " + fnn + ": state column '" + fs.name + "' (" + fs.type.str() + ") is not the expected 'is_set' (bool) after " +
+                                  std::to_string(nk) + " ordering column(s)");
+          check_first_last_type("Final " + fnn + " state column '" + fv.name + "'", fv.type);
+          for (size_t k = 0; k < nk; k++) {
+            SortKey sk;
+            sk.expr = make_col((int)(state_col + 1 + k), c->schema);
+            sk.asc = ob.at(k).get_bool("asc", true);
+            sk.nulls_first = ob.at(k).get_bool("nulls_first", !sk.asc);
+            check_first_last_type("Final " + fnn + " ordering state column '" + c->schema[state_col + 1 + k].name + "'", sk.expr->type);
+            ae.order_by.push_back(sk);
+          }
+          ae.input_type = fv.type;
+          state_col += ae.n_state_cols();
+        } else {
+          if (!a.has("args") || a.at("args").size() != 1) throw std::runtime_error(fnn + " takes 1 argument(s)");
+          ae.arg = parse_expr(a.at("args").at(0), c->schema);
+          check_first_last_type(fnn + " argument", ae.arg->type);
+          ae.order_by = parse_sort_keys(ob, c->schema);
+          for (auto& k : ae.order_by) check_first_last_type(fnn + " ordering key", k.expr->type);
+          ae.input_type = ae.arg->type;
+        }
+        ae.sum_type = ae.input_type;
+        ae.result_type = ae.input_type;
+      } else if (from_states && agg_is_stat(ae.fn)) {
         // states are read positionally; a column whose name does not end in the expected suffix means a layout this
         // engine does not know, which is refused rather than misread
         const std::vector<std::string> sfx = stat_state_suffixes(ae.fn);
@@ -1365,6 +1427,15 @@ inline PlanPtr parse_plan(const Json& j) {
           n->schema.push_back(Field{ae.name + "[sum]", ae.sum_type, true});
         } else if (agg_is_bitwise(ae.fn)) {
           n->schema.push_back(Field{ae.name + "[" + bitwise_state_suffix(ae.fn) + "]", ae.sum_type, true});
+        } else if (agg_is_first_last(ae.fn)) {
+          // [EXT-unverified] the ordering columns are named by the sort expression's display string ("ts@2" for a column)
+          n->schema.push_back(Field{ae.name + "[" + first_last_state_suffix(ae.fn) + "]", ae.result_type, true});
+          for (size_t k = 0; k < ae.order_by.size(); k++) {
+            const Expr& e = *ae.order_by[k].expr;
+            const std::string nm = e.kind == Expr::Col ? c->schema[(size_t)e.col].name + "@" + std::to_string(e.col) : ae.name + "[order_" + std::to_string(k) + "]";
+            n->schema.push_back(Field{nm, e.type, true});
+          }
+          n->schema.push_back(Field{"is_set", DataType(TypeId::Bool), true});
         } else {
           n->schema.push_back(Field{ae.name + (ae.fn == AggFn::Min ? "[min]" : "[max]"), ae.sum_type, true});
         }
@@ -1372,7 +1443,7 @@ inline PlanPtr parse_plan(const Json& j) {
         // [EXT] COUNT and regr_count are never NULL (0 for an empty group)
         n->schema.push_back(Field{ae.name, ae.result_type, ae.fn != AggFn::Count && ae.fn != AggFn::RegrCount});
       }
-      if (!n->grouping_sets.empty() && agg_is_stat(ae.fn))
+      if (!n->grouping_sets.empty() && (agg_is_stat(ae.fn) || agg_is_first_last(ae.fn)))
         throw PlanUnsupported(a.at("fn").str() + " (" + ae.name + ") alongside grouping sets is not supported");
     }
   } else if (op == "HashJoinExec" || op == "SortMergeJoinExec" || op == "NestedLoopJoinExec") {

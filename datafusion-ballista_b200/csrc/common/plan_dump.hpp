@@ -86,7 +86,7 @@ inline std::string dump_plan(const PlanNode& n) {
   static const char* agg_modes[] = {"Partial", "Final", "FinalPartitioned", "Single", "SinglePartitioned"};
   static const char* agg_fns[] = {"sum", "min", "max", "count", "avg", "var_samp", "var_pop", "stddev_samp", "stddev_pop", "covar_samp", "covar_pop", "corr",
                                   "regr_slope", "regr_intercept", "regr_count", "regr_r2", "regr_avgx", "regr_avgy", "regr_sxx", "regr_syy", "regr_sxy",
-                                  "bool_and", "bool_or", "bit_and", "bit_or", "bit_xor"};
+                                  "bool_and", "bool_or", "bit_and", "bit_or", "bit_xor", "first_value", "last_value"};
   std::string o = "{\"op\":" + pbp::jstr(n.op_name);
   auto child = [&](size_t i) { return dump_plan(*n.children[i]); };
   switch (n.op) {
@@ -120,7 +120,8 @@ inline std::string dump_plan(const PlanNode& n) {
       for (size_t i = 0; i < n.aggs.size(); i++) {
         const AggExpr& a = n.aggs[i];
         o += std::string(i ? "," : "") + "{\"fn\":\"" + agg_fns[(int)a.fn] + "\",\"name\":" + pbp::jstr(a.name) + ",\"args\":[" + (a.arg ? dump_expr(a.arg) : std::string()) + (a.arg2 ? "," + dump_expr(a.arg2) : std::string()) +
-             "],\"input_type\":" + type_json(a.input_type) + ",\"sum_type\":" + type_json(a.sum_type) + ",\"result_type\":" + type_json(a.result_type) + "}";
+             "],\"input_type\":" + type_json(a.input_type) + ",\"sum_type\":" + type_json(a.sum_type) + ",\"result_type\":" + type_json(a.result_type) +
+             (agg_is_first_last(a.fn) ? ",\"order_by\":" + dump_sort_keys(a.order_by) + ",\"ignore_nulls\":" + (a.ignore_nulls ? "true" : "false") : std::string()) + "}";
       }
       o += "],\"input\":" + child(0);
       break;

@@ -693,9 +693,19 @@ inline std::string plan_json(const Msg& n, const std::string& override_job) {
         std::string fn = a.str(4);
         for (auto& ch : fn) ch = (char)tolower((unsigned char)ch);
         if (fn == "mean") fn = "avg";
-        if (!a.subs(5).empty()) throw Unsupported("ordered aggregates are not supported by the device engine");
+        // ordering_req = 5 (PhysicalSortExprNode) and ignore_nulls = 6: first_value / last_value only; every other ordered
+        // aggregate stays refused
+        const bool first_last = fn == "first_value" || fn == "last_value";
+        if (!first_last && !a.subs(5).empty()) throw Unsupported("ordered aggregates are not supported by the device engine");
         o += std::string(i ? "," : "") + "{\"fn\":" + jstr(fn) + ",\"name\":" + jstr(an[i]) + ",\"args\":" + exprs_json(a.subs(2));
         if (a.boolean(3)) o += ",\"distinct\":true";
+        if (first_last && !a.subs(5).empty()) {
+          const std::vector<Msg> req = a.subs(5);  // bare PhysicalSortExprNodes (no PhysicalExprNode wrapper)
+          o += ",\"order_by\":[";
+          for (size_t k = 0; k < req.size(); k++) o += std::string(k ? "," : "") + sort_expr_json(req[k]);
+          o += "]";
+        }
+        if (first_last && a.boolean(6)) o += ",\"ignore_nulls\":true";
         o += "}";
       }
       o += "]";

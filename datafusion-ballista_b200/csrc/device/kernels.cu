@@ -12,6 +12,7 @@
 #include "../common/hash.hpp"
 #include "../common/tpch_gen.hpp"
 #include "kernels.h"
+#include "sort_word.cuh"
 
 namespace b200 {
 
@@ -580,55 +581,43 @@ __global__ void sort_word_kernel(SortWordArgs A, const uint32_t* perm, uint64_t*
   for (int64_t k = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; k < n; k += (int64_t)gridDim.x * blockDim.x) {
     const int64_t i = perm ? perm[k] : k;
     const bool valid = !A.valid || A.valid[i];
-    uint64_t w = 0;
     if (A.word < 0) {  // null-rank word: decides where NULLs go
-      w = valid ? (A.nulls_first ? 1 : 0) : (A.nulls_first ? 0 : 1);
-      out[k] = w;
+      out[k] = sort_null_word(valid, A.nulls_first);
       continue;
     }
+    uint64_t w = 0;
     if (valid) {
+      int kind = SWK_UINT;
+      uint64_t lo = 0, hi = 0;
       switch (A.phys) {
-        case PH_I8: w = (uint64_t)(int64_t)((const int8_t*)A.data)[i] ^ 0x8000000000000000ull; break;
-        case PH_I16: w = (uint64_t)(int64_t)((const int16_t*)A.data)[i] ^ 0x8000000000000000ull; break;
-        case PH_I32: w = (uint64_t)(int64_t)((const int32_t*)A.data)[i] ^ 0x8000000000000000ull; break;
-        case PH_I64: w = (uint64_t)((const int64_t*)A.data)[i] ^ 0x8000000000000000ull; break;
+        case PH_I8: kind = SWK_INT; lo = (uint64_t)(int64_t)((const int8_t*)A.data)[i]; break;
+        case PH_I16: kind = SWK_INT; lo = (uint64_t)(int64_t)((const int16_t*)A.data)[i]; break;
+        case PH_I32: kind = SWK_INT; lo = (uint64_t)(int64_t)((const int32_t*)A.data)[i]; break;
+        case PH_I64: kind = SWK_INT; lo = (uint64_t)((const int64_t*)A.data)[i]; break;
         case PH_U8:
-        case PH_BOOL8: w = ((const uint8_t*)A.data)[i]; break;
-        case PH_U16: w = ((const uint16_t*)A.data)[i]; break;
-        case PH_U32: w = ((const uint32_t*)A.data)[i]; break;
-        case PH_U64: w = ((const uint64_t*)A.data)[i]; break;
+        case PH_BOOL8: lo = ((const uint8_t*)A.data)[i]; break;
+        case PH_U16: lo = ((const uint16_t*)A.data)[i]; break;
+        case PH_U32: lo = ((const uint32_t*)A.data)[i]; break;
+        case PH_U64: lo = ((const uint64_t*)A.data)[i]; break;
         case PH_F32:
-        case PH_F64: {
-          // raw bits as an INTEGER: if the compiler sees a double here it turns `bits ^ signbit` into an
-          // FP negate, and neg.f64 of a NaN does not return the sign-flipped bit pattern (NaN keys were
-          // ordered below -0.0); found by tests/test_gpu_sort.py
-          long long x = A.phys == PH_F32 ? __double_as_longlong((double)((const float*)A.data)[i]) : ((const long long*)A.data)[i];
-          asm volatile("" : "+l"(x));
-          x ^= (long long)((unsigned long long)(x >> 63) >> 1);  // IEEE total order
-          w = (uint64_t)x ^ 0x8000000000000000ull;
+        case PH_F64:
+          kind = SWK_F64;
+          lo = A.phys == PH_F32 ? (uint64_t)__double_as_longlong((double)((const float*)A.data)[i]) : ((const uint64_t*)A.data)[i];
           break;
-        }
-        case PH_DEC128: {
-          const uint64_t* p = (const uint64_t*)A.data + 2 * i;
-          w = A.word == 0 ? (p[1] ^ 0x8000000000000000ull) : p[0];  // word 0 = high (signed), word 1 = low
+        case PH_DEC128:
+          kind = SWK_DEC128;
+          lo = ((const uint64_t*)A.data)[2 * i];
+          hi = ((const uint64_t*)A.data)[2 * i + 1];
           break;
-        }
-        case PH_STRVIEW: {
-          const unsigned long long* v = (const unsigned long long*)A.data + 2 * i;
-          const uint8_t* s = (const uint8_t*)v[0];
-          uint32_t len = (uint32_t)v[1];
-          uint32_t base = (uint32_t)A.word * 7;  // 7 data bytes per word + 1 "has more/len" byte keeps prefixes ordered
-          for (int b = 0; b < 7; b++) {
-            uint32_t p = base + b;
-            w = (w << 8) | (p < len ? s[p] : 0);
-          }
-          uint32_t rem = len > base ? len - base : 0;
-          w = (w << 8) | (rem > 7 ? 8 : rem);  // bytes present in this word (8 = continues)
+        case PH_STRVIEW:
+          kind = SWK_STR;
+          lo = ((const unsigned long long*)A.data)[2 * i];
+          hi = ((const unsigned long long*)A.data)[2 * i + 1];
           break;
-        }
-        default: break;
+        default: kind = -1; break;
       }
-      if (!A.asc) w = ~w;
+      if (kind >= 0) w = sort_value_word(kind, lo, hi, A.word, A.asc);
+      else if (!A.asc) w = ~w;
     }
     out[k] = w;
   }
@@ -637,7 +626,7 @@ void launch_sort_word(const SortWordArgs& A, const uint32_t* perm, uint64_t* out
   launch_kernel(sort_word_kernel, grid_for(n, 256, 4), 256, 0, st, A, perm, out, n);
 }
 // ---- small-n comparison sort ---------------------------------------------------------------------
-// three-way compare of rows i and j under one key; mirrors the word encoding of sort_word_kernel
+// three-way compare of rows i and j under one key; mirrors the word encoding of sort_word.cuh
 __device__ __forceinline__ int small_sort_cmp(const SortWordArgs& A, int64_t i, int64_t j) {
   const bool vi = !A.valid || A.valid[i], vj = !A.valid || A.valid[j];
   if (vi != vj) {  // the null-rank word is not affected by asc/desc

@@ -27,6 +27,7 @@
 #include "../common/regex_dfa.hpp"
 #include "kernels.h"
 #include "program.h"
+#include "sort_word.cuh"
 
 namespace b200 {
 
@@ -3187,6 +3188,93 @@ __device__ __forceinline__ void mom_reg_flush(double (&acc)[G][VM_MAX_MOM][3], M
 }
 
 // ------------------------------------------------------------------------------------------------
+// first_value / last_value passes (program.h FlChain; DESIGN.md §4.1).  Compiled only into the pipeline_kernel variant
+// of the global sink with MOM = true, behind Program::fl_pass, whatever sink pass 1 used: every group pass 1 found is in
+// the global table by then.
+// ------------------------------------------------------------------------------------------------
+// row r's word (key, word) of chain ch, in the form the cells fold: the word for last_value, its complement for first_value
+__device__ __noinline__ unsigned long long fl_folded(const Lane L, int c, int key, int word, int r, int64_t row) {
+  const FlChain& ch = PROG.fl[c];
+  uint64_t w;
+  if (key >= ch.n_keys) {
+    w = (uint64_t)row;
+  } else {
+    const FlKey k = ch.key[key];
+    KeyVal kv;
+    load_key(L, k.v, r, &kv);
+    if (word < 0) w = sort_null_word(kv.valid, k.nulls_first);
+    else w = kv.valid ? sort_value_word(k.kind, kv.w0, kv.w1, word, k.asc) : 0ull;  // a NULL's value words are 0, as in the sort
+  }
+  return ch.last ? w : ~w;
+}
+
+__device__ __noinline__ uint32_t sink_first_last(const Lane L, uint32_t active, int64_t row0) {
+  if (*(volatile unsigned int*)&PROG.status->overflow) return active;
+  const int c = PROG.fl_chain;
+  const FlChain& ch = PROG.fl[c];
+  const AggTable& T = PROG.table;
+  const int n_keys = PROG.n_keys;
+  const bool capture = PROG.fl_pass == 2;
+  const int slot_now = PROG.fl_slot, slot_prev = (slot_now + 2) % 3, slot_next = (slot_now + 1) % 3;
+  const uint32_t cand = ch.cand.kind == OPD_NONE ? 0xFFFFFFFFu : fetch_valid(L, ch.cand);
+#pragma unroll 1
+  for (int r = 0; r < VM_R; r++) {
+    if (!((active >> r) & 1)) continue;
+    if (ch.cand.kind != OPD_NONE && (!((cand >> r) & 1) || ld1_i64(L, ch.cand, r) == 0)) continue;
+    const int64_t row = row0 + r * L.B + L.tid;
+    if (!capture && ch.dead[row]) continue;
+    KeyVal kv[VM_MAX_KEYS];
+    for (int k = 0; k < n_keys; k++) load_key(L, PROG.keys[k], r, &kv[k]);
+    const unsigned long long h = n_keys ? (unsigned long long)ld1_i64(L, PROG.key_hash, r) : 0ull;
+    const unsigned long long slot = table_upsert(n_keys, h, kv);  // pass 1 published every group: a lookup
+    if (slot == ~0ull) {
+      atomicExch(&PROG.status->overflow, 1u);
+      continue;
+    }
+    auto cell = [&](int s) -> unsigned long long* {
+      return s < 2 ? &T.acc[((unsigned long long)ch.col * T.cap + slot) * 2 + s] : &T.acc[((unsigned long long)(ch.col + 1) * T.cap + slot) * 2];
+    };
+    if (!capture) *cell(slot_next) = 0ull;  // the slot of the next pass; nothing reads it in this one
+    if (PROG.fl_prev_key >= 0) {
+      const unsigned long long best = *(volatile unsigned long long*)cell(slot_prev);
+      if (fl_folded(L, c, PROG.fl_prev_key, PROG.fl_prev_word, r, row) != best) {
+        if (!capture) ch.dead[row] = 1;  // lost on the previous word: out of the chain from now on
+        continue;
+      }
+    }
+    if (capture) {  // the one row left (the position word is unique): its values into the group's cells
+      for (int j = 0; j < PROG.n_flcap; j++) {
+        const FlCapture cp = PROG.flcap[j];
+        if (cp.chain != c) continue;
+        KeyVal v;
+        load_key(L, cp.v, r, &v);
+        unsigned long long w0 = v.w0, w1 = v.w1;
+        if (v.vk == VK_F64) {
+          w0 ^= (unsigned long long)((long long)w0 >> 63) >> 1;  // the total-order key, as MIN_F64 / MAX_F64 keep it
+        } else if (v.vk != VK_I128 && v.vk != VK_STR) {
+          w1 = (unsigned long long)((long long)w0 >> 63);
+        }
+        unsigned long long* dst = &T.acc[((unsigned long long)cp.col * T.cap + slot) * 2];
+        dst[0] = w0;
+        dst[1] = w1;
+        T.acc[((unsigned long long)(cp.col + 1) * T.cap + slot) * 2] = v.valid;
+      }
+      if (ch.set_col != 255) T.acc[((unsigned long long)ch.set_col * T.cap + slot) * 2] = 1ull;
+      continue;
+    }
+    const unsigned long long f = fl_folded(L, c, PROG.fl_key, PROG.fl_word, r, row);
+    unsigned long long* dst = cell(slot_now);
+    if (f > *(volatile unsigned long long*)dst) atomicMax(dst, f);
+    if (PROG.fl_key < ch.n_keys && PROG.fl_word >= 0 && ch.key[PROG.fl_key].kind == SWK_STR) {
+      KeyVal kv1;
+      load_key(L, ch.key[PROG.fl_key].v, r, &kv1);
+      if (kv1.valid && kv1.w1 > 7ull * (unsigned long long)(PROG.fl_word + 1)) atomicExch(&PROG.status->fl_more, 1u);
+    }
+  }
+  return active;
+}
+
+// ------------------------------------------------------------------------------------------------
 // The kernel
 // ------------------------------------------------------------------------------------------------
 template <int SINK, int G, bool ADD_ONLY, bool SIDE, bool MOM = false, bool SFN = false, bool GSETS = false>
@@ -3295,7 +3383,7 @@ __global__ void __launch_bounds__(512, 1) pipeline_kernel() {
       active = run_program<SFN>(L, active, mops, n_instr);
     }
     if (MOM) {
-      if (SINK == SINK_AGG_GLOBAL) active = sink_mom_global(L, active);
+      if (SINK == SINK_AGG_GLOBAL) active = PROG.fl_pass ? sink_first_last(L, active, row0) : sink_mom_global(L, active);
       else active = sink_mom_reg<(MOM ? G : 1)>(L, active, macc, &gtable, mom_centres());
       live_rows += __popc(active);
     } else if (SINK == SINK_MATERIALIZE) {
@@ -3405,6 +3493,8 @@ bool pipeline_add_only(const Program& P, int grid, int block) {
 template <bool SFN>
 static cudaError_t launch_variant(const Program& P, int reg_groups, int grid, int block, size_t smem, cudaStream_t st) {
   const bool add_only = pipeline_add_only(P, grid, block);
+  // the first_value / last_value passes: the global sink's pass-2 variant, after either sink (every group is in the table)
+  if (P.fl_pass) return launch_one<SFN, SINK_AGG_GLOBAL, 1, true, false, true>(grid, block, smem, st);
   if (P.mom_pass) {  // pass 2 of VAR / STDDEV / COVAR / CORR
     if (P.sink == SINK_AGG_GLOBAL) return launch_one<SFN, SINK_AGG_GLOBAL, 1, true, false, true>(grid, block, smem, st);
     return reg_groups <= 1 ? launch_one<SFN, SINK_AGG_REG, 1, false, false, true>(grid, block, smem, st)

@@ -24,6 +24,9 @@ static const int VM_REG_ACC = 6;      // accumulators held in registers by the A
 static const int VM_REG_GROUPS = 4;   // groups held in registers by the AGG_REG sink
 static const int VM_MAX_STAGES = 4;
 static const int VM_MAX_MOM = 6;      // centred co-moments of one aggregate sink (VAR / STDDEV / COVAR / CORR)
+static const int VM_MAX_FL_CHAINS = 4; // first_value / last_value ordering chains of one aggregate sink
+static const int VM_MAX_FL_KEYS = 4;   // ordering keys of one chain (plan.hpp kMaxFirstLastKeys)
+static const int VM_MAX_FL_CAP = 16;   // values the capture passes of one aggregate sink write (results and state columns)
 
 // physical (in-HBM) column encodings
 enum Phys : uint8_t {
@@ -204,6 +207,43 @@ struct MomDesc {
   uint8_t _pad[4];
 };
 
+// first_value / last_value (DESIGN.md §4.1, §6 (xvii)).  A chain is one ordering over one candidate set, shared by every
+// aggregate with both; it runs after pass 1 as a series of launches of the same program ("first/last passes").  Pass p
+// folds one order-preserving word (sort_word.cuh) of every live candidate into a per-group 64-bit atomic max -- the word
+// itself for last_value, its complement for first_value, so that every cell starts at 0 -- over the rows that are still
+// tied with the group's best on every earlier word.  A row that differs from the group's cell on the previous word is
+// marked in `dead` and skipped from then on.  The last word is the row's position in the pipeline's source, which makes
+// the winner unique; the capture pass then lets that row write its values into the group's cells.
+// Three rotating word slots live in the table columns col (lo, hi) and col + 1 (lo): pass p folds slot p % 3, compares
+// against slot (p - 1) % 3 and clears slot (p + 1) % 3 for the next pass.
+// a sort key value's encoding (sort_word.cuh): lo / hi hold an int64, a uint64 (bools and zero-extended unsigned integers), a double's bits,
+// a Decimal128's low / high words, or a string's {ptr, len}
+enum SortWordKind : uint8_t { SWK_INT = 0, SWK_UINT, SWK_F64, SWK_DEC128, SWK_STR };
+struct FlKey {
+  Operand v;
+  uint8_t kind;         // SortWordKind
+  uint8_t asc, nulls_first;
+  uint8_t _pad;
+};
+struct FlChain {
+  FlKey key[VM_MAX_FL_KEYS];
+  Operand cand;         // Bool operand: the candidates are the live rows where it is TRUE; OPD_NONE: every live row
+  uint8_t n_keys;
+  uint8_t last;         // 1: last_value (the largest word wins); 0: first_value
+  uint8_t col;          // first of the two table columns of the word slots
+  uint8_t set_col;      // table column whose lo the capture sets to 1 (the partial state's is_set); 255: none
+  uint8_t _pad[4];
+  uint8_t* dead;        // one byte per source row, zeroed before the chain's first pass
+};
+// a value the winner of chain `chain` writes in the capture pass: its 16-byte image into table column col (floats as
+// their total-order key, integers sign-extended, strings as views) and its validity into the lo of column col + 1
+struct FlCapture {
+  Operand v;
+  uint8_t chain;
+  uint8_t col;
+  uint8_t _pad[2];
+};
+
 struct AggTable {
   unsigned long long* hash;   // [cap] 0 = empty
   unsigned int* state;        // [cap] 0 empty, 1 claimed, 2 keys published
@@ -222,7 +262,7 @@ struct RunStatus {
   unsigned long long out_rows;   // materialize sink: rows written
   unsigned long long in_active;  // rows that passed all filters
   unsigned int pack_overflow;    // OP_STR_PACK8 met a string longer than 7 bytes: re-lower without packing
-  unsigned int _pad;             // (keeps the struct 8-byte aligned; the group-by kernel reports "outside my pattern" through pack_overflow too)
+  unsigned int fl_more;          // first_value / last_value pass over a string word: some live row's key continues past it
   unsigned long long arena_need; // string builders: bytes reserved in the character arena, counted past its capacity
 };
 
@@ -275,6 +315,16 @@ struct Program {
   // string builders (OP_CONCAT and up): the launch's character arena; a reservation beyond arena_cap writes nothing
   uint8_t* arena;
   unsigned long long arena_cap;
+  // first_value / last_value (FlChain above): all the fields above describe pass 1 and stay as they are for these passes
+  uint8_t n_fl, n_flcap;
+  uint8_t fl_pass;              // 0: not a first/last pass; 1: a refinement pass of chain fl_chain; 2: its capture pass
+  uint8_t fl_chain;
+  int8_t fl_key, fl_prev_key;  // the word this pass folds: key fl_key (n_keys: the row position), word fl_word (-1: NULL
+  int32_t fl_word, fl_prev_word; // rank); the word the previous pass folded (fl_prev_key < 0: this is the chain's first pass)
+  uint8_t fl_slot;              // the slot this pass folds (the capture pass: the slot after the position's)
+  uint8_t _pad4[3];
+  FlChain fl[VM_MAX_FL_CHAINS];
+  FlCapture flcap[VM_MAX_FL_CAP];
 };
 
 // ---- fused fast path (scan -> filter -> decimal products -> <=4-group SUM/COUNT aggregate) -----------

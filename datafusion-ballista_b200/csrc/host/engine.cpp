@@ -102,6 +102,7 @@ struct b200_engine {
   std::atomic<uint64_t> narrowed_bytes_saved{0};         // PCIe bytes not sent thanks to narrowing (b200_engine_counter)
   std::atomic<uint64_t> n_window_sorts{0};               // sorts the window operator ran itself (b200_engine_counter)
   std::atomic<uint64_t> nlj_pairs{0};                    // (build row, probe row) pairs the nested-loop join evaluated (b200_engine_counter)
+  std::atomic<uint64_t> first_last_passes{0};            // first_value / last_value pass launches (b200_engine_counter)
   std::atomic<uint64_t> string_arena_retries{0};         // launches re-run because their character arena was too small
   std::atomic<uint64_t> host_syncs{0};                   // host waits on the stream inside tasks, exchanges and exports (host_wait)
   // parsed stage plans by plan text with the job id taken out (b200_stage_prepare): the next job that runs the same stage
@@ -1122,6 +1123,7 @@ RunOutcome launch_program(const Exec& x, PipelineBuilder& pb, int reg_groups, co
   if (P.sink == SINK_MATERIALIZE)
     for (int j = 0; j < P.n_out; j++) kt_bytes += (uint64_t)phys_width((Phys)P.out[j].phys) * (uint64_t)P.n_rows;  // upper bound: every row kept
   KernelTimer kt(x, ff ? "filter_compact" : gb ? "groupby_hash_agg" : fused ? "pipeline_fused_agg" : P.sink == SINK_MATERIALIZE ? "pipeline_materialize"
+                   : P.fl_pass ? "pipeline_agg_first_last"
                    : P.mom_pass ? (P.sink == SINK_AGG_REG ? "pipeline_agg_reg_pass2" : "pipeline_agg_global_pass2")
                    : P.sink == SINK_AGG_REG ? "pipeline_agg_reg" : P.n_sets ? "pipeline_agg_gsets" : "pipeline_agg_global", kt_bytes);
   cudaEvent_t e0, e1;
@@ -1277,6 +1279,11 @@ struct AggLowered {
   std::vector<ColRef> acc_src;
   std::vector<MomDesc> moms;         // VAR / STDDEV / COVAR / CORR: co-moments of pass 2 (table columns after the accs)
   std::vector<ColRef> key_hashes;    // grouping sets: the hash of each key on its own
+  // first_value / last_value: chains and captures (program.h FlChain); their table columns follow the co-moments'
+  std::vector<FlChain> fl;
+  std::vector<FlCapture> flcap;
+  std::vector<bool> fl_key_nullable;  // [chain * VM_MAX_FL_KEYS + key]: the key has a NULL-rank word
+  size_t fl_cols = 0;
   struct OutRecipe {
     uint8_t kind, a, b;
     Phys phys;
@@ -1688,9 +1695,103 @@ void lower_aggregate(PipelineBuilder& pb, const PlanNode& node, AggLowered& L, i
     }
     push_stat(ae, cnt, sx, sy, mxx, myy, mxy);
   };
+  // first_value / last_value: one chain per (ordering, candidate set, first or last), one capture per value the winner
+  // writes; recipes reference captures (a = capture index, kind AO_*) or a chain's is_set (b = 254) until the table
+  // columns are laid out below
+  std::vector<std::pair<size_t, int>> fl_recipes;  // (recipe, capture index; -1 - chain: that chain's is_set)
+  auto lower_first_last = [&](const AggExpr& ae) {
+    const size_t nk = ae.order_by.size();
+    ColRef xv, cand;
+    bool has_cand = false;
+    std::vector<ColRef> keys;
+    if (from_states) {
+      xv = pb.cols.at(state_col);
+      for (size_t k = 0; k < nk; k++) keys.push_back(pb.cols.at(state_col + 1 + k));
+      cand = pb.cols.at(state_col + 1 + nk);  // is_set
+      has_cand = true;
+    } else {
+      xv = pb.compile(*ae.arg);
+      for (auto& k : ae.order_by) keys.push_back(pb.compile(*k.expr));
+      if (ae.ignore_nulls && xv.nullable) {
+        auto nn = std::make_shared<Expr>();
+        nn->kind = Expr::IsNotNull;
+        nn->type = DataType(TypeId::Bool);
+        nn->nullable = false;
+        nn->args = {ae.arg};
+        cand = pb.compile(*nn);
+        has_cand = true;
+      }
+    }
+    FlChain ch;
+    memset(&ch, 0, sizeof ch);
+    ch.n_keys = (uint8_t)nk;
+    ch.last = ae.fn == AggFn::LastValue ? 1 : 0;
+    if (has_cand) {
+      pb.pin(cand);
+      ch.cand = pb.resolve(cand);
+    }
+    for (size_t k = 0; k < nk; k++) {
+      pb.pin(keys[k]);
+      FlKey& fk = ch.key[k];
+      fk.v = pb.resolve(keys[k]);
+      const DataType& t = keys[k].type;
+      fk.kind = t.id == TypeId::Utf8 ? SWK_STR : t.is_decimal() ? SWK_DEC128 : t.is_float() ? SWK_F64 : (t.id == TypeId::UInt64 || t.id == TypeId::Bool) ? SWK_UINT : SWK_INT;
+      fk.asc = ae.order_by[k].asc ? 1 : 0;
+      fk.nulls_first = ae.order_by[k].nulls_first ? 1 : 0;
+    }
+    int c = -1;
+    for (size_t i = 0; i < L.fl.size() && c < 0; i++) {
+      FlChain seen = L.fl[i];
+      seen.set_col = 0;  // whether an earlier aggregate emits is_set does not make it another chain
+      if (memcmp(&seen, &ch, sizeof ch) == 0) c = (int)i;
+    }
+    if (c < 0) {
+      if (L.fl.size() >= (size_t)VM_MAX_FL_CHAINS)
+        throw EngineError(B200_ERR_UNSUPPORTED, "more than " + std::to_string(VM_MAX_FL_CHAINS) + " first_value / last_value orderings in one AggregateExec (" + ae.name + ")");
+      L.fl.push_back(ch);
+      for (size_t k = 0; k < (size_t)VM_MAX_FL_KEYS; k++) L.fl_key_nullable.push_back(k < nk && keys[k].nullable);
+      c = (int)L.fl.size() - 1;
+    }
+    auto capture = [&](const ColRef& v) {
+      pb.pin(v);
+      FlCapture cp;
+      memset(&cp, 0, sizeof cp);
+      cp.v = pb.resolve(v);
+      cp.chain = (uint8_t)c;
+      for (size_t i = 0; i < L.flcap.size(); i++)
+        if (memcmp(&L.flcap[i], &cp, sizeof cp) == 0) return (int)i;
+      if (L.flcap.size() >= (size_t)VM_MAX_FL_CAP)
+        throw EngineError(B200_ERR_UNSUPPORTED, "more than " + std::to_string(VM_MAX_FL_CAP) + " first_value / last_value values in one AggregateExec (" + ae.name + ")");
+      L.flcap.push_back(cp);
+      return (int)L.flcap.size() - 1;
+    };
+    auto push_value = [&](const ColRef& v, const DataType& t, const std::string& name) {
+      const uint8_t kind = t.id == TypeId::Utf8 ? AO_MINMAX_STR : t.pk() == PK::F64 ? AO_MINMAX_F64 : t.pk() == PK::I128 ? AO_ACC_I128 : AO_ACC_I64;
+      fl_recipes.emplace_back(L.outs.size(), capture(v));
+      push(kind, 0, 0, t, name, true);
+      if (kind == AO_MINMAX_STR) L.outs.back().phys = PH_STRVIEW;  // copied into a buffer of its own after the extraction
+    };
+    if (!emit_states) {
+      push_value(xv, ae.result_type, ae.name);
+      return;
+    }
+    const size_t first = node.group_by.size();
+    size_t out_col = first;  // the node's schema names the state columns
+    for (size_t i = 0; i < node.aggs.size() && &node.aggs[i] != &ae; i++) out_col += (size_t)node.aggs[i].n_state_cols();
+    push_value(xv, ae.result_type, node.schema.at(out_col).name);
+    for (size_t k = 0; k < nk; k++) push_value(keys[k], keys[k].type, node.schema.at(out_col + 1 + k).name);
+    L.fl[(size_t)c].set_col = 1;  // laid out below
+    fl_recipes.emplace_back(L.outs.size(), -1 - c);
+    push(AO_COUNT, 0, 255, DataType(TypeId::Bool), "is_set", false);
+  };
   for (size_t ai = 0; ai < node.aggs.size(); ai++) {
     const AggExpr& ae = node.aggs[ai];
     const std::string& nm = ae.name;
+    if (agg_is_first_last(ae.fn)) {
+      lower_first_last(ae);
+      if (from_states) state_col += (size_t)ae.n_state_cols();
+      continue;
+    }
     if (agg_is_stat(ae.fn)) {
       if (from_states) {
         lower_stat_states(ae);
@@ -1792,6 +1893,30 @@ void lower_aggregate(PipelineBuilder& pb, const PlanNode& node, AggLowered& L, i
   for (auto& r : L.outs)
     if (r.kind == AO_STAT)
       for (int k = 3; k < 6; k++) r.st[k] = (uint8_t)(n_acc + 3 * r.st[k]);
+  // first_value / last_value after them: two word-slot columns per chain (and its is_set when it emits states), two per
+  // capture (the value, its validity); every column starts at 0
+  size_t col = n_acc + 3 * L.moms.size();
+  for (auto& ch : L.fl) {
+    ch.col = (uint8_t)col;
+    col += 2;
+    if (ch.set_col) ch.set_col = (uint8_t)col++;
+    else ch.set_col = 255;
+  }
+  for (auto& cp : L.flcap) {
+    cp.col = (uint8_t)col;
+    col += 2;
+  }
+  if (col > 250) throw EngineError(B200_ERR_UNSUPPORTED, "too many aggregate table columns in one AggregateExec (first_value / last_value)");
+  L.fl_cols = col - n_acc - 3 * L.moms.size();
+  for (auto& fr : fl_recipes) {
+    auto& r = L.outs[fr.first];
+    if (fr.second >= 0) {
+      r.a = L.flcap[(size_t)fr.second].col;
+      r.b = (uint8_t)(r.a + 1);
+    } else {
+      r.a = L.fl[(size_t)(-1 - fr.second)].set_col;
+    }
+  }
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1811,6 +1936,7 @@ bool match_fused(const Program& P, FusedPlan& FP) {
   memset(&F, 0, sizeof F);
   if (P.sink != SINK_AGG_REG) return false;
   if (P.n_mom) return false;  // VAR / STDDEV / COVAR / CORR need the second pass of the VM sinks
+  if (P.n_fl) return false;   // first_value / last_value need the first/last passes of the VM sinks
   if (P.n_sets) return false;  // grouping sets run on the global sink's grouping-set variant only
   if (getenv("B200_NO_FUSED")) return false;
   for (int a = 0; a < P.n_acc; a++)
@@ -2089,6 +2215,7 @@ bool match_groupby(const Program& P, GroupBySpec& S) {
   memset(&S, 0, sizeof S);
   if (getenv("B200_NO_GROUPBY")) return false;
   if (P.n_mom) return false;  // VAR / STDDEV / COVAR / CORR need the second pass of the VM sinks
+  if (P.n_fl) return false;   // first_value / last_value need the first/last passes of the VM sinks
   if (P.n_sets) return false;  // grouping sets run on the global sink's grouping-set variant only
   if (P.n_keys < 1 || P.n_keys > 2 || P.n_acc > GB_MAX_ACC || P.n_cols > FUSED_MAX_COLS || P.n_cols == 0) return false;
   for (int c = 0; c < P.n_cols; c++) {
@@ -2317,6 +2444,51 @@ TableMem alloc_table(const Exec& x, uint64_t cap, int n_keys, const std::vector<
 
 typedef std::function<std::unique_ptr<PipelineBuilder>()> BuilderFactory;
 
+// first_value / last_value (program.h FlChain): per chain, one refinement pass per order-preserving word of its ordering
+// (a NULL-rank word for a nullable key, one value word, two for Decimal128, and for Utf8 as many 7-byte words as the
+// longest live key needs), one for the row position, then the capture pass.  Every pass reruns the lowered program over
+// the same rows; an overflow means a group of pass 1 was not found again.
+static void run_first_last_passes(const Exec& x, PipelineBuilder& pb, AggLowered& L, int reg_groups, OpMetrics* met) {
+  Program& P = pb.prog;
+  const int64_t n = std::max<int64_t>(P.n_rows, 1);
+  DevPtr dead = dev_alloc((size_t)n * L.fl.size(), x.st());
+  CUDA_CHECK(cudaMemsetAsync(dead->ptr, 0, (size_t)n * L.fl.size(), x.st()));
+  for (size_t c = 0; c < L.fl.size(); c++) P.fl[c].dead = (uint8_t*)dead->ptr + (size_t)n * c;
+  for (size_t c = 0; c < L.fl.size(); c++) {
+    const FlChain& ch = P.fl[c];
+    P.fl_chain = (uint8_t)c;
+    P.fl_prev_key = -1;
+    P.fl_prev_word = 0;
+    P.fl_slot = 0;
+    auto pass = [&](int kind, int key, int word) {
+      x.check_cancel();
+      P.fl_pass = (uint8_t)kind;
+      P.fl_key = (int8_t)key;
+      P.fl_word = word;
+      RunOutcome r = launch_program(x, pb, reg_groups, nullptr, true, met);
+      x.e->first_last_passes++;
+      if (r.status.overflow) throw EngineError(B200_ERR_EXECUTION, "aggregate: a group of the first pass was not found by a first_value / last_value pass");
+      P.fl_prev_key = (int8_t)key;
+      P.fl_prev_word = word;
+      P.fl_slot = (uint8_t)((P.fl_slot + 1) % 3);
+      return r.status.fl_more != 0;
+    };
+    for (int k = 0; k < ch.n_keys; k++) {
+      if (L.fl_key_nullable[c * VM_MAX_FL_KEYS + (size_t)k]) pass(1, k, -1);
+      if (ch.key[k].kind == SWK_STR) {
+        // a Utf8 key: one more word while some live row's key continues past the last one
+        for (int w = 0; pass(1, k, w); w++) {
+        }
+      } else {
+        for (int w = 0; w < (ch.key[k].kind == SWK_DEC128 ? 2 : 1); w++) pass(1, k, w);
+      }
+    }
+    pass(1, ch.n_keys, 0);  // the row position: one winner per group
+    pass(2, ch.n_keys, 0);  // capture
+  }
+  P.fl_pass = 0;
+}
+
 DevBatchPtr run_aggregate(const Exec& x, const BuilderFactory& make_pb, const PlanNode& node, const DevBatchPtr& src, OpMetrics* met) {
   const int n_keys = (int)node.group_by.size();
   if (n_keys > VM_MAX_KEYS) throw EngineError(B200_ERR_UNSUPPORTED, "too many group-by columns");
@@ -2383,6 +2555,10 @@ DevBatchPtr run_aggregate(const Exec& x, const BuilderFactory& make_pb, const Pl
     for (size_t a = 0; a < L.accs.size(); a++) P.acc[a] = L.accs[a];
     P.n_mom = (uint8_t)L.moms.size();
     for (size_t m = 0; m < L.moms.size(); m++) P.mom[m] = L.moms[m];
+    P.n_fl = (uint8_t)L.fl.size();
+    for (size_t c = 0; c < L.fl.size(); c++) P.fl[c] = L.fl[c];
+    P.n_flcap = (uint8_t)L.flcap.size();
+    for (size_t j = 0; j < L.flcap.size(); j++) P.flcap[j] = L.flcap[j];
     memset(&P.key_hash, 0, sizeof P.key_hash);
     P.keys_all_i64 = L.fast ? 1 : 0;
     P.n_sets = (uint8_t)n_sets;
@@ -2425,7 +2601,7 @@ DevBatchPtr run_aggregate(const Exec& x, const BuilderFactory& make_pb, const Pl
     }
     {
       ScopeTimer t_alloc("    agg: alloc_table");
-      tm = alloc_table(x, cap, table_keys, L.accs, 3 * L.moms.size());
+      tm = alloc_table(x, cap, table_keys, L.accs, 3 * L.moms.size() + L.fl_cols);
     }
     P.table = tm.T;
     pb.finalize_layout((size_t)VM_REG_ACC * 512 * 16 + 256);
@@ -2511,6 +2687,7 @@ DevBatchPtr run_aggregate(const Exec& x, const BuilderFactory& make_pb, const Pl
     if (P.arena && r2.status.arena_need > P.arena_cap) throw EngineError(B200_ERR_EXECUTION, "aggregate: the second pass built more string bytes than the first");
     if (r2.status.overflow) throw EngineError(B200_ERR_EXECUTION, "aggregate: a group of the first pass was not found by the second");
   }
+  if (!L.fl.empty()) run_first_last_passes(x, *pbp, L, reg_groups, met);
   {
     // remember the smallest table class that holds this many groups (not the level that happened to be used: a small
     // input jumps straight to a table sized for its row count)
@@ -5846,6 +6023,7 @@ uint64_t b200_engine_counter(b200_engine* e, const char* name) {
   if (n == "host_syncs") return e->host_syncs;
   if (n == "regex_compiles") return e->regex.compiles;
   if (n == "string_arena_retries") return e->string_arena_retries;
+  if (n == "first_last_passes") return e->first_last_passes;
   return 0;
 }
 

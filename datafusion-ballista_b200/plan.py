@@ -192,11 +192,17 @@ def project(exprs: Sequence, input: Json) -> Json:
     return {"op": "ProjectionExec", "exprs": [{"expr": e, "name": n} for e, n in exprs], "input": input}
 
 
-def agg(fn_: str, arg: Optional[Json], name: str, input_type=None, arg2: Optional[Json] = None) -> Json:
-    """arg2: the second argument of covar / corr."""
+def agg(fn_: str, arg: Optional[Json], name: str, input_type=None, arg2: Optional[Json] = None,
+        order_by: Optional[Sequence[Json]] = None, ignore_nulls: bool = False) -> Json:
+    """arg2: the second argument of covar / corr.  order_by (`sort_key` entries) and ignore_nulls: first_value /
+    last_value (DESIGN.md §6 (xvii)); in Final modes order_by carries the directions of the state's ordering columns."""
     a: Json = {"fn": fn_, "name": name, "args": ([] if arg is None else [arg]) + ([] if arg2 is None else [arg2])}
     if input_type is not None:
         a["input_type"] = input_type
+    if order_by:
+        a["order_by"] = list(order_by)
+    if ignore_nulls:
+        a["ignore_nulls"] = True
     return a
 
 
