@@ -537,6 +537,22 @@ inline bool is_refused_string_fn(const std::string& f) {
   return false;
 }
 
+// The one-argument float math functions (DESIGN.md §6 (xviii)) in the order of MathFn1 (csrc/device/program.h); -1 for
+// another name.  isnan and iszero give Bool, the others their argument's type.
+inline int math_fn1_index(const std::string& f) {
+  static const char* const names[] = {"sqrt",  "cbrt",  "exp",   "ln",    "log2",  "log10", "sin",     "cos",
+                                      "tan",   "asin",  "acos",  "atan",  "sinh",  "cosh",  "tanh",    "asinh",
+                                      "acosh", "atanh", "cot",   "degrees", "radians", "signum", "isnan", "iszero"};
+  for (int i = 0; i < (int)(sizeof(names) / sizeof(names[0])); i++)
+    if (f == names[i]) return i;
+  return -1;
+}
+enum { MATH_ISNAN = 22, MATH_ISZERO = 23 };
+inline bool is_math_fn(const std::string& f) {
+  return math_fn1_index(f) >= 0 || f == "log" || f == "atan2" || f == "nanvl" || f == "power" || f == "trunc" || f == "gcd" ||
+         f == "lcm" || f == "factorial" || f == "pi";
+}
+
 // Result type and nullability of a scalar function call (DESIGN.md §3, rules [EXT] in §6).  A known function over an
 // argument type it does not take is refused with PlanUnsupported naming the type; an unknown name or a wrong argument
 // count is a malformed plan.
@@ -581,6 +597,36 @@ inline void type_scalar_fn(Expr& e) {
         throw PlanUnsupported("round to " + std::to_string(d.lit.i) + " digits is not supported (|digits| <= 22)");
     }
     e.type = arg_t(0);
+    e.nullable = any_nullable();
+  } else if (is_math_fn(f)) {
+    // DESIGN.md §6 (xviii): floats keep their type (Float32 computes in f32); power takes (Float64, Float64) or
+    // (Int64, Int64); gcd / lcm / factorial take Int64; every other type is refused, naming it
+    const int m1 = math_fn1_index(f);
+    const bool two = f == "atan2" || f == "nanvl" || f == "power" || f == "gcd" || f == "lcm";
+    if (f == "pi") arity(0, 0);
+    else if (f == "log" || f == "trunc") arity(1, 2);
+    else arity(two ? 2 : 1, two ? 2 : 1);
+    auto need = [&](size_t i, bool ok) {
+      if (!ok) refuse(i);
+    };
+    if (f == "gcd" || f == "lcm" || f == "factorial") {
+      for (size_t i = 0; i < n; i++) need(i, arg_t(i).id == TypeId::Int64);
+    } else if (f == "power") {
+      need(0, arg_t(0).id == TypeId::Int64 || arg_t(0).id == TypeId::Float64);
+      need(1, arg_t(1) == arg_t(0));
+    } else if (f == "trunc") {
+      need(0, arg_t(0).is_float());
+      if (n == 2) {
+        need(1, arg_t(1).is_integer());
+        const Expr& d = *e.args[1];
+        // round's factor and limit (the lowering refuses a non-literal digit count)
+        if (d.kind == Expr::Lit && !d.lit.is_null && (d.lit.i > 22 || d.lit.i < -22))
+          throw PlanUnsupported("trunc to " + std::to_string(d.lit.i) + " digits is not supported (|digits| <= 22)");
+      }
+    } else {
+      for (size_t i = 0; i < n; i++) need(i, arg_t(i).is_float() && arg_t(i) == arg_t(0));
+    }
+    e.type = f == "pi" ? DataType(TypeId::Float64) : (m1 == MATH_ISNAN || m1 == MATH_ISZERO) ? DataType(TypeId::Bool) : arg_t(0);
     e.nullable = any_nullable();
   } else if (f == "nullif") {
     arity(2, 2);

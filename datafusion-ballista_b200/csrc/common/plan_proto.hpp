@@ -417,7 +417,20 @@ inline std::string expr_json(const Msg& e) {
           {"rtrim", "rtrim"},     {"regexp_like", "regexp_like"},
           {"regexp_count", "regexp_count"},                 {"regexp_replace", "regexp_replace"},
           {"concat", "concat"},   {"concat_ws", "concat_ws"}, {"repeat", "repeat"},
-          {"reverse", "reverse"}};
+          {"reverse", "reverse"},
+          // the math functions of DESIGN §6 (xviii)
+          {"sqrt", "sqrt"},       {"cbrt", "cbrt"},         {"exp", "exp"},
+          {"ln", "ln"},           {"log", "log"},           {"log2", "log2"},
+          {"log10", "log10"},     {"sin", "sin"},           {"cos", "cos"},
+          {"tan", "tan"},         {"asin", "asin"},         {"acos", "acos"},
+          {"atan", "atan"},       {"sinh", "sinh"},         {"cosh", "cosh"},
+          {"tanh", "tanh"},       {"asinh", "asinh"},       {"acosh", "acosh"},
+          {"atanh", "atanh"},     {"cot", "cot"},           {"degrees", "degrees"},
+          {"radians", "radians"}, {"signum", "signum"},     {"atan2", "atan2"},
+          {"nanvl", "nanvl"},     {"power", "power"},       {"pow", "power"},
+          {"trunc", "trunc"},     {"gcd", "gcd"},           {"lcm", "lcm"},
+          {"factorial", "factorial"},                       {"isnan", "isnan"},
+          {"iszero", "iszero"},   {"pi", "pi"}};
       for (auto& kv : fns)
         if (name == kv.first) return "{\"fn\":\"" + std::string(kv.second) + "\",\"args\":" + exprs_json(args) + "}";
       throw Unsupported("scalar function " + name + " is not supported by the device engine");

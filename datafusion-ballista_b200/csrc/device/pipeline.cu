@@ -1034,6 +1034,191 @@ __device__ __noinline__ void scalar_regex_replace_op(const Lane L, const uint32_
 }
 
 // ------------------------------------------------------------------------------------------------
+// Math functions (OP_MATH1 / OP_MATH2 / OP_MATH_I64 / OP_TRUNC; DESIGN.md §6 (xviii)).  Float values are CUDA's
+// non-fast-math library results with the NaN bits glibc gives on x86-64: a NaN operand comes back with its own bits,
+// quieted (CUDA arithmetic would return its canonical NaN), and a NaN a function makes carries the sign glibc's gives.
+// A Float32 value sits widened in binary64 with its NaN payload shifted along (f32_bits_to_f64_bits), so binary64's
+// quiet bit and the NaN words below are the f32 ones too.
+// ------------------------------------------------------------------------------------------------
+#define MATH_NAN_NEG 0xFFF8000000000000ull  // x86 SSE's default NaN (an invalid operation): sqrt(-1), log(-1), sin(inf), ...
+#define MATH_NAN_POS 0x7FF8000000000000ull  // glibc's log10 / asin / acos domain errors; Rust's f64::NAN / f32::NAN
+__device__ __forceinline__ double math_quiet(double x) { return __longlong_as_double(__double_as_longlong(x) | 0x0008000000000000ll); }
+__device__ __forceinline__ double math_word(unsigned long long w) { return __longlong_as_double((long long)w); }
+// x86's divsd / divss: a NaN dividend comes back quieted, else a NaN divisor, else the quotient (0/0, inf/inf: default NaN)
+__device__ __forceinline__ double math_x86_div(double a, double b, bool f32) {
+  if (a != a) return math_quiet(a);
+  if (b != b) return math_quiet(b);
+  const double q = f32 ? (double)__fdiv_rn((float)a, (float)b) : __ddiv_rn(a, b);
+  return q != q ? math_word(MATH_NAN_NEG) : q;
+}
+// one-argument float function fn (MathFn1) of x, in f32 arithmetic when f32; isnan / iszero are not computed here
+__device__ __noinline__ double math1(int fn, bool f32, double x) {
+  if (x != x) return fn == MF_SIGNUM ? math_word(MATH_NAN_POS) : math_quiet(x);
+  const int g = fn == MF_COT ? MF_TAN : fn;  // cot = 1.0 / x.tan(), as Rust writes it
+  double r;
+  if (f32) {
+    const float v = (float)x;
+    float o;
+    switch (g) {
+      case MF_SQRT: o = sqrtf(v); break;
+      case MF_CBRT: o = cbrtf(v); break;
+      case MF_EXP: o = expf(v); break;
+      case MF_LN: o = logf(v); break;
+      case MF_LOG2: o = log2f(v); break;
+      case MF_LOG10: o = log10f(v); break;
+      case MF_SIN: o = sinf(v); break;
+      case MF_COS: o = cosf(v); break;
+      case MF_TAN: o = tanf(v); break;
+      case MF_ASIN: o = asinf(v); break;
+      case MF_ACOS: o = acosf(v); break;
+      case MF_ATAN: o = atanf(v); break;
+      case MF_SINH: o = sinhf(v); break;
+      case MF_COSH: o = coshf(v); break;
+      case MF_TANH: o = tanhf(v); break;
+      case MF_ASINH: o = asinhf(v); break;
+      case MF_ACOSH: o = acoshf(v); break;
+      case MF_ATANH: o = atanhf(v); break;
+      case MF_DEGREES: o = __fmul_rn(v, __int_as_float(0x42652ee1)); break;  // Rust's f32 to_degrees constant
+      case MF_RADIANS: o = __fmul_rn(v, __int_as_float(0x3c8efa35)); break;  // (PI as f32) / 180.0f32
+      default: o = v == 0.0f ? 0.0f : copysignf(1.0f, v); break;         // signum: DataFusion maps ±0 to 0.0
+    }
+    r = (double)o;
+  } else {
+    switch (g) {
+      case MF_SQRT: r = sqrt(x); break;
+      case MF_CBRT: r = cbrt(x); break;
+      case MF_EXP: r = exp(x); break;
+      case MF_LN: r = log(x); break;
+      case MF_LOG2: r = log2(x); break;
+      case MF_LOG10: r = log10(x); break;
+      case MF_SIN: r = sin(x); break;
+      case MF_COS: r = cos(x); break;
+      case MF_TAN: r = tan(x); break;
+      case MF_ASIN: r = asin(x); break;
+      case MF_ACOS: r = acos(x); break;
+      case MF_ATAN: r = atan(x); break;
+      case MF_SINH: r = sinh(x); break;
+      case MF_COSH: r = cosh(x); break;
+      case MF_TANH: r = tanh(x); break;
+      case MF_ASINH: r = asinh(x); break;
+      case MF_ACOSH: r = acosh(x); break;
+      case MF_ATANH: r = atanh(x); break;
+      case MF_DEGREES: r = __dmul_rn(x, math_word(0x404ca5dc1a63c1f8ull)); break;  // 180.0 / PI, correctly rounded
+      case MF_RADIANS: r = __dmul_rn(x, math_word(0x3f91df46a2529d39ull)); break;  // PI / 180.0
+      default: r = x == 0.0 ? 0.0 : copysign(1.0, x); break;
+    }
+  }
+  if (r != r) r = math_word(g == MF_LOG10 || g == MF_ASIN || g == MF_ACOS ? MATH_NAN_POS : MATH_NAN_NEG);
+  return fn == MF_COT ? math_x86_div(1.0, r, f32) : r;
+}
+// two-argument float function fn (MathFn2)
+__device__ __noinline__ double math2(int fn, bool f32, double a, double b) {
+  switch (fn) {
+    case MF2_NANVL: return a != a ? b : a;  // the operand itself, bits included
+    case MF2_LOG: return math_x86_div(math1(MF_LN, f32, b), math1(MF_LN, f32, a), f32);  // Rust x.log(base) = ln(x) / ln(base)
+    case MF2_ATAN2:  // glibc's atan2(y, x) returns a NaN x before a NaN y
+      if (b != b) return math_quiet(b);
+      if (a != a) return math_quiet(a);
+      return f32 ? (double)atan2f((float)a, (float)b) : atan2(a, b);
+    default: {  // pow (Float64 only), as glibc's: C99 Annex F's pow(x, ±0) = 1 and pow(1, y) = 1 even for a quiet NaN (a
+                // signalling one comes back quieted), then a NaN x before a NaN y; a NaN x to an odd integer power loses its sign
+      const bool snan_a = a != a && !(__double_as_longlong(a) & 0x0008000000000000ll);
+      const bool snan_b = b != b && !(__double_as_longlong(b) & 0x0008000000000000ll);
+      if ((b == 0.0 && !snan_a) || (a == 1.0 && !snan_b)) return 1.0;
+      if (a != a) {
+        const bool odd = fabs(b) < 9007199254740992.0 && trunc(b) == b && fmod(b, 2.0) != 0.0;
+        return math_word((unsigned long long)__double_as_longlong(math_quiet(a)) & (odd ? 0x7FFFFFFFFFFFFFFFull : ~0ull));
+      }
+      if (b != b) return math_quiet(b);
+      const double r = pow(a, b);
+      return r == r ? r : math_word(MATH_NAN_NEG);
+    }
+  }
+}
+// Int64 function fn (MathFnI); *err = the error word's code (0: none)
+__device__ __noinline__ int64_t math_i64(int fn, int64_t a, int64_t b, unsigned int* err) {
+  if (fn == MFI_FACTORIAL) {
+    if (a > 20) *err = 1;  // 21! > i64::MAX
+    int64_t r = 1;
+    for (int64_t i = 2; i <= a && i <= 20; i++) r *= i;
+    return r;
+  }
+  if (fn == MFI_POW) {  // Rust's i64::checked_pow(a, b as u32)
+    if (b < 0 || b > 0xFFFFFFFFll) {
+      *err = 8;
+      return 0;
+    }
+    int64_t acc = 1, base = a;
+    uint64_t e = (uint64_t)b;
+    while (e) {
+      if (e & 1) {
+        const __int128 p = (__int128)acc * base;
+        if (p != (__int128)(int64_t)p) return *err = 1, 0;
+        acc = (int64_t)p;
+        if (e == 1) break;
+      }
+      e >>= 1;
+      const __int128 q = (__int128)base * base;
+      if (q != (__int128)(int64_t)q) return *err = 1, 0;
+      base = (int64_t)q;
+    }
+    return acc;
+  }
+  // gcd / lcm over the magnitudes (unsigned: |i64::MIN| = 2^63)
+  const uint64_t ua = a < 0 ? 0 - (uint64_t)a : (uint64_t)a, ub = b < 0 ? 0 - (uint64_t)b : (uint64_t)b;
+  uint64_t x = ua, y = ub;
+  while (y) {
+    const uint64_t t = x % y;
+    x = y;
+    y = t;
+  }
+  if (fn == MFI_GCD) {
+    if (x > (uint64_t)INT64_MAX) *err = 1;  // gcd(i64::MIN, 0) and gcd(i64::MIN, i64::MIN) are 2^63
+    return (int64_t)x;
+  }
+  if (ua == 0 || ub == 0) return 0;
+  const uint64_t q = ua / x;
+  if (__umul64hi(q, ub) != 0 || q * ub > (uint64_t)INT64_MAX) *err = 1;
+  return (int64_t)(q * ub);
+}
+__device__ __noinline__ void scalar_math_op(const Lane L, const uint32_t active, const int pc) {
+  const VInstr ins = PROG.code[pc];
+  const uint32_t va = fetch_valid(L, ins.a);
+  const uint32_t vb = ins.b.kind != OPD_NONE ? fetch_valid(L, ins.b) : 0xFFFFFFFFu;
+  const uint32_t live = active & va & vb;
+  const bool boolean = ins.op == OP_MATH1 && (ins.aux == MF_ISNAN || ins.aux == MF_ISZERO);
+  uint32_t bmask = 0;
+#pragma unroll 1
+  for (int r = 0; r < VM_R; r++) {
+    if (ins.op == OP_MATH_I64) {
+      unsigned int err = 0;
+      const int64_t o = math_i64(ins.aux, ld1_i64(L, ins.a, r), ins.b.kind != OPD_NONE ? ld1_i64(L, ins.b, r) : 0, &err);
+      if (err && ((live >> r) & 1)) raise(err);
+      st1_i64(L, ins.dst, r, o);
+      continue;
+    }
+    const double x = ld1_f64(L, ins.a, r);
+    const bool f32 = (ins.op == OP_TRUNC ? ins.aux : ins.imm) == PH_F32;
+    if (boolean) {
+      bmask |= (ins.aux == MF_ISNAN ? x != x : x == 0.0) ? 1u << r : 0u;
+    } else if (ins.op == OP_MATH1) {
+      st1_f64(L, ins.dst, r, math1(ins.aux, f32, x));
+    } else if (ins.op == OP_MATH2) {
+      st1_f64(L, ins.dst, r, math2(ins.aux, f32, x, ld1_f64(L, ins.b, r)));
+    } else {  // OP_TRUNC: trunc(x * f) / f, each step rounded once, as OP_ROUND
+      const double f = __longlong_as_double((long long)PROG.imms[ins.imm].lo);
+      double o = math_quiet(x);
+      if (x != x) {
+      } else if (f32) o = (double)__fdiv_rn(truncf(__fmul_rn((float)x, (float)f)), (float)f);
+      else o = __ddiv_rn(trunc(__dmul_rn(x, f)), f);
+      st1_f64(L, ins.dst, r, o);
+    }
+  }
+  if (boolean) store_bool(L, ins.dst, bmask);
+  store_valid(L, ins.dst, va & vb);
+}
+
+// ------------------------------------------------------------------------------------------------
 // Cold operations: one rolled loop over the thread's rows; every body exists once in the binary.
 // ------------------------------------------------------------------------------------------------
 template <bool SFN>
@@ -1041,6 +1226,7 @@ __device__ __noinline__ void cold_op(const Lane L, const uint32_t active, const 
   if (SFN && PROG.code[pc].op >= OP_ABS) {  // the scalar functions (see run_generic)
     const uint8_t op = PROG.code[pc].op;
     if (op <= OP_CEIL) scalar_num_op(L, active, pc);
+    else if (op >= OP_MATH1) scalar_math_op(L, active, pc);
     else if (op == OP_NULLIF) scalar_nullif_op(L, active, pc);
     else if (op == OP_REGEX) scalar_regex_op(L, active, pc);
     else if (op == OP_REGEX_COUNT) scalar_regex_count_op(L, active, pc);

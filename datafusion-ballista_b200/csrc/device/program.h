@@ -102,8 +102,20 @@ enum VOp : uint8_t {
   // immediates, the forward DFA and the reverse one (device pointer in lo, shape in hi); the first one's _pad holds the
   // code points the count skips (start - 1, saturated)
   OP_REGEX_COUNT,   // a: STR -> I64, never NULL (scalar_regex_count_op)
-  OP_REGEX_REPLACE  // a: STR, b: the replacement (STR literal) -> STR in the arena; aux: 1 = every match (g) (scalar_regex_replace_op)
+  OP_REGEX_REPLACE, // a: STR, b: the replacement (STR literal) -> STR in the arena; aux: 1 = every match (g) (scalar_regex_replace_op)
+  // math functions (scalar_math_op; DESIGN.md §6 (xviii)).  t = VK_F64 for the float ones, which hold a Float32 value
+  // widened to binary64 and compute in f32 when imm (OP_MATH1 / OP_MATH2) or aux (OP_TRUNC) says PH_F32
+  OP_MATH1,      // dst = f(a); aux = MathFn1; imm = PH_F32 or 0.  MF_ISNAN / MF_ISZERO give BOOL
+  OP_MATH2,      // dst = f(a, b), both of one float type; aux = MathFn2; imm = PH_F32 or 0
+  OP_MATH_I64,   // dst = f(a[, b]) over Int64, checked (raise 1 on overflow, 8 on a power exponent outside 0..2^32-1); aux = MathFnI
+  OP_TRUNC       // t = VK_F64; trunc(a * f) / f; imm = immediate idx of the factor f (round's); aux = PH_F32 for f32 arithmetic
 };
+enum MathFn1 : uint8_t {
+  MF_SQRT = 0, MF_CBRT, MF_EXP, MF_LN, MF_LOG2, MF_LOG10, MF_SIN, MF_COS, MF_TAN, MF_ASIN, MF_ACOS, MF_ATAN, MF_SINH,
+  MF_COSH, MF_TANH, MF_ASINH, MF_ACOSH, MF_ATANH, MF_COT, MF_DEGREES, MF_RADIANS, MF_SIGNUM, MF_ISNAN, MF_ISZERO
+};
+enum MathFn2 : uint8_t { MF2_LOG = 0, MF2_ATAN2, MF2_NANVL, MF2_POW };  // MF2_LOG: a = base, b = x
+enum MathFnI : uint8_t { MFI_POW = 0, MFI_GCD, MFI_LCM, MFI_FACTORIAL };
 enum BuildFlags : uint8_t {
   BUILD_NULLS = 1,  // `||`: NULL if any argument is NULL (else NULL arguments are skipped: concat, concat_ws)
   BUILD_WS = 2      // concat_ws: operand a is the separator, written between the present arguments; NULL iff it is

@@ -995,6 +995,7 @@ static void throw_run_error(unsigned int error) {
   if (error == 5) throw EngineError(B200_ERR_EXECUTION, "repeat: a result row is longer than 2147483647 bytes");
   if (error == 6) throw EngineError(B200_ERR_EXECUTION, "CAST(Date32 AS Utf8): a date outside chrono's range (years -262144..262143)");
   if (error == 7) throw EngineError(B200_ERR_EXECUTION, "regexp_replace: a result row is longer than 2147483647 bytes");
+  if (error == 8) throw EngineError(B200_ERR_EXECUTION, "power: an Int64 exponent outside 0..4294967295");
   if (error) throw EngineError(B200_ERR_EXECUTION, "execution error in expression");
 }
 

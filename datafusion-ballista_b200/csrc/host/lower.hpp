@@ -513,6 +513,73 @@ class PipelineBuilder {
     return *e.args[i];
   }
 
+  // round's and trunc's factor f = 10^n (1 / 10^-n for n < 0; in f32 for a Float32 result) as an immediate, fi = its
+  // index; false when the digit count n is a NULL literal (the result is NULL)
+  bool digit_factor(const Expr& e, int& fi) {
+    int64_t n = 0;
+    if (e.args.size() > 1) {
+      const Expr& d = literal_arg(e, 1, "the digit count");
+      if (d.lit.is_null) return false;
+      n = d.lit.i;
+    }
+    if (n > 22 || n < -22) throw EngineError(B200_ERR_UNSUPPORTED, e.fn + " to " + std::to_string(n) + " digits is not supported (|digits| <= 22)");
+    double p = 1;
+    for (int64_t i = 0; i < (n < 0 ? -n : n); i++) p *= 10;  // exact: 10^22 is the largest power of ten binary64 holds
+    const bool f32 = e.type.id == TypeId::Float32;
+    LitValue fl;
+    fl.f = f32 ? (n >= 0 ? (double)(float)p : (double)(1.0f / (float)p)) : (n >= 0 ? p : 1.0 / p);
+    fi = literal(DataType(TypeId::Float64), fl).op.idx;
+    return true;
+  }
+
+  // two-operand function: dst = op(a, b), NULL where either is
+  ColRef binary_fn(const Expr& e, uint8_t op, uint8_t t, uint8_t aux, int32_t imm) {
+    ColRef a = compile(*e.args[0]);
+    pin(a);
+    ColRef b = compile(*e.args[1]);
+    unpin(a);
+    ColRef r = new_reg(e.type, a.nullable || b.nullable);
+    VInstr ins = blank(op, t);
+    ins.a = resolve(a);
+    ins.b = resolve(b);
+    ins.dst = r.op;
+    ins.aux = aux;
+    ins.imm = imm;
+    if (a.nullable || b.nullable) ins.flags |= IF_NULLCHK;
+    emit(ins);
+    release(a);
+    release(b);
+    return r;
+  }
+
+  // the math functions of DESIGN.md §6 (xviii); typing has checked the argument types and counts
+  ColRef compile_math_fn(const Expr& e) {
+    const std::string& f = e.fn;
+    const int32_t f32 = e.args.size() && e.args[0]->type.id == TypeId::Float32 ? PH_F32 : 0;
+    const int m1 = math_fn1_index(f);
+    if (m1 >= 0) return unary_fn(e, OP_MATH1, VK_F64, (uint8_t)m1, f32);
+    if (f == "pi") {
+      LitValue l;
+      l.f = 3.14159265358979323846;  // std::f64::consts::PI
+      return literal(DataType(TypeId::Float64), l);
+    }
+    if (f == "log") {
+      if (e.args.size() == 1) return unary_fn(e, OP_MATH1, VK_F64, MF_LOG10, f32);
+      return binary_fn(e, OP_MATH2, VK_F64, MF2_LOG, f32);
+    }
+    if (f == "atan2" || f == "nanvl") return binary_fn(e, OP_MATH2, VK_F64, f == "atan2" ? MF2_ATAN2 : MF2_NANVL, f32);
+    if (f == "power") {
+      if (e.type.id == TypeId::Float64) return binary_fn(e, OP_MATH2, VK_F64, MF2_POW, 0);
+      return binary_fn(e, OP_MATH_I64, VK_I64, MFI_POW, 0);
+    }
+    if (f == "gcd" || f == "lcm") return binary_fn(e, OP_MATH_I64, VK_I64, f == "gcd" ? MFI_GCD : MFI_LCM, 0);
+    if (f == "factorial") return unary_fn(e, OP_MATH_I64, VK_I64, MFI_FACTORIAL, 0);
+    // trunc
+    int fi = -1;
+    if (!digit_factor(e, fi)) return null_of(e.type);
+    return unary_fn(e, OP_TRUNC, VK_F64, (uint8_t)f32, fi);
+  }
+
   // the scalar functions of DESIGN.md §3 besides date_part and substr; typing (plan.hpp) has checked the argument types
   ColRef compile_scalar_fn(const Expr& e) {
     const std::string& f = e.fn;
@@ -523,21 +590,11 @@ class PipelineBuilder {
     }
     if (f == "floor" || f == "ceil") return unary_fn(e, f == "floor" ? OP_FLOOR : OP_CEIL, VK_F64, 0, 0);
     if (f == "round") {
-      int64_t n = 0;
-      if (e.args.size() > 1) {
-        const Expr& d = literal_arg(e, 1, "the digit count");
-        if (d.lit.is_null) return null_of(e.type);
-        n = d.lit.i;
-      }
-      if (n > 22 || n < -22) throw EngineError(B200_ERR_UNSUPPORTED, "round to " + std::to_string(n) + " digits is not supported (|digits| <= 22)");
-      double p = 1;
-      for (int64_t i = 0; i < (n < 0 ? -n : n); i++) p *= 10;  // exact: 10^22 is the largest power of ten binary64 holds
-      const bool f32 = e.type.id == TypeId::Float32;
-      LitValue fl;
-      fl.f = f32 ? (n >= 0 ? (double)(float)p : (double)(1.0f / (float)p)) : (n >= 0 ? p : 1.0 / p);
-      const int fi = literal(DataType(TypeId::Float64), fl).op.idx;
-      return unary_fn(e, OP_ROUND, VK_F64, f32 ? PH_F32 : 0, fi);
+      int fi = -1;
+      if (!digit_factor(e, fi)) return null_of(e.type);
+      return unary_fn(e, OP_ROUND, VK_F64, e.type.id == TypeId::Float32 ? PH_F32 : 0, fi);
     }
+    if (is_math_fn(f)) return compile_math_fn(e);
     if (f == "character_length" || f == "octet_length") return unary_fn(e, f == "octet_length" ? OP_OCTET_LENGTH : OP_CHAR_LENGTH, VK_STR, 0, 0);
     if (f == "btrim" || f == "ltrim" || f == "rtrim") {
       int set = -1;
